@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- KKT LDL^T factor+solve throughput of the B200 backend (contract: see the task statement).
+"""bench.py -- KKT LDL^T factor+solve throughput of the GPU backend on an H100.
 
 A "step" = the linear algebra of ONE interior-point iteration: one numeric factorisation of a new KKT matrix (inertia
 check on) + two back-solves (step + one refinement), the call pattern measured on the reference's IP loop (SURVEY.md 8c:
@@ -13,19 +13,23 @@ the single-GPU time of the same N=800 step measured in the same run and printed 
   e2e   : the same through the reference-facing C-ABI calls with HOST buffers (b200ldlt_factor reads the pinned
           values array Ipopt fills, b200ldlt_solve takes/returns host rhs) -- H2D/D2H inside the timed region.
   roofline : the HBM-bound triangular solve (bottom-level kernels + the two persistent sweeps): algorithmic bytes 2*8*nnz(L) +
-          vector traffic (SURVEY.md 8d) / their measured duration, against MEASURED_PEAKS.json's hbm_gbs;
-          roofline_schur: the Schur-complement GEMM's pipe utilisation from the committed ncu export.
+          vector traffic (SURVEY.md 8d) / their measured duration, against MEASURED_PEAKS.json's hbm_gbs when present,
+          else the H100 SXM data-sheet HBM3 bandwidth (3350 GB/s).
   cpu_baseline : the CPU oracle (oracle/cpu_ldlt.cpp, "port") on the host cores on the same matrix.  The reference's own
           comparator, MUMPS, is probed for at run time (ldconfig / pkg-config) and is absent from this image.
   ip_loop : the reference's unmodified interior-point loop (tests/driver/ipopt_driver) on the same problem with the
-          B200 backend and with the CPU oracle: iterations, wall seconds, IP iterations per second.
+          GPU backend and with the CPU oracle: iterations, wall seconds, IP iterations per second.
 --impl reference times the CPU path alone, same steps / warm-up as the product arm.
+--dump-outputs DIR writes, after the timed steps, what the timed path returned to its caller in its last step: the
+          solution vector (solution.npy, float64) and the inertia / status of the factorisation (factor.npy, float64:
+          [status, number of negative eigenvalues]).  The inputs are the same from run to run with the same arguments.
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -82,7 +86,7 @@ def get_snapshots(rank, N=None, backend="oracle"):
     import struct
     N = N or WORKLOAD_N
     drv = os.path.join(ROOT, "tests", "driver", "ipopt_driver")
-    cache = os.path.join("/tmp", "b200_bench_snap_%d" % N)
+    cache = os.path.join(tempfile.gettempdir(), "b200_bench_snap_%d" % N)
     paths = [cache + "_%d.bin" % k for k in SNAP_ITERS]
     src = "reference IP loop (MBndryCntrl1 N=%d) KKT snapshots at factorisations %s" % (N, SNAP_ITERS)
     if rank == 0 and not all(os.path.exists(p) for p in paths) and os.path.exists(drv):
@@ -151,6 +155,7 @@ def time_oracle(snaps, steps, warmup, threads):
     o = OracleLdlt()
     o.InitializeStructure(s0["dim"], len(s0["irn"]), s0["irn"], s0["jcn"])
     t_steps = []
+    last = None
     for it in range(warmup + steps):
         sn = snaps[it % len(snaps)]
         t0 = time.perf_counter()
@@ -163,7 +168,15 @@ def time_oracle(snaps, steps, warmup, threads):
         dt = time.perf_counter() - t0
         if it >= warmup:
             t_steps.append(dt)
-    return float(np.mean(t_steps)), o.stats()
+        last = (x, st, neg)
+    return float(np.mean(t_steps)), o.stats(), last
+
+
+def dump_outputs(out_dir, x, status, neg):
+    """What the timed path handed its caller in the last timed step (float64, a few MB at the benchmark sizes)."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "solution.npy"), np.ascontiguousarray(x, dtype=np.float64))
+    np.save(os.path.join(out_dir, "factor.npy"), np.array([status, neg], dtype=np.float64))
 
 
 def main():
@@ -172,6 +185,8 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (solution, inertia) as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -184,7 +199,7 @@ def main():
     wl_dim = wl_N * wl_N * 2 + 4 * wl_N
     config = {"workload": "MBndryCntrl1 N=%d KKT (dim %d): 1 numeric LDL^T + 2 back-solves per step" % (wl_N, wl_dim),
               "parallelism": ("elimination-tree sharding over %d GPUs" % world) if world > 1 else "single GPU",
-              "l2_policy": "working set (L + contribution blocks: hundreds of MB) exceeds the 126 MB L2; 3 different matrices cycled",
+              "l2_policy": "working set (L + contribution blocks: hundreds of MB) exceeds the 50 MB L2; 3 different matrices cycled",
               "scaling_note": "one KKT system per step on all GPUs (strong scaling); --gpus 1 runs BASELINE config 3 (N=400, the metric's configuration), --gpus > 1 config 5 (N=800, the one north_star shards) with its single-GPU time in the same line"}
 
     if args.impl == "reference":
@@ -193,7 +208,9 @@ def main():
         if rank != 0:
             return 0
         snaps, src = get_snapshots_nodist(wl_N)
-        sec, st = time_oracle(snaps, K, W, cpu_threads)
+        sec, st, (x_last, st_last, neg_last) = time_oracle(snaps, K, W, cpu_threads)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, x_last, st_last, neg_last)
         line = {"impl": "reference", "metric": "kkt_factor_solve_iters_per_sec", "value": 1.0 / sec, "unit": "iter/s",
                 "n_gpus": args.gpus, "steps": K, "warmup": W, "ms_per_step": sec * 1e3, "higher_is_better": True,
                 "scaling": "strong", "vs_baseline": None, "dtype": "f64", "data": src, "config": config,
@@ -212,7 +229,7 @@ def main():
     from ipopt_b200 import B200Ldlt
 
     if world > 1:
-        # config 5 (N=800): the snapshots come from the reference IP loop driven by the B200 backend itself on rank 0
+        # config 5 (N=800): the snapshots come from the reference IP loop driven by the GPU backend itself on rank 0
         # (the CPU oracle needs minutes per run at this size)
         snaps, src = get_snapshots(rank, SHARDED_N, backend="b200")
         return run_sharded(args, snaps, src, config, rank, local_rank, world, K, W, host_cores)
@@ -236,12 +253,14 @@ def main():
     d_work = torch.empty(dim, dtype=torch.float64, device="cuda")
     h_rhs = [sn["rhs"].copy() for sn in snaps]
     launches = 0
+    last_factor = [None, None]
 
     def step_device(i):
         nonlocal launches
         sn = snaps[i % len(snaps)]
         st, neg = solver.factor_device(d_vals[i % len(snaps)].data_ptr(), True, sn["neg"])
         assert st == 0, (st, solver.last_error())
+        last_factor[:] = [st, neg]
         launches += solver.info()["launches_factor"]
         for _ in range(2):
             d_work.copy_(d_rhs0[i % len(snaps)])
@@ -287,6 +306,8 @@ def main():
     launches = 0
     ms_dev, _ = timed(step_device)
     launches_timed = launches * K // (K + W)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_work.cpu().numpy(), *last_factor)
     ms_e2e, wall_e2e = timed(step_host)
     ms_e2e = max(ms_e2e, wall_e2e)   # host fill + memcpy of the step are part of the end-to-end time
 
@@ -317,38 +338,13 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        ncu = {}
-        try:   # figures read from the committed ncu exports (profiles/r2_ncu_metrics.json, made by scripts/ncu_extract.py)
-            ncu = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_metrics.json")))
-        except Exception:
-            pass
-        # DRAM bytes of ONE solve (all its launches) and the pipe utilisation of the Schur-complement kernels, from the committed
-        # `ncu --set full` exports of this workload (profiles/r2_final_*_raw.csv, summarised in r2_ncu_metrics.json)
-        kern = ncu.get("kernels", {})
-        solve_traffic, solve_traffic_src, schur_entry = None, None, None
-        if dim == 321600 and kern.get("r2final_solve"):
-            solve_traffic = sum((r.get("dram_read_bytes") or 0) + (r.get("dram_write_bytes") or 0) for r in kern["r2final_solve"])
-            solve_traffic_src = "profiles/r2_r2final_solve_raw.csv: dram__bytes_read.sum + dram__bytes_write.sum over the %d launches of one solve" % len(kern["r2final_solve"])
-        if kern.get("r2final_schur") or kern.get("r2e_tc"):
-            def pick(rows, name):
-                rows = [r for r in rows if name in r["kernel"]]
-                if not rows:
-                    return None
-                return {"launches": len(rows), "fp64_pipe_pct": float(np.mean([r.get("fp64_pipe_pct") or 0 for r in rows])),
-                        "tensor_pipe_pct": float(np.mean([r.get("tensor_pipe_pct") or 0 for r in rows])),
-                        "mean_us": float(np.mean([r.get("duration_s") or 0 for r in rows]))}
-            schur_entry = {"default_path": "k_big_update_cb: FP64 DFMA rank-32 updates of the contribution block, one per panel, behind the pivot chain",
-                           "k_big_update_cb": pick(kern.get("r2final_schur", []), "k_big_update_cb"),
-                           "tensor_core_path_opt_in": "k_tc_schur: tcgen05.mma kind::i8 Ozaki split (tc_schur_min_r), MBndryCntrl1 N=800",
-                           "k_tc_schur": pick(kern.get("r2e_tc", []), "k_tc_schur"),
-                           "source": "profiles/r2_r2final_schur_raw.csv, profiles/r2_r2e_tc_raw.csv (sm__pipe_fp64_cycles_active / sm__pipe_tensor_cycles_active, % of peak)"}
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
         nnzL = info["nnz_L"]
         tri_bytes = 2 * 8 * nnzL + 8 * 4 * dim   # L streamed twice + 2 reads/2 writes of the vector (SURVEY.md 8d)
         ach = tri_bytes / (tri_ms * 1e-3) / 1e9
         # CPU baseline, bounded sample on the host cores of this box
         # the oracle's rank-1 updates are memory-bound: more threads are not always faster -> report the best of a few
-        skip_cpu = bool(os.environ.get("B200_BENCH_SKIP_CPU"))   # profiling runs under ncu only (the CPU leg is minutes there)
+        skip_cpu = bool(os.environ.get("B200_BENCH_SKIP_CPU"))   # GPU-only runs (the CPU legs take minutes)
         cands = sorted({t for t in (8, 16, cpu_threads) if t <= cpu_threads})
         trials = [(time_oracle(snaps, 1, 0, t)[0], t) for t in cands[:-1]] if len(cands) > 1 and not skip_cpu else []
         best_t = min(trials)[1] if trials else cpu_threads
@@ -374,10 +370,8 @@ def main():
                                              "factor_ms": fac_ms, "solve_ms_per_rhs": tri_ms},
             "roofline": {"kernel": "supernodal triangular solve, all launches of one right-hand side (k_rhs_in, k_solve_direct x2 levels, k_solve<fwd>, k_solve<bwd>, k_solve_direct x2, k_sol_out)",
                          "bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak,
-                         "traffic": solve_traffic, "traffic_source": solve_traffic_src,
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (burst)" if peaks else "fallback 6650",
+                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (burst)" if peaks else "H100 SXM data sheet (3.35 TB/s HBM3)",
                          "algorithmic_bytes_per_solve": tri_bytes},
-            "roofline_schur": schur_entry,
             "factor": {"flops_panel": info["flops_panel"], "flops_schur": info["flops_schur"],
                        "gflops_achieved": (info["flops_panel"] + info["flops_schur"]) / (fac_ms * 1e-3) / 1e9,
                        "nnz_L": nnzL, "supernodes": info["nsupernodes"], "levels": info["nlevels"], "max_front": info["max_front"]},
@@ -437,12 +431,15 @@ def run_sharded(args, snaps, src, config, rank, local_rank, world, K, W, host_co
     d_vals = [torch.from_numpy(sn["val"]).cuda() for sn in snaps]
     d_rhs = [torch.from_numpy(sn["rhs"]).cuda() for sn in snaps]
 
+    last = [None, None, None]
+
     def step_device(i):
         sn = snaps[i % len(snaps)]
         st, neg = sh.factor_device(d_vals[i % len(snaps)], True, sn["neg"])
         assert st == 0 and neg == sn["neg"], (st, neg)
         for _ in range(2):
-            sh.solve_device(d_rhs[i % len(snaps)])
+            x = sh.solve_device(d_rhs[i % len(snaps)])
+        last[:] = [x, st, neg]
 
     def step_host(i):
         sn = snaps[i % len(snaps)]
@@ -473,6 +470,8 @@ def run_sharded(args, snaps, src, config, rank, local_rank, world, K, W, host_co
     if rank == 0:
         sampler.start()
     ms_dev, wall_dev = timed(step_device)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[0].cpu().numpy(), last[1], last[2])
     ms_e2e, wall_e2e = timed(step_host)
     ms_dev, ms_e2e = max(ms_dev, wall_dev), max(ms_e2e, wall_e2e)
     sampler.stop_flag = True

@@ -1,4 +1,4 @@
-/* b200ldlt -- C ABI of the B200-native sparse symmetric-indefinite LDL^T backend.
+/* b200ldlt -- C ABI of the H100-native sparse symmetric-indefinite LDL^T backend.
  *
  * This is the drop-in boundary: one entry point per virtual of Ipopt's
  * SparseSymLinearSolverInterface (reference file
@@ -47,7 +47,7 @@ typedef struct b200ldlt_options {
   int use_graph;       /* 1 = replay numeric phases from CUDA graphs */
   int verbose;
   int tc_schur_min_r;  /* fronts with >= this many contribution rows form their Schur complement on the tensor cores
-                          (tcgen05 int8 Ozaki split, csrc/schur_tc.cu); 0 = off (FP64 DFMA tiles everywhere) */
+                          (wgmma int8 Ozaki split, csrc/schur_tc.cu); 0 = off (FP64 DFMA tiles everywhere) */
 } b200ldlt_options;
 
 /* statistics of the last analyse/factor/solve (algorithmic work per SURVEY.md section 8d) */

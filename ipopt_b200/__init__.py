@@ -1,4 +1,4 @@
-"""ipopt_b200 -- B200-native KKT (symmetric indefinite LDL^T) backend for coin-or/Ipopt.
+"""ipopt_b200 -- H100-native KKT (symmetric indefinite LDL^T) backend for coin-or/Ipopt.
 
 The product is the C-ABI shared library ``ipopt_b200/lib/libb200ldlt.so`` (see ``include/b200ldlt.h``);
 this package holds its sources (``csrc/``), the Ipopt-side plugin (``plugin/``) and a thin ctypes

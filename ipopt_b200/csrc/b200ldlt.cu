@@ -1,4 +1,4 @@
-// Host orchestration + extern "C" shim of the B200 LDL^T backend (see include/b200ldlt.h).
+// Host orchestration + extern "C" shim of the GPU LDL^T backend (see include/b200ldlt.h), H100 / sm_90a.
 // One translation unit: the kernels are included so nvcc sees launch sites and definitions together.
 #include "../../include/b200ldlt.h"
 #include "../../include/b200vec.h"
@@ -118,7 +118,8 @@ struct DebugSwitches {
     if (const char* e = getenv("B200_BUCKETS")) {
       for (const char* p = e; *p;) { buckets.push_back(atoi(p)); while (*p && *p != ',') ++p; if (*p) ++p; }
     } else {
-      buckets = {48, 96};   // the classes of a level run side by side, so a finer split costs no serial launches (measured: -0.1 ms at N=400)
+      buckets = {48, 96};   // the classes of a level run side by side, so a finer split costs no serial launches
+                            // (H100 SXM, 700 W, factorisation at N=400 / 800: {96} and {32,64,96} within 0.4 %)
     }
   }
 };
@@ -192,7 +193,7 @@ struct Solver {
   std::vector<char> solve_direct_front;   // per supernode: solved by k_solve_direct (see build_solve_tables)
   int solve_epoch = 0, df_grid = 0;
   unsigned long long ticket_f = 0, ticket_b = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   struct Shard {
     bool active = false;
     int rank = 0, world = 1, nsub = 0;
@@ -1094,7 +1095,7 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
         const TcFront* tf = SL.d_f.p + P.tc_f_off;
         k_tc_slice<<<dim3(cdiv(P.tc_rmax, 8), P.tc_f_cnt), 256, 0, st>>>(D, N, tf, 0, sv->d_tc_dig.p, sv->d_tc_exp.p); ++L;
         k_tc_slice<<<dim3(cdiv(P.tc_rmax, 8), P.tc_f_cnt), 256, 0, st>>>(D, N, tf, 1, sv->d_tc_dig.p, sv->d_tc_exp.p); ++L;
-        k_tc_schur<<<P.tc_t_cnt, 192, TC_SMEM_BYTES, st>>>(D, N, tf, SL.d_t.p + P.tc_t_off, sv->d_tc_dig.p, sv->d_tc_exp.p); ++L;
+        k_tc_schur<<<P.tc_t_cnt, TC_THREADS, TC_SMEM_BYTES, st>>>(D, N, tf, SL.d_t.p + P.tc_t_off, sv->d_tc_dig.p, sv->d_tc_exp.p); ++L;
       }
       if (!cb_panel && P.df_cnt > 0) {
         k_big_schur84<<<dim3(cdiv(P.df_rmax, TM), cdiv(P.df_rmax, TM), P.df_cnt), 128, 0, st>>>(D, N, SL.d_dfl.p + P.df_off); ++L;
@@ -1348,12 +1349,14 @@ void b200ldlt_default_options(b200ldlt_options* o) {
   o->ordering = 0;
   o->pair_saddle = 1;
   o->leaf_k = 32;
-  o->relax_frac = 0.05;   // measured on the B200 (profiles/r2_summary.md): 0.05 gives the shortest factorisation at N=400 and N=800 (0.15: +5..8 %)
+  o->relax_frac = 0.05;   // 5 % relaxed amalgamation (H100 SXM, 700 W: N=400 5.83 ms vs 6.13 at 0.02, 6.28 at 0.10;
+                          // N=800 21.2 ms vs 21.0 at 0.02, 22.8 at 0.10)
   o->scaling = 2;
   o->pivtol = 1e-8;
   o->pivtolmax = 1e-4;
   o->tiny = 1e-15;
-  o->smem_front_max = 96;    // measured (profiles/r2_summary.md): 64: 4.84, 96: 4.77, 128: 4.89 ms per N=400 factorisation
+  o->smem_front_max = 96;    // fronts of order 65..96 in shared memory, larger ones through the panel pipeline
+                             // (H100 SXM, 700 W: 64 and 128 are 1-2.5 % slower at N=400 and N=800)
   o->tc_schur_min_r = 0;
   o->use_graph = 1;   /* 1 = CUDA-graph replay of the factorisation + dataflow solve; 0 = plain launches; 2 = level-per-launch solve */
   o->verbose = 0;

@@ -258,7 +258,7 @@ __device__ __forceinline__ void tile_syrk(double* __restrict__ C, long long ldc,
 
 // --------------------------------------------------------------------------------------------
 // FP64 tensor-pipe version of the Schur-complement contraction: C[i,j] -= sum_t A[i,t] * B[j,t], lower tiles only,
-// with mma.sync.m8n8k4.f64 (DMMA - the only FP64 path of the tensor pipe; tcgen05 has no f64 kind).
+// with mma.sync.m8n8k4.f64 (DMMA - the only FP64 path of the tensor pipe; wgmma has no f64 type).
 // CTA tile 128x128, K step 16, 8 warps as 4(M) x 2(N), each warp 32x64 = 4 x 8 DMMA tiles (64 accumulators/thread).
 // Shared tiles As/Bs[16][132]: row stride 132 doubles (== 4 mod 16) makes the 64-bit fragment loads conflict-free.
 // --------------------------------------------------------------------------------------------

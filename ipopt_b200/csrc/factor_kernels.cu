@@ -1,4 +1,4 @@
-// Numeric factorisation kernels of the B200 supernodal multifrontal LDL^T (sm_100a).
+// Numeric factorisation kernels of the supernodal multifrontal LDL^T (sm_90a).
 //
 // What the reference delegates to the vendor library's numeric phase (MUMPS job=2,
 // reference src/Algorithm/LinearSolvers/IpMumpsSolverInterface.cpp:448-541): per front
@@ -99,12 +99,14 @@ __device__ __forceinline__ double warp_max(double v) {
   return v;
 }
 
-// warp-wide max of non-negative floats in ONE instruction (CREDUX.MAX.F32, sm_100a).  The pivot SEARCH runs on
-// float-rounded magnitudes (the tests are inequalities with slack >= 1e-8, the selected entries are then re-read exactly).
+// warp-wide max of floats in ONE reduction instruction: REDUX.MAX on an order-preserving integer image of the float
+// (non-negative floats keep their bits, negative ones -- the -1 "no candidate" sentinels -- get their magnitude bits
+// flipped), NaN ignored unless every lane holds one, as redux.sync.max.f32 does.  The pivot SEARCH runs on float-rounded
+// magnitudes (the tests are inequalities with slack >= 1e-8, the selected entries are then re-read exactly).
 __device__ __forceinline__ float wredux_max(float v) {
-  float m;
-  asm volatile("redux.sync.max.f32 %0, %1, 0xffffffff;" : "=f"(m) : "f"(v));
-  return m;
+  const int b = __float_as_int(v);
+  const int m = __reduce_max_sync(0xffffffffu, (v != v) ? INT_MIN : (b ^ ((b >> 31) & 0x7fffffff)));
+  return (m == INT_MIN) ? __int_as_float(0x7fffffff) : __int_as_float(m ^ ((m >> 31) & 0x7fffffff));
 }
 
 // The pivoted front factorisation runs either on a whole CTA (WARP=false, __syncthreads) or on a single

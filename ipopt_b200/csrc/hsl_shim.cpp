@@ -6,7 +6,7 @@
 //   ma97_default_control_d, ma97_analyse_d, ma97_factor_d, ma97_factor_solve_d, ma97_solve_d, ma97_finalise_d,
 //   ma97_free_akeep_d
 // with the prototypes and the ma97_control_d / ma97_info_d layouts of reference
-// src/Algorithm/LinearSolvers/hsl_ma97d.h:67-178.  This file exports those seven entry points on top of the B200
+// src/Algorithm/LinearSolvers/hsl_ma97d.h:67-178.  This file exports those seven entry points on top of the GPU
 // backend, so an UNMODIFIED Ipopt (AMPL ipopt, cyipopt, ...) runs its KKT factorisations on the GPU with an options-file
 // change only.  How the adapter uses them: :473-608 (analyse: CSC lower triangle, 1-based when f_arrays != 0, values may
 // be NULL), :610-800 (factor with matrix_type 4 = real symmetric indefinite, then solve job 0; info.num_neg is the

@@ -1,4 +1,4 @@
-// Device-side data descriptors shared by the numeric kernels (sm_100a).
+// Device-side data descriptors shared by the numeric kernels (sm_90a).
 #pragma once
 #include <cstdint>
 

@@ -1,23 +1,24 @@
-// Schur-complement contraction of the big fronts on the 5th-generation tensor cores (tcgen05 / TMEM), sm_100a.
+// Schur-complement contraction of the big fronts on the Hopper tensor cores (warpgroup MMA, wgmma), sm_90a.
 //
 //   CB -= L21 * (L21 D)^T            (the dense GEMM of a front: SURVEY.md 8d "Schur update GEMM")
 //
-// tcgen05.mma has no FP64 kind, so the FP64 product is computed EXACTLY-in-integers by an Ozaki split:
+// wgmma has no FP64 type, so the FP64 product is computed EXACTLY-in-integers by an Ozaki split:
 //   1. every row of A = L21 and of B = W21 = L21 D is scaled by a power of two so that |entry| <= 1/2, and cut into
 //      NS = 8 signed base-128 digits  x = sum_s d_s 2^(-7(s+1)),  |d_s| <= 64  (int8).  All steps are exact in FP64.
 //   2. for every digit pair (s, s') with s + s' < NS the int8 GEMM  A_s B_s'^T  runs on the tensor cores
-//      (tcgen05.mma.kind::i8, int32 accumulation in TMEM: exact -- |sum| <= 64*64*k*(NS) < 2^31 for k < 65536).
-//      Pairs with the same d = s + s' share one TMEM accumulator (same weight 2^(-7(d+2))): 8 accumulators of 64
-//      columns = the 512 TMEM columns of an SM.
-//   3. epilogue: tcgen05.ld the 8 accumulators, recombine in FP64 (int32 -> double is exact), undo the row scalings
-//      (exact) and subtract from the contribution block.
+//      (wgmma.mma_async .s32.s8.s8, int32 accumulation in registers: exact -- |sum| <= 64*64*k*(NS) < 2^31 for
+//      k < 65536).  Pairs with the same d = s + s' share one accumulator (same weight 2^(-7(d+2))): 8 accumulators.
+//   3. epilogue: recombine the 8 accumulators in FP64 (int32 -> double is exact), undo the row scalings (exact) and
+//      subtract from the contribution block.
 // The dropped pairs (s + s' >= NS) bound the error by ~ (NS+1) k 2^(12-7(NS+2)) = 9k 2^-58 relative to
 // rowscale_i * rowscale_j, i.e. below the rounding error k*2^-53*|A||B| of an FP64 GEMM for the k seen here.
 //
-// Data movement: the digit matrices are written by k_tc_slice directly in the shared-memory operand layout of UMMA
-// (K-major, no swizzle: 8-row x 16-byte core matrices), one contiguous unit per (row block, 32-column K step) holding all
-// 8 digits, so the GEMM kernel stages them with plain 1-D TMA bulk copies (cp.async.bulk + mbarrier) -- no tensor maps.
-// Warp roles (CTA = 192 threads): warp 0 = TMA producer, warp 1 = MMA issuer (one elected lane), warps 2-5 = epilogue.
+// Data movement: the digit matrices are written by k_tc_slice directly in the shared-memory operand layout of wgmma
+// (K-major, no swizzle: 8-row x 16-byte core matrices), one contiguous unit per (64-row block, 32-column K step) holding
+// all 8 digits, so the GEMM kernel stages them with plain 1-D TMA bulk copies (cp.async.bulk + mbarrier) -- no tensor maps.
+// Tile and warp roles: one CTA per 64 x 64 lower tile of the contribution block, 288 threads.  Warpgroups 0 and 1
+// (warps 0-7) each own 32 columns of the tile: 8 accumulators of m64n32 = 128 int32 registers per thread, which is what
+// bounds the tile (the 8 accumulators of a 64 x 64 tile fill half the register file of an SM).  Warp 8 is the TMA producer.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -26,16 +27,18 @@
 namespace b200 {
 
 #define TC_NS 8            // digits per operand
-#define TC_BM 128          // rows of A per tile (= UMMA M)
-#define TC_BN 64           // rows of B per tile (= UMMA N): 8 accumulators x 64 columns = 512 TMEM columns
-#define TC_BK 32           // K per UMMA instruction (int8)
+#define TC_BM 64           // rows of A per tile (= wgmma M)
+#define TC_BN 64           // rows of B per tile: two warpgroups x wgmma N = 32
+#define TC_WN 32           // columns of the tile per consumer warpgroup (wgmma N)
+#define TC_BK 32           // K per wgmma instruction (int8)
 #define TC_STAGES 4
-#define TC_A_UNIT (TC_NS * 2 * TC_BM * 16)   // bytes of one (128-row block, K step) unit of A digits  = 32 KB
-#define TC_B_UNIT (TC_NS * 2 * TC_BN * 16)   // bytes of one (64-row block, K step) unit of B digits   = 16 KB
+#define TC_THREADS 288     // 2 consumer warpgroups + 1 producer warp
+#define TC_A_UNIT (TC_NS * 2 * TC_BM * 16)   // bytes of one (64-row block, K step) unit of A digits  = 16 KB
+#define TC_B_UNIT (TC_NS * 2 * TC_BN * 16)   // bytes of one (64-row block, K step) unit of B digits  = 16 KB
 #define TC_STAGE_BYTES (TC_A_UNIT + TC_B_UNIT)
 #define TC_SMEM_BYTES (TC_STAGES * TC_STAGE_BYTES + 1024)
 
-// one big front's digit storage: A (L21) in 128-row blocks, B (W21) in 64-row blocks, nks = ceil(k / 32) K steps
+// one big front's digit storage: A (L21) and B (W21) in 64-row blocks, nks = ceil(k / 32) K steps
 struct TcFront {
   int s;                 // supernode
   int nks;               // K steps
@@ -43,14 +46,14 @@ struct TcFront {
   long long b_off;       // byte offset of its B units: [row block][K step] x TC_B_UNIT
   long long e_off;       // offset (ints) of its row exponents: ea[r] then eb[r]
 };
-struct TcTile { int fi, ti, tj; };   // front index in the TcFront list, 128-row block, 64-row block (lower tiles only)
+struct TcTile { int fi, ti, tj; };   // front index in the TcFront list, row block of A, row block of B (lower tiles only)
 
 // ------------------------------------------------------------------------------------------------
 // digit extraction.  One warp per row of the front's L21 / W21 (r rows, k columns, ld = f):
-// pass 1: row maximum -> exponent e with |x| 2^-e <= 1/2 ; pass 2: digits, written in the UMMA operand layout
+// pass 1: row maximum -> exponent e with |x| 2^-e <= 1/2 ; pass 2: digits, written in the wgmma operand layout
 //   unit(rowblock, kstep) : [digit s][k chunk j (16 bytes)][row in block][16 bytes]
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_tc_slice(DevSym S, DevNum N, const TcFront* __restrict__ fronts, int which /*0: A = L21 (128-row blocks), 1: B = W21 (64-row blocks)*/,
+__global__ void __launch_bounds__(256) k_tc_slice(DevSym S, DevNum N, const TcFront* __restrict__ fronts, int which /*0: A = L21, 1: B = W21*/,
                                                   int8_t* __restrict__ dig, int* __restrict__ expo) {
   const TcFront F = fronts[blockIdx.y];
   const int s = F.s;
@@ -117,152 +120,136 @@ __device__ __forceinline__ void tc_bulk_g2s(void* dst, const void* src, unsigned
                "l"(src), "r"(bytes), "r"(tc_smem_u32(bar))
                : "memory");
 }
-// UMMA shared-memory descriptor, K-major operand without swizzle (canonical layout ((8,m),2):((1,SBO),LBO) in 16-byte
-// units: cute/atom/mma_traits_sm100.hpp make_umma_desc<Major::K>, LayoutType::SWIZZLE_NONE)
+// wgmma shared-memory descriptor, K-major operand without swizzle (canonical layout ((8,m),(16 B,2)):((16 B,SBO),(1,LBO)):
+// LBO = byte distance of the two 16-byte K chunks, SBO = byte distance of consecutive 8-row core matrices)
 __device__ __forceinline__ unsigned long long tc_smem_desc(unsigned addr_bytes, unsigned lbo_bytes, unsigned sbo_bytes) {
   unsigned long long d = 0;
   d |= (unsigned long long)((addr_bytes >> 4) & 0x3fff);           // start address   bits [0,14)
   d |= (unsigned long long)((lbo_bytes >> 4) & 0x3fff) << 16;      // leading (K) byte offset  bits [16,30)
   d |= (unsigned long long)((sbo_bytes >> 4) & 0x3fff) << 32;      // stride (M/N) byte offset bits [32,46)
-  d |= 1ull << 46;                                                  // descriptor version 1 (Blackwell)  bits [46,48)
-  return d;                                                         // base offset 0, lbo mode 0, layout type 0 (no swizzle)
+  return d;                                                         // base offset 0, layout type 0 (no swizzle)
 }
-// instruction descriptor of tcgen05.mma.kind::i8: s8 x s8 -> s32, A and B K-major, M = 128, N = 64
-__device__ __forceinline__ unsigned tc_idesc() {
-  return (2u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(TC_BN >> 3) << 17) | ((unsigned)(TC_BM >> 4) << 24);
-}
-__device__ __forceinline__ void tc_mma_i8(unsigned tmem_d, unsigned long long adesc, unsigned long long bdesc, unsigned idesc, unsigned accumulate) {
+// D(64 x 32, s32) += A(64 x 32, s8, smem) * B(32 x 32, s8, smem)^T
+__device__ __forceinline__ void tc_wgmma_i8(int (&c)[16], unsigned long long adesc, unsigned long long bdesc) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n"
+      "}\n"
+      : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3]), "+r"(c[4]), "+r"(c[5]), "+r"(c[6]), "+r"(c[7]), "+r"(c[8]), "+r"(c[9]),
+        "+r"(c[10]), "+r"(c[11]), "+r"(c[12]), "+r"(c[13]), "+r"(c[14]), "+r"(c[15])
+      : "l"(adesc), "l"(bdesc), "r"(1)
       : "memory");
 }
-__device__ __forceinline__ void tc_commit(unsigned long long* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(tc_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_ld16(unsigned taddr, int (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
+__device__ __forceinline__ void tc_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void tc_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void tc_wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the accumulators in registers across the asynchronous MMAs (no spill / copy between issue and wait)
+__device__ __forceinline__ void tc_fence_acc(int (&c)[16]) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) asm volatile("" : "+r"(c[j])::"memory");
 }
 
 // ------------------------------------------------------------------------------------------------
-// the GEMM: one CTA per (front, 128 x 64) lower tile of the contribution block
+// the GEMM: one CTA per (front, 64 x 64) lower tile of the contribution block
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(192, 1) k_tc_schur(DevSym S, DevNum N, const TcFront* __restrict__ fronts,
-                                                      const TcTile* __restrict__ tiles, const int8_t* __restrict__ dig,
-                                                      const int* __restrict__ expo) {
+__global__ void __launch_bounds__(TC_THREADS, 1) k_tc_schur(DevSym S, DevNum N, const TcFront* __restrict__ fronts,
+                                                             const TcTile* __restrict__ tiles, const int8_t* __restrict__ dig,
+                                                             const int* __restrict__ expo) {
   extern __shared__ __align__(1024) unsigned char tc_smem[];
-  __shared__ unsigned long long full_bar[TC_STAGES], empty_bar[TC_STAGES], acc_bar;
-  __shared__ unsigned tmem_base_s;
+  __shared__ unsigned long long full_bar[TC_STAGES], empty_bar[TC_STAGES];
   const TcTile T = tiles[blockIdx.x];
   const TcFront F = fronts[T.fi];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nks = F.nks;
 
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < TC_STAGES; ++i) { tc_mbar_init(&full_bar[i], 1); tc_mbar_init(&empty_bar[i], 1); }
-    tc_mbar_init(&acc_bar, 1);
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < TC_STAGES; ++i) { tc_mbar_init(&full_bar[i], 1); tc_mbar_init(&empty_bar[i], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {   // one warp allocates all 512 TMEM columns (1 CTA per SM: launch bounds + shared memory)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&tmem_base_s)), "n"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const unsigned tmem_base = tmem_base_s;
 
-  if (warp == 0) {
-    // ===== TMA producer: per K step one 32 KB unit of A digits and one 16 KB unit of B digits =====
+  if (warp == 8) {
+    // ===== TMA producer: per K step one 16 KB unit of A digits and one 16 KB unit of B digits =====
     if (lane == 0) {
       const int8_t* a_src = dig + F.a_off + (long long)T.ti * nks * TC_A_UNIT;
       const int8_t* b_src = dig + F.b_off + (long long)T.tj * nks * TC_B_UNIT;
       for (int ks = 0; ks < nks; ++ks) {
         const int st = ks % TC_STAGES;
         const unsigned ph = (ks / TC_STAGES) & 1;
-        tc_mbar_wait(&empty_bar[st], ph ^ 1);                       // consumer freed the slot (first pass: immediate)
+        tc_mbar_wait(&empty_bar[st], ph ^ 1);                       // consumers freed the slot (first pass: immediate)
         unsigned char* sa = tc_smem + (size_t)st * TC_STAGE_BYTES;
         tc_mbar_expect_tx(&full_bar[st], TC_STAGE_BYTES);
-        tc_bulk_g2s(sa, a_src + (long long)ks * TC_A_UNIT, TC_A_UNIT / 2, &full_bar[st]);
-        tc_bulk_g2s(sa + TC_A_UNIT / 2, a_src + (long long)ks * TC_A_UNIT + TC_A_UNIT / 2, TC_A_UNIT / 2, &full_bar[st]);
+        tc_bulk_g2s(sa, a_src + (long long)ks * TC_A_UNIT, TC_A_UNIT, &full_bar[st]);
         tc_bulk_g2s(sa + TC_A_UNIT, b_src + (long long)ks * TC_B_UNIT, TC_B_UNIT, &full_bar[st]);
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer: for every K step the 36 digit pairs (s, s'), s + s' < 8, into accumulator d = s + s' =====
-    if (lane == 0) {
-      const unsigned idesc = tc_idesc();
-      for (int ks = 0; ks < nks; ++ks) {
-        const int st = ks % TC_STAGES;
-        const unsigned ph = (ks / TC_STAGES) & 1;
-        tc_mbar_wait(&full_bar[st], ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const unsigned sa = tc_smem_u32(tc_smem + (size_t)st * TC_STAGE_BYTES);
-        const unsigned sb = sa + TC_A_UNIT;
+    return;
+  }
+
+  // ===== consumer warpgroup wg (warps 4wg .. 4wg+3): columns 32 wg .. 32 wg + 31 of the tile =====
+  const int wg = warp >> 2;
+  int acc[TC_NS][16];
 #pragma unroll
-        for (int d = 0; d < TC_NS; ++d) {
+  for (int d = 0; d < TC_NS; ++d)
 #pragma unroll
-          for (int q = 0; q <= d; ++q) {
-            // A digit q, B digit d - q ; within a unit: digit stride 2*rows*16 bytes, K-chunk (LBO) rows*16, 8-row group (SBO) 128
-            const unsigned long long ad = tc_smem_desc(sa + q * (2 * TC_BM * 16), TC_BM * 16, 128);
-            const unsigned long long bd = tc_smem_desc(sb + (d - q) * (2 * TC_BN * 16), TC_BN * 16, 128);
-            tc_mma_i8(tmem_base + d * TC_BN, ad, bd, idesc, (ks > 0 || q > 0) ? 1u : 0u);
-          }
-        }
-        tc_commit(&empty_bar[st]);     // smem slot free when these MMAs have read it
+    for (int j = 0; j < 16; ++j) acc[d][j] = 0;
+  for (int ks = 0; ks < nks; ++ks) {
+    const int st = ks % TC_STAGES;
+    const unsigned ph = (ks / TC_STAGES) & 1;
+    tc_mbar_wait(&full_bar[st], ph);
+    const unsigned sa = tc_smem_u32(tc_smem + (size_t)st * TC_STAGE_BYTES);
+    const unsigned sb = sa + TC_A_UNIT + wg * (TC_WN * 16);
+    tc_wgmma_fence();
+    // the 36 digit pairs (s, s'), s + s' < 8, into accumulator d = s + s'
+#pragma unroll
+    for (int d = 0; d < TC_NS; ++d) {
+#pragma unroll
+      for (int q = 0; q <= d; ++q) {
+        // A digit q, B digit d - q ; within a unit: digit stride 2*rows*16 bytes, K-chunk (LBO) rows*16, 8-row group (SBO) 128
+        const unsigned long long ad = tc_smem_desc(sa + q * (2 * TC_BM * 16), TC_BM * 16, 128);
+        const unsigned long long bd = tc_smem_desc(sb + (d - q) * (2 * TC_BN * 16), TC_BN * 16, 128);
+        tc_wgmma_i8(acc[d], ad, bd);
       }
-      tc_commit(&acc_bar);             // accumulators complete
     }
-  } else {
-    // ===== epilogue: warps 2..5 own TMEM lanes 32 (warp % 4) .. +31; thread = row of the 128-row tile =====
-    const int q4 = warp & 3;
-    const int s = F.s;
-    const int k = S.sn_start[s + 1] - S.sn_start[s];
-    const int r = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
-    const int gi = T.ti * TC_BM + q4 * 32 + lane;      // row of the contribution block
-    const int gj0 = T.tj * TC_BN;
-    const int* __restrict__ ea = expo + F.e_off;
-    const int* __restrict__ eb = ea + r;
-    const int ei = (gi < r) ? ea[gi] : 0;
-    double* __restrict__ C = N.CB + S.cb_off[s];
-    (void)k;
-    tc_mbar_wait(&acc_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const unsigned lane_addr = tmem_base + ((unsigned)(q4 * 32) << 16);
-    for (int c0 = 0; c0 < TC_BN; c0 += 16) {
-      double acc[16];
+    tc_wgmma_commit();
 #pragma unroll
-      for (int j = 0; j < 16; ++j) acc[j] = 0.0;
+    for (int d = 0; d < TC_NS; ++d) tc_fence_acc(acc[d]);
+    // the previous K step's MMAs have read their slot once at most this step's group is in flight
+    tc_wgmma_wait<1>();
+    if (ks > 0 && (threadIdx.x & 127) == 0) tc_mbar_arrive(&empty_bar[(ks - 1) % TC_STAGES]);
+  }
+  tc_wgmma_wait<0>();
+#pragma unroll
+  for (int d = 0; d < TC_NS; ++d) tc_fence_acc(acc[d]);
+
+  // ===== epilogue: accumulator fragment of m64n32 -- register 4i+h of a thread holds row 16 (warp % 4) + lane / 4 + 8 (h / 2),
+  // column 8 i + 2 (lane % 4) + (h % 2) of the warpgroup's 64 x 32 block =====
+  const int s = F.s;
+  const int r = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
+  const int* __restrict__ ea = expo + F.e_off;
+  const int* __restrict__ eb = ea + r;
+  double* __restrict__ C = N.CB + S.cb_off[s];
+  const int gi0 = T.ti * TC_BM + 16 * (warp & 3) + (lane >> 2);
+  const int gj0 = T.tj * TC_BN + wg * TC_WN + 2 * (lane & 3);
+#pragma unroll
+  for (int h2 = 0; h2 < 2; ++h2) {
+    const int gi = gi0 + 8 * h2;
+    if (gi >= r) continue;
+    const int ei = ea[gi];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int reg = 4 * (j >> 1) + 2 * h2 + (j & 1);
+      double a = 0.0;
       // smallest weight first
 #pragma unroll
-      for (int d = TC_NS - 1; d >= 0; --d) {
-        int v[16];
-        tc_ld16(lane_addr + d * TC_BN + c0, v);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        const double w = ldexp(1.0, -7 * (d + 2));
-#pragma unroll
-        for (int j = 0; j < 16; ++j) acc[j] = fma((double)v[j], w, acc[j]);
-      }
-      if (gi < r) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int gj = gj0 + c0 + j;
-          if (gj < r && gj <= gi) C[gi + (long long)gj * r] -= ldexp(acc[j], ei + eb[gj]);
-        }
-      }
+      for (int d = TC_NS - 1; d >= 0; --d) a = fma((double)acc[d][reg], ldexp(1.0, -7 * (d + 2)), a);
+      const int gj = gj0 + 8 * (j >> 1) + (j & 1);
+      if (gj < r && gj <= gi) C[gi + (long long)gj * r] -= ldexp(a, ei + eb[gj]);
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
   }
 }
 

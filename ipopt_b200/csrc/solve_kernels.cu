@@ -1,4 +1,4 @@
-// Supernodal triangular-solve kernels (forward L, block-diagonal D^-1, backward L^T), sm_100a.
+// Supernodal triangular-solve kernels (forward L, block-diagonal D^-1, backward L^T), sm_90a.
 //
 // Replaces the vendor back-solve the reference calls once per right-hand side
 // (MUMPS job=3, reference src/Algorithm/LinearSolvers/IpMumpsSolverInterface.cpp:543-583).

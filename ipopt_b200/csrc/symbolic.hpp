@@ -1,4 +1,4 @@
-// Symbolic analysis for the B200 supernodal multifrontal LDL^T (host side, runs once).
+// Symbolic analysis for the supernodal multifrontal LDL^T (host side, runs once).
 //
 // Replaces what the reference delegates to the vendor solver's analysis phase
 // (MUMPS job=1, reference src/Algorithm/LinearSolvers/IpMumpsSolverInterface.cpp:385-446;

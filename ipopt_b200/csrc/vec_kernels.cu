@@ -1,4 +1,4 @@
-// Device-resident dense-vector, expansion-matrix and triplet-SpMV kernels (C ABI: include/b200vec.h), sm_100a.
+// Device-resident dense-vector, expansion-matrix and triplet-SpMV kernels (C ABI: include/b200vec.h), sm_90a.
 //
 // Replaces the host loops of the reference's src/LinAlg on the interior-point hot path (SURVEY.md 8a rows V1-V9):
 // IpDenseVector.cpp:93-1500, IpBlas.cpp:270-298, IpExpansionMatrix.cpp:27-372, TMatrices/IpGenTMatrix.cpp:46-130,
@@ -30,7 +30,7 @@ struct Ctx {
   unsigned* d_cnt = nullptr;    // arrival counter of the reductions
   double* d_out = nullptr;
   double* h_out = nullptr;      // pinned
-  int max_blocks = 1184;        // 148 SMs x 8 CTAs
+  int max_blocks = 1056;        // 132 SMs (H100 SXM) x 8 CTAs; set from the device in b200vec_create
   int64_t launches = 0;
   std::string err;
 };
@@ -324,7 +324,7 @@ b200vec_ctx b200vec_create(int device, void* stream) {
   if (cudaSetDevice(c->dev) != cudaSuccess) { delete c; return nullptr; }
   if (stream) c->st = (cudaStream_t)stream;
   else { cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking); c->own = true; }
-  int sms = 148;
+  int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->dev);
   c->max_blocks = sms * 8;
   cudaMalloc((void**)&c->d_part, c->max_blocks * sizeof(double));

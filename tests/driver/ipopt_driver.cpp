@@ -1,11 +1,13 @@
 // TEST / BENCH INFRASTRUCTURE: runs the reference's UNMODIFIED interior-point loop (libipopt built from
-// /root/reference into oracle/_ref) on the reference's own benchmark TNLPs (compiled from where they lie:
+// the reference sources into oracle/_ref) on the reference's own benchmark TNLPs (oracle/_ref/lib/libreftnlp.so:
 // examples/ScalableProblems/*.cpp, examples/hs071_cpp/hs071_nlp.cpp) with the KKT linear solver injected
 // through the reference's custom-solver hook, exactly as SURVEY.md section 8(b) describes:
 //   new AlgorithmBuilder(new StdAugSystemSolver(*new TSymLinearSolver(iface, NULL)), name) + linear_solver=custom
 //   (reference src/Algorithm/IpAlgBuilder.hpp:55-58, IpAlgBuilder.cpp:576-584; driver modelled on
 //    examples/ScalableProblems/solve_problem.cpp:103-260).
 // Backends: "b200" = the product (libb200ldlt.so via ipopt_b200/plugin), "oracle" = oracle/cpu_ldlt.cpp.
+#include <dlfcn.h>
+
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -109,7 +111,6 @@ static double wall_now()
    return duration<double>(steady_clock::now().time_since_epoch()).count();
 }
 
-extern "C" void openblas_set_num_threads(int);
 extern "C" int omp_get_max_threads(void);
 
 int main(int argc, char** argv)
@@ -118,9 +119,11 @@ int main(int argc, char** argv)
    // container's quota; on a many-core GPU box that turns every level-1 BLAS call of the IP loop into a storm of
    // spinning workers.  Level-1 ops on <1e6 doubles are memory-bound anyway: keep the host BLAS single-threaded
    // unless asked otherwise.
+   // (looked up at run time: the BLAS is libipopt.so's dependency, not linked here; absent for a non-OpenBLAS BLAS)
    {
       const char* e = getenv("B200_HOST_BLAS_THREADS");
-      openblas_set_num_threads(e ? atoi(e) : 1);
+      void (*set_threads)(int) = (void (*)(int))dlsym(RTLD_DEFAULT, "openblas_set_num_threads");
+      if( set_threads ) set_threads(e ? atoi(e) : 1);
    }
    std::string backend = "b200", problem = "hs071", json_path, final_path, dump_prefix;
    bool reopt = false;   // second solve of the same NLP with warm_start_same_structure=yes (ReOptimizeNLP)

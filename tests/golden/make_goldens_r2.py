@@ -1,5 +1,5 @@
 """Round-2 golden fixtures, all produced by the REFERENCE's own interior-point loop (oracle/_ref libipopt.so) with the
-CPU oracle as linear solver (tests/driver/ipopt_driver --backend oracle).  Needs /root/reference (driver build).
+CPU oracle as linear solver (tests/driver/ipopt_driver --backend oracle).  Needs the reference sources (driver build).
 
   python tests/golden/make_goldens_r2.py [small] [full] [control]
 

@@ -1,6 +1,6 @@
 """The Ipopt-side adapter (ipopt_b200/plugin/B200LdltSolverInterface) driven by the reference's own IP loop with the CPU
 oracle as its backend -- host logic only, no GPU: warm_start_same_structure, counters.  Test infrastructure: the oracle is
-the checker's stand-in here, not a product path.  Needs tests/driver/ipopt_driver (built where /root/reference exists)."""
+the checker's stand-in here, not a product path.  Needs tests/driver/ipopt_driver (built against the reference artefacts in oracle/_ref)."""
 import json, os, subprocess
 import pytest
 
@@ -10,7 +10,7 @@ DRIVER = os.path.join(ROOT, "tests", "driver", "ipopt_driver")
 
 def run_driver(args, tmp_path):
     if not os.path.exists(DRIVER):
-        pytest.skip("tests/driver/ipopt_driver not built (needs /root/reference at build time)")
+        pytest.skip("tests/driver/ipopt_driver not built (needs the reference artefacts in oracle/_ref at build time)")
     js = str(tmp_path / "r.json")
     env = dict(os.environ, OMP_NUM_THREADS="4")
     p = subprocess.run([DRIVER, "--backend", "oracle", "--print-level", "0", "--json", js] + args, capture_output=True,

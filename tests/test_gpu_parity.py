@@ -275,10 +275,10 @@ def test_full_size_lukvle1():
     s.close()
 
 
-# ---- end-to-end through the reference's own IP loop (driver binary built where /root/reference exists) -------
+# ---- end-to-end through the reference's own IP loop (driver binary built against oracle/_ref) -------
 def _run_driver(backend, problem, N, tmp_path, opts=None, extra=()):
     if not os.path.exists(DRIVER):
-        pytest.skip("tests/driver/ipopt_driver not built (needs /root/reference at build time)")
+        pytest.skip("tests/driver/ipopt_driver not built (needs the reference artefacts in oracle/_ref at build time)")
     js, fin = str(tmp_path / "r.json"), str(tmp_path / "f.bin")
     env = dict(os.environ, OMP_NUM_THREADS=str(min(16, os.cpu_count() or 1)),
                B200_HSLLIB=os.path.join(ROOT, "ipopt_b200", "lib", "libb200ldlt.so"))

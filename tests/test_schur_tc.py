@@ -1,4 +1,4 @@
-"""Tensor-core Schur complement (tcgen05 int8 Ozaki split, ipopt_b200/csrc/schur_tc.cu) against the FP64 DFMA kernel and
+"""Tensor-core Schur complement (wgmma int8 Ozaki split, ipopt_b200/csrc/schur_tc.cu) against the FP64 DFMA kernel and
 against numpy, on a matrix whose elimination tree is two dense children under one dense root, so the contribution block
 of a child IS the quantity under test:  CB = - A21 A11^-1 A12  (r x r, lower triangle)."""
 import ctypes as C

@@ -1,6 +1,6 @@
 """GPU parity of the b200vec kernels (SURVEY.md 8a rows V1-V9) against the REFERENCE's own classes: every case runs the
 same inputs through Ipopt::DenseVector / ExpansionMatrix / GenTMatrix / SymTMatrix of the unmodified libipopt.so
-(tests/driver/libvecref.so, built from /root/reference into oracle/_ref) and through the CUDA kernels.
+(tests/driver/libvecref.so, built against the unmodified libipopt.so in oracle/_ref) and through the CUDA kernels.
 Bars: representation (homogeneous flag + scalar) identical; element-wise results BIT-IDENTICAL for everything the
 reference computes with its own loops; <= 1 ulp-level relative error where the reference delegates to BLAS (Axpy -> daxpy);
 min/max-type reductions exact; sum-type reductions within n*eps*sum|terms| (different summation order)."""
@@ -17,7 +17,7 @@ SCALARS = [0.0, 1.0, -1.0, 2.5]
 @pytest.fixture(scope="module")
 def ctx():
     if not R.available():
-        pytest.skip("tests/driver/libvecref.so not built (needs /root/reference at build time)")
+        pytest.skip("tests/driver/libvecref.so not built (needs the reference artefacts in oracle/_ref at build time)")
     from ipopt_b200.vec import VecContext
     c = VecContext()
     yield c
