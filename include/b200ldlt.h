@@ -91,7 +91,12 @@ int b200ldlt_factor(b200ldlt_handle h, int check_inertia, int expected_neg, int*
 /* Same, values already resident in device memory (nonzeros doubles). */
 int b200ldlt_factor_device(b200ldlt_handle h, const double* d_vals, int check_inertia, int expected_neg, int* num_neg);
 
-/* <-> MultiSolve part 2: rhs is dim x nrhs column-major, overwritten with the solution (host memory). */
+/* <-> MultiSolve part 2: rhs is dim x nrhs column-major, overwritten with the solution (host memory).
+ * nrhs > 1: the columns are solved in blocks of up to 8 (environment B200_SOLVE_BLOCK=n at b200ldlt_create caps the
+ * width, 1 = one solve per column), one forward and one backward sweep per block; every column is bit-identical to a
+ * solve of that column alone.  The first such call after an analysis allocates per-column device state for the full width
+ * (before its timing starts); if that allocation fails, the columns are solved one by one.  info.launches_solve /
+ * ms_solve_gpu describe the whole call. */
 int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs);
 /* Same with a device-resident rhs/solution. */
 int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs);

@@ -17,6 +17,7 @@
 #include "factor_kernels.cu"
 #include "solve_kernels.cu"
 #include "solve_dataflow.cu"
+#include "solve_multi.cu"
 #include "schur_tc.cu"
 #include "symbolic.hpp"
 
@@ -101,6 +102,7 @@ struct DebugSwitches {
   bool cb_at_end = false;         // B200_CB_AT_END=1: Schur complements as one GEMM per level (k_big_schur84) instead of per-panel updates
   int solve_direct = 2;           // B200_SOLVE_DIRECT=D: the D lowest tree levels are solved by k_solve_direct (0 = all inside the subtrees)
   bool solve_nopair = false;      // B200_SOLVE_NOPAIR=1: one subtree per CTA in the solve sweeps (no side-by-side pairs)
+  int solve_block = MS_NB_MAX;    // B200_SOLVE_BLOCK=n: nrhs > 1 solved in blocks of at most n columns (1 = one solve per column)
   bool no_warp2 = false;          // B200_NO_WARP2=1: fronts of order 33..64 by the shared-memory kernel (one CTA each) instead of k_front_warp2
   bool no_pdl = false;            // B200_NO_PDL=1: chain kernels launched without programmatic dependent launch
   bool factor_timeline = false;   // B200_FACTOR_TIMELINE=1: %globaltimer records of the factorisation kernels (b200ldlt_dump_factor_timeline)
@@ -113,6 +115,7 @@ struct DebugSwitches {
     cb_at_end = getenv("B200_CB_AT_END") != nullptr;
     solve_nopair = getenv("B200_SOLVE_NOPAIR") != nullptr;
     if (const char* e = getenv("B200_SOLVE_DIRECT")) solve_direct = atoi(e);
+    if (const char* e = getenv("B200_SOLVE_BLOCK")) solve_block = std::min(std::max(atoi(e), 1), MS_NB_MAX);
     no_pdl = getenv("B200_NO_PDL") != nullptr;
     no_warp2 = getenv("B200_NO_WARP2") != nullptr;
     if (const char* e = getenv("B200_BUCKETS")) {
@@ -175,6 +178,19 @@ struct Solver {
   DevSym DS;
   DevNum DN;
   int launches = 0;
+  // blocked multi-column solve (solve_multi.cu): per-column copies of the sweep state, allocated at the first nrhs > 1
+  // solve after an analysis for B200_SOLVE_BLOCK columns (width 0: the column loop)
+  struct BlockSolve {
+    int width = 0;
+    DevBuf<double> d_x, d_cbv, d_bigv, d_bigy, d_part;
+    DevBuf<int> d_done_f, d_done_b, d_bflag_f, d_bflag_b, d_bcnt, d_bcnt_b, d_ccnt;
+    DevBuf<unsigned long long> d_ticket;
+    unsigned long long ticket_f = 0, ticket_b = 0;
+    DevSolve V;                       // the single-column plan's lists, this state's (column 0) arrays
+    MultiStride M;
+    int grid = 0;
+  };
+  std::unique_ptr<BlockSolve> blk;
   // solve (solve_dataflow.cu): shared flag / scratch arrays + one plan per front set
   DevBuf<int> d_done_f, d_done_b, d_bflag_f, d_bflag_b, d_bcnt, d_bcnt_b, d_boff;
   DevBuf<long long> d_bigv_off;
@@ -720,6 +736,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   sv->reanalyse = false;
   if (sv->h_rhs) { cudaFreeHost(sv->h_rhs); sv->h_rhs = nullptr; }
   sv->rhs_cap = 0;
+  sv->blk.reset();
   if (sv->fgraph_exec) { cudaGraphExecDestroy(sv->fgraph_exec); sv->fgraph_exec = nullptr; }
   if (sv->fgraph) { cudaGraphDestroy(sv->fgraph); sv->fgraph = nullptr; }
   AnalyseOptions ao;
@@ -1291,6 +1308,140 @@ static int enqueue_solve(Solver* sv, const double* d_b, double* d_out) {
   return B200LDLT_SUCCESS;
 }
 
+// Per-column sweep state of the blocked solve, for the full block width B200_SOLVE_BLOCK: allocated once per analysis,
+// at the first nrhs > 1 solve, before that solve's timing starts.  Returns false (and the columns are then solved one by
+// one, as with B200_SOLVE_BLOCK=1) when the device memory for it cannot be had.
+static bool block_solve_state(Solver* sv) {
+  if (sv->blk) return sv->blk->width > 1;
+  const int nb = sv->dbg.solve_block;
+  sv->blk.reset(new Solver::BlockSolve());
+  if (nb < 2) return false;
+  cudaStream_t st = sv->stream;
+  Solver::BlockSolve& B = *sv->blk;
+  const SolvePlan& SP = sv->splan;
+  MultiStride& M = B.M;
+  M.nb = nb;
+  M.nsn = sv->S.nsn;
+  M.nbo = (int)sv->d_bflag_f.n;
+  M.nccnt = (int)SP.d_ccnt.n;
+  M.x = sv->n;
+  M.cbv = (long long)sv->d_cbv.n;
+  M.bigv = (long long)sv->d_bigv.n;
+  M.part = (long long)SP.d_part.n;
+  DevBuf<int>* flags[] = {&B.d_done_f, &B.d_done_b, &B.d_bcnt, &B.d_bcnt_b, &B.d_bflag_f, &B.d_bflag_b, &B.d_ccnt};
+  const long long per_col[] = {M.nsn, M.nsn, M.nsn, M.nsn, M.nbo, M.nbo, M.nccnt};
+  int occ = 1, occ_b = 1;
+  auto setup = [&]() -> cudaError_t {
+    cudaError_t e;
+    if ((e = B.d_x.alloc(M.x * nb)) != cudaSuccess || (e = B.d_cbv.alloc(M.cbv * nb)) != cudaSuccess ||
+        (e = B.d_bigv.alloc(M.bigv * nb)) != cudaSuccess || (e = B.d_bigy.alloc(M.bigv * nb)) != cudaSuccess ||
+        (e = B.d_part.alloc(M.part * nb)) != cudaSuccess || (e = B.d_ticket.alloc(2)) != cudaSuccess)
+      return e;
+    for (int i = 0; i < 7; ++i) {
+      if ((e = flags[i]->alloc(std::max<long long>(per_col[i] * nb, 1))) != cudaSuccess) return e;
+      if ((e = cudaMemsetAsync(flags[i]->p, 0, flags[i]->n * sizeof(int), st)) != cudaSuccess) return e;
+    }
+    if ((e = cudaMemsetAsync(B.d_ticket.p, 0, 2 * sizeof(unsigned long long), st)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(k_solve_multi<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM)) != cudaSuccess ||
+        (e = cudaFuncSetAttribute(k_solve_multi<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM)) != cudaSuccess ||
+        (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_solve_multi<true>, DF_THREADS, DF_DYN_SMEM)) != cudaSuccess ||
+        (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_solve_multi<false>, DF_THREADS, DF_DYN_SMEM)) != cudaSuccess)
+      return e;
+    return cudaStreamSynchronize(st);
+  };
+  const cudaError_t e = setup();
+  if (e != cudaSuccess) {
+    if (sv->opt.verbose) fprintf(stderr, "[b200ldlt] blocked solve unavailable (%s): one solve per column\n", cudaGetErrorString(e));
+    cudaGetLastError();
+    sv->blk.reset(new Solver::BlockSolve());   // width 0: not retried before the next analysis
+    return false;
+  }
+  B.width = nb;
+  DevSolve& V = B.V;
+  V = SP.V;
+  V.done_f = B.d_done_f.p; V.done_b = B.d_done_b.p;
+  V.bflag_f = B.d_bflag_f.p; V.bflag_b = B.d_bflag_b.p; V.bcnt = B.d_bcnt.p; V.bcnt_b = B.d_bcnt_b.p;
+  V.bigv = B.d_bigv.p; V.bigy = B.d_bigy.p;
+  V.part = B.d_part.p; V.ccnt = B.d_ccnt.p;
+  V.ticket = B.d_ticket.p;
+  V.tlog = nullptr;
+  B.grid = std::max(1, std::min(occ, occ_b)) * sv->num_sms;
+  if (sv->opt.verbose)
+    fprintf(stderr, "[b200ldlt] blocked solve: %d columns, %.1f MB of per-column state, grid %d\n", nb,
+            (double)(8 * (B.d_x.n + B.d_cbv.n + B.d_bigv.n + B.d_bigy.n + B.d_part.n) +
+                     4 * (B.d_done_f.n + B.d_done_b.n + B.d_bcnt.n + B.d_bcnt_b.n + B.d_bflag_f.n + B.d_bflag_b.n + B.d_ccnt.n)) / 1e6,
+            B.grid);
+  return true;
+}
+
+// one sweep of the blocked solve: the launches of launch_sweep, each carrying all nb columns
+static int launch_sweep_block(Solver* sv, int nb, bool fwd) {
+  cudaStream_t st = sv->stream;
+  Solver::BlockSolve& B = *sv->blk;
+  const SolvePlan& SP = sv->splan;
+  MultiStride M = B.M;
+  M.nb = nb;
+  const long long nt = ((long long)(fwd ? SP.ntf : SP.ntb) + SP.npair) * nb;
+  const int grid = (int)std::min<long long>(B.grid, nt);
+  const int nd = (int)SP.direct_cnt.size();
+  auto direct = [&](int l) {
+    if (SP.direct_cnt[l] <= 0) return;
+    const unsigned g = cdiv(SP.direct_cnt[l] * nb, DF_THREADS / 32);
+    if (fwd) k_solve_direct_multi<true><<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, B.V, M, SP.d_direct[l]->p, SP.direct_cnt[l], sv->solve_epoch, B.d_x.p, B.d_cbv.p);
+    else k_solve_direct_multi<false><<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, B.V, M, SP.d_direct[l]->p, SP.direct_cnt[l], sv->solve_epoch, B.d_x.p, B.d_cbv.p);
+    ++sv->launches;
+  };
+  if (fwd) {
+    for (int l = 0; l < nd; ++l) direct(l);
+    if (nt > 0) {
+      k_solve_multi<true><<<grid, DF_THREADS, DF_DYN_SMEM, st>>>(sv->DS, sv->DN, B.V, M, sv->solve_epoch, B.ticket_f, B.d_x.p, B.d_cbv.p);
+      B.ticket_f += (unsigned long long)nt + grid;
+      ++sv->launches;
+    }
+  } else {
+    if (nt > 0) {
+      k_solve_multi<false><<<grid, DF_THREADS, DF_DYN_SMEM, st>>>(sv->DS, sv->DN, B.V, M, sv->solve_epoch, B.ticket_b, B.d_x.p, B.d_cbv.p);
+      B.ticket_b += (unsigned long long)nt + grid;
+      ++sv->launches;
+    }
+    for (int l = nd - 1; l >= 0; --l) direct(l);
+  }
+  CU(cudaGetLastError());
+  return B200LDLT_SUCCESS;
+}
+
+// nb (>= 2) columns of d_rhs (leading dimension n), solved in place by one forward and one backward sweep
+static int enqueue_solve_block(Solver* sv, double* d_rhs, int nb) {
+  int rc;
+  Solver::BlockSolve& B = *sv->blk;
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  const dim3 g(cdiv(n, 256), nb);
+  k_rhs_in_multi<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_rhs, B.d_x.p, B.M.x); ++sv->launches;
+  sv->solve_epoch++;
+  rc = launch_sweep_block(sv, nb, true);
+  if (rc == B200LDLT_SUCCESS) rc = launch_sweep_block(sv, nb, false);
+  if (rc != B200LDLT_SUCCESS) return rc;
+  k_sol_out_multi<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, B.d_x.p, B.M.x, d_rhs); ++sv->launches;
+  CU(cudaGetLastError());
+  return B200LDLT_SUCCESS;
+}
+
+// nrhs columns of d_rhs (leading dimension n), in place: blocks of up to B200_SOLVE_BLOCK columns through the blocked
+// sweeps, single columns (and every column of the level-per-launch solve, use_graph == 2) through enqueue_solve.
+// `blocked`: the result of block_solve_state, called by the entry point before its timing starts.
+static int enqueue_solve_columns(Solver* sv, double* d_rhs, int nrhs, bool blocked) {
+  const int cap = blocked ? sv->blk->width : 1;
+  for (int c = 0; c < nrhs;) {
+    const int w = std::min(cap, nrhs - c);
+    double* col = d_rhs + (size_t)c * sv->n;
+    const int rc = w == 1 ? enqueue_solve(sv, col, col) : enqueue_solve_block(sv, col, w);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    c += w;
+  }
+  return B200LDLT_SUCCESS;
+}
+
 static int shard_setup(Solver* sv, int rank, int world) {
   Symbolic& S = sv->S;
   cudaStream_t st = sv->stream;
@@ -1463,11 +1614,11 @@ int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs) {
   if (!sv || !sv->factored) { if (sv) sv->err = "solve before factor"; return B200LDLT_FATAL_ERROR; }
   CU(cudaSetDevice(sv->dev));
   cudaStream_t st = sv->stream;
+  const bool blocked = nrhs > 1 && sv->opt.use_graph != 2 && block_solve_state(sv);
   sv->launches = 0;
   CU(cudaEventRecord(sv->ev0, st));
-  for (int c = 0; c < nrhs; ++c) {
-    double* col = d_rhs + (size_t)c * sv->n;
-    int rc = enqueue_solve(sv, col, col);
+  {
+    int rc = enqueue_solve_columns(sv, d_rhs, nrhs, blocked);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   CU(cudaEventRecord(sv->ev1, st));
@@ -1495,6 +1646,7 @@ int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs) {
   // caller's array is pageable: Ipopt allocates it per call, IpTSymLinearSolver.cpp:222-241); same on the way back.
   const size_t total = n * (size_t)nrhs;
   const size_t chunk = std::max<size_t>((total + 3) / 4, 32768);
+  const bool blocked = nrhs > 1 && sv->opt.use_graph != 2 && block_solve_state(sv);
   sv->launches = 0;
   CU(cudaEventRecord(sv->ev0, st));
   for (size_t o = 0; o < total; o += chunk) {
@@ -1502,9 +1654,8 @@ int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs) {
     memcpy(sv->h_rhs + o, rhs + o, m * sizeof(double));
     CU(cudaMemcpyAsync(sv->d_rhs.p + o, sv->h_rhs + o, m * sizeof(double), cudaMemcpyHostToDevice, st));
   }
-  for (int c = 0; c < nrhs; ++c) {
-    double* col = sv->d_rhs.p + (size_t)c * n;
-    int rc = enqueue_solve(sv, col, col);
+  {
+    int rc = enqueue_solve_columns(sv, sv->d_rhs.p, nrhs, blocked);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   int nchunk = 0;
