@@ -44,7 +44,7 @@ typedef struct b200ldlt_options {
   double pivtolmax;    /* cap for increase_quality; cf. ma57_pivtolmax 1e-4 */
   double tiny;         /* |pivot| below this (after scaling) is treated as zero -> SINGULAR */
   int smem_front_max;  /* fronts of order <= this are factored by one CTA in shared memory */
-  int use_graph;       /* 1 = replay numeric phases from CUDA graphs */
+  int use_graph;       /* 1 = replay the factorisation from a CUDA graph; any other value = plain launches */
   int verbose;
   int tc_schur_min_r;  /* fronts with >= this many contribution rows form their Schur complement on the tensor cores
                           (wgmma int8 Ozaki split, csrc/schur_tc.cu); 0 = off (FP64 DFMA tiles everywhere) */

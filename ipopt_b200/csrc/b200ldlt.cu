@@ -17,7 +17,6 @@
 #include "factor_kernels.cu"
 #include "solve_kernels.cu"
 #include "solve_dataflow.cu"
-#include "solve_multi.cu"
 #include "schur_tc.cu"
 #include "symbolic.hpp"
 
@@ -66,9 +65,22 @@ struct SolvePlan {
   std::vector<std::unique_ptr<DevBuf<int>>> d_direct;   // per bottom level: the fronts k_solve_direct owns
   std::vector<int> direct_cnt;
   DevBuf<double> d_part;
-  DevSolve V;
   int nsub = 0, npair = 0, ntf = 0, ntb = 0;
   long long sub_bytes = 0;
+  unsigned long long* tlog = nullptr;   // B200_SOLVE_TIMELINE (splan only): records of its single-column sweeps
+};
+
+// what the solve sweeps write, for `width` columns: column c of each array at its base + c * its stride in M.  The chunk
+// partials and counters belong to a plan (a counter counts modulo its task's nq, so plans must not share them): one column
+// uses those of the plan it sweeps, a block (width > 1) has its own copies of splan's in d_part / d_ccnt.
+struct SweepState {
+  int width = 0;
+  DevBuf<double> d_x, d_cbv, d_bigv, d_bigy, d_part;
+  DevBuf<int> d_done_f, d_done_b, d_bflag_f, d_bflag_b, d_bcnt, d_bcnt_b, d_ccnt;
+  DevBuf<unsigned long long> d_ticket;   // [0] fwd, [1] bwd (monotonic)
+  unsigned long long ticket_f = 0, ticket_b = 0;   // their values when the next sweep starts
+  MultiStride M;
+  int grid = 0;                          // CTAs of the persistent sweep kernel
 };
 
 struct LevelPlan {
@@ -77,7 +89,6 @@ struct LevelPlan {
   long long big_entmax = 0, big_zero_max = 0;
   struct Bucket { int off, cnt, fmax, kmax, threads; size_t smem; int kind = 0; };   // kind 2: k_front_warp2 (order 33..64, <= 32 pivots)
   std::vector<Bucket> small;
-  int all_off = 0, all_cnt = 0, fmax = 0;  // whole level (solve)
   // Schur complements of the level's big fronts: tensor-core (Ozaki int8, schur_tc.cu) for r >= tc_min_r, DFMA tiles else
   int tc_f_off = 0, tc_f_cnt = 0, tc_t_off = 0, tc_t_cnt = 0, tc_rmax = 0;
   int df_off = 0, df_cnt = 0, df_rmax = 0;
@@ -171,31 +182,20 @@ struct Solver {
   DevBuf<int> d_useg_src, d_u_row, d_u_col, d_irn, d_jcn;
   DevBuf<long long> d_rows_ptr, d_uent_ptr, d_u_dst64, d_L_off, d_cb_off, d_useg_ptr;
   DevBuf<unsigned> d_u_dst;
-  DevBuf<double> d_vals, d_uval, d_L, d_W, d_CB, d_dinv, d_doff, d_scale, d_x, d_cbv, d_rhs, d_res, d_colmax;
+  DevBuf<double> d_vals, d_uval, d_L, d_W, d_CB, d_dinv, d_doff, d_scale, d_rhs, d_res, d_colmax;
   DevBuf<int> d_ptype, d_lperm, d_bperm, d_counters, d_einv;
   DevBuf<long long> d_einv_off;
   DevBuf<unsigned long long> d_rmax;
   DevSym DS;
   DevNum DN;
   int launches = 0;
-  // blocked multi-column solve (solve_multi.cu): per-column copies of the sweep state, allocated at the first nrhs > 1
-  // solve after an analysis for B200_SOLVE_BLOCK columns (width 0: the column loop)
-  struct BlockSolve {
-    int width = 0;
-    DevBuf<double> d_x, d_cbv, d_bigv, d_bigy, d_part;
-    DevBuf<int> d_done_f, d_done_b, d_bflag_f, d_bflag_b, d_bcnt, d_bcnt_b, d_ccnt;
-    DevBuf<unsigned long long> d_ticket;
-    unsigned long long ticket_f = 0, ticket_b = 0;
-    DevSolve V;                       // the single-column plan's lists, this state's (column 0) arrays
-    MultiStride M;
-    int grid = 0;
-  };
-  std::unique_ptr<BlockSolve> blk;
-  // solve (solve_dataflow.cu): shared flag / scratch arrays + one plan per front set
-  DevBuf<int> d_done_f, d_done_b, d_bflag_f, d_bflag_b, d_bcnt, d_bcnt_b, d_boff;
+  // solve (solve_dataflow.cu): per-front tables, sweep states + one plan per front set
+  SweepState sweep;                 // one column: every single-column solve (also the sharded one), device_ptr "x" / "cbv"
+  std::unique_ptr<SweepState> blk;  // blocked solve: B200_SOLVE_BLOCK columns, allocated at the first nrhs > 1 solve after
+                                    // an analysis (width 0: the column loop)
+  DevBuf<int> d_boff;
   DevBuf<long long> d_bigv_off;
-  DevBuf<double> d_bigv, d_bigy;
-  DevBuf<unsigned long long> d_ticket, d_tlog, d_flog;
+  DevBuf<unsigned long long> d_tlog, d_flog;
   DevBuf<double> d_linv;
   DevBuf<double> d_linv_part;       // partial tiles of the chunked k_linv_gemm items (one launch at a time uses it)
   DevBuf<int> d_linv_cnt;           // their arrival counters (self-resetting)
@@ -207,8 +207,7 @@ struct Solver {
   std::vector<SolveTask> h_tasks;   // fwd then bwd (debug timeline)
   SolvePlan splan;                  // all fronts
   std::vector<char> solve_direct_front;   // per supernode: solved by k_solve_direct (see build_solve_tables)
-  int solve_epoch = 0, df_grid = 0;
-  unsigned long long ticket_f = 0, ticket_b = 0;
+  int solve_epoch = 0;
   int num_sms = 132;
   struct Shard {
     bool active = false;
@@ -284,12 +283,10 @@ static void build_level_plans(const Symbolic& S, int smax, const std::vector<cha
   plan.assign(S.nlevels, LevelPlan());
   for (int l = 0; l < S.nlevels; ++l) {
     LevelPlan& P = plan[l];
-    P.all_off = (int)fl.size();
     P.big_off = (int)fl.size();
     for (int q = S.level_ptr[l]; q < S.level_ptr[l + 1]; ++q) {
       int s = S.level_sn[q];
       if (!take[s]) continue;
-      P.fmax = std::max(P.fmax, S.f(s));
       if (S.f(s) > smax) {
         fl.push_back(s);
         P.big_cnt++;
@@ -373,7 +370,6 @@ static void build_level_plans(const Symbolic& S, int smax, const std::vector<cha
       for (int s : w2) fl.push_back(s);
       P.small.insert(P.small.begin(), bk);     // the most numerous class first (it gets the main stream when there are no big fronts)
     }
-    P.all_cnt = (int)fl.size() - P.all_off;
   }
 }
 
@@ -655,20 +651,7 @@ static int build_solve_plan(Solver* sv, const Symbolic& S, const std::vector<cha
   CU(SP.d_ccnt.alloc(std::max(ncidx, 1)));
   CU(cudaMemsetAsync(SP.d_ccnt.p, 0, SP.d_ccnt.n * sizeof(int), st));
   CU(SP.d_part.alloc(std::max<long long>(npart, 1) * 64));
-  DevSolve& V = SP.V;
-  V.tasks = SP.d_tf.p; V.tasks_bwd = SP.d_tb.p; V.ntasks_fwd = SP.ntf; V.ntasks_bwd = SP.ntb;
-  V.bundle = SP.d_bundle.p;
-  V.done_f = sv->d_done_f.p; V.done_b = sv->d_done_b.p;
-  V.bflag_f = sv->d_bflag_f.p; V.bflag_b = sv->d_bflag_b.p; V.bcnt = sv->d_bcnt.p; V.bcnt_b = sv->d_bcnt_b.p;
-  V.boff = sv->d_boff.p; V.bigv_off = sv->d_bigv_off.p; V.bigv = sv->d_bigv.p; V.bigy = sv->d_bigy.p;
-  V.part = SP.d_part.p; V.ccnt = SP.d_ccnt.p;
-  V.ticket = sv->d_ticket.p;
-  V.linv = sv->d_linv.p; V.linv_off = sv->d_linv_off.p;
-  V.fdesc = sv->d_fdesc.p; V.gmap = sv->d_gmap.p; V.gmap_off = sv->d_gmap_off.p;
-  V.subs = SP.d_subs.p; V.sub_meta = SP.d_sub_meta.p; V.subrow = SP.d_subrow.p; V.nsub = nsub;
-  V.subpair = SP.d_subpair.p; V.npair = SP.npair; V.sub_Loff = SP.d_sub_Loff.p;
-  V.upper_max = sv->opt.smem_front_max;
-  V.tlog = nullptr;
+  SP.tlog = nullptr;
   return B200LDLT_SUCCESS;
 }
 
@@ -730,6 +713,42 @@ static int upload_schur_lists(Solver* sv, SchurLists& SL, cudaStream_t st) {
   return B200LDLT_SUCCESS;
 }
 
+// the persistent sweep kernel for one column (multi = false) or a block of columns
+static auto sweep_kernel(bool fwd, bool multi) {
+  return fwd ? (multi ? k_solve<true, true> : k_solve<true, false>) : (multi ? k_solve<false, true> : k_solve<false, false>);
+}
+
+// Allocates and zeroes the sweep state of M.nb columns, M giving the per-column sizes, and sizes its sweep grid.
+static cudaError_t alloc_sweep_state(Solver* sv, SweepState& W, const MultiStride& M) {
+  cudaStream_t st = sv->stream;
+  const int nb = M.nb;
+  W.width = 0;
+  W.M = M;
+  cudaError_t e;
+  if ((e = W.d_x.alloc(M.x * nb)) != cudaSuccess || (e = W.d_cbv.alloc(M.cbv * nb)) != cudaSuccess ||
+      (e = W.d_bigv.alloc(M.bigv * nb)) != cudaSuccess || (e = W.d_bigy.alloc(M.bigv * nb)) != cudaSuccess ||
+      (e = W.d_part.alloc(M.part * nb)) != cudaSuccess || (e = W.d_ticket.alloc(2)) != cudaSuccess)
+    return e;
+  DevBuf<int>* flags[] = {&W.d_done_f, &W.d_done_b, &W.d_bcnt, &W.d_bcnt_b, &W.d_bflag_f, &W.d_bflag_b, &W.d_ccnt};
+  const long long per_col[] = {M.nsn, M.nsn, M.nsn, M.nsn, M.nbo, M.nbo, M.nccnt};
+  for (int i = 0; i < 7; ++i) {
+    if ((e = flags[i]->alloc(per_col[i] * nb)) != cudaSuccess) return e;
+    if (flags[i]->n && (e = cudaMemsetAsync(flags[i]->p, 0, flags[i]->n * sizeof(int), st)) != cudaSuccess) return e;
+  }
+  if ((e = cudaMemsetAsync(W.d_ticket.p, 0, 2 * sizeof(unsigned long long), st)) != cudaSuccess) return e;
+  W.ticket_f = W.ticket_b = 0;
+  int occ = 1, occ_b = 1;
+  if ((e = cudaFuncSetAttribute(sweep_kernel(true, nb > 1), cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM)) != cudaSuccess ||
+      (e = cudaFuncSetAttribute(sweep_kernel(false, nb > 1), cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM)) != cudaSuccess ||
+      (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, sweep_kernel(true, nb > 1), DF_THREADS, DF_DYN_SMEM)) != cudaSuccess ||
+      (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, sweep_kernel(false, nb > 1), DF_THREADS, DF_DYN_SMEM)) != cudaSuccess)
+    return e;
+  W.grid = std::max(1, std::min(occ, occ_b)) * sv->num_sms;
+  if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return e;
+  W.width = nb;
+  return cudaSuccess;
+}
+
 static int run_analysis(Solver* sv, const double* vals) {
   // a (re-)analysis invalidates the factors and every buffer sized by the old plan
   sv->factored = false;
@@ -775,8 +794,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   CU(sv->d_W.alloc(S.L_off[S.nsn]));
   CU(sv->d_CB.alloc(std::max<int64_t>(S.cb_off[S.nsn], 1)));
   CU(sv->d_dinv.alloc(n)); CU(sv->d_doff.alloc(n)); CU(sv->d_scale.alloc(n));
-  CU(sv->d_x.alloc(n)); CU(sv->d_rhs.alloc(n)); CU(sv->d_res.alloc(n));
-  CU(sv->d_cbv.alloc(std::max<size_t>(S.rows.size(), 1)));
+  CU(sv->d_rhs.alloc(n)); CU(sv->d_res.alloc(n));
   CU(sv->d_ptype.alloc(n)); CU(sv->d_lperm.alloc(n)); CU(sv->d_bperm.alloc(n));
   CU(sv->d_counters.alloc(CNT_N));
   CU(sv->d_colmax.alloc(n));
@@ -836,8 +854,6 @@ static int run_analysis(Solver* sv, const double* vals) {
   CU(cudaFuncSetAttribute(k_front_warp2, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * S2_SMEM_PER_WARP));
   CU(cudaFuncSetAttribute(k_front_smem<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   CU(cudaFuncSetAttribute(k_front_smem<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-  CU(cudaFuncSetAttribute(k_fwd_front, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  CU(cudaFuncSetAttribute(k_bwd_front, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   CU(cudaStreamSynchronize(st));
 
 
@@ -877,19 +893,11 @@ static int run_analysis(Solver* sv, const double* vals) {
     }
     CU(sv->d_boff.upload(boff, st));
     CU(sv->d_bigv_off.upload(bigv_off, st));
-    CU(sv->d_done_f.alloc(S.nsn)); CU(sv->d_done_b.alloc(S.nsn));
-    CU(sv->d_bcnt.alloc(S.nsn)); CU(sv->d_bcnt_b.alloc(S.nsn));
-    CU(sv->d_bflag_f.alloc(std::max(bo, 1))); CU(sv->d_bflag_b.alloc(std::max(bo, 1)));
-    CU(sv->d_bigv.alloc(std::max<long long>(bv, 1))); CU(sv->d_bigy.alloc(std::max<long long>(bv, 1)));
-    CU(sv->d_ticket.alloc(2));
-    CU(cudaMemsetAsync(sv->d_done_f.p, 0, S.nsn * sizeof(int), st));
-    CU(cudaMemsetAsync(sv->d_done_b.p, 0, S.nsn * sizeof(int), st));
-    CU(cudaMemsetAsync(sv->d_bcnt.p, 0, S.nsn * sizeof(int), st));
-    CU(cudaMemsetAsync(sv->d_bcnt_b.p, 0, S.nsn * sizeof(int), st));
-    CU(cudaMemsetAsync(sv->d_bflag_f.p, 0, std::max(bo, 1) * sizeof(int), st));
-    CU(cudaMemsetAsync(sv->d_bflag_b.p, 0, std::max(bo, 1) * sizeof(int), st));
-    CU(cudaMemsetAsync(sv->d_ticket.p, 0, 2 * sizeof(unsigned long long), st));
-    sv->solve_epoch = 0; sv->ticket_f = sv->ticket_b = 0;
+    CU(cudaDeviceGetAttribute(&sv->num_sms, cudaDevAttrMultiProcessorCount, sv->dev));
+    const MultiStride one{1, S.nsn, std::max(bo, 1), 0, n, (long long)std::max<size_t>(S.rows.size(), 1),
+                          std::max<long long>(bv, 1), 0};
+    CU(alloc_sweep_state(sv, sv->sweep, one));
+    sv->solve_epoch = 0;
     {
       int rc2 = build_solve_tables(sv, S, st);
       if (rc2 != B200LDLT_SUCCESS) return rc2;
@@ -897,21 +905,13 @@ static int run_analysis(Solver* sv, const double* vals) {
       rc2 = build_solve_plan(sv, S, take, sv->splan, st);
       if (rc2 != B200LDLT_SUCCESS) return rc2;
     }
-    CU(cudaFuncSetAttribute(k_solve<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM));
-    CU(cudaFuncSetAttribute(k_solve<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM));
     if (sv->dbg.solve_timeline) {
       CU(sv->d_tlog.alloc(2 * (size_t)(sv->splan.ntf + sv->splan.ntb) + 8 * (size_t)sv->splan.nsub + 8));
-      sv->splan.V.tlog = sv->d_tlog.p;
+      sv->splan.tlog = sv->d_tlog.p;
     }
-    int occ = 1;
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_solve<true>, DF_THREADS, DF_DYN_SMEM));
-    int occ_b = 1;
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_solve<false>, DF_THREADS, DF_DYN_SMEM));
-    CU(cudaDeviceGetAttribute(&sv->num_sms, cudaDevAttrMultiProcessorCount, sv->dev));
-    sv->df_grid = std::max(1, std::min(occ, occ_b)) * sv->num_sms;
     if (sv->opt.verbose)
-      fprintf(stderr, "[b200ldlt] solve: %d big-front blocks, top grid %d x %d thr (%d/%d CTAs per SM)\n",
-              bo, sv->df_grid, DF_THREADS, occ, occ_b);
+      fprintf(stderr, "[b200ldlt] solve: %d big-front blocks, top grid %d x %d thr (%d CTAs per SM)\n",
+              bo, sv->sweep.grid, DF_THREADS, sv->sweep.grid / sv->num_sms);
     CU(cudaStreamSynchronize(st));
   }
 
@@ -1244,128 +1244,94 @@ __global__ void k_mark_flags(int* flags, const int* __restrict__ list, int n, in
   if (i < n) flags[list[i]] = value;
 }
 
-// one sweep over the fronts of a plan: ONE persistent kernel (forward: subtrees then top tasks; backward: the reverse)
-static int launch_sweep(Solver* sv, const SolvePlan& SP, bool fwd) {
+// the DevSolve of a sweep: the handle's per-front tables, the plan's work lists, the state's arrays (column 0; the
+// kernels find the other columns through MultiStride)
+static DevSolve sweep_view(const Solver* sv, const SolvePlan& SP, const SweepState& W) {
+  DevSolve V;
+  V.tasks = SP.d_tf.p; V.tasks_bwd = SP.d_tb.p; V.ntasks_fwd = SP.ntf; V.ntasks_bwd = SP.ntb;
+  V.bundle = SP.d_bundle.p;
+  V.done_f = W.d_done_f.p; V.done_b = W.d_done_b.p;
+  V.bflag_f = W.d_bflag_f.p; V.bflag_b = W.d_bflag_b.p; V.bcnt = W.d_bcnt.p; V.bcnt_b = W.d_bcnt_b.p;
+  V.boff = sv->d_boff.p; V.bigv_off = sv->d_bigv_off.p; V.bigv = W.d_bigv.p; V.bigy = W.d_bigy.p;
+  V.part = W.width > 1 ? W.d_part.p : SP.d_part.p; V.ccnt = W.width > 1 ? W.d_ccnt.p : SP.d_ccnt.p;
+  V.ticket = W.d_ticket.p;
+  V.linv = sv->d_linv.p; V.linv_off = sv->d_linv_off.p;
+  V.fdesc = sv->d_fdesc.p; V.gmap = sv->d_gmap.p; V.gmap_off = sv->d_gmap_off.p;
+  V.subs = SP.d_subs.p; V.sub_meta = SP.d_sub_meta.p; V.subrow = SP.d_subrow.p; V.nsub = SP.nsub;
+  V.subpair = SP.d_subpair.p; V.npair = SP.npair; V.sub_Loff = SP.d_sub_Loff.p;
+  V.upper_max = sv->opt.smem_front_max;
+  V.tlog = W.width > 1 ? nullptr : SP.tlog;
+  return V;
+}
+
+// one sweep of nb columns (nb <= W.width) over the fronts of a plan: the bottom levels one launch each, and ONE persistent
+// kernel (forward: bottom levels, then subtrees, then top tasks; backward: the reverse)
+static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, bool fwd) {
   cudaStream_t st = sv->stream;
-  const DevSolve& V = SP.V;
-  const long long nt = (long long)(fwd ? SP.ntf : SP.ntb) + SP.npair;
-  const int grid = (int)std::min<long long>(sv->df_grid, nt);
+  const DevSolve V = sweep_view(sv, SP, W);
+  MultiStride M = W.M;
+  M.nb = nb;
+  const bool multi = nb > 1;
+  const long long nt = ((long long)(fwd ? SP.ntf : SP.ntb) + SP.npair) * nb;
+  const int grid = (int)std::min<long long>(W.grid, nt);
   const int nd = (int)SP.direct_cnt.size();
+  const auto k_direct = fwd ? (multi ? k_solve_direct<true, true> : k_solve_direct<true, false>)
+                            : (multi ? k_solve_direct<false, true> : k_solve_direct<false, false>);
+  const auto k_sweep = sweep_kernel(fwd, multi);
   auto direct = [&](int l) {
     if (SP.direct_cnt[l] <= 0) return;
-    const unsigned g = cdiv(SP.direct_cnt[l], DF_THREADS / 32);
-    if (fwd) k_solve_direct<true><<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, V, SP.d_direct[l]->p, SP.direct_cnt[l], sv->solve_epoch, sv->d_x.p, sv->d_cbv.p);
-    else k_solve_direct<false><<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, V, SP.d_direct[l]->p, SP.direct_cnt[l], sv->solve_epoch, sv->d_x.p, sv->d_cbv.p);
+    const unsigned g = cdiv(SP.direct_cnt[l] * nb, DF_THREADS / 32);
+    k_direct<<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, V, M, SP.d_direct[l]->p, SP.direct_cnt[l], sv->solve_epoch, W.d_x.p, W.d_cbv.p);
     ++sv->launches;
   };
-  if (fwd) {
-    for (int l = 0; l < nd; ++l) direct(l);      // bottom levels first, one launch per level
-    if (nt > 0) {
-      k_solve<true><<<grid, DF_THREADS, DF_DYN_SMEM, st>>>(sv->DS, sv->DN, V, sv->solve_epoch, sv->ticket_f, sv->d_x.p, sv->d_cbv.p);
-      sv->ticket_f += (unsigned long long)nt + grid;
-      ++sv->launches;
-    }
-  } else {
-    if (nt > 0) {
-      k_solve<false><<<grid, DF_THREADS, DF_DYN_SMEM, st>>>(sv->DS, sv->DN, V, sv->solve_epoch, sv->ticket_b, sv->d_x.p, sv->d_cbv.p);
-      sv->ticket_b += (unsigned long long)nt + grid;
-      ++sv->launches;
-    }
-    for (int l = nd - 1; l >= 0; --l) direct(l);
+  if (fwd) for (int l = 0; l < nd; ++l) direct(l);
+  if (nt > 0) {
+    unsigned long long& ticket = fwd ? W.ticket_f : W.ticket_b;
+    k_sweep<<<grid, DF_THREADS, DF_DYN_SMEM, st>>>(sv->DS, sv->DN, V, M, sv->solve_epoch, ticket, W.d_x.p, W.d_cbv.p);
+    ticket += (unsigned long long)nt + grid;
+    ++sv->launches;
   }
+  if (!fwd) for (int l = nd - 1; l >= 0; --l) direct(l);
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
 }
 
-static int enqueue_solve(Solver* sv, const double* d_b, double* d_out) {
-  Symbolic& S = sv->S;
+// nb columns of d_in (leading dimension n) -> d_out (in place when they are the same) by one forward and one backward
+// sweep over all fronts, nb <= W.width
+static int enqueue_solve(Solver* sv, SweepState& W, const double* d_in, double* d_out, int nb) {
   cudaStream_t st = sv->stream;
-  const int n = S.n;
-  int& L = sv->launches;
-  k_rhs_in<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_b, sv->d_x.p); ++L;
-  if (sv->opt.use_graph != 2) {   // default: subtree + task-queue sweeps (use_graph == 2 selects the level-per-launch kernels)
-    sv->solve_epoch++;
-    int rc = launch_sweep(sv, sv->splan, true);
-    if (rc == B200LDLT_SUCCESS) rc = launch_sweep(sv, sv->splan, false);
-    if (rc != B200LDLT_SUCCESS) return rc;
-    k_sol_out<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, sv->d_x.p, d_out); ++L;
-    CU(cudaGetLastError());
-    return B200LDLT_SUCCESS;
-  }
-  const int* fl = sv->d_front_list.p;
-  for (int l = 0; l < S.nlevels; ++l) {
-    const LevelPlan& P = sv->plan[l];
-    int threads = P.fmax <= 64 ? 64 : (P.fmax <= 256 ? 256 : 1024);
-    k_fwd_front<<<P.all_cnt, threads, 2 * (size_t)P.fmax * sizeof(double), st>>>(sv->DS, sv->DN, fl + P.all_off, sv->d_x.p, sv->d_cbv.p); ++L;
-  }
-  for (int l = S.nlevels - 1; l >= 0; --l) {
-    const LevelPlan& P = sv->plan[l];
-    int threads = P.fmax <= 64 ? 64 : (P.fmax <= 256 ? 256 : 1024);
-    k_bwd_front<<<P.all_cnt, threads, (size_t)P.fmax * sizeof(double), st>>>(sv->DS, sv->DN, fl + P.all_off, sv->d_x.p); ++L;
-  }
-  k_sol_out<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, sv->d_x.p, d_out); ++L;
+  const int n = sv->n;
+  const dim3 g(cdiv(n, 256), nb);
+  k_rhs_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_in, W.d_x.p, W.M.x); ++sv->launches;
+  sv->solve_epoch++;
+  int rc = launch_sweep(sv, sv->splan, W, nb, true);
+  if (rc == B200LDLT_SUCCESS) rc = launch_sweep(sv, sv->splan, W, nb, false);
+  if (rc != B200LDLT_SUCCESS) return rc;
+  k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, W.M.x, d_out); ++sv->launches;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
 }
 
-// Per-column sweep state of the blocked solve, for the full block width B200_SOLVE_BLOCK: allocated once per analysis,
-// at the first nrhs > 1 solve, before that solve's timing starts.  Returns false (and the columns are then solved one by
-// one, as with B200_SOLVE_BLOCK=1) when the device memory for it cannot be had.
+// The sweep state of the blocked solve, B200_SOLVE_BLOCK columns wide: allocated once per analysis, at the first nrhs > 1
+// solve, before that solve's timing starts.  Returns false (and the columns are then solved one by one, as with
+// B200_SOLVE_BLOCK=1) when the device memory for it cannot be had.
 static bool block_solve_state(Solver* sv) {
   if (sv->blk) return sv->blk->width > 1;
   const int nb = sv->dbg.solve_block;
-  sv->blk.reset(new Solver::BlockSolve());
+  sv->blk.reset(new SweepState());   // width 0: not retried before the next analysis
   if (nb < 2) return false;
-  cudaStream_t st = sv->stream;
-  Solver::BlockSolve& B = *sv->blk;
-  const SolvePlan& SP = sv->splan;
-  MultiStride& M = B.M;
+  SweepState& B = *sv->blk;
+  MultiStride M = sv->sweep.M;
   M.nb = nb;
-  M.nsn = sv->S.nsn;
-  M.nbo = (int)sv->d_bflag_f.n;
-  M.nccnt = (int)SP.d_ccnt.n;
-  M.x = sv->n;
-  M.cbv = (long long)sv->d_cbv.n;
-  M.bigv = (long long)sv->d_bigv.n;
-  M.part = (long long)SP.d_part.n;
-  DevBuf<int>* flags[] = {&B.d_done_f, &B.d_done_b, &B.d_bcnt, &B.d_bcnt_b, &B.d_bflag_f, &B.d_bflag_b, &B.d_ccnt};
-  const long long per_col[] = {M.nsn, M.nsn, M.nsn, M.nsn, M.nbo, M.nbo, M.nccnt};
-  int occ = 1, occ_b = 1;
-  auto setup = [&]() -> cudaError_t {
-    cudaError_t e;
-    if ((e = B.d_x.alloc(M.x * nb)) != cudaSuccess || (e = B.d_cbv.alloc(M.cbv * nb)) != cudaSuccess ||
-        (e = B.d_bigv.alloc(M.bigv * nb)) != cudaSuccess || (e = B.d_bigy.alloc(M.bigv * nb)) != cudaSuccess ||
-        (e = B.d_part.alloc(M.part * nb)) != cudaSuccess || (e = B.d_ticket.alloc(2)) != cudaSuccess)
-      return e;
-    for (int i = 0; i < 7; ++i) {
-      if ((e = flags[i]->alloc(std::max<long long>(per_col[i] * nb, 1))) != cudaSuccess) return e;
-      if ((e = cudaMemsetAsync(flags[i]->p, 0, flags[i]->n * sizeof(int), st)) != cudaSuccess) return e;
-    }
-    if ((e = cudaMemsetAsync(B.d_ticket.p, 0, 2 * sizeof(unsigned long long), st)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k_solve_multi<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM)) != cudaSuccess ||
-        (e = cudaFuncSetAttribute(k_solve_multi<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM)) != cudaSuccess ||
-        (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_solve_multi<true>, DF_THREADS, DF_DYN_SMEM)) != cudaSuccess ||
-        (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, k_solve_multi<false>, DF_THREADS, DF_DYN_SMEM)) != cudaSuccess)
-      return e;
-    return cudaStreamSynchronize(st);
-  };
-  const cudaError_t e = setup();
+  M.nccnt = (int)sv->splan.d_ccnt.n;
+  M.part = (long long)sv->splan.d_part.n;
+  const cudaError_t e = alloc_sweep_state(sv, B, M);
   if (e != cudaSuccess) {
     if (sv->opt.verbose) fprintf(stderr, "[b200ldlt] blocked solve unavailable (%s): one solve per column\n", cudaGetErrorString(e));
     cudaGetLastError();
-    sv->blk.reset(new Solver::BlockSolve());   // width 0: not retried before the next analysis
+    sv->blk.reset(new SweepState());
     return false;
   }
-  B.width = nb;
-  DevSolve& V = B.V;
-  V = SP.V;
-  V.done_f = B.d_done_f.p; V.done_b = B.d_done_b.p;
-  V.bflag_f = B.d_bflag_f.p; V.bflag_b = B.d_bflag_b.p; V.bcnt = B.d_bcnt.p; V.bcnt_b = B.d_bcnt_b.p;
-  V.bigv = B.d_bigv.p; V.bigy = B.d_bigy.p;
-  V.part = B.d_part.p; V.ccnt = B.d_ccnt.p;
-  V.ticket = B.d_ticket.p;
-  V.tlog = nullptr;
-  B.grid = std::max(1, std::min(occ, occ_b)) * sv->num_sms;
   if (sv->opt.verbose)
     fprintf(stderr, "[b200ldlt] blocked solve: %d columns, %.1f MB of per-column state, grid %d\n", nb,
             (double)(8 * (B.d_x.n + B.d_cbv.n + B.d_bigv.n + B.d_bigy.n + B.d_part.n) +
@@ -1374,68 +1340,15 @@ static bool block_solve_state(Solver* sv) {
   return true;
 }
 
-// one sweep of the blocked solve: the launches of launch_sweep, each carrying all nb columns
-static int launch_sweep_block(Solver* sv, int nb, bool fwd) {
-  cudaStream_t st = sv->stream;
-  Solver::BlockSolve& B = *sv->blk;
-  const SolvePlan& SP = sv->splan;
-  MultiStride M = B.M;
-  M.nb = nb;
-  const long long nt = ((long long)(fwd ? SP.ntf : SP.ntb) + SP.npair) * nb;
-  const int grid = (int)std::min<long long>(B.grid, nt);
-  const int nd = (int)SP.direct_cnt.size();
-  auto direct = [&](int l) {
-    if (SP.direct_cnt[l] <= 0) return;
-    const unsigned g = cdiv(SP.direct_cnt[l] * nb, DF_THREADS / 32);
-    if (fwd) k_solve_direct_multi<true><<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, B.V, M, SP.d_direct[l]->p, SP.direct_cnt[l], sv->solve_epoch, B.d_x.p, B.d_cbv.p);
-    else k_solve_direct_multi<false><<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, B.V, M, SP.d_direct[l]->p, SP.direct_cnt[l], sv->solve_epoch, B.d_x.p, B.d_cbv.p);
-    ++sv->launches;
-  };
-  if (fwd) {
-    for (int l = 0; l < nd; ++l) direct(l);
-    if (nt > 0) {
-      k_solve_multi<true><<<grid, DF_THREADS, DF_DYN_SMEM, st>>>(sv->DS, sv->DN, B.V, M, sv->solve_epoch, B.ticket_f, B.d_x.p, B.d_cbv.p);
-      B.ticket_f += (unsigned long long)nt + grid;
-      ++sv->launches;
-    }
-  } else {
-    if (nt > 0) {
-      k_solve_multi<false><<<grid, DF_THREADS, DF_DYN_SMEM, st>>>(sv->DS, sv->DN, B.V, M, sv->solve_epoch, B.ticket_b, B.d_x.p, B.d_cbv.p);
-      B.ticket_b += (unsigned long long)nt + grid;
-      ++sv->launches;
-    }
-    for (int l = nd - 1; l >= 0; --l) direct(l);
-  }
-  CU(cudaGetLastError());
-  return B200LDLT_SUCCESS;
-}
-
-// nb (>= 2) columns of d_rhs (leading dimension n), solved in place by one forward and one backward sweep
-static int enqueue_solve_block(Solver* sv, double* d_rhs, int nb) {
-  int rc;
-  Solver::BlockSolve& B = *sv->blk;
-  cudaStream_t st = sv->stream;
-  const int n = sv->n;
-  const dim3 g(cdiv(n, 256), nb);
-  k_rhs_in_multi<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_rhs, B.d_x.p, B.M.x); ++sv->launches;
-  sv->solve_epoch++;
-  rc = launch_sweep_block(sv, nb, true);
-  if (rc == B200LDLT_SUCCESS) rc = launch_sweep_block(sv, nb, false);
-  if (rc != B200LDLT_SUCCESS) return rc;
-  k_sol_out_multi<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, B.d_x.p, B.M.x, d_rhs); ++sv->launches;
-  CU(cudaGetLastError());
-  return B200LDLT_SUCCESS;
-}
-
 // nrhs columns of d_rhs (leading dimension n), in place: blocks of up to B200_SOLVE_BLOCK columns through the blocked
-// sweeps, single columns (and every column of the level-per-launch solve, use_graph == 2) through enqueue_solve.
-// `blocked`: the result of block_solve_state, called by the entry point before its timing starts.
+// state, single columns through the one-column state.  `blocked`: the result of block_solve_state, called by the entry
+// point before its timing starts.
 static int enqueue_solve_columns(Solver* sv, double* d_rhs, int nrhs, bool blocked) {
   const int cap = blocked ? sv->blk->width : 1;
   for (int c = 0; c < nrhs;) {
     const int w = std::min(cap, nrhs - c);
     double* col = d_rhs + (size_t)c * sv->n;
-    const int rc = w == 1 ? enqueue_solve(sv, col, col) : enqueue_solve_block(sv, col, w);
+    const int rc = enqueue_solve(sv, w == 1 ? sv->sweep : *sv->blk, col, col, w);
     if (rc != B200LDLT_SUCCESS) return rc;
     c += w;
   }
@@ -1509,7 +1422,7 @@ void b200ldlt_default_options(b200ldlt_options* o) {
   o->smem_front_max = 96;    // fronts of order 65..96 in shared memory, larger ones through the panel pipeline
                              // (H100 SXM, 700 W: 64 and 128 are 1-2.5 % slower at N=400 and N=800)
   o->tc_schur_min_r = 0;
-  o->use_graph = 1;   /* 1 = CUDA-graph replay of the factorisation + dataflow solve; 0 = plain launches; 2 = level-per-launch solve */
+  o->use_graph = 1;   /* 1 = CUDA-graph replay of the factorisation; any other value = plain launches */
   o->verbose = 0;
 }
 
@@ -1614,7 +1527,7 @@ int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs) {
   if (!sv || !sv->factored) { if (sv) sv->err = "solve before factor"; return B200LDLT_FATAL_ERROR; }
   CU(cudaSetDevice(sv->dev));
   cudaStream_t st = sv->stream;
-  const bool blocked = nrhs > 1 && sv->opt.use_graph != 2 && block_solve_state(sv);
+  const bool blocked = nrhs > 1 && block_solve_state(sv);
   sv->launches = 0;
   CU(cudaEventRecord(sv->ev0, st));
   {
@@ -1646,7 +1559,7 @@ int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs) {
   // caller's array is pageable: Ipopt allocates it per call, IpTSymLinearSolver.cpp:222-241); same on the way back.
   const size_t total = n * (size_t)nrhs;
   const size_t chunk = std::max<size_t>((total + 3) / 4, 32768);
-  const bool blocked = nrhs > 1 && sv->opt.use_graph != 2 && block_solve_state(sv);
+  const bool blocked = nrhs > 1 && block_solve_state(sv);
   sv->launches = 0;
   CU(cudaEventRecord(sv->ev0, st));
   for (size_t o = 0; o < total; o += chunk) {
@@ -1704,7 +1617,7 @@ int b200ldlt_dump_factor_timeline(b200ldlt_handle h, const char* path) {
 /* debug: write the per-task timeline of the last solve (needs env B200_SOLVE_TIMELINE=1 at analyse time) */
 int b200ldlt_dump_solve_timeline(b200ldlt_handle h, const char* path) {
   Solver* sv = (Solver*)h;
-  if (!sv || !sv->splan.V.tlog) return B200LDLT_FATAL_ERROR;
+  if (!sv || !sv->splan.tlog) return B200LDLT_FATAL_ERROR;
   std::vector<unsigned long long> t(sv->d_tlog.n);
   CU(cudaMemcpy(t.data(), sv->d_tlog.p, t.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   FILE* fp = fopen(path, "w");
@@ -1759,8 +1672,8 @@ void* b200ldlt_device_ptr(b200ldlt_handle h, const char* name) {
   if (nm == "vals") return sv->d_vals.p;        // exists before the (lazy) analysis: assemble_augsys_device fills it
   if (!sv->analysed) return nullptr;
   if (nm == "CB") return sv->d_CB.p;
-  if (nm == "cbv") return sv->d_cbv.p;
-  if (nm == "x") return sv->d_x.p;
+  if (nm == "cbv") return sv->sweep.d_cbv.p;
+  if (nm == "x") return sv->sweep.d_x.p;
   if (nm == "counters") return sv->d_counters.p;
   return nullptr;
 }
@@ -1812,18 +1725,18 @@ int b200ldlt_shard_solve(b200ldlt_handle h, int phase, double* d_rhs) {
   int rc = B200LDLT_SUCCESS;
   if (phase == 0) {
     sv->launches = 0;
-    k_rhs_in<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_rhs, sv->d_x.p);
+    k_rhs_in<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_rhs, sv->sweep.d_x.p, n);
     sv->solve_epoch++;
-    rc = launch_sweep(sv, H.splan[0], true);
+    rc = launch_sweep(sv, H.splan[0], sv->sweep, 1, true);
   } else if (phase == 1) {
-    if (H.d_mark_cut.n) k_mark_flags<<<cdiv((long long)H.d_mark_cut.n, 256), 256, 0, st>>>(sv->d_done_f.p, H.d_mark_cut.p, (int)H.d_mark_cut.n, sv->solve_epoch);
-    rc = launch_sweep(sv, H.splan[1], true);
-    if (rc == B200LDLT_SUCCESS) rc = launch_sweep(sv, H.splan[1], false);
+    if (H.d_mark_cut.n) k_mark_flags<<<cdiv((long long)H.d_mark_cut.n, 256), 256, 0, st>>>(sv->sweep.d_done_f.p, H.d_mark_cut.p, (int)H.d_mark_cut.n, sv->solve_epoch);
+    rc = launch_sweep(sv, H.splan[1], sv->sweep, 1, true);
+    if (rc == B200LDLT_SUCCESS) rc = launch_sweep(sv, H.splan[1], sv->sweep, 1, false);
   } else if (phase == 2) {
-    if (H.rank != 0 && H.d_mark_top.n) k_mark_flags<<<cdiv((long long)H.d_mark_top.n, 256), 256, 0, st>>>(sv->d_done_b.p, H.d_mark_top.p, (int)H.d_mark_top.n, sv->solve_epoch);
-    rc = launch_sweep(sv, H.splan[0], false);
+    if (H.rank != 0 && H.d_mark_top.n) k_mark_flags<<<cdiv((long long)H.d_mark_top.n, 256), 256, 0, st>>>(sv->sweep.d_done_b.p, H.d_mark_top.p, (int)H.d_mark_top.n, sv->solve_epoch);
+    rc = launch_sweep(sv, H.splan[0], sv->sweep, 1, false);
   } else if (phase == 3) {
-    k_sol_out<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, sv->d_x.p, d_rhs);
+    k_sol_out<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, sv->sweep.d_x.p, n, d_rhs);
   } else return B200LDLT_FATAL_ERROR;
   CU(cudaGetLastError());
   return rc;
@@ -1896,7 +1809,7 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
   cudaStream_t st = sv->stream;
   CU(cudaMemcpyAsync(sv->d_ref_b.p, d_rhs, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
   sv->launches = 0;
-  int rc = enqueue_solve(sv, d_rhs, d_rhs);
+  int rc = enqueue_solve(sv, sv->sweep, d_rhs, d_rhs, 1);
   if (rc != B200LDLT_SUCCESS) return rc;
   b200vec vb{sv->d_ref_b.p, n, 0, 0.0}, vx{d_rhs, n, 0, 0.0}, vr{sv->d_ref_r.p, n, 0, 0.0};
   double nb = 0.0, ratio = 0.0;
@@ -1910,7 +1823,7 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
     if (b200vec_amax(sv->vec, &vr, &nr) || b200vec_amax(sv->vec, &vx, &nx)) { sv->err = b200vec_last_error(sv->vec); return B200LDLT_FATAL_ERROR; }
     ratio = (nb + nx == 0.0) ? nr : nr / (std::min(nx, 1e6 * nb) + nb);
     if (step >= max_steps || (step >= min_steps && ratio <= tol)) break;
-    rc = enqueue_solve(sv, sv->d_ref_r.p, sv->d_ref_r.p);     // d = A^-1 r
+    rc = enqueue_solve(sv, sv->sweep, sv->d_ref_r.p, sv->d_ref_r.p, 1);     // d = A^-1 r
     if (rc != B200LDLT_SUCCESS) return rc;
     if (b200vec_axpy(sv->vec, 1.0, &vr, &vx)) { sv->err = b200vec_last_error(sv->vec); return B200LDLT_FATAL_ERROR; }
     ++step;

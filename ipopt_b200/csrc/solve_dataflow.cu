@@ -19,6 +19,7 @@
 //                      sorted) list and every ticket holder is resident, so the scheme cannot deadlock.  Chunk partials
 //                      are combined by the last-arriving CTA in chunk order (fence + counter): bit-reproducible.
 // Forward: direct levels, then subtrees before top tasks; backward: top tasks before subtrees, then the direct levels.
+// A block of right-hand sides takes the same launches through the MULTI instantiations of both kernels (see MultiStride).
 // L is streamed exactly once per sweep (HBM-bound, SURVEY.md 8d: 2*8*nnz(L) bytes per right-hand side); children ->
 // parent data flows through per-front update vectors gathered by the parent (no atomics on the data path).
 // Replaces the vendor back-solve of the reference (MUMPS job=3,
@@ -1210,11 +1211,59 @@ __device__ void solve_subtree(const DevSym& S, const DevNum& N, const DevSolve& 
 }
 
 // ------------------------------------------------------------------------------------------------
-// ONE persistent kernel per sweep.  Work items are taken with an atomic ticket: forward = subtrees (largest first), then
-// the top tasks by level; backward = top tasks (levels descending), then the subtrees.
+// A block of nb right-hand sides (2 <= nb <= MS_NB_MAX) goes through the same launches: the MULTI instantiations of
+// k_solve / k_solve_direct turn every work item into nb items, one per column, issued next to each other in the ticket
+// order: (item 0, col 0), (item 0, col 1), ..., (item 1, col 0), ...  Each column has its own copy of everything a sweep
+// writes -- x, update vectors, bigv / bigy, chunk partials and counters, done / block flags -- so an item runs the same
+// front routines on its column's slices: the arithmetic of every column is the arithmetic of a single-column solve, bit for
+// bit.  The block shares the launches and the dependency latency of the sweep (direct levels, subtree walks, flag hops
+// between top tasks).  It does not share panel traffic: every (item, column) stages its own panels, loads its own L / Linv
+// tiles and waits on its own flags (the items of a front are adjacent tickets, so the later copies may find the panel in
+// L2).  Deadlock freedom carries over: an item only waits for items of its own column that are EARLIER in the ticket order
+// (their single-column predecessors, nb times further back), and every ticket holder is resident.
 // ------------------------------------------------------------------------------------------------
-template <bool FWD>
-__global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, DevSolve V, int epoch,
+#define MS_NB_MAX 8          // widest block; wider calls are cut into blocks of this many columns
+
+// where column c of the sweep state lives: base pointer (DevSolve / kernel argument) + c * stride
+struct MultiStride {
+  int nb;                    // columns
+  int nsn;                   // done_f, done_b, bcnt, bcnt_b
+  int nbo;                   // bflag_f, bflag_b (big-front blocks)
+  int nccnt;                 // chunk counters
+  long long x, cbv;          // x (n), update vectors (rows)
+  long long bigv;            // bigv, bigy
+  long long part;            // chunk partials (64 doubles per slot)
+};
+
+__device__ __forceinline__ DevSolve column_view(const DevSolve& V, const MultiStride& M, int c) {
+  DevSolve W = V;
+  W.done_f += (long long)c * M.nsn; W.done_b += (long long)c * M.nsn;
+  W.bcnt += (long long)c * M.nsn; W.bcnt_b += (long long)c * M.nsn;
+  W.bflag_f += (long long)c * M.nbo; W.bflag_b += (long long)c * M.nbo;
+  W.ccnt += (long long)c * M.nccnt;
+  W.bigv += c * M.bigv; W.bigy += c * M.bigv;
+  W.part += c * M.part;
+  return W;
+}
+
+// the front routines on global memory (outside a subtree): x and update vectors of one column
+__device__ __forceinline__ void global_io(FrontIO& io, const DevSym& S, const DevNum& N, const DevSolve& V, double* x,
+                                          double* cbv) {
+  io.Lbase = N.L; io.L0 = 0; io.xs = x; io.col0 = 0; io.uv = cbv; io.ro0 = 0;
+  io.dinv = N.dinv; io.doff = N.doff; io.ptype = N.ptype; io.lperm = N.lperm;
+  io.rel = S.rel; io.subrow = nullptr; io.rootx = nullptr;
+  io.fd = V.fdesc; io.s0 = 0; io.sR = S.nsn - 1; io.chi = S.child_idx; io.ch00 = 0;
+  io.gfd = V.fdesc; io.gcbv = cbv; io.grel = S.rel; io.grows = S.rows; io.gx = x;
+}
+
+// ------------------------------------------------------------------------------------------------
+// ONE persistent kernel per sweep.  Work items are taken with an atomic ticket: forward = subtrees (largest first), then
+// the top tasks by level; backward = top tasks (levels descending), then the subtrees.  MULTI: (item, column) tickets over
+// M.nb columns.  Otherwise the ticket is the item and the column a compile-time 0 (no per-ticket division, the column view
+// is the identity), and the top tasks are recorded in V.tlog when it is set.
+// ------------------------------------------------------------------------------------------------
+template <bool FWD, bool MULTI>
+__global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, DevSolve V, MultiStride M, int epoch,
                                                          unsigned long long ticket_base,
                                                          double* __restrict__ x, double* __restrict__ cbv) {
   extern __shared__ __align__(16) unsigned char smraw[];
@@ -1228,13 +1277,8 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
   const long long stage_doubles = (DF_DYN_SMEM / 8) - ((DF_THREADS / 32) * DF_WSCR + DF_MIDSCR);
   const SolveTask* tasks = FWD ? V.tasks : V.tasks_bwd;
   const int ntasks = FWD ? V.ntasks_fwd : V.ntasks_bwd;
-  const unsigned long long total = (unsigned long long)ntasks + V.npair;
-  FrontIO io;
-  io.Lbase = N.L; io.L0 = 0; io.xs = x; io.col0 = 0; io.uv = cbv; io.ro0 = 0;
-  io.dinv = N.dinv; io.doff = N.doff; io.ptype = N.ptype; io.lperm = N.lperm;
-  io.rel = S.rel; io.subrow = nullptr; io.rootx = nullptr;
-  io.fd = V.fdesc; io.s0 = 0; io.sR = S.nsn - 1; io.chi = S.child_idx; io.ch00 = 0;
-  io.gfd = V.fdesc; io.gcbv = cbv; io.grel = S.rel; io.grows = S.rows; io.gx = x;
+  const unsigned long long nb = MULTI ? (unsigned long long)M.nb : 1ull;
+  const unsigned long long total = ((unsigned long long)ntasks + V.npair) * nb;
   unsigned mphase = 0, mphase1 = 0;
   const Team cta{(int)threadIdx.x, DF_THREADS, 0};
   if (threadIdx.x == 0) { mbar_init(&s_mbar, 1); mbar_init(&s_mbar1, 1); }
@@ -1245,30 +1289,37 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
     const unsigned long long tk = s_ticket;
     __syncthreads();
     if (tk >= total) return;
-    const bool is_sub = FWD ? (tk < (unsigned long long)V.npair) : (tk >= (unsigned long long)ntasks);
+    const unsigned long long item = MULTI ? tk / nb : tk;
+    const int c = MULTI ? (int)(tk - item * nb) : 0;
+    const DevSolve Vc = column_view(V, M, c);
+    double* xc = x + c * M.x;
+    double* cbvc = cbv + c * M.cbv;
+    const bool is_sub = FWD ? (item < (unsigned long long)V.npair) : (item >= (unsigned long long)ntasks);
     if (is_sub) {
-      const int2 pr = V.subpair[FWD ? tk : tk - ntasks];
+      const int2 pr = V.subpair[FWD ? item : item - ntasks];
       // (u0, -1): one subtree by the whole CTA.  (u0, u1): two subtrees side by side -- threads 0..127 walk u0 in the lower
       // part of the shared memory, threads 128..255 walk u1 above it (own transaction barrier, own hardware barrier).
       const bool second = pr.y >= 0 && threadIdx.x >= DF_THREADS / 2;
       const Team tm = pr.y < 0 ? cta : Team{(int)threadIdx.x - (second ? DF_THREADS / 2 : 0), DF_THREADS / 2, second ? 2 : 1};
-      solve_subtree<FWD>(S, N, V, second ? pr.y : pr.x, epoch, second ? smraw + V.subs[pr.x].sbytes : smraw,
-                         second ? &s_mbar1 : &s_mbar, second ? mphase1 : mphase, x, cbv, tm);
+      solve_subtree<FWD>(S, N, Vc, second ? pr.y : pr.x, epoch, second ? smraw + V.subs[pr.x].sbytes : smraw,
+                         second ? &s_mbar1 : &s_mbar, second ? mphase1 : mphase, xc, cbvc, tm);
       mphase ^= 1;
       if (pr.y >= 0) mphase1 ^= 1;
       __syncthreads();
       continue;
     }
-    const unsigned long long ti = FWD ? tk - V.npair : tk;
+    const unsigned long long ti = FWD ? item - V.npair : item;
     const SolveTask T = tasks[ti];
+    FrontIO io;
+    global_io(io, S, N, Vc, xc, cbvc);
     unsigned long long t_start = 0;
-    if (V.tlog && threadIdx.x == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
+    if (!MULTI && V.tlog && threadIdx.x == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
     if (T.type == ST_SMALL) {
       const int w = threadIdx.x >> 5;
       if (w < T.blk) {
         const int s = V.bundle[T.s + w];
-        if (FWD) w64_fwd<false>(io, V, s, epoch, sm + w * DF_WSCR);
-        else w64_bwd<false>(io, V, s, epoch, S.sn_parent[s], V.upper_max);
+        if (FWD) w64_fwd<false>(io, Vc, s, epoch, sm + w * DF_WSCR);
+        else w64_bwd<false>(io, Vc, s, epoch, S.sn_parent[s], V.upper_max);
       }
     } else if (T.type == ST_MID) {
       // stage the whole panel in shared memory with one bulk copy when it fits (it does not depend on the right-hand
@@ -1287,19 +1338,19 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
         Lp = stage; mb = &s_mbar; ph = mphase;
         mphase ^= 1;
       }
-      if (FWD) mid_fwd<false>(io, V, T.s, epoch, midscr, Lp, mb, ph, cta);
-      else mid_bwd<false>(io, V, T.s, epoch, S.sn_parent[T.s], midscr, Lp, mb, ph, V.upper_max, cta);
+      if (FWD) mid_fwd<false>(io, Vc, T.s, epoch, midscr, Lp, mb, ph, cta);
+      else mid_bwd<false>(io, Vc, T.s, epoch, S.sn_parent[T.s], midscr, Lp, mb, ph, V.upper_max, cta);
     } else if (T.type == ST_FP) {
-      big_fp(S, N, V, T, epoch, sm, &s_flag, x, cbv);
+      big_fp(S, N, Vc, T, epoch, sm, &s_flag, xc, cbvc);
     } else if (T.type == ST_FC) {
-      big_fc(S, N, V, T, epoch, sm, &s_flag, x, cbv);
+      big_fc(S, N, Vc, T, epoch, sm, &s_flag, xc, cbvc);
     } else if (T.type == ST_BT) {
-      big_bt(S, N, V, T, epoch, sm, &s_flag, x);
+      big_bt(S, N, Vc, T, epoch, sm, &s_flag, xc);
     } else {
-      big_bx(S, N, V, T, epoch, sm, &s_flag, x);
+      big_bx(S, N, Vc, T, epoch, sm, &s_flag, xc);
     }
     __syncthreads();
-    if (V.tlog && threadIdx.x == 0) {
+    if (!MULTI && V.tlog && threadIdx.x == 0) {
       unsigned long long t_end;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_end));
       unsigned long long* rec = V.tlog + 2 * ((FWD ? 0 : (unsigned long long)V.ntasks_fwd) + ti);
@@ -1314,25 +1365,25 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
 // gives every front its own warp straight from global memory (column loads issued ahead of the shuffle chain) with every
 // warp slot of the GPU busy -- instead of walking them inside the shared-memory subtrees, where they are serialised behind
 // each other on a handful of warps.  Forward: these launches precede k_solve<fwd>; backward: they follow k_solve<bwd>.
-// Their parents find the update vectors in global memory (FrontDesc::direct).
+// Their parents find the update vectors in global memory (FrontDesc::direct).  MULTI: one warp per (front, column), the
+// M.nb warps of a front side by side (the panel comes from L1 / L2 after the first).
 // ------------------------------------------------------------------------------------------------
-template <bool FWD>
-__global__ void __launch_bounds__(DF_THREADS, 2) k_solve_direct(DevSym S, DevNum N, DevSolve V, const int* __restrict__ list,
-                                                                int cnt, int epoch, double* __restrict__ x,
-                                                                double* __restrict__ cbv) {
+template <bool FWD, bool MULTI>
+__global__ void __launch_bounds__(DF_THREADS, 2) k_solve_direct(DevSym S, DevNum N, DevSolve V, MultiStride M,
+                                                                const int* __restrict__ list, int cnt, int epoch,
+                                                                double* __restrict__ x, double* __restrict__ cbv) {
   __shared__ double wscr[(DF_THREADS / 32) * DF_WSCR];
   const int w = threadIdx.x >> 5;
   const int g = blockIdx.x * (DF_THREADS / 32) + w;
-  if (g >= cnt) return;
+  const int nb = MULTI ? M.nb : 1;
+  if (g >= cnt * nb) return;
+  const int c = MULTI ? g % nb : 0;
+  const DevSolve Vc = column_view(V, M, c);
   FrontIO io;
-  io.Lbase = N.L; io.L0 = 0; io.xs = x; io.col0 = 0; io.uv = cbv; io.ro0 = 0;
-  io.dinv = N.dinv; io.doff = N.doff; io.ptype = N.ptype; io.lperm = N.lperm;
-  io.rel = S.rel; io.subrow = nullptr; io.rootx = nullptr;
-  io.fd = V.fdesc; io.s0 = 0; io.sR = S.nsn - 1; io.chi = S.child_idx; io.ch00 = 0;
-  io.gfd = V.fdesc; io.gcbv = cbv; io.grel = S.rel; io.grows = S.rows; io.gx = x;
-  const int s = list[g];
-  if (FWD) w64_fwd<false>(io, V, s, epoch, wscr + w * DF_WSCR);
-  else w64_bwd<false>(io, V, s, epoch, -1, V.upper_max);
+  global_io(io, S, N, Vc, x + c * M.x, cbv + c * M.cbv);
+  const int s = list[MULTI ? g / nb : g];
+  if (FWD) w64_fwd<false>(io, Vc, s, epoch, wscr + w * DF_WSCR);
+  else w64_bwd<false>(io, Vc, s, epoch, -1, Vc.upper_max);
 }
 
 }  // namespace b200
