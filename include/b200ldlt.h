@@ -101,6 +101,28 @@ int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs);
 /* Same with a device-resident rhs/solution. */
 int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs);
 
+/* ---- partial solves and factor inspection (cf. MA57 / HSL_MA97 job 1-4, Pardiso phases 331-333) ---------------------
+ * The factor call computes  S A S = P L D L^T P^T :  S the diagonal (power-of-two) equilibration of that call
+ * (device_ptr "scale"), P the fill-reducing permutation composed with the pivoting inside the supernodes, L unit lower
+ * triangular, D block diagonal with 1x1 and 2x2 blocks.  Intermediate vectors are indexed by PIVOT POSITION p = 0..n-1.
+ *   job 0 : x = A^-1 b                      (= b200ldlt_solve)
+ *   job 1 : x = L^-1 P^T S b                original -> pivot order
+ *   job 2 : x = D^-1 b                      pivot -> pivot
+ *   job 3 : x = S P L^-T b                  pivot -> original
+ *   job 4 : x = S P L^-T D^-1 b             pivot -> original
+ * job 3 . 2 . 1 = job 4 . 1 = job 0, bit for bit: the parts run the arithmetic of the full solve.  nrhs > 1 is blocked
+ * like b200ldlt_solve, and every column is bit-identical to a partial solve of that column alone.  Kernel launches per
+ * block (info.launches_solve; ms_solve_gpu as for job 0): job 1, 3, 4: 5 and job 2: 1 (job 0: 8) -- with the default
+ * B200_SOLVE_DIRECT=2; in general job 1, 3, 4 take 3 + D and job 0 takes 4 + 2 D for D direct levels.
+ * FATAL_ERROR (message in last_error) for a job outside 0..4, without factors (also after a SINGULAR factorisation) and
+ * on a sharded handle.  With info.num_forced > 0, D holds the lifted pivots: the parts describe the perturbed matrix. */
+int b200ldlt_solve_partial(b200ldlt_handle h, int job, int nrhs, double* rhs);
+int b200ldlt_solve_partial_device(b200ldlt_handle h, int job, int nrhs, double* d_rhs);
+/* Per pivot position p (any pointer may be NULL): pivot_var[p] = the 0-based original variable; pivot_type[p] = 1 (1x1),
+ * 2 (first of a 2x2), 3 (second of a 2x2); dinv2[2p] = diagonal entry of D^-1, dinv2[2p+1] = off-diagonal entry
+ * (p, p+1) of D^-1 when p opens a 2x2 pivot, else 0.  D^-1 is that of the scaled matrix S A S. */
+int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, double* dinv2);
+
 /* <-> NumberOfNegEVals() (hpp:207) */
 int b200ldlt_num_neg(b200ldlt_handle h);
 /* <-> IncreaseQuality() (hpp:220): pivtol <- min(pivtolmax, pivtol^0.75); returns 0 if already at max.
@@ -166,7 +188,8 @@ int b200ldlt_shard_setup(b200ldlt_handle h, int rank, int world);
 /* "owner" (per supernode: owning rank, -1 = top part on rank 0), "cut_roots", "top_fronts" */
 int64_t b200ldlt_shard_array(b200ldlt_handle h, const char* name, int64_t* out, int64_t cap);
 /* device arrays of the handle: "CB" (contribution blocks, offsets cb_off), "cbv" (update vectors, offsets rows_ptr),
- * "x" (permuted solution vector), "counters" (8 ints), "vals" (triplet values) */
+ * "x" (permuted solution vector), "counters" (8 ints), "vals" (triplet values), "scale" (the n equilibration factors
+ * S of the last factor call, original order) */
 void* b200ldlt_device_ptr(b200ldlt_handle h, const char* name);
 int b200ldlt_shard_factor(b200ldlt_handle h, int phase, int from_host);
 int b200ldlt_shard_factor_finish(b200ldlt_handle h, const int* counters_total, int check_inertia, int expected_neg, int* num_neg);

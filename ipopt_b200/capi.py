@@ -55,7 +55,8 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_solve", "b200ldlt_solve_device", "b200ldlt_num_neg", "b200ldlt_increase_quality",
             "b200ldlt_refactor", "b200ldlt_get_info", "b200ldlt_symbolic_array", "b200ldlt_analyse_now",
             "b200ldlt_residual", "b200ldlt_set_pivtol",
-            "b200ldlt_assemble_augsys_device", "b200ldlt_solve_refine_device"]
+            "b200ldlt_assemble_augsys_device", "b200ldlt_solve_refine_device",
+            "b200ldlt_solve_partial", "b200ldlt_solve_partial_device", "b200ldlt_enquire_indef"]
 
 _lib = None
 
@@ -90,6 +91,9 @@ def load_library():
     L.b200ldlt_device_ptr.restype = vp
     L.b200ldlt_solve.argtypes = [vp, C.c_int, dp]
     L.b200ldlt_solve_device.argtypes = [vp, C.c_int, vp]
+    L.b200ldlt_solve_partial.argtypes = [vp, C.c_int, C.c_int, dp]
+    L.b200ldlt_solve_partial_device.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.b200ldlt_enquire_indef.argtypes = [vp, ip, ip, dp]
     L.b200ldlt_num_neg.argtypes = [vp]
     L.b200ldlt_increase_quality.argtypes = [vp]
     L.b200ldlt_get_info.argtypes = [vp, C.POINTER(Info)]
@@ -239,6 +243,27 @@ class B200Ldlt:
 
     def solve_device(self, d_rhs_ptr, nrhs=1):
         return self._L.b200ldlt_solve_device(self._h, int(nrhs), C.c_void_p(d_rhs_ptr))
+
+    def solve_partial(self, job, rhs, nrhs=1):
+        """One part of the solve, in place on float64 rhs (dim*nrhs, column-major): job 0 = A^-1 b, 1 = L^-1 P^T S b,
+        2 = D^-1 b, 3 = S P L^-T b, 4 = S P L^-T D^-1 b (intermediate vectors in pivot order, see b200ldlt.h)."""
+        return self._L.b200ldlt_solve_partial(self._h, int(job), int(nrhs), _dptr(rhs))
+
+    def solve_partial_device(self, job, d_rhs_ptr, nrhs=1):
+        return self._L.b200ldlt_solve_partial_device(self._h, int(job), int(nrhs), C.c_void_p(d_rhs_ptr))
+
+    def enquire_indef(self):
+        """(pivot_var, pivot_type, dinv) per pivot position: the 0-based original variable, 1 / 2 / 3 (1x1 / first /
+        second of a 2x2 pivot), and an (n, 2) array of the diagonal and off-diagonal entry of D^-1 (scaled matrix)."""
+        n = self.dim
+        var, ty, d = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros((n, 2), np.float64)
+        if self._L.b200ldlt_enquire_indef(self._h, _iptr(var), _iptr(ty), _dptr(d)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return var, ty, d
+
+    def device_ptr(self, name):
+        """Device address of a named array of the handle (b200ldlt_device_ptr: "scale", "x", "cbv", ...), 0 if none."""
+        return self._L.b200ldlt_device_ptr(self._h, name.encode()) or 0
 
     def assemble_augsys_device(self, n_x, n_s, n_c, nnz_w, nnz_jc, nnz_jd, W=0, W_factor=1.0, D_x=0, delta_x=0.0, D_s=0,
                                delta_s=0.0, J_c=0, D_c=0, delta_c=0.0, J_d=0, D_d=0, delta_d=0.0):

@@ -195,6 +195,7 @@ struct Solver {
                                     // an analysis (width 0: the column loop)
   DevBuf<int> d_boff;
   DevBuf<long long> d_bigv_off;
+  DevBuf<long long> d_piv_big;      // n : per pivot position, its index in bigv (pivots of big fronts) or -1 (partial solves)
   DevBuf<unsigned long long> d_tlog, d_flog;
   DevBuf<double> d_linv;
   DevBuf<double> d_linv_part;       // partial tiles of the chunked k_linv_gemm items (one launch at a time uses it)
@@ -713,8 +714,10 @@ static int upload_schur_lists(Solver* sv, SchurLists& SL, cudaStream_t st) {
   return B200LDLT_SUCCESS;
 }
 
-// the persistent sweep kernel for one column (multi = false) or a block of columns
-static auto sweep_kernel(bool fwd, bool multi) {
+// the persistent sweep kernel for one column (multi = false) or a block of columns; apply_d = false: the forward sweep
+// of the partial solves (L only)
+static auto sweep_kernel(bool fwd, bool multi, bool apply_d = true) {
+  if (fwd && !apply_d) return multi ? k_solve<true, true, false> : k_solve<true, false, false>;
   return fwd ? (multi ? k_solve<true, true> : k_solve<true, false>) : (multi ? k_solve<false, true> : k_solve<false, false>);
 }
 
@@ -737,13 +740,17 @@ static cudaError_t alloc_sweep_state(Solver* sv, SweepState& W, const MultiStrid
   }
   if ((e = cudaMemsetAsync(W.d_ticket.p, 0, 2 * sizeof(unsigned long long), st)) != cudaSuccess) return e;
   W.ticket_f = W.ticket_b = 0;
-  int occ = 1, occ_b = 1;
+  int occ = 1, occ_b = 1, occ_l = 1;
   if ((e = cudaFuncSetAttribute(sweep_kernel(true, nb > 1), cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM)) != cudaSuccess ||
       (e = cudaFuncSetAttribute(sweep_kernel(false, nb > 1), cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM)) != cudaSuccess ||
+      (e = cudaFuncSetAttribute(sweep_kernel(true, nb > 1, false), cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM)) != cudaSuccess ||
       (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, sweep_kernel(true, nb > 1), DF_THREADS, DF_DYN_SMEM)) != cudaSuccess ||
-      (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, sweep_kernel(false, nb > 1), DF_THREADS, DF_DYN_SMEM)) != cudaSuccess)
+      (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, sweep_kernel(false, nb > 1), DF_THREADS, DF_DYN_SMEM)) != cudaSuccess ||
+      (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_l, sweep_kernel(true, nb > 1, false), DF_THREADS, DF_DYN_SMEM)) != cudaSuccess)
     return e;
-  W.grid = std::max(1, std::min(occ, occ_b)) * sv->num_sms;
+  // every CTA of a persistent sweep must be resident: the grid fits all three sweep kernels (the same in practice: the
+  // launch bounds cap each at 128 registers)
+  W.grid = std::max(1, std::min(std::min(occ, occ_b), occ_l)) * sv->num_sms;
   if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return e;
   W.width = nb;
   return cudaSuccess;
@@ -893,6 +900,13 @@ static int run_analysis(Solver* sv, const double* vals) {
     }
     CU(sv->d_boff.upload(boff, st));
     CU(sv->d_bigv_off.upload(bigv_off, st));
+    {
+      // partial solves: where a pivot position's value lives between the sweeps (k_piv_out / k_piv_in)
+      std::vector<long long> piv_big(n, -1);
+      for (int s = 0; s < S.nsn; ++s) if (S.f(s) > DF_MIDMAX)
+        for (int t = 0; t < S.k(s); ++t) piv_big[S.sn_start[s] + t] = bigv_off[s] + t;
+      CU(sv->d_piv_big.upload(piv_big, st));
+    }
     CU(cudaDeviceGetAttribute(&sv->num_sms, cudaDevAttrMultiProcessorCount, sv->dev));
     const MultiStride one{1, S.nsn, std::max(bo, 1), 0, n, (long long)std::max<size_t>(S.rows.size(), 1),
                           std::max<long long>(bv, 1), 0};
@@ -1265,8 +1279,9 @@ static DevSolve sweep_view(const Solver* sv, const SolvePlan& SP, const SweepSta
 }
 
 // one sweep of nb columns (nb <= W.width) over the fronts of a plan: the bottom levels one launch each, and ONE persistent
-// kernel (forward: bottom levels, then subtrees, then top tasks; backward: the reverse)
-static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, bool fwd) {
+// kernel (forward: bottom levels, then subtrees, then top tasks; backward: the reverse).  apply_d = false: a forward
+// sweep that leaves D^-1 out (partial solves)
+static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, bool fwd, bool apply_d = true) {
   cudaStream_t st = sv->stream;
   const DevSolve V = sweep_view(sv, SP, W);
   MultiStride M = W.M;
@@ -1275,9 +1290,10 @@ static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, 
   const long long nt = ((long long)(fwd ? SP.ntf : SP.ntb) + SP.npair) * nb;
   const int grid = (int)std::min<long long>(W.grid, nt);
   const int nd = (int)SP.direct_cnt.size();
-  const auto k_direct = fwd ? (multi ? k_solve_direct<true, true> : k_solve_direct<true, false>)
-                            : (multi ? k_solve_direct<false, true> : k_solve_direct<false, false>);
-  const auto k_sweep = sweep_kernel(fwd, multi);
+  const auto k_direct = (fwd && !apply_d) ? (multi ? k_solve_direct<true, true, false> : k_solve_direct<true, false, false>)
+                        : fwd ? (multi ? k_solve_direct<true, true> : k_solve_direct<true, false>)
+                              : (multi ? k_solve_direct<false, true> : k_solve_direct<false, false>);
+  const auto k_sweep = sweep_kernel(fwd, multi, apply_d);
   auto direct = [&](int l) {
     if (SP.direct_cnt[l] <= 0) return;
     const unsigned g = cdiv(SP.direct_cnt[l] * nb, DF_THREADS / 32);
@@ -1312,6 +1328,40 @@ static int enqueue_solve(Solver* sv, SweepState& W, const double* d_in, double* 
   return B200LDLT_SUCCESS;
 }
 
+// One part of the solve (job 1..4, include/b200ldlt.h) for nb columns of d_in -> d_out (leading dimension n, in place
+// when they are the same), nb <= W.width.  The parts are the pieces of enqueue_solve: job 1 is its first half with the
+// forward sweep leaving D^-1 out, copied out in pivot order; job 3 its second half, fed in pivot order; job 2 (and the
+// front of job 4) applies D^-1 through the helper the fused sweep uses.  So job 3 . 2 . 1 and job 4 . 1 reproduce
+// enqueue_solve bit for bit.  Launches: job 1, 3, 4: 2 + one sweep (the direct levels + 1); job 2: 1.
+static int enqueue_partial(Solver* sv, SweepState& W, int job, const double* d_in, double* d_out, int nb) {
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  const dim3 g(cdiv(n, 256), nb);
+  const long long ldx = W.M.x, ldb = W.M.bigv;
+  int rc = B200LDLT_SUCCESS;
+  if (job == 1) {
+    k_rhs_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_in, W.d_x.p, ldx); ++sv->launches;
+    sv->solve_epoch++;
+    rc = launch_sweep(sv, sv->splan, W, nb, true, false);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    k_piv_out<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb, d_out); ++sv->launches;
+  } else if (job == 2) {
+    // (through the sweep state's x: d_in and d_out may be the same array, and k_dinv reads partners from its input)
+    k_dinv<<<g, 256, 0, st>>>(n, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, d_in, nullptr, W.d_x.p, n, nullptr, 0); ++sv->launches;
+    CU(cudaMemcpyAsync(d_out, W.d_x.p, (size_t)n * nb * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  } else {
+    if (job == 3) k_piv_in<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, d_in, W.d_x.p, ldx, W.d_bigv.p, ldb);
+    else k_dinv<<<g, 256, 0, st>>>(n, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, d_in, sv->d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb);
+    ++sv->launches;
+    sv->solve_epoch++;
+    rc = launch_sweep(sv, sv->splan, W, nb, false);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, d_out); ++sv->launches;
+  }
+  CU(cudaGetLastError());
+  return rc;
+}
+
 // The sweep state of the blocked solve, B200_SOLVE_BLOCK columns wide: allocated once per analysis, at the first nrhs > 1
 // solve, before that solve's timing starts.  Returns false (and the columns are then solved one by one, as with
 // B200_SOLVE_BLOCK=1) when the device memory for it cannot be had.
@@ -1342,13 +1392,14 @@ static bool block_solve_state(Solver* sv) {
 
 // nrhs columns of d_rhs (leading dimension n), in place: blocks of up to B200_SOLVE_BLOCK columns through the blocked
 // state, single columns through the one-column state.  `blocked`: the result of block_solve_state, called by the entry
-// point before its timing starts.
-static int enqueue_solve_columns(Solver* sv, double* d_rhs, int nrhs, bool blocked) {
+// point before its timing starts.  job 0: the solve; 1..4: enqueue_partial.
+static int enqueue_solve_columns(Solver* sv, double* d_rhs, int nrhs, bool blocked, int job = 0) {
   const int cap = blocked ? sv->blk->width : 1;
   for (int c = 0; c < nrhs;) {
     const int w = std::min(cap, nrhs - c);
     double* col = d_rhs + (size_t)c * sv->n;
-    const int rc = enqueue_solve(sv, w == 1 ? sv->sweep : *sv->blk, col, col, w);
+    SweepState& W = w == 1 ? sv->sweep : *sv->blk;
+    const int rc = job == 0 ? enqueue_solve(sv, W, col, col, w) : enqueue_partial(sv, W, job, col, col, w);
     if (rc != B200LDLT_SUCCESS) return rc;
     c += w;
   }
@@ -1522,16 +1573,18 @@ int b200ldlt_refactor(b200ldlt_handle h, int check_inertia, int expected_neg, in
   return do_factor(sv, sv->d_vals.p, false, check_inertia, expected_neg, num_neg);
 }
 
-int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs) {
-  Solver* sv = (Solver*)h;
-  if (!sv || !sv->factored) { if (sv) sv->err = "solve before factor"; return B200LDLT_FATAL_ERROR; }
+}  // extern "C"
+
+namespace b200 {
+// the solve (job 0) or one part of it (job 1..4) on device-resident columns
+static int solve_device_job(Solver* sv, int job, int nrhs, double* d_rhs) {
   CU(cudaSetDevice(sv->dev));
   cudaStream_t st = sv->stream;
   const bool blocked = nrhs > 1 && block_solve_state(sv);
   sv->launches = 0;
   CU(cudaEventRecord(sv->ev0, st));
   {
-    int rc = enqueue_solve_columns(sv, d_rhs, nrhs, blocked);
+    int rc = enqueue_solve_columns(sv, d_rhs, nrhs, blocked, job);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   CU(cudaEventRecord(sv->ev1, st));
@@ -1541,9 +1594,8 @@ int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs) {
   return B200LDLT_SUCCESS;
 }
 
-int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs) {
-  Solver* sv = (Solver*)h;
-  if (!sv || !sv->factored) { if (sv) sv->err = "solve before factor"; return B200LDLT_FATAL_ERROR; }
+// the same on host columns: staged through pinned memory in chunks (see b200ldlt_solve)
+static int solve_host_job(Solver* sv, int job, int nrhs, double* rhs) {
   if (nrhs <= 0) return B200LDLT_SUCCESS;
   CU(cudaSetDevice(sv->dev));
   cudaStream_t st = sv->stream;
@@ -1568,7 +1620,7 @@ int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs) {
     CU(cudaMemcpyAsync(sv->d_rhs.p + o, sv->h_rhs + o, m * sizeof(double), cudaMemcpyHostToDevice, st));
   }
   {
-    int rc = enqueue_solve_columns(sv, sv->d_rhs.p, nrhs, blocked);
+    int rc = enqueue_solve_columns(sv, sv->d_rhs.p, nrhs, blocked, job);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   int nchunk = 0;
@@ -1587,6 +1639,71 @@ int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs) {
   CU(cudaStreamSynchronize(st));
   cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
   sv->info.launches_solve = sv->launches;
+  return B200LDLT_SUCCESS;
+}
+
+// job 1..4 are refused (FATAL_ERROR + last_error) out of range, without factors and on a sharded handle
+static bool partial_refused(Solver* sv, int job) {
+  if (job < 1 || job > 4) sv->err = "solve_partial: job must be 0..4";
+  else if (!sv->factored) sv->err = "solve_partial: no factors (factorise first; a SINGULAR factorisation leaves none)";
+  else if (sv->shard.active) sv->err = "solve_partial: not available on a sharded handle";
+  else return false;
+  return true;
+}
+}  // namespace b200
+
+extern "C" {
+
+int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs) {
+  Solver* sv = (Solver*)h;
+  if (!sv || !sv->factored) { if (sv) sv->err = "solve before factor"; return B200LDLT_FATAL_ERROR; }
+  return solve_device_job(sv, 0, nrhs, d_rhs);
+}
+
+int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs) {
+  Solver* sv = (Solver*)h;
+  if (!sv || !sv->factored) { if (sv) sv->err = "solve before factor"; return B200LDLT_FATAL_ERROR; }
+  return solve_host_job(sv, 0, nrhs, rhs);
+}
+
+int b200ldlt_solve_partial(b200ldlt_handle h, int job, int nrhs, double* rhs) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  if (job == 0) return b200ldlt_solve(h, nrhs, rhs);
+  if (partial_refused(sv, job)) return B200LDLT_FATAL_ERROR;
+  return solve_host_job(sv, job, nrhs, rhs);
+}
+
+int b200ldlt_solve_partial_device(b200ldlt_handle h, int job, int nrhs, double* d_rhs) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  if (job == 0) return b200ldlt_solve_device(h, nrhs, d_rhs);
+  if (partial_refused(sv, job)) return B200LDLT_FATAL_ERROR;
+  return solve_device_job(sv, job, nrhs, d_rhs);
+}
+
+int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, double* dinv2) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  if (!sv->factored) { sv->err = "enquire_indef: no factors (factorise first; a SINGULAR factorisation leaves none)"; return B200LDLT_FATAL_ERROR; }
+  CU(cudaSetDevice(sv->dev));
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  std::vector<int> lperm(n), ptype(n);
+  std::vector<double> dinv(n), doff(n);
+  CU(cudaMemcpyAsync(lperm.data(), sv->d_lperm.p, n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(ptype.data(), sv->d_ptype.p, n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(dinv.data(), sv->d_dinv.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(doff.data(), sv->d_doff.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const Symbolic& S = sv->S;
+  for (int s = 0; s < S.nsn; ++s)
+    for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) {
+      // pivot t of front s holds the front's local column lperm[p]: permuted column sn_start[s] + lperm[p]
+      if (pivot_var) pivot_var[p] = S.perm[S.sn_start[s] + lperm[p]];
+      if (pivot_type) pivot_type[p] = ptype[p];
+      if (dinv2) { dinv2[2 * (size_t)p] = dinv[p]; dinv2[2 * (size_t)p + 1] = ptype[p] == 2 ? doff[p] : 0.0; }
+    }
   return B200LDLT_SUCCESS;
 }
 
@@ -1675,6 +1792,7 @@ void* b200ldlt_device_ptr(b200ldlt_handle h, const char* name) {
   if (nm == "cbv") return sv->sweep.d_cbv.p;
   if (nm == "x") return sv->sweep.d_x.p;
   if (nm == "counters") return sv->d_counters.p;
+  if (nm == "scale") return sv->d_scale.p;
   return nullptr;
 }
 

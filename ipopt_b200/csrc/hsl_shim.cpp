@@ -11,6 +11,14 @@
 // change only.  How the adapter uses them: :473-608 (analyse: CSC lower triangle, 1-based when f_arrays != 0, values may
 // be NULL), :610-800 (factor with matrix_type 4 = real symmetric indefinite, then solve job 0; info.num_neg is the
 // inertia; info.flag 7 / -7 = singular), :802-860 (IncreaseQuality raises control.u and re-factors).
+//
+// Beyond what Ipopt resolves, the shim also serves the other MA97 callers of the same library:
+//   ma97_solve_d job 1..4  the partial solves (b200ldlt_solve_partial: L, D, L^T on their own, in pivot order);
+//   ma97_enquire_indef_d   the pivot order and D^-1 (b200ldlt_enquire_indef), declared at hsl_ma97d.h:158-160;
+//   scale[]                of ma97_factor_d / ma97_factor_solve_d: the equilibration factors of that factorisation.
+// Not provided: ma97_alter_d, ma97_enquire_posdef_d, ma97_solve_fredholm_d and the sparse-rhs / 64-bit variants.
+#include <cuda_runtime_api.h>
+
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -96,6 +104,12 @@ void fill_info(Keep* K, ma97_info_d* info) {
   info->ordering = 3;                     // nested dissection (METIS)
 }
 
+// scale[] of the factor calls: the n equilibration factors of the factorisation just done (device_ptr "scale")
+bool copy_scale(Keep* K, double* scale) {
+  const void* d = b200ldlt_device_ptr(K->h, "scale");
+  return d && cudaMemcpy(scale, d, (size_t)K->n * sizeof(double), cudaMemcpyDeviceToHost) == cudaSuccess;
+}
+
 }  // namespace
 
 extern "C" {
@@ -156,7 +170,7 @@ void ma97_analyse_d(int check, int n, const int ptr[], const int row[], double v
 
 void ma97_factor_d(int matrix_type, const int ptr[], const int row[], const double val[], void** akeep, void** fkeep,
                    const ma97_control_d* control, ma97_info_d* info, double scale[]) {
-  (void)ptr; (void)row; (void)scale;
+  (void)ptr; (void)row;
   memset(info, 0, sizeof(*info));
   Keep* K = akeep ? (Keep*)*akeep : nullptr;
   if (!K || !K->h || !val || (matrix_type != 4 && matrix_type != 3)) { info->flag = -1; return; }
@@ -171,24 +185,50 @@ void ma97_factor_d(int matrix_type, const int ptr[], const int row[], const doub
   if (st == B200LDLT_SINGULAR) { info->flag = (control && control->action) ? 7 : -7; K->factored = false; }
   else if (st != B200LDLT_SUCCESS) { info->flag = -1; K->factored = false; }
   else { info->flag = 0; K->factored = true; }
+  if (K->factored && scale && !copy_scale(K, scale)) info->flag = -1;
   if (fkeep) *fkeep = K;
 }
 
+// job 0: A x = b; 1: P L x = S b; 2: D x = b; 3: (P L)^T S^-1 x = b; 4: D (P L)^T S^-1 x = b, i.e. the jobs of
+// b200ldlt_solve_partial (include/b200ldlt.h) -- intermediate vectors in pivot order
 void ma97_solve_d(int job, int nrhs, double x[], int ldx, void** akeep, void** fkeep, const ma97_control_d* control,
                   ma97_info_d* info) {
   (void)control; (void)fkeep;
   memset(info, 0, sizeof(*info));
   Keep* K = akeep ? (Keep*)*akeep : nullptr;
-  if (!K || !K->h || !K->factored || job != 0 || nrhs < 0) { info->flag = -1; return; }
+  if (!K || !K->h || !K->factored || job < 0 || job > 4 || nrhs < 0) { info->flag = -1; return; }
   if (nrhs == 0) return;
   int st;
-  if (ldx == K->n) st = b200ldlt_solve(K->h, nrhs, x);
+  if (ldx == K->n) st = b200ldlt_solve_partial(K->h, job, nrhs, x);
   else {
     st = B200LDLT_SUCCESS;
-    for (int c = 0; c < nrhs && st == B200LDLT_SUCCESS; ++c) st = b200ldlt_solve(K->h, 1, x + (size_t)c * ldx);
+    for (int c = 0; c < nrhs && st == B200LDLT_SUCCESS; ++c) st = b200ldlt_solve_partial(K->h, job, 1, x + (size_t)c * ldx);
   }
   fill_info(K, info);
   info->flag = (st == B200LDLT_SUCCESS) ? 0 : -1;
+}
+
+// piv_order[i] (variable i, 0-based index; values 1-based): the position of variable i in the pivot order, negative for
+// both variables of a 2x2 pivot.  d[2p] / d[2p+1]: diagonal / off-diagonal (p, p+1) entry of D^-1 at pivot position p,
+// the off-diagonal 0 unless p opens a 2x2 pivot.  Either output may be NULL.  This is our reading of MA97's documented
+// convention; the HSL user documentation was not available to check it against, so callers that depend on the exact
+// signs or on D^-1 versus D should verify it with their HSL version.
+void ma97_enquire_indef_d(void** akeep, void** fkeep, const ma97_control_d* control, ma97_info_d* info, int piv_order[],
+                          double d[]) {
+  (void)fkeep; (void)control;
+  memset(info, 0, sizeof(*info));
+  Keep* K = akeep ? (Keep*)*akeep : nullptr;
+  if (!K || !K->h || !K->factored) { info->flag = -1; return; }
+  std::vector<int> var, ty;
+  if (piv_order) { var.resize(K->n); ty.resize(K->n); }
+  if (b200ldlt_enquire_indef(K->h, piv_order ? var.data() : nullptr, piv_order ? ty.data() : nullptr, d) != B200LDLT_SUCCESS) {
+    info->flag = -1;
+    return;
+  }
+  if (piv_order)
+    for (int p = 0; p < K->n; ++p) piv_order[var[p]] = ty[p] == 1 ? p + 1 : -(p + 1);
+  fill_info(K, info);
+  info->flag = 0;
 }
 
 void ma97_factor_solve_d(int matrix_type, const int ptr[], const int row[], const double val[], int nrhs, double x[], int ldx,

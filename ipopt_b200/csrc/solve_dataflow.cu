@@ -20,6 +20,8 @@
 //                      are combined by the last-arriving CTA in chunk order (fence + counter): bit-reproducible.
 // Forward: direct levels, then subtrees before top tasks; backward: top tasks before subtrees, then the direct levels.
 // A block of right-hand sides takes the same launches through the MULTI instantiations of both kernels (see MultiStride).
+// The partial solves (L, D, L^T on their own) use the forward sweep with APPLY_D = false, the backward sweep as is, and
+// the pivot-order copies / D^-1 pass of solve_kernels.cu.
 // L is streamed exactly once per sweep (HBM-bound, SURVEY.md 8d: 2*8*nnz(L) bytes per right-hand side); children ->
 // parent data flows through per-front update vectors gathered by the parent (no atomics on the data path).
 // Replaces the vendor back-solve of the reference (MUMPS job=3,
@@ -209,7 +211,8 @@ __device__ __forceinline__ void w64_fstep8(int k, int tb, const double (&l0)[8],
   }
 }
 
-template <bool SUB>
+// D^-1 of the pivot rows: dinv_entry (solve_kernels.cu).  APPLY_D = false (partial solve, L only): the pivot rows keep v = the L-solve value instead of D^-1 v
+template <bool SUB, bool APPLY_D = true>
 __device__ void w64_fwd(const FrontIO& io, const DevSolve& V, int s, int epoch, double* w) {
   const int lane = threadIdx.x & 31;
   const FrontDesc fd = load_fd(io.fd + (s - io.s0));
@@ -284,11 +287,13 @@ __device__ void w64_fwd(const FrontIO& io, const DevSolve& V, int s, int epoch, 
     const int i = lane + 32 * h;
     const double v = h ? v1 : v0;
     if (i < k) {
-      const int ty = io.ptype[cl + i];
-      double y;
-      if (ty == 1) y = v * io.dinv[cl + i];
-      else if (ty == 2) y = v * io.dinv[cl + i] + w[i + 1] * io.doff[cl + i];
-      else y = w[i - 1] * io.doff[cl + i - 1] + v * io.dinv[cl + i];
+      double y = v;
+      if (APPLY_D) {
+        const int ty = io.ptype[cl + i];
+        if (ty == 1) y = dinv_entry(1, v, 0.0, io.dinv[cl + i], 0.0);
+        else if (ty == 2) y = dinv_entry(2, v, w[i + 1], io.dinv[cl + i], io.doff[cl + i]);
+        else y = dinv_entry(3, v, w[i - 1], io.dinv[cl + i], io.doff[cl + i - 1]);
+      }
       io.xs[cl + i] = y;
     } else if (i < f) io.uv[rol + i - k] = v;
   }
@@ -430,7 +435,7 @@ __device__ void w64_bwd(const FrontIO& io, const DevSolve& V, int s, int epoch, 
 // ------------------------------------------------------------------------------------------------
 // mid fronts (65 .. 256): one CTA, blocked by 32; scratch: v[f] | w[f]
 // ------------------------------------------------------------------------------------------------
-template <bool SUB>
+template <bool SUB, bool APPLY_D = true>
 __device__ void mid_fwd(const FrontIO& io, const DevSolve& V, int s, int epoch, double* scr, const double* Lp_override,
                         unsigned long long* mbar, unsigned mphase, const Team tm) {
   const FrontDesc fd = load_fd(io.fd + (s - io.s0));
@@ -494,11 +499,13 @@ __device__ void mid_fwd(const FrontIO& io, const DevSolve& V, int s, int epoch, 
     team_sync(tm);
   }
   for (int t = tid; t < k; t += nt) {
-    const int ty = io.ptype[cl + t];
-    double y;
-    if (ty == 1) y = v[t] * io.dinv[cl + t];
-    else if (ty == 2) y = v[t] * io.dinv[cl + t] + v[t + 1] * io.doff[cl + t];
-    else y = v[t - 1] * io.doff[cl + t - 1] + v[t] * io.dinv[cl + t];
+    double y = v[t];
+    if (APPLY_D) {
+      const int ty = io.ptype[cl + t];
+      if (ty == 1) y = dinv_entry(1, v[t], 0.0, io.dinv[cl + t], 0.0);
+      else if (ty == 2) y = dinv_entry(2, v[t], v[t + 1], io.dinv[cl + t], io.doff[cl + t]);
+      else y = dinv_entry(3, v[t], v[t - 1], io.dinv[cl + t], io.doff[cl + t - 1]);
+    }
     io.xs[cl + t] = y;
   }
   double* __restrict__ out = io.uv + rol;
@@ -638,7 +645,8 @@ __device__ __forceinline__ void reduce_cols(double (&pacc)[16], double* red, dou
   __syncthreads();
 }
 
-// FP: pivot rows [64 blk, +64) of front s, tiles [t0, t1) of Linv's block row
+// FP: pivot rows [64 blk, +64) of front s, tiles [t0, t1) of Linv's block row.  APPLY_D = false: bigv gets y, not D^-1 y.
+template <bool APPLY_D>
 __device__ void big_fp(const DevSym& S, const DevNum& N, const DevSolve& V, const SolveTask& T, int epoch, double* sm,
                        int* s_flag, const double* __restrict__ x, const double* __restrict__ cbv) {
   const int s = T.s, rb = T.blk;
@@ -717,10 +725,12 @@ __device__ void big_fp(const DevSym& S, const DevNum& N, const DevSolve& V, cons
     const int i = r0 + tid;
     const long long o = V.bigv_off[s];
     V.bigy[o + i] = ys[tid];              // y block for the contribution rows (pivoted order)
-    double z;                              // 2x2 partners never straddle a 32-column panel, so they sit in this block
-    if (ty2 == 1) z = ys[tid] * dv;
-    else if (ty2 == 2) z = ys[tid] * dv + ys[tid + 1] * dof;
-    else z = ys[tid - 1] * dofm + ys[tid] * dv;
+    double z = ys[tid];                    // 2x2 partners never straddle a 32-column panel, so they sit in this block
+    if (APPLY_D) {
+      if (ty2 == 1) z = dinv_entry(1, ys[tid], 0.0, dv, 0.0);
+      else if (ty2 == 2) z = dinv_entry(2, ys[tid], ys[tid + 1], dv, dof);
+      else z = dinv_entry(3, ys[tid], ys[tid - 1], dv, dofm);
+    }
     V.bigv[o + i] = z;
   }
   __syncthreads();
@@ -1089,7 +1099,7 @@ struct SubLayout {
 };
 
 // one subtree, by the whole CTA (see the file header).  `mbar` / `mphase`: the CTA's transaction barrier and its phase.
-template <bool FWD>
+template <bool FWD, bool APPLY_D>
 __device__ void solve_subtree(const DevSym& S, const DevNum& N, const DevSolve& V, int u, int epoch, unsigned char* smraw,
                               unsigned long long* mbar, unsigned mphase, double* __restrict__ x, double* __restrict__ cbv,
                               const Team tm) {
@@ -1181,12 +1191,12 @@ __device__ void solve_subtree(const DevSym& S, const DevNum& N, const DevSolve& 
     const int b = lvl[e], en = lvl[e + 1], ns = nsm[e];
     for (int q = b + warp; q < b + ns; q += NT / 32) {
       const int s = fl[q];
-      if (FWD) w64_fwd<true>(io, V, s, epoch, wscr + warp * DF_WSCR);
+      if (FWD) w64_fwd<true, APPLY_D>(io, V, s, epoch, wscr + warp * DF_WSCR);
       else w64_bwd<true>(io, V, s, epoch, -1, V.upper_max);
     }
     for (int q = b + ns; q < en; ++q) {   // (mid fronts use their own scratch: no barrier needed before them)
       const int s = fl[q];
-      if (FWD) mid_fwd<true>(io, V, s, epoch, midscr, nullptr, nullptr, 0, tm);
+      if (FWD) mid_fwd<true, APPLY_D>(io, V, s, epoch, midscr, nullptr, nullptr, 0, tm);
       else mid_bwd<true>(io, V, s, epoch, -1, midscr, nullptr, nullptr, 0, V.upper_max, tm);
     }
     team_sync(tm);
@@ -1260,9 +1270,10 @@ __device__ __forceinline__ void global_io(FrontIO& io, const DevSym& S, const De
 // ONE persistent kernel per sweep.  Work items are taken with an atomic ticket: forward = subtrees (largest first), then
 // the top tasks by level; backward = top tasks (levels descending), then the subtrees.  MULTI: (item, column) tickets over
 // M.nb columns.  Otherwise the ticket is the item and the column a compile-time 0 (no per-ticket division, the column view
-// is the identity), and the top tasks are recorded in V.tlog when it is set.
+// is the identity), and the top tasks are recorded in V.tlog when it is set.  APPLY_D = false (forward only): the L
+// solve alone -- the pivot rows keep the values the fused sweep has before D^-1, in x (bigv for the big fronts).
 // ------------------------------------------------------------------------------------------------
-template <bool FWD, bool MULTI>
+template <bool FWD, bool MULTI, bool APPLY_D = true>
 __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, DevSolve V, MultiStride M, int epoch,
                                                          unsigned long long ticket_base,
                                                          double* __restrict__ x, double* __restrict__ cbv) {
@@ -1301,7 +1312,7 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
       // part of the shared memory, threads 128..255 walk u1 above it (own transaction barrier, own hardware barrier).
       const bool second = pr.y >= 0 && threadIdx.x >= DF_THREADS / 2;
       const Team tm = pr.y < 0 ? cta : Team{(int)threadIdx.x - (second ? DF_THREADS / 2 : 0), DF_THREADS / 2, second ? 2 : 1};
-      solve_subtree<FWD>(S, N, Vc, second ? pr.y : pr.x, epoch, second ? smraw + V.subs[pr.x].sbytes : smraw,
+      solve_subtree<FWD, APPLY_D>(S, N, Vc, second ? pr.y : pr.x, epoch, second ? smraw + V.subs[pr.x].sbytes : smraw,
                          second ? &s_mbar1 : &s_mbar, second ? mphase1 : mphase, xc, cbvc, tm);
       mphase ^= 1;
       if (pr.y >= 0) mphase1 ^= 1;
@@ -1318,7 +1329,7 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
       const int w = threadIdx.x >> 5;
       if (w < T.blk) {
         const int s = V.bundle[T.s + w];
-        if (FWD) w64_fwd<false>(io, Vc, s, epoch, sm + w * DF_WSCR);
+        if (FWD) w64_fwd<false, APPLY_D>(io, Vc, s, epoch, sm + w * DF_WSCR);
         else w64_bwd<false>(io, Vc, s, epoch, S.sn_parent[s], V.upper_max);
       }
     } else if (T.type == ST_MID) {
@@ -1338,10 +1349,10 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
         Lp = stage; mb = &s_mbar; ph = mphase;
         mphase ^= 1;
       }
-      if (FWD) mid_fwd<false>(io, Vc, T.s, epoch, midscr, Lp, mb, ph, cta);
+      if (FWD) mid_fwd<false, APPLY_D>(io, Vc, T.s, epoch, midscr, Lp, mb, ph, cta);
       else mid_bwd<false>(io, Vc, T.s, epoch, S.sn_parent[T.s], midscr, Lp, mb, ph, V.upper_max, cta);
     } else if (T.type == ST_FP) {
-      big_fp(S, N, Vc, T, epoch, sm, &s_flag, xc, cbvc);
+      big_fp<APPLY_D>(S, N, Vc, T, epoch, sm, &s_flag, xc, cbvc);
     } else if (T.type == ST_FC) {
       big_fc(S, N, Vc, T, epoch, sm, &s_flag, xc, cbvc);
     } else if (T.type == ST_BT) {
@@ -1366,9 +1377,9 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
 // warp slot of the GPU busy -- instead of walking them inside the shared-memory subtrees, where they are serialised behind
 // each other on a handful of warps.  Forward: these launches precede k_solve<fwd>; backward: they follow k_solve<bwd>.
 // Their parents find the update vectors in global memory (FrontDesc::direct).  MULTI: one warp per (front, column), the
-// M.nb warps of a front side by side (the panel comes from L1 / L2 after the first).
+// M.nb warps of a front side by side (the panel comes from L1 / L2 after the first).  APPLY_D: as in k_solve.
 // ------------------------------------------------------------------------------------------------
-template <bool FWD, bool MULTI>
+template <bool FWD, bool MULTI, bool APPLY_D = true>
 __global__ void __launch_bounds__(DF_THREADS, 2) k_solve_direct(DevSym S, DevNum N, DevSolve V, MultiStride M,
                                                                 const int* __restrict__ list, int cnt, int epoch,
                                                                 double* __restrict__ x, double* __restrict__ cbv) {
@@ -1382,7 +1393,7 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve_direct(DevSym S, DevNum
   FrontIO io;
   global_io(io, S, N, Vc, x + c * M.x, cbv + c * M.cbv);
   const int s = list[MULTI ? g / nb : g];
-  if (FWD) w64_fwd<false>(io, Vc, s, epoch, wscr + w * DF_WSCR);
+  if (FWD) w64_fwd<false, APPLY_D>(io, Vc, s, epoch, wscr + w * DF_WSCR);
   else w64_bwd<false>(io, Vc, s, epoch, -1, Vc.upper_max);
 }
 

@@ -1,5 +1,5 @@
 // Around the triangular solve (solve_dataflow.cu), sm_90a: permutation + scaling of the right-hand sides in and of the
-// solutions out, and the residual helpers.
+// solutions out, the pivot-order copies and the D^-1 pass of the partial solves, and the residual helpers.
 #include <cuda_runtime.h>
 #include <math.h>
 
@@ -20,6 +20,57 @@ __global__ void k_sol_out(int n, const int* __restrict__ perm, const double* __r
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const long long c = blockIdx.y;
   if (i < n) { const int o = perm[i]; x[c * n + o] = scale[o] * xp[c * ldx + i]; }
+}
+
+// Entry p of y = D^-1 v, pivot order.  ty = ptype[p], d = dinv[p]; for a 2x2 pivot vq = v at the partner and o = the
+// pair's off-diagonal (doff at its first pivot).  Each row of a pair is "first entry x its coefficient" fused onto the
+// rounded product of the second entry: exactly what the fused forward sweeps compiled to before this helper existed
+// (sm_90a SASS: DMUL, then DFMA).  The intrinsics pin that rounding, so the fused sweeps (solve_dataflow.cu) and
+// k_dinv produce the same bits whatever the compiler would contract.
+__device__ __forceinline__ double dinv_entry(int ty, double v, double vq, double d, double o) {
+  if (ty == 1) return __dmul_rn(v, d);
+  if (ty == 2) return __fma_rn(v, d, __dmul_rn(vq, o));   // first of the pair:  d v + o vq
+  return __fma_rn(vq, o, __dmul_rn(v, d));                // second of the pair: o vq + d v
+}
+
+// Partial solves: vectors in pivot order (position p = sn_start[s] + t for pivot t of front s).  Between the sweeps the
+// value of position p lives in xp[p], or in big[piv_big[p]] when p is a pivot of a big front (piv_big[p] >= 0: those
+// keep their forward result in bigv, see solve_dataflow.cu).  Column blockIdx.y; b / out: leading dimension n.
+// out = sweep values (after a forward sweep without D)
+__global__ void k_piv_out(int n, const long long* __restrict__ piv_big, const double* __restrict__ xp, long long ldx,
+                          const double* __restrict__ big, long long ldbig, double* __restrict__ out) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long c = blockIdx.y;
+  if (p < n) { const long long q = piv_big[p]; out[c * n + p] = q >= 0 ? big[c * ldbig + q] : xp[c * ldx + p]; }
+}
+// sweep values = b (before a backward sweep)
+__global__ void k_piv_in(int n, const long long* __restrict__ piv_big, const double* __restrict__ b,
+                         double* __restrict__ xp, long long ldx, double* __restrict__ big, long long ldbig) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long c = blockIdx.y;
+  if (p < n) {
+    const long long q = piv_big[p];
+    const double v = b[c * n + p];
+    if (q >= 0) big[c * ldbig + q] = v; else xp[c * ldx + p] = v;
+  }
+}
+// out = D^-1 b, pivot order, the partner of a 2x2 pivot read from b (b and out must not overlap).  piv_big == nullptr:
+// out[p] (leading dimension n); else the sweep values, as k_piv_in writes them (out = xp, leading dimension ldx).
+__global__ void k_dinv(int n, const int* __restrict__ ptype, const double* __restrict__ dinv,
+                       const double* __restrict__ doff, const double* __restrict__ b, const long long* __restrict__ piv_big,
+                       double* __restrict__ out, long long ldx, double* __restrict__ big, long long ldbig) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long c = blockIdx.y;
+  if (p >= n) return;
+  const double* bc = b + c * n;
+  const int ty = ptype[p];
+  double y;
+  if (ty == 1) y = dinv_entry(1, bc[p], 0.0, dinv[p], 0.0);
+  else if (ty == 2) y = dinv_entry(2, bc[p], bc[p + 1], dinv[p], doff[p]);
+  else y = dinv_entry(3, bc[p], bc[p - 1], dinv[p], doff[p - 1]);
+  if (!piv_big) { out[c * n + p] = y; return; }
+  const long long q = piv_big[p];
+  if (q >= 0) big[c * ldbig + q] = y; else out[c * ldx + p] = y;
 }
 
 // r = b - A x from the original triplets (tests / bench parity helper)
