@@ -123,6 +123,29 @@ int b200ldlt_solve_partial_device(b200ldlt_handle h, int job, int nrhs, double* 
  * (p, p+1) of D^-1 when p opens a 2x2 pivot, else 0.  D^-1 is that of the scaled matrix S A S. */
 int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, double* dinv2);
 
+/* ---- multiplication by the factors and alteration of D (cf. HSL_MA97 ma97_lmultiply / ma97_alter) --------------------
+ * Same conventions as the partial solves (S A S = P L D L^T P^T, vectors in pivot order indexed by pivot position p):
+ *   trans = 0 :  y = S^-1 P L x        x in pivot order, y in original order   (the inverse of job 1)
+ *   trans = 1 :  y = L^T P^T S^-1 x    x in original order, y in pivot order   (the inverse of job 3)
+ * x and y are n x nrhs column-major; they may be the same array (in place), otherwise they must not overlap.  L is read
+ * as the factorisation left it, so  lmultiply(0, D lmultiply(1, v))  =  A v  up to rounding (with
+ * info.num_forced > 0: the perturbed matrix).  Results are bit-reproducible; nrhs > 1 runs in blocks of up to 8 columns
+ * (B200_SOLVE_BLOCK, as for the solves), L streamed once per block, every column bit-identical to a call on that column
+ * alone.  Kernel launches: 2 per block (trans 0: multiply + gather; trans 1: copy-in + multiply), in info.launches_solve;
+ * info.ms_solve_gpu is the call's device time (host entry point: with its copies).  The first call after an analysis
+ * builds the work lists and slot map (about 8 bytes per panel row and column chunk: 9 MB per column at MBndryCntrl1
+ * N=400) before its timing starts; a handle that never multiplies allocates none of it.
+ * FATAL_ERROR (message in last_error) for trans other than 0 / 1, without factors (also after SINGULAR) and on a sharded
+ * handle. */
+int b200ldlt_lmultiply(b200ldlt_handle h, int trans, int nrhs, const double* x, double* y);
+int b200ldlt_lmultiply_device(b200ldlt_handle h, int trans, int nrhs, const double* d_x, double* d_y);
+/* Replace D^-1 by the caller's, 2n doubles in the layout of enquire_indef (dinv2[2p] diagonal, dinv2[2p+1] off-diagonal
+ * (p, p+1), host memory); the pivot types stay.  Refused with FATAL_ERROR -- and D left exactly as it was -- when an
+ * entry is not finite or an off-diagonal entry is non-zero at a p that does not open a 2x2 pivot (also in the cases
+ * lmultiply refuses).  Every later solve, partial solve and enquire_indef use the new D until the next factor or refactor
+ * call, which computes D afresh.  num_neg and b200ldlt_info keep describing the factorisation, not the altered D. */
+int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2);
+
 /* <-> NumberOfNegEVals() (hpp:207) */
 int b200ldlt_num_neg(b200ldlt_handle h);
 /* <-> IncreaseQuality() (hpp:220): pivtol <- min(pivtolmax, pivtol^0.75); returns 0 if already at max.

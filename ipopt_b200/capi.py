@@ -56,7 +56,8 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_refactor", "b200ldlt_get_info", "b200ldlt_symbolic_array", "b200ldlt_analyse_now",
             "b200ldlt_residual", "b200ldlt_set_pivtol",
             "b200ldlt_assemble_augsys_device", "b200ldlt_solve_refine_device",
-            "b200ldlt_solve_partial", "b200ldlt_solve_partial_device", "b200ldlt_enquire_indef"]
+            "b200ldlt_solve_partial", "b200ldlt_solve_partial_device", "b200ldlt_enquire_indef",
+            "b200ldlt_lmultiply", "b200ldlt_lmultiply_device", "b200ldlt_alter_d"]
 
 _lib = None
 
@@ -94,6 +95,9 @@ def load_library():
     L.b200ldlt_solve_partial.argtypes = [vp, C.c_int, C.c_int, dp]
     L.b200ldlt_solve_partial_device.argtypes = [vp, C.c_int, C.c_int, vp]
     L.b200ldlt_enquire_indef.argtypes = [vp, ip, ip, dp]
+    L.b200ldlt_lmultiply.argtypes = [vp, C.c_int, C.c_int, dp, dp]
+    L.b200ldlt_lmultiply_device.argtypes = [vp, C.c_int, C.c_int, vp, vp]
+    L.b200ldlt_alter_d.argtypes = [vp, dp]
     L.b200ldlt_num_neg.argtypes = [vp]
     L.b200ldlt_increase_quality.argtypes = [vp]
     L.b200ldlt_get_info.argtypes = [vp, C.POINTER(Info)]
@@ -260,6 +264,26 @@ class B200Ldlt:
         if self._L.b200ldlt_enquire_indef(self._h, _iptr(var), _iptr(ty), _dptr(d)) != SYMSOLVER_SUCCESS:
             raise RuntimeError(self.last_error())
         return var, ty, d
+
+    def lmultiply(self, trans, x, nrhs=1):
+        """Multiply by the factors: trans 0: S^-1 P L x (pivot -> original order), trans 1: L^T P^T S^-1 x (original ->
+        pivot order), x float64 dim*nrhs column-major.  Returns y (a new array); raises on a refusal."""
+        x = np.ascontiguousarray(x, dtype=np.float64).ravel()
+        y = np.empty_like(x)
+        if self._L.b200ldlt_lmultiply(self._h, int(trans), int(nrhs), _dptr(x), _dptr(y)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return y
+
+    def lmultiply_device(self, trans, d_x_ptr, d_y_ptr, nrhs=1):
+        """The same on device addresses (d_y may be d_x); returns the status."""
+        return self._L.b200ldlt_lmultiply_device(self._h, int(trans), int(nrhs), C.c_void_p(d_x_ptr), C.c_void_p(d_y_ptr))
+
+    def alter_d(self, dinv):
+        """Replace D^-1 by an (n, 2) array in the layout enquire_indef returns; returns the status (FATAL_ERROR and D
+        unchanged for a non-finite entry or an off-diagonal entry where no 2x2 pivot opens)."""
+        d = np.ascontiguousarray(dinv, dtype=np.float64)
+        assert d.size == 2 * self.dim
+        return self._L.b200ldlt_alter_d(self._h, _dptr(d))
 
     def device_ptr(self, name):
         """Device address of a named array of the handle (b200ldlt_device_ptr: "scale", "x", "cbv", ...), 0 if none."""

@@ -17,6 +17,7 @@
 #include "factor_kernels.cu"
 #include "solve_kernels.cu"
 #include "solve_dataflow.cu"
+#include "lmul_kernels.cu"
 #include "schur_tc.cu"
 #include "symbolic.hpp"
 
@@ -81,6 +82,18 @@ struct SweepState {
   unsigned long long ticket_f = 0, ticket_b = 0;   // their values when the next sweep starts
   MultiStride M;
   int grid = 0;                          // CTAs of the persistent sweep kernel
+};
+
+// multiplication by the factors (lmul_kernels.cu): the work lists and the slot map of k_lmul_n / k_lmul_gather, built at
+// the first lmultiply call after an analysis (a handle that never multiplies allocates nothing), and a scratch of `width`
+// columns of `ld` doubles (the slots for trans = 0, w for trans = 1)
+struct LmulPlan {
+  DevBuf<LmulItem> d_items_n;
+  DevBuf<int2> d_items_t;
+  DevBuf<int> d_pcol0, d_own_ptr, d_own, d_desc_ptr, d_desc;
+  DevBuf<double> d_scr;
+  long long ld = 0;
+  int width = 0;
 };
 
 struct LevelPlan {
@@ -196,6 +209,9 @@ struct Solver {
   DevBuf<int> d_boff;
   DevBuf<long long> d_bigv_off;
   DevBuf<long long> d_piv_big;      // n : per pivot position, its index in bigv (pivots of big fronts) or -1 (partial solves)
+  std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call after an analysis
+  DevBuf<double> d_alter;           // alter_d: the caller's 2n entries of D^-1 (allocated at the first call)
+  DevBuf<int> d_alter_bad;
   DevBuf<unsigned long long> d_tlog, d_flog;
   DevBuf<double> d_linv;
   DevBuf<double> d_linv_part;       // partial tiles of the chunked k_linv_gemm items (one launch at a time uses it)
@@ -763,6 +779,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   if (sv->h_rhs) { cudaFreeHost(sv->h_rhs); sv->h_rhs = nullptr; }
   sv->rhs_cap = 0;
   sv->blk.reset();
+  sv->lmul.reset();
   if (sv->fgraph_exec) { cudaGraphExecDestroy(sv->fgraph_exec); sv->fgraph_exec = nullptr; }
   if (sv->fgraph) { cudaGraphDestroy(sv->fgraph); sv->fgraph = nullptr; }
   AnalyseOptions ao;
@@ -1406,6 +1423,114 @@ static int enqueue_solve_columns(Solver* sv, double* d_rhs, int nrhs, bool block
   return B200LDLT_SUCCESS;
 }
 
+// The work lists and the slot map of the multiply (lmul_kernels.cu).  The pivot columns of a front are cut into chunks
+// of LM_CH; chunk [t0, ..) of front s owns f - t0 slots, one per panel row from t0 on.  Pivot position p (panel row
+// i = p - c0 of its front) sums its own front's chunks with t0 <= i (own, by p) and, as permuted column q, the
+// contribution rows equal to q of its descendants (desc, by q: fronts ascending, then chunks).  All of it depends on the
+// analysis only.
+static int build_lmul_plan(Solver* sv, LmulPlan& M) {
+  const Symbolic& S = sv->S;
+  const int n = sv->n;
+  cudaStream_t st = sv->stream;
+  std::vector<LmulItem> itn;
+  std::vector<int2> itt;
+  std::vector<int> pcol0(n), own_ptr(n + 1, 0), desc_ptr(n + 1, 0);
+  std::vector<long long> cbase;
+  long long ns = 0;
+  for (int s = 0; s < S.nsn; ++s) {
+    const int c0 = S.sn_start[s], k = S.sn_start[s + 1] - c0, r = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]), f = k + r;
+    for (int i = 0; i < k; ++i) { pcol0[c0 + i] = c0; own_ptr[c0 + i + 1] = i / LM_CH + 1; }
+    for (int t0 = 0; t0 < k; t0 += LM_CH) {
+      cbase.push_back(ns);
+      for (int g = 0; 32 * g < f - t0; ++g) itn.push_back(LmulItem{s, t0, g, 0, ns});
+      for (int j = 0; j < r; ++j) desc_ptr[S.rows[S.rows_ptr[s] + j] + 1]++;
+      ns += f - t0;
+    }
+    for (int t0 = 0; t0 < k; t0 += LM_CW) itt.push_back(make_int2(s, t0));
+  }
+  if (ns >= (1ll << 31)) { sv->err = "lmultiply: the factors are too large for the slot map"; return B200LDLT_FATAL_ERROR; }
+  for (int p = 0; p < n; ++p) { own_ptr[p + 1] += own_ptr[p]; desc_ptr[p + 1] += desc_ptr[p]; }
+  std::vector<int> own(own_ptr[n]), desc(std::max(desc_ptr[n], 1)), fill(desc_ptr.begin(), desc_ptr.end() - 1);
+  size_t ci = 0;
+  for (int s = 0; s < S.nsn; ++s) {
+    const int c0 = S.sn_start[s], k = S.sn_start[s + 1] - c0, r = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
+    for (int t0 = 0; t0 < k; t0 += LM_CH, ++ci) {
+      const long long b = cbase[ci];
+      for (int i = t0; i < k; ++i) own[own_ptr[c0 + i] + t0 / LM_CH] = (int)(b + i - t0);
+      for (int j = 0; j < r; ++j) desc[fill[S.rows[S.rows_ptr[s] + j]]++] = (int)(b + k + j - t0);
+    }
+  }
+  CU(M.d_items_n.upload(itn, st));
+  CU(M.d_items_t.upload(itt, st));
+  CU(M.d_pcol0.upload(pcol0, st));
+  CU(M.d_own_ptr.upload(own_ptr, st));
+  CU(M.d_own.upload(own, st));
+  CU(M.d_desc_ptr.upload(desc_ptr, st));
+  CU(M.d_desc.upload(desc, st));
+  M.ld = std::max<long long>(ns, n);
+  if (sv->opt.verbose)
+    fprintf(stderr, "[b200ldlt] lmultiply map: %zu + %zu warp items, %lld slots (%.1f MB per column)\n", itn.size(),
+            itt.size(), ns, 8e-6 * (double)M.ld);
+  return B200LDLT_SUCCESS;
+}
+
+// the multiply's state for calls of nrhs columns (before the call's timing starts): the map at the first call after an
+// analysis, the scratch for the widest block the call uses
+static int lmul_state(Solver* sv, int nrhs) {
+  if (!sv->lmul) {
+    std::unique_ptr<LmulPlan> M(new LmulPlan());
+    const int rc = build_lmul_plan(sv, *M);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    sv->lmul = std::move(M);
+  }
+  LmulPlan& M = *sv->lmul;
+  const int w = std::min(nrhs, sv->dbg.solve_block);
+  if (w > M.width) {
+    M.width = 0;
+    CU(M.d_scr.alloc((size_t)M.ld * w));
+    M.width = w;
+  }
+  return B200LDLT_SUCCESS;
+}
+
+// nb <= MS_NB_MAX columns (leading dimension n) of d_x -> d_y: two launches
+static int enqueue_lmul(Solver* sv, int trans, const double* d_x, double* d_y, int nb) {
+  using KN = void (*)(const FrontDesc*, const double*, const LmulItem*, int, const double*, int, double*, long long);
+  using KT = void (*)(const FrontDesc*, const double*, const int2*, int, const int*, const int*, const double*, int, double*);
+  static_assert(MS_NB_MAX == 8, "one instantiation per block width");
+  static const KN kn[8] = {k_lmul_n<1>, k_lmul_n<2>, k_lmul_n<3>, k_lmul_n<4>, k_lmul_n<5>, k_lmul_n<6>, k_lmul_n<7>, k_lmul_n<8>};
+  static const KT kt[8] = {k_lmul_t<1>, k_lmul_t<2>, k_lmul_t<3>, k_lmul_t<4>, k_lmul_t<5>, k_lmul_t<6>, k_lmul_t<7>, k_lmul_t<8>};
+  const LmulPlan& M = *sv->lmul;
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  const dim3 g(cdiv(n, 256), nb);
+  if (trans == 0) {
+    const int ni = (int)M.d_items_n.n;
+    kn[nb - 1]<<<cdiv(ni, 8), 256, 0, st>>>(sv->d_fdesc.p, sv->d_L.p, M.d_items_n.p, ni, d_x, n, M.d_scr.p, M.ld);
+    k_lmul_gather<<<g, 256, 0, st>>>(n, M.d_pcol0.p, sv->d_lperm.p, M.d_own_ptr.p, M.d_own.p, M.d_desc_ptr.p, M.d_desc.p,
+                                     sv->d_perm.p, sv->d_scale.p, M.d_scr.p, M.ld, d_y);
+  } else {
+    const int ni = (int)M.d_items_t.n;
+    k_lmul_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_x, M.d_scr.p);
+    kt[nb - 1]<<<cdiv(ni, 8), 256, 0, st>>>(sv->d_fdesc.p, sv->d_L.p, M.d_items_t.p, ni, sv->d_lperm.p, sv->d_rows.p,
+                                            M.d_scr.p, n, d_y);
+  }
+  sv->launches += 2;
+  CU(cudaGetLastError());
+  return B200LDLT_SUCCESS;
+}
+
+// nrhs columns in blocks of up to B200_SOLVE_BLOCK (lmul_state called before)
+static int enqueue_lmul_columns(Solver* sv, int trans, int nrhs, const double* d_x, double* d_y) {
+  for (int c = 0; c < nrhs;) {
+    const int w = std::min(sv->lmul->width, nrhs - c);
+    const int rc = enqueue_lmul(sv, trans, d_x + (size_t)c * sv->n, d_y + (size_t)c * sv->n, w);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    c += w;
+  }
+  return B200LDLT_SUCCESS;
+}
+
 static int shard_setup(Solver* sv, int rank, int world) {
   Symbolic& S = sv->S;
   cudaStream_t st = sv->stream;
@@ -1650,6 +1775,15 @@ static bool partial_refused(Solver* sv, int job) {
   else return false;
   return true;
 }
+
+// lmultiply / alter_d are refused in the same cases as the partial solves (alter_d passes trans = 0)
+static bool factors_refused(Solver* sv, const char* what, int trans) {
+  if (trans != 0 && trans != 1) sv->err = std::string(what) + ": trans must be 0 or 1";
+  else if (!sv->factored) sv->err = std::string(what) + ": no factors (factorise first; a SINGULAR factorisation leaves none)";
+  else if (sv->shard.active) sv->err = std::string(what) + ": not available on a sharded handle";
+  else return false;
+  return true;
+}
 }  // namespace b200
 
 extern "C" {
@@ -1704,6 +1838,81 @@ int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, d
       if (pivot_type) pivot_type[p] = ptype[p];
       if (dinv2) { dinv2[2 * (size_t)p] = dinv[p]; dinv2[2 * (size_t)p + 1] = ptype[p] == 2 ? doff[p] : 0.0; }
     }
+  return B200LDLT_SUCCESS;
+}
+
+int b200ldlt_lmultiply_device(b200ldlt_handle h, int trans, int nrhs, const double* d_x, double* d_y) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  if (factors_refused(sv, "lmultiply", trans)) return B200LDLT_FATAL_ERROR;
+  if (nrhs <= 0) return B200LDLT_SUCCESS;
+  CU(cudaSetDevice(sv->dev));
+  cudaStream_t st = sv->stream;
+  { const int rc = lmul_state(sv, nrhs); if (rc != B200LDLT_SUCCESS) return rc; }
+  sv->launches = 0;
+  CU(cudaEventRecord(sv->ev0, st));
+  { const int rc = enqueue_lmul_columns(sv, trans, nrhs, d_x, d_y); if (rc != B200LDLT_SUCCESS) return rc; }
+  CU(cudaEventRecord(sv->ev1, st));
+  CU(cudaStreamSynchronize(st));
+  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
+  sv->info.launches_solve = sv->launches;
+  return B200LDLT_SUCCESS;
+}
+
+int b200ldlt_lmultiply(b200ldlt_handle h, int trans, int nrhs, const double* x, double* y) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  if (factors_refused(sv, "lmultiply", trans)) return B200LDLT_FATAL_ERROR;
+  if (nrhs <= 0) return B200LDLT_SUCCESS;
+  CU(cudaSetDevice(sv->dev));
+  cudaStream_t st = sv->stream;
+  const size_t n = sv->n, total = n * (size_t)nrhs;
+  if (nrhs > sv->rhs_cap) {
+    if (sv->h_rhs) cudaFreeHost(sv->h_rhs);
+    sv->h_rhs = nullptr;
+    sv->rhs_cap = 0;
+    CU(cudaHostAlloc((void**)&sv->h_rhs, total * sizeof(double), cudaHostAllocDefault));
+    CU(sv->d_rhs.alloc(total));
+    sv->rhs_cap = nrhs;
+  }
+  { const int rc = lmul_state(sv, nrhs); if (rc != B200LDLT_SUCCESS) return rc; }
+  // through the pinned staging of the solves, in place on the device (both kernel pairs allow it)
+  memcpy(sv->h_rhs, x, total * sizeof(double));
+  sv->launches = 0;
+  CU(cudaEventRecord(sv->ev0, st));
+  CU(cudaMemcpyAsync(sv->d_rhs.p, sv->h_rhs, total * sizeof(double), cudaMemcpyHostToDevice, st));
+  { const int rc = enqueue_lmul_columns(sv, trans, nrhs, sv->d_rhs.p, sv->d_rhs.p); if (rc != B200LDLT_SUCCESS) return rc; }
+  CU(cudaMemcpyAsync(sv->h_rhs, sv->d_rhs.p, total * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(sv->ev1, st));
+  CU(cudaStreamSynchronize(st));
+  memcpy(y, sv->h_rhs, total * sizeof(double));
+  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
+  sv->info.launches_solve = sv->launches;
+  return B200LDLT_SUCCESS;
+}
+
+int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  if (factors_refused(sv, "alter_d", 0)) return B200LDLT_FATAL_ERROR;
+  if (!dinv2) { sv->err = "alter_d: no entries"; return B200LDLT_FATAL_ERROR; }
+  CU(cudaSetDevice(sv->dev));
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  if (sv->d_alter.n != 2 * (size_t)n) CU(sv->d_alter.alloc(2 * (size_t)n));
+  if (!sv->d_alter_bad.p) CU(sv->d_alter_bad.alloc(1));
+  int bad = 0;
+  CU(cudaMemcpyAsync(sv->d_alter.p, dinv2, 2 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
+  CU(cudaMemsetAsync(sv->d_alter_bad.p, 0, sizeof(int), st));
+  k_alter_check<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_ptype.p, sv->d_alter.p, sv->d_alter_bad.p);
+  k_alter<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_ptype.p, sv->d_alter.p, sv->d_alter_bad.p, sv->d_dinv.p, sv->d_doff.p);
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(&bad, sv->d_alter_bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (bad) {
+    sv->err = "alter_d: refused (an entry is not finite, or an off-diagonal entry is non-zero where no 2x2 pivot opens); D is unchanged";
+    return B200LDLT_FATAL_ERROR;
+  }
   return B200LDLT_SUCCESS;
 }
 

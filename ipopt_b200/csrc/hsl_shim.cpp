@@ -15,8 +15,15 @@
 // Beyond what Ipopt resolves, the shim also serves the other MA97 callers of the same library:
 //   ma97_solve_d job 1..4  the partial solves (b200ldlt_solve_partial: L, D, L^T on their own, in pivot order);
 //   ma97_enquire_indef_d   the pivot order and D^-1 (b200ldlt_enquire_indef), declared at hsl_ma97d.h:158-160;
-//   scale[]                of ma97_factor_d / ma97_factor_solve_d: the equilibration factors of that factorisation.
-// Not provided: ma97_alter_d, ma97_enquire_posdef_d, ma97_solve_fredholm_d and the sparse-rhs / 64-bit variants.
+//   scale[]                of ma97_factor_d / ma97_factor_solve_d: the equilibration factors of that factorisation;
+//   ma97_lmultiply_d       multiplication by S^-1 P L or its transpose (b200ldlt_lmultiply), hsl_ma97d.h:169-171;
+//   ma97_alter_d           writes D^-1 back in the layout ma97_enquire_indef_d returns (b200ldlt_alter_d);
+//   ma97_enquire_posdef_d  the diagonal of the Cholesky factor L D^1/2 when every pivot is a positive 1x1 pivot.
+// Not provided: ma97_solve_fredholm_d (it needs the factors of a singular matrix, and the backend keeps none after
+// SINGULAR), ma97_sparse_fwd_solve_d (it needs a sweep pruned to the rows a sparse right-hand side reaches) and the
+// 64-bit variants.
+// The conventions of the inspection calls (enquire_indef / enquire_posdef / alter / lmultiply) are our reading of the
+// reference header; they have not been checked against the HSL user documentation.
 #include <cuda_runtime_api.h>
 
 #include <cmath>
@@ -227,6 +234,56 @@ void ma97_enquire_indef_d(void** akeep, void** fkeep, const ma97_control_d* cont
   }
   if (piv_order)
     for (int p = 0; p < K->n; ++p) piv_order[var[p]] = ty[p] == 1 ? p + 1 : -(p + 1);
+  fill_info(K, info);
+  info->flag = 0;
+}
+
+// y = (S^-1 P L) x for trans = 0, its transpose for trans = 1: the operator of job 1 inverted (b200ldlt_lmultiply).
+// k columns; ldx / ldy != n: column by column, as ma97_solve_d does.  k = 0 does nothing.
+void ma97_lmultiply_d(int trans, int k, const double x[], int ldx, double y[], int ldy, void** akeep, void** fkeep,
+                      const ma97_control_d* control, ma97_info_d* info) {
+  (void)control; (void)fkeep;
+  memset(info, 0, sizeof(*info));
+  Keep* K = akeep ? (Keep*)*akeep : nullptr;
+  if (!K || !K->h || !K->factored || k < 0 || (trans != 0 && trans != 1) || ldx < K->n || ldy < K->n) { info->flag = -1; return; }
+  if (k == 0) return;
+  int st;
+  if (ldx == K->n && ldy == K->n) st = b200ldlt_lmultiply(K->h, trans, k, x, y);
+  else {
+    st = B200LDLT_SUCCESS;
+    for (int c = 0; c < k && st == B200LDLT_SUCCESS; ++c)
+      st = b200ldlt_lmultiply(K->h, trans, 1, x + (size_t)c * ldx, y + (size_t)c * ldy);
+  }
+  fill_info(K, info);
+  info->flag = (st == B200LDLT_SUCCESS) ? 0 : -1;
+}
+
+// d[2p] / d[2p+1]: the new diagonal / off-diagonal entry of D^-1 at pivot position p -- the convention of
+// ma97_enquire_indef_d, so that enquire followed by alter changes nothing.  Refused (flag -1, D unchanged) for a
+// non-finite entry or a non-zero off-diagonal entry where no 2x2 pivot opens.  Lasts until the next factorisation.
+void ma97_alter_d(const double d[], void** akeep, void** fkeep, const ma97_control_d* control, ma97_info_d* info) {
+  (void)fkeep; (void)control;
+  memset(info, 0, sizeof(*info));
+  Keep* K = akeep ? (Keep*)*akeep : nullptr;
+  if (!K || !K->h || !K->factored || !d) { info->flag = -1; return; }
+  const int st = b200ldlt_alter_d(K->h, d);
+  fill_info(K, info);
+  info->flag = (st == B200LDLT_SUCCESS) ? 0 : -1;
+}
+
+// d[p] = sqrt(D_pp), pivot order: the diagonal of the Cholesky factor L D^1/2 of the scaled matrix.  Defined only when
+// every pivot is a positive 1x1 pivot (a positive-definite factorisation); otherwise flag -1 and d untouched.
+void ma97_enquire_posdef_d(void** akeep, void** fkeep, const ma97_control_d* control, ma97_info_d* info, double d[]) {
+  (void)fkeep; (void)control;
+  memset(info, 0, sizeof(*info));
+  Keep* K = akeep ? (Keep*)*akeep : nullptr;
+  if (!K || !K->h || !K->factored || !d) { info->flag = -1; return; }
+  std::vector<int> ty(K->n);
+  std::vector<double> dinv2(2 * (size_t)K->n);
+  if (b200ldlt_enquire_indef(K->h, nullptr, ty.data(), dinv2.data()) != B200LDLT_SUCCESS) { info->flag = -1; return; }
+  for (int p = 0; p < K->n; ++p)
+    if (ty[p] != 1 || !(dinv2[2 * (size_t)p] > 0.0)) { fill_info(K, info); info->flag = -1; return; }
+  for (int p = 0; p < K->n; ++p) d[p] = std::sqrt(1.0 / dinv2[2 * (size_t)p]);
   fill_info(K, info);
   info->flag = 0;
 }
