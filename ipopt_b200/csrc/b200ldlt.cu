@@ -68,7 +68,6 @@ struct SolvePlan {
   DevBuf<double> d_part;
   int nsub = 0, npair = 0, ntf = 0, ntb = 0;
   long long sub_bytes = 0;
-  unsigned long long* tlog = nullptr;   // B200_SOLVE_TIMELINE (splan only): records of its single-column sweeps
 };
 
 // what the solve sweeps write, for `width` columns: column c of each array at its base + c * its stride in M.  The chunk
@@ -120,34 +119,21 @@ struct SchurLists {
 
 // environment switches for profiling / A-B runs, read ONCE at b200ldlt_create (never on the enqueue path)
 struct DebugSwitches {
-  bool factor_sections = false;   // B200_FACTOR_SECTIONS=1 (with use_graph=0): timed section marks
   bool one_stream = false;        // B200_ONE_STREAM=1: big-front pipeline on a single stream
-  bool solve_timeline = false;    // B200_SOLVE_TIMELINE=1: per-task %globaltimer log of the top solve kernel
   bool cb_at_end = false;         // B200_CB_AT_END=1: Schur complements as one GEMM per level (k_big_schur84) instead of per-panel updates
   int solve_direct = 2;           // B200_SOLVE_DIRECT=D: the D lowest tree levels are solved by k_solve_direct (0 = all inside the subtrees)
   bool solve_nopair = false;      // B200_SOLVE_NOPAIR=1: one subtree per CTA in the solve sweeps (no side-by-side pairs)
   int solve_block = MS_NB_MAX;    // B200_SOLVE_BLOCK=n: nrhs > 1 solved in blocks of at most n columns (1 = one solve per column)
   bool no_warp2 = false;          // B200_NO_WARP2=1: fronts of order 33..64 by the shared-memory kernel (one CTA each) instead of k_front_warp2
   bool no_pdl = false;            // B200_NO_PDL=1: chain kernels launched without programmatic dependent launch
-  bool factor_timeline = false;   // B200_FACTOR_TIMELINE=1: %globaltimer records of the factorisation kernels (b200ldlt_dump_factor_timeline)
-  std::vector<int> buckets;       // B200_BUCKETS=a,b,c: soft split points of the shared-memory front classes
   void read() {
-    factor_sections = getenv("B200_FACTOR_SECTIONS") != nullptr;
     one_stream = getenv("B200_ONE_STREAM") != nullptr;
-    solve_timeline = getenv("B200_SOLVE_TIMELINE") != nullptr;
-    factor_timeline = getenv("B200_FACTOR_TIMELINE") != nullptr;
     cb_at_end = getenv("B200_CB_AT_END") != nullptr;
     solve_nopair = getenv("B200_SOLVE_NOPAIR") != nullptr;
     if (const char* e = getenv("B200_SOLVE_DIRECT")) solve_direct = atoi(e);
     if (const char* e = getenv("B200_SOLVE_BLOCK")) solve_block = std::min(std::max(atoi(e), 1), MS_NB_MAX);
     no_pdl = getenv("B200_NO_PDL") != nullptr;
     no_warp2 = getenv("B200_NO_WARP2") != nullptr;
-    if (const char* e = getenv("B200_BUCKETS")) {
-      for (const char* p = e; *p;) { buckets.push_back(atoi(p)); while (*p && *p != ',') ++p; if (*p) ++p; }
-    } else {
-      buckets = {48, 96};   // the classes of a level run side by side, so a finer split costs no serial launches
-                            // (H100 SXM, 700 W, factorisation at N=400 / 800: {96} and {32,64,96} within 0.4 %)
-    }
   }
 };
 
@@ -212,7 +198,6 @@ struct Solver {
   std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call after an analysis
   DevBuf<double> d_alter;           // alter_d: the caller's 2n entries of D^-1 (allocated at the first call)
   DevBuf<int> d_alter_bad;
-  DevBuf<unsigned long long> d_tlog, d_flog;
   DevBuf<double> d_linv;
   DevBuf<double> d_linv_part;       // partial tiles of the chunked k_linv_gemm items (one launch at a time uses it)
   DevBuf<int> d_linv_cnt;           // their arrival counters (self-resetting)
@@ -221,7 +206,6 @@ struct Solver {
   DevBuf<int> d_gmap;
   LinvPlan linv_plan;               // explicit inverses of the big fronts' pivot blocks (all fronts)
   std::vector<std::unique_ptr<LinvPlan>> linv_level;   // the same work, split by tree level (issued behind each level's chain)
-  std::vector<SolveTask> h_tasks;   // fwd then bwd (debug timeline)
   SolvePlan splan;                  // all fronts
   std::vector<char> solve_direct_front;   // per supernode: solved by k_solve_direct (see build_solve_tables)
   int solve_epoch = 0;
@@ -258,22 +242,6 @@ struct Solver {
     for (auto& q : side) if (q) cudaStreamDestroy(q);
     if (own_stream && stream) cudaStreamDestroy(stream);
   }
-  // debug (B200_FACTOR_SECTIONS=1 with use_graph=0): timed section marks of the last factorisation
-  std::vector<std::pair<std::string, cudaEvent_t>> sect;
-  void mark(const char* label, int level) {
-    if (!dbg.factor_sections || opt.use_graph != 0) return;
-    cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, stream);
-    sect.emplace_back(std::string(label) + " L" + std::to_string(level), e);
-  }
-  void dump_sections() {
-    if (sect.empty()) return;
-    for (size_t i = 1; i < sect.size(); ++i) {
-      float ms = 0; cudaEventElapsedTime(&ms, sect[i - 1].second, sect[i].second);
-      fprintf(stderr, "[sections] %-18s %8.1f us\n", sect[i].first.c_str(), ms * 1e3);
-    }
-    for (auto& pr : sect) cudaEventDestroy(pr.second);
-    sect.clear();
-  }
   cudaEvent_t next_event() {
     if (ev_next == ev_pool.size()) { cudaEvent_t e; cudaEventCreateWithFlags(&e, cudaEventDisableTiming); ev_pool.push_back(e); }
     return ev_pool[ev_next++];
@@ -292,7 +260,7 @@ struct Solver {
 
 // per level: big fronts first, then the shared-memory classes by descending front order; only fronts with take[s]
 static void build_level_plans(const Symbolic& S, int smax, const std::vector<char>& take, std::vector<int>& fl,
-                              std::vector<LevelPlan>& plan, const std::vector<int>& soft, SchurLists& SL, int tc_min_r,
+                              std::vector<LevelPlan>& plan, SchurLists& SL, int tc_min_r,
                               bool use_warp2) {
   SL.f.clear(); SL.t.clear(); SL.dfl.clear(); SL.dig_bytes = 0; SL.exp_ints = 0;
   fl.clear();
@@ -347,8 +315,9 @@ static void build_level_plans(const Symbolic& S, int smax, const std::vector<cha
     // Size classes: (64, smax] 256 threads, (32, 64] 128 threads, <= 32 one warp per front.  Inside a class the
     // fronts are split again at the soft limits below (shared memory per CTA follows the largest front of a launch,
     // so finer buckets raise the number of resident CTAs per SM); a soft split only happens once the current bucket
-    // holds enough fronts to fill the GPU.
-    // (soft: splits at 48 and 96 by default, DebugSwitches::buckets)
+    // holds enough fronts to fill the GPU.  Soft limits at 48 and 96: the classes of a level run side by side, so a finer
+    // split costs no serial launches (H100 SXM, 700 W, factorisation at N=400 / 800: {96} and {32,64,96} within 0.4 %).
+    const int kSoft[] = {48, 96};
     const int kMinBucket = 296;
     auto threads_of = [](int f) { return f > 64 ? 256 : (f > 32 ? 128 : 64); };
     LevelPlan::Bucket cur{(int)fl.size(), 0, 0, 0, 256, 0};
@@ -369,7 +338,7 @@ static void build_level_plans(const Symbolic& S, int smax, const std::vector<cha
       if (cur.cnt == 0) {
         cur.threads = threads_of(f);
         cur_lo = 0;
-        for (int v : soft) if (v < f) cur_lo = std::max(cur_lo, v);
+        for (int v : kSoft) if (v < f) cur_lo = std::max(cur_lo, v);
       }
       fl.push_back(s);
       cur.cnt++;
@@ -657,7 +626,6 @@ static int build_solve_plan(Solver* sv, const Symbolic& S, const std::vector<cha
   if (sv->opt.verbose)
     fprintf(stderr, "[b200ldlt] solve plan: %d subtrees in %d work items (%.1f MB of L, largest %.0f KB), top: %d fwd / %d bwd tasks, %lld partial slots\n",
             nsub, SP.npair, SP.sub_bytes / 1e6, nsub ? (ownL[roots[0] + 1] - ownL[roots[0] - size[roots[0]] + 1]) * 8 / 1e3 : 0.0, SP.ntf, SP.ntb, npart);
-  if (sv->dbg.solve_timeline) { sv->h_tasks = tf; sv->h_tasks.insert(sv->h_tasks.end(), tb.begin(), tb.end()); }
   if (tf.empty()) tf.push_back(SolveTask{ST_SMALL, 0, 0, 0, 0, 0, 1, 0, 0, 0});
   if (tb.empty()) tb.push_back(SolveTask{ST_SMALL, 0, 0, 0, 0, 0, 1, 0, 0, 0});
   if (bundle.empty()) bundle.push_back(0);
@@ -668,7 +636,6 @@ static int build_solve_plan(Solver* sv, const Symbolic& S, const std::vector<cha
   CU(SP.d_ccnt.alloc(std::max(ncidx, 1)));
   CU(cudaMemsetAsync(SP.d_ccnt.p, 0, SP.d_ccnt.n * sizeof(int), st));
   CU(SP.d_part.alloc(std::max<long long>(npart, 1) * 64));
-  SP.tlog = nullptr;
   return B200LDLT_SUCCESS;
 }
 
@@ -837,14 +804,6 @@ static int run_analysis(Solver* sv, const double* vals) {
   N.L = sv->d_L.p; N.W = sv->d_W.p; N.CB = sv->d_CB.p; N.uval = sv->d_uval.p;
   N.dinv = sv->d_dinv.p; N.doff = sv->d_doff.p; N.ptype = sv->d_ptype.p;
   N.lperm = sv->d_lperm.p; N.bperm = sv->d_bperm.p; N.counters = sv->d_counters.p; N.colmax = sv->d_colmax.p;
-  N.flog = nullptr;
-  if (sv->dbg.factor_timeline) {
-    const unsigned long long cap = 1ull << 16;
-    CU(sv->d_flog.alloc(2 + cap * FLOG_WORDS));
-    const unsigned long long hdr[2] = {0ull, cap};
-    CU(cudaMemcpy(sv->d_flog.p, hdr, sizeof(hdr), cudaMemcpyHostToDevice));
-    N.flog = sv->d_flog.p;
-  }
 
   // inverse row maps of the children of the (factorisation-)big fronts, for the one-launch extend-add
   {
@@ -869,15 +828,14 @@ static int run_analysis(Solver* sv, const double* vals) {
   std::vector<int> fl;
   {
     std::vector<char> take(S.nsn, 1);
-    build_level_plans(S, sv->opt.smem_front_max, take, fl, sv->plan, sv->dbg.buckets, sv->schur, sv->tc_min_r, !sv->dbg.no_warp2);
+    build_level_plans(S, sv->opt.smem_front_max, take, fl, sv->plan, sv->schur, sv->tc_min_r, !sv->dbg.no_warp2);
   }
   CU(sv->d_front_list.upload(fl, st));
   { int rc2 = upload_schur_lists(sv, sv->schur, st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
   CU(cudaFuncSetAttribute(k_tc_schur, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
   CU(cudaFuncSetAttribute(k_big_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, CHAIN_SMEM));
   CU(cudaFuncSetAttribute(k_front_warp2, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * S2_SMEM_PER_WARP));
-  CU(cudaFuncSetAttribute(k_front_smem<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  CU(cudaFuncSetAttribute(k_front_smem<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+  CU(cudaFuncSetAttribute(k_front_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   CU(cudaStreamSynchronize(st));
 
 
@@ -935,10 +893,6 @@ static int run_analysis(Solver* sv, const double* vals) {
       std::vector<char> take(S.nsn, 1);
       rc2 = build_solve_plan(sv, S, take, sv->splan, st);
       if (rc2 != B200LDLT_SUCCESS) return rc2;
-    }
-    if (sv->dbg.solve_timeline) {
-      CU(sv->d_tlog.alloc(2 * (size_t)(sv->splan.ntf + sv->splan.ntb) + 8 * (size_t)sv->splan.nsub + 8));
-      sv->splan.tlog = sv->d_tlog.p;
     }
     if (sv->opt.verbose)
       fprintf(stderr, "[b200ldlt] solve: %d big-front blocks, top grid %d x %d thr (%d CTAs per SM)\n",
@@ -1000,7 +954,6 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
   sv->ev_next = 0;
   CU(cudaMemsetAsync(sv->d_counters.p, 0, CNT_N * sizeof(int), st));
   CU(cudaMemsetAsync(sv->d_colmax.p, 0, (size_t)n * sizeof(double), st));
-  if (sv->DN.flog) CU(cudaMemsetAsync(sv->DN.flog, 0, sizeof(unsigned long long), st));
   k_sum_dups<<<cdiv(nu, 256), 256, 0, st>>>(nu, sv->d_useg_ptr.p, sv->d_useg_src.p, sv->d_vals.p, sv->d_uval.p); ++L;
   k_fill<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_scale.p, 1.0); ++L;
   for (int sw = 0; sw < sv->opt.scaling; ++sw) {
@@ -1032,7 +985,6 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
     }
   }
   bool linv_forked = false;
-  sv->mark("prologue", -1);
   for (int l = 0; l < S.nlevels; ++l) {
     const LevelPlan& P = plan[l];
     if (P.big_cnt) {
@@ -1042,7 +994,6 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
         k_big_extend_all<<<dim3(cdiv(P.big_fmax, 8), P.big_cnt), 256, 0, st>>>(D, N, bl); ++L;
       }
     }
-    if (P.big_cnt) sv->mark("big-assemble", l);
     unsigned used_side = 0;
     {
       // the front classes of a level are independent: issue them side by side (forked from / joined to the main stream)
@@ -1065,14 +1016,13 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
         } else if (bk.fmax <= 32) {  // one warp per front (registers), 4 fronts per CTA
           k_front_warp<<<cdiv(bk.cnt, 4), 128, 4 * XS_SMEM_PER_WARP, sq>>>(D, N, fl + bk.off, bk.cnt); ++L;
         } else {
-          k_front_smem<false><<<bk.cnt, bk.threads, bk.smem, sq>>>(D, N, fl + bk.off, bk.cnt, 0); ++L;
+          k_front_smem<<<bk.cnt, bk.threads, bk.smem, sq>>>(D, N, fl + bk.off, bk.cnt); ++L;
         }
       }
       used_side = used;
       // (the side streams are joined at the END of the level: this level's big fronts do not depend on its small fronts,
       //  so the panel chain below runs next to them)
     }
-    sv->mark("small-fronts", l);
     if (P.big_cnt) {
       const int* bl = fl + P.big_off;
       if (P.big_chmax <= 0) {   // (with children the extend-add kernel has recorded the column maxima of the first panels)
@@ -1125,7 +1075,6 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
         CU(cudaEventRecord(e, su));
         CU(cudaStreamWaitEvent(st, e, 0));
       }
-      sv->mark("big-chain", l);
       if (!linv_p && !sv->dbg.one_stream && l < (int)sv->linv_level.size() && sv->linv_level[l]->ndiag > 0) {
         // explicit L11 inverses of this level's fronts: behind the chain on their own stream, concurrent with the Schur
         // complements and the levels above (they only read the finished pivot blocks; k_linv_gemm<1> uses the top k x k
@@ -1155,7 +1104,6 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
       CU(cudaStreamWaitEvent(st, e, 0));
     }
   }
-  sv->mark("big-schur(last)", S.nlevels);
   if (linv_forked) {
     cudaEvent_t e = sv->next_event();
     CU(cudaEventRecord(e, sv->stream3));
@@ -1164,7 +1112,6 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
     int rc = enqueue_linv(sv, linv_p ? *linv_p : sv->linv_plan, st);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
-  sv->mark("linv", S.nlevels);
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
 }
@@ -1191,7 +1138,6 @@ static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* n
   CU(cudaStreamSynchronize(st));
   float ms = 0;
   cudaEventElapsedTime(&ms, sv->ev0, sv->ev1);
-  sv->dump_sections();
   b200ldlt_info& I = sv->info;
   I.ms_factor_gpu = ms;
   I.launches_factor = sv->launches;
@@ -1291,7 +1237,6 @@ static DevSolve sweep_view(const Solver* sv, const SolvePlan& SP, const SweepSta
   V.subs = SP.d_subs.p; V.sub_meta = SP.d_sub_meta.p; V.subrow = SP.d_subrow.p; V.nsub = SP.nsub;
   V.subpair = SP.d_subpair.p; V.npair = SP.npair; V.sub_Loff = SP.d_sub_Loff.p;
   V.upper_max = sv->opt.smem_front_max;
-  V.tlog = W.width > 1 ? nullptr : SP.tlog;
   return V;
 }
 
@@ -1551,7 +1496,7 @@ static int shard_setup(Solver* sv, int rank, int world) {
   }
   for (int ph = 0; ph < 2; ++ph) {
     std::vector<int> fl;
-    build_level_plans(S, sv->opt.smem_front_max, take[ph], fl, H.plan[ph], sv->dbg.buckets, H.schur[ph], sv->tc_min_r, !sv->dbg.no_warp2);
+    build_level_plans(S, sv->opt.smem_front_max, take[ph], fl, H.plan[ph], H.schur[ph], sv->tc_min_r, !sv->dbg.no_warp2);
     { int rc2 = upload_schur_lists(sv, H.schur[ph], st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
     { int rc2 = build_linv_plan(sv, S, take[ph], H.linv_plan[ph], st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
     { int rc2 = build_solve_plan(sv, S, take[ph], H.splan[ph], st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
@@ -1913,55 +1858,6 @@ int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2) {
     sv->err = "alter_d: refused (an entry is not finite, or an off-diagonal entry is non-zero where no 2x2 pivot opens); D is unchanged";
     return B200LDLT_FATAL_ERROR;
   }
-  return B200LDLT_SUCCESS;
-}
-
-/* debug: write the kernel timeline of the last factorisation (needs env B200_FACTOR_TIMELINE=1 at create time):
- * one line per record: kind s jb level k f t0 t1 ...  (kind: 1 chain role, 2 panel rows, 3 bulk update, 4 front (smem),
- * 5 front (warp), 6 Schur, 7 extend-add, 10-12 L11 inverse; times in ns of %globaltimer) */
-int b200ldlt_dump_factor_timeline(b200ldlt_handle h, const char* path) {
-  Solver* sv = (Solver*)h;
-  if (!sv || !sv->DN.flog) return B200LDLT_FATAL_ERROR;
-  std::vector<unsigned long long> t(sv->d_flog.n);
-  CU(cudaMemcpy(t.data(), sv->d_flog.p, t.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  FILE* fp = fopen(path, "w");
-  if (!fp) return B200LDLT_FATAL_ERROR;
-  const unsigned long long nrec = std::min(t[0], t[1]);
-  for (unsigned long long i = 0; i < nrec; ++i) {
-    const unsigned long long* r = t.data() + 2 + i * FLOG_WORDS;
-    const int s = (int)(long long)r[1];
-    const int k = sv->S.sn_start[s + 1] - sv->S.sn_start[s];
-    const int f = k + (int)(sv->S.rows_ptr[s + 1] - sv->S.rows_ptr[s]);
-    fprintf(fp, "%d %d %d %d %d %d", (int)r[0], s, (int)(long long)r[2], sv->S.sn_level[s], k, f);
-    for (unsigned long long q = 0; q < r[3] && q < FLOG_WORDS - 4; ++q) fprintf(fp, " %llu", r[4 + q]);
-    fprintf(fp, "\n");
-  }
-  fclose(fp);
-  return B200LDLT_SUCCESS;
-}
-
-/* debug: write the per-task timeline of the last solve (needs env B200_SOLVE_TIMELINE=1 at analyse time) */
-int b200ldlt_dump_solve_timeline(b200ldlt_handle h, const char* path) {
-  Solver* sv = (Solver*)h;
-  if (!sv || !sv->splan.tlog) return B200LDLT_FATAL_ERROR;
-  std::vector<unsigned long long> t(sv->d_tlog.n);
-  CU(cudaMemcpy(t.data(), sv->d_tlog.p, t.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  FILE* fp = fopen(path, "w");
-  if (!fp) return B200LDLT_FATAL_ERROR;
-  for (size_t i = 0; i < sv->h_tasks.size(); ++i) {
-    const SolveTask& T = sv->h_tasks[i];
-    int s = T.type == ST_SMALL ? -1 : T.s;
-    fprintf(fp, "%zu %d %d %d %d %d %llu %llu\n", i, i < (size_t)sv->splan.ntf ? 0 : 1, T.type, T.s, T.blk,
-            s >= 0 ? sv->S.sn_level[s] : -1, t[2 * i], t[2 * i + 1]);
-  }
-  // subtree records: "S pass index start loaded end nfront nlv"
-  const size_t base = 2 * (size_t)(sv->splan.ntf + sv->splan.ntb);
-  for (int pass = 0; pass < 2; ++pass)
-    for (int u = 0; u < sv->splan.nsub; ++u) {
-      const unsigned long long* r = t.data() + base + 4 * ((size_t)pass * sv->splan.nsub + u);
-      fprintf(fp, "S %d %d %llu %llu %llu %llu %llu\n", pass, u, r[0], r[1], r[2], r[3] >> 32, r[3] & 0xffffffffull);
-    }
-  fclose(fp);
   return B200LDLT_SUCCESS;
 }
 

@@ -109,16 +109,11 @@ __device__ __forceinline__ float wredux_max(float v) {
   return (m == INT_MIN) ? __int_as_float(0x7fffffff) : __int_as_float(m ^ ((m >> 31) & 0x7fffffff));
 }
 
-// The pivoted front factorisation runs either on a whole CTA (WARP=false, __syncthreads) or on a single
-// warp (WARP=true, __syncwarp; several fronts per CTA).
-template <bool WARP>
-__device__ __forceinline__ void gsync() { if (WARP) __syncwarp(); else __syncthreads(); }
-
-template <bool WARP>
+// The pivoted front factorisation of k_front_smem: barriers inside, so every thread of the CTA calls these.
 __device__ void swap_sym(double* F, int ld, int f, int p, int q) {
   // symmetric interchange of rows/cols p < q of a matrix whose LOWER triangle is stored (the strictly upper part
   // of F is never read); one pass, index t handled by one thread; caller syncs before.
-  const int tid = WARP ? (threadIdx.x & 31) : threadIdx.x, nt = WARP ? 32 : blockDim.x;
+  const int tid = threadIdx.x, nt = blockDim.x;
   if (p > q) { const int x = p; p = q; q = x; }
   for (int t = tid; t < f; t += nt) {
     double* u; double* v;
@@ -130,14 +125,13 @@ __device__ void swap_sym(double* F, int ld, int f, int p, int q) {
     const double a = *u, b = *v;
     *u = b; *v = a;
   }
-  gsync<WARP>();
+  __syncthreads();
 }
 
-template <bool WARP>
 __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int* pt, double* cv1,
                                   double* cv2, volatile int* sh, double u, double tiny,
                                   double* dinv, double* doff, int* ptype_g, int* counters) {
-  const int tid = WARP ? (threadIdx.x & 31) : threadIdx.x, nt = WARP ? 32 : blockDim.x;
+  const int tid = threadIdx.x, nt = blockDim.x;
   const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;
   for (int t = tid; t < k; t += nt) lp[t] = t;
   if (tid == 0) { sh[2] = 0; sh[6] = 0; }
@@ -145,7 +139,7 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
   int c_neg = 0, c_forced = 0, c_tiny = 0, c_2x2 = 0;  // only meaningful on thread 0
   int j = 0, kend = k, progress = 0;
   bool forced = false;
-  gsync<WARP>();
+  __syncthreads();
   while (j < k) {
     if (j == kend) {  // no candidate left in this pass
       if (progress > 0) { kend = k; progress = 0; }
@@ -211,23 +205,23 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
       }
       if (lane == 0) { sh[4 * par] = type; sh[4 * par + 1] = r; }
     }
-    gsync<WARP>();
+    __syncthreads();
     const int type = sh[4 * par], r = sh[4 * par + 1], noise = sh[4 * par + 2];
     par ^= 1;
     if (type == 0) {  // reject for now: park column j at the end of the candidate range
       if (j != kend - 1) {
-        swap_sym<WARP>(F, ld, f, j, kend - 1);
+        swap_sym(F, ld, f, j, kend - 1);
         if (tid == 0) { int t = lp[j]; lp[j] = lp[kend - 1]; lp[kend - 1] = t; }
       }
       --kend;
       continue;
     }
     if (type == 2 && r != j) {
-      swap_sym<WARP>(F, ld, f, j, r);
+      swap_sym(F, ld, f, j, r);
       if (tid == 0) { int t = lp[j]; lp[j] = lp[r]; lp[r] = t; }
     }
     if (type == 3 && r != j + 1) {
-      swap_sym<WARP>(F, ld, f, j + 1, r);
+      swap_sym(F, ld, f, j + 1, r);
       if (tid == 0) { int t = lp[j + 1]; lp[j + 1] = lp[r]; lp[r] = t; }
     }
     if (type != 3) {
@@ -272,7 +266,7 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
         }
         for (; m <= mend; m += nwarp) F[i + m * ld] = fma(-li, cj[m], F[i + m * ld]);
       }
-      gsync<WARP>();
+      __syncthreads();
       j += 1;
     } else {
       // ---------------- 2x2 pivot at (j, j+1) ----------------
@@ -308,7 +302,7 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
         }
         for (; m <= mend; m += nwarp) F[i + m * ld] = fma(-l2, cj1[m], fma(-l1, cj[m], F[i + m * ld]));
       }
-      gsync<WARP>();
+      __syncthreads();
       j += 2;
     }
     ++progress;
@@ -350,7 +344,7 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
     if (c_tiny) atomicAdd(counters + CNT_TINY, c_tiny);
     if (c_2x2) atomicAdd(counters + CNT_2X2, c_2x2);
   }
-  gsync<WARP>();
+  __syncthreads();
 }
 
 // --------------------------------------------------------------------------------------------
@@ -610,36 +604,30 @@ __device__ void warp_ldlt32(double (&a)[32], double (&b)[32], const int f, const
 // Class S/M: one CTA per front, everything in shared memory.
 // smem: F[ld*f] | cv1[f] | cv2[f] | lp[k] | pt[k] | sh[8]
 // --------------------------------------------------------------------------------------------
-template <bool WARP>
-__global__ void k_front_smem(DevSym S, DevNum N, const int* __restrict__ front_list, int nfronts,
-                             int smem_per_group /*bytes, WARP mode only*/) {
+__global__ void k_front_smem(DevSym S, DevNum N, const int* __restrict__ front_list, int nfronts) {
   extern __shared__ double smem[];
-  const int group = WARP ? (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) : blockIdx.x;
-  if (group >= nfronts) return;
-  const int s = front_list[group];
+  if (blockIdx.x >= nfronts) return;
+  const int s = front_list[blockIdx.x];
   const int c0 = S.sn_start[s], k = S.sn_start[s + 1] - c0;
   const int r = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
   const int f = k + r, ld = f | 1;
-  double* F = WARP ? (double*)((char*)smem + (size_t)(threadIdx.x >> 5) * smem_per_group) : smem;
+  double* F = smem;
   double* cv1 = F + (size_t)ld * f;
   double* cv2 = cv1 + f;
   int* lp = (int*)(cv2 + f);
   int* pt = lp + k;
   int* sh = pt + k;
-  const int tid = WARP ? (threadIdx.x & 31) : threadIdx.x, nt = WARP ? 32 : blockDim.x;
-  unsigned long long ts[4];
-  const bool tlog = N.flog != nullptr && threadIdx.x == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1);
-  if (tlog) ts[0] = flog_now();
+  const int tid = threadIdx.x, nt = blockDim.x;
 
   for (int t = tid; t < ld * f; t += nt) F[t] = 0.0;
-  gsync<WARP>();
+  __syncthreads();
   // original entries (unique -> no write conflicts)
   for (long long uu = S.uent_ptr[s] + tid; uu < S.uent_ptr[s + 1]; uu += nt) {
     unsigned d = S.u_dst[uu];
     int lr = d & 0xffffu, lc = d >> 16;
     F[lr + lc * ld] = N.uval[uu];   // lower triangle only (lr >= lc)
   }
-  gsync<WARP>();
+  __syncthreads();
   // extend-add of the children contribution blocks, one child at a time (deterministic)
   for (int q = S.child_ptr[s]; q < S.child_ptr[s + 1]; ++q) {
     const int c = S.child_idx[q];
@@ -653,13 +641,11 @@ __global__ void k_front_smem(DevSym S, DevNum N, const int* __restrict__ front_l
         F[li + lj * ld] += cb[ii + (size_t)jj * rc];   // rel is increasing: li >= lj
       }
     }
-    gsync<WARP>();
+    __syncthreads();
   }
 
-  if (tlog) ts[1] = flog_now();
-  factor_front_smem<WARP>(F, ld, f, k, lp, pt, cv1, cv2, sh, N.u, N.tiny, N.dinv + c0, N.doff + c0,
-                          N.ptype + c0, N.counters);
-  if (tlog) ts[2] = flog_now();
+  factor_front_smem(F, ld, f, k, lp, pt, cv1, cv2, sh, N.u, N.tiny, N.dinv + c0, N.doff + c0,
+                    N.ptype + c0, N.counters);
 
   // write L panel (f x k, ld = f), unit diagonal.  The strictly-upper part of the k x k pivot block receives L11^T
   // (entry (i, t), i < t, = L[t][i]): the backward solve of the small fronts reads row t of L11 as the contiguous
@@ -686,7 +672,6 @@ __global__ void k_front_smem(DevSym S, DevNum N, const int* __restrict__ front_l
   double* __restrict__ cbo = N.CB + S.cb_off[s];
   for (int m = tid >> 5; m < r; m += (nt >> 5))
     for (int i = m + (tid & 31); i < r; i += 32) cbo[i + (size_t)m * r] = F[(k + i) + (k + m) * ld];
-  if (tlog) { ts[3] = flog_now(); flog_put(N, 4, s, f, ts, 4); }
 }
 
 // --------------------------------------------------------------------------------------------
@@ -699,7 +684,6 @@ __global__ void __launch_bounds__(128) k_front_warp(DevSym S, DevNum N, const in
   const int group = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (group >= nfronts) return;
   const int s = front_list[group];
-  FlogScope fs(N, 5, s, 0);
   const int c0 = S.sn_start[s], k = S.sn_start[s + 1] - c0;
   const int r = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
   const int f = k + r;
@@ -766,7 +750,6 @@ __global__ void __launch_bounds__(128) k_front_warp(DevSym S, DevNum N, const in
 #pragma unroll
   for (int c = 0; c < 32; ++c)
     if (lane >= k && lane < f && c <= lane - k) cbo[(lane - k) + (size_t)c * r] = a[c];
-  fs.done();
 }
 
 // --------------------------------------------------------------------------------------------
@@ -784,7 +767,6 @@ __global__ void __launch_bounds__(128, 2) k_front_warp2(DevSym S, DevNum N, cons
   const int group = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (group >= nfronts) return;
   const int s = front_list[group];
-  FlogScope fs(N, 5, s, 1);
   const int c0 = S.sn_start[s], k = S.sn_start[s + 1] - c0;
   const int r = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
   const int f = k + r, f1 = f - 32;            // 32 < f <= 64, k <= 32 (guaranteed by the launch plan)
@@ -916,7 +898,6 @@ __global__ void __launch_bounds__(128, 2) k_front_warp2(DevSym S, DevNum N, cons
       if (j <= lane && lane < f1) cbo[(32 - k + lane) + (size_t)(32 - k + j) * r] = C22[lane + j * 33] - acc;
     }
   }
-  fs.done();
 }
 
 // --------------------------------------------------------------------------------------------
@@ -956,9 +937,6 @@ __global__ void __launch_bounds__(256) k_big_extend_all(DevSym S, DevNum N, cons
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int lj = blockIdx.x * 8 + warp;
   if (lj >= fp) return;
-  unsigned long long ts[2];
-  const bool tlog = N.flog != nullptr && threadIdx.x == 0 && (blockIdx.x == 0 || (blockIdx.x + 1) * 8 >= fp);
-  if (tlog) ts[0] = flog_now();
   // destination column indexed by the parent row li >= lj
   double* __restrict__ dst = (lj < kp) ? N.L + S.L_off[p] + (size_t)lj * fp
                                        : N.CB + S.cb_off[p] + (size_t)(lj - kp) * rp - kp;
@@ -1002,7 +980,6 @@ __global__ void __launch_bounds__(256) k_big_extend_all(DevSym S, DevNum N, cons
     m = warp_max(m);
     if (lane == 0) N.colmax[c0p + lj] = m;
   }
-  if (tlog) { ts[1] = flog_now(); flog_put(N, 7, p, 0, ts, 2); }
 }
 
 // column maxima of the first panel below its diagonal block (later panels get theirs from k_big_update)
@@ -1052,8 +1029,7 @@ __device__ __forceinline__ double fast_rcp(const double d) {
 __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const double tiny,
                             double* __restrict__ As, double* __restrict__ Lraw, int* __restrict__ order, int* __restrict__ pt,
                             double* __restrict__ dinv_s, double* __restrict__ doff_s, const double* __restrict__ gext_s,
-                            int* counters, unsigned long long* prof = nullptr /* debug: [0] fast steps<<40|cycles, [1] other steps<<40|cycles */) {
-  unsigned long long pf_fast = 0, pf_slow = 0; long long pf_t0 = 0; bool pf_pending = false;
+                            int* counters) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   unsigned cand = (f >= 32) ? 0xffffffffu : ((1u << f) - 1u);
   unsigned parked = 0;
@@ -1093,11 +1069,6 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
       avail = cand;
     }
     const int g0 = __ffs(avail) - 1;
-    if (prof) {
-      const long long now = clock64();
-      if (pf_pending) pf_slow += (1ull << 40) + (unsigned long long)(now - pf_t0);
-      pf_t0 = now; pf_pending = true;
-    }
     __syncthreads();                                   // the previous step's column stores are visible
     const double* __restrict__ cA = As + g0 * 33;
     // everything a 1x1 pivot on g0 needs is loaded (and its reciprocal started) before the search
@@ -1117,7 +1088,6 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
     const float gam_up = __double2float_ru(gam), lam_up = fmaxf(lamf, 0.0f);
     if (!forced && ajj_dn > tiny_up && ajj_dn >= __fmul_ru(u_up, fmaxf(lam_up, gam_up)) && ajj_dn >= __fmul_ru(alpha_up, lam_up)) {
       apply1(a0, pa0, rinv0, g0, pr0);                 // proven: |pivot| > tiny, >= u * column max, >= alpha * lam
-      if (prof) { pf_fast += (1ull << 40) + (unsigned long long)(clock64() - pf_t0); pf_pending = false; }
       continue;
     }
     int r = -1;
@@ -1210,10 +1180,6 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
     }
     parked |= 1u << g0;                                // nothing acceptable now: retry after the other candidates
   }
-  if (prof) {
-    if (pf_pending) pf_slow += (1ull << 40) + (unsigned long long)(clock64() - pf_t0);
-    prof[0] = pf_fast; prof[1] = pf_slow;
-  }
   if (w == 0) {
     if (lane < f) { order[lane] = my_order; pt[lane] = my_pt; dinv_s[lane] = my_dinv; doff_s[lane] = my_doff; }
     if (lane == 0) {
@@ -1298,9 +1264,6 @@ __device__ void chain_role(const DevSym& S, const DevNum& N, const int s, const 
   double* __restrict__ P = N.L + S.L_off[s];
   double* __restrict__ Wp = N.W + S.L_off[s];
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  unsigned long long ts[8];
-  const bool tlog = N.flog != nullptr && tid == 0;
-  if (tlog) ts[0] = flog_now();
   // ---- all global loads in flight at once (asynchronous copies straight into the tiles, zero-filled where masked) ----
 #pragma unroll
   for (int e8 = 0; e8 < 8; ++e8) {
@@ -1331,14 +1294,12 @@ __device__ void chain_role(const DevSym& S, const DevNum& N, const int s, const 
   const double gext = (lane < nbn) ? N.colmax[c0 + o + lane] : 0.0;
   asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncthreads();
-  if (tlog) ts[1] = flog_now();
   if (has_pp) {
     // B. panel p-1's update of the two tiles (independent of each other: no barrier in between)
     chain_tile_update<false>(A1, Lr, WrP);
     chain_tile_update<true>(A2, Lr, WrN);
     __syncthreads();
   }
-  if (tlog) ts[2] = flog_now();
   if (has_p) {
     // C. rows of the new block at panel p: X = A_perm L_bb^-T (= L D), L = X D^-1.  Warp w solves rows 8w..8w+7; lane q
     // holds entry q of each row and row q of L_bb, the pivot entry x[t] travels by shuffle (31 steps of 8 independent
@@ -1386,7 +1347,6 @@ __device__ void chain_role(const DevSym& S, const DevNum& N, const int s, const 
     __syncthreads();
   }
   // D. pivoted LDL^T of the new diagonal block
-  if (tlog) ts[3] = flog_now();
   double a[8];
 #pragma unroll
   for (int q = 0; q < 8; ++q) { const int c = 8 * w + q; a[q] = (c <= lane) ? A2[lane * 33 + c] : A2[c * 33 + lane]; }
@@ -1394,9 +1354,7 @@ __device__ void chain_role(const DevSym& S, const DevNum& N, const int s, const 
   __syncthreads();   // A2 becomes the full symmetric working copy of cta_ldlt32s: A2[c * 33 + i] = A[i][c]
 #pragma unroll
   for (int q = 0; q < 8; ++q) A2[(8 * w + q) * 33 + lane] = a[q];
-  __shared__ unsigned long long prof_s[2];
-  cta_ldlt32s(a, nbn, N.u, N.tiny, A2, Ln, order, pt, dinv_s, doff_s, gext_s, N.counters, tlog ? prof_s : nullptr);
-  if (tlog) ts[4] = flog_now();
+  cta_ldlt32s(a, nbn, N.u, N.tiny, A2, Ln, order, pt, dinv_s, doff_s, gext_s, N.counters);
   const int mine = (lane < nbn) ? order[lane] : 0;
 #pragma unroll
   for (int q = 0; q < 8; ++q) {
@@ -1416,7 +1374,6 @@ __device__ void chain_role(const DevSym& S, const DevNum& N, const int s, const 
     N.doff[c0 + o + lane] = doff_s[lane];
     N.ptype[c0 + o + lane] = pt[lane];
   }
-  if (tlog) { ts[5] = flog_now(); ts[6] = prof_s[0]; ts[7] = prof_s[1]; flog_put(N, 1, s, jbp, ts, 8); }
 }
 
 // --------------------------------------------------------------------------------------------
@@ -1484,9 +1441,6 @@ __global__ void __launch_bounds__(128) k_big_panel(DevSym S, DevNum N, const int
   const bool active = i < f;
   const bool has_q = jb >= NB;                 // there is a panel p-1 whose update this kernel applies
   const int jbq = jb - NB;
-  unsigned long long ts[2];
-  const bool tlog = N.flog != nullptr && tid == 0 && (bx == 0 || (long long)(bx + 1) * blockDim.x >= f - row0 - nxt);
-  if (tlog) ts[0] = flog_now();
   // issue all global loads up front: the diagonal block, its D, the W rows of this block at panel p-1 (permuted), and this
   // thread's rows (panel p-1: L; panel p: A, columns in pivot order)
   if (tid < NB) {
@@ -1580,7 +1534,6 @@ __global__ void __launch_bounds__(128) k_big_panel(DevSym S, DevNum N, const int
       if (t < nb) { Wp[i + (size_t)(jb + t) * f] = x[t]; P[i + (size_t)(jb + t) * f] = l[t]; }
   }
   if (active && lmax > lim) atomicAdd(N.counters + CNT_GROWTH, 1);
-  if (tlog) { ts[1] = flog_now(); flog_put(N, 2, s, jb, ts, 2); }
 }
 
 #define TM 64
@@ -1603,9 +1556,6 @@ __global__ void __launch_bounds__(256) k_big_update(DevSym S, DevNum N, const in
   const int M = f - o, Nk = k - o;            // rows below; remaining pivot columns
   const int i0 = blockIdx.x * TM, j0 = blockIdx.y * TM;
   if (i0 >= M || j0 >= Nk || i0 + TM - 1 < j0) return;
-  unsigned long long ts[2];
-  const bool tlog = N.flog != nullptr && threadIdx.x == 0 && j0 == 0 && (i0 == 0 || i0 + TM >= M);
-  if (tlog) ts[0] = flog_now();
   const long long ld = f;
   double* __restrict__ C = N.L + S.L_off[s] + o + (long long)o * ld;
   const double* __restrict__ A = N.L + S.L_off[s] + o + (long long)jb * ld;
@@ -1670,7 +1620,6 @@ __global__ void __launch_bounds__(256) k_big_update(DevSym S, DevNum N, const in
       }
     }
   }
-  if (tlog) { ts[1] = flog_now(); flog_put(N, 3, s, jb, ts, 2); }
 }
 
 // Contribution-block share of a panel's update: CB -= L21[:, panel] * W21[:, panel]^T (rank nb) on the lower 64x64 tiles of
@@ -1692,9 +1641,6 @@ __global__ void __launch_bounds__(256) k_big_update_cb(DevSym S, DevNum N, const
   const double* __restrict__ A = N.L + S.L_off[s] + k + (long long)jb * ld;
   const double* __restrict__ Bm = N.W + S.L_off[s] + k + (long long)jb * ld;
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  unsigned long long ts[2];
-  const bool tlog = N.flog != nullptr && tid == 0 && j0 == 0 && (i0 == 0 || i0 + TM >= r);
-  if (tlog) ts[0] = flog_now();
   {
     double av[8], bv[8];
 #pragma unroll
@@ -1735,7 +1681,6 @@ __global__ void __launch_bounds__(256) k_big_update_cb(DevSym S, DevNum N, const
       const int gi = i0 + tx + 16 * q, gj = j0 + ty + 16 * p;
       if (gi < r && gj < r && gi >= gj) C[gi + (long long)gj * r] = c[q][p];
     }
-  if (tlog) { ts[1] = flog_now(); flog_put(N, 8, s, jb, ts, 2); }
 }
 
 // --------------------------------------------------------------------------------------------
@@ -1752,9 +1697,6 @@ __global__ void __launch_bounds__(128) k_big_schur84(DevSym S, DevNum N, const i
   const long long f = k + r;
   const int i0 = blockIdx.x * TM, j0 = blockIdx.y * TM;
   if (i0 >= r || j0 >= r || i0 + TM - 1 < j0) return;
-  unsigned long long ts[2];
-  const bool tlog = N.flog != nullptr && threadIdx.x == 0 && j0 == 0 && (i0 == 0 || i0 + TM >= r);
-  if (tlog) ts[0] = flog_now();
   double* __restrict__ C = N.CB + S.cb_off[s];
   const double* __restrict__ A = N.L + S.L_off[s] + k;
   const double* __restrict__ Bm = N.W + S.L_off[s] + k;
@@ -1801,7 +1743,6 @@ __global__ void __launch_bounds__(128) k_big_schur84(DevSym S, DevNum N, const i
       const int gi = i0 + tx + 8 * q, gj = j0 + ty + 16 * p2;
       if (gi < r && gj < r && gi >= gj) C[gi + (long long)gj * r] -= acc[q][p2];
     }
-  if (tlog) { ts[1] = flog_now(); flog_put(N, 6, s, 0, ts, 2); }
 }
 
 }  // namespace b200

@@ -41,37 +41,6 @@ struct DevNum {
   int* counters;    // CNT_N
   double u;         // pivot threshold
   double tiny;      // zero-pivot threshold (scaled matrix)
-  unsigned long long* flog;   // debug (B200_FACTOR_TIMELINE): [0] = next record, [1] = capacity, then 12 words per record
-};
-
-// ---- debug timeline of the factorisation: %globaltimer stamps written by the first / last CTA of a launch ----
-#define FLOG_WORDS 12
-__device__ __forceinline__ unsigned long long flog_now() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-__device__ __forceinline__ void flog_put(const DevNum& N, int kind, int s, int jb, const unsigned long long* ts, int nts) {
-  const unsigned long long slot = atomicAdd(N.flog, 1ull);
-  if (slot >= N.flog[1]) return;
-  unsigned long long* r = N.flog + 2 + slot * FLOG_WORDS;
-  r[0] = (unsigned long long)kind; r[1] = (unsigned long long)(long long)s; r[2] = (unsigned long long)(long long)jb; r[3] = (unsigned long long)nts;
-  for (int i = 0; i < nts && i < FLOG_WORDS - 4; ++i) r[4 + i] = ts[i];
-}
-// start/end of the first and the last CTA of a grid (kernels that are not on the chain)
-struct FlogScope {
-  const DevNum& N; int kind, s, jb; unsigned long long t0; bool on;
-  __device__ __forceinline__ FlogScope(const DevNum& N_, int kind_, int s_, int jb_) : N(N_), kind(kind_), s(s_), jb(jb_), t0(0), on(false) {
-    if (N.flog && threadIdx.x == 0) {
-      const unsigned long long nb = (unsigned long long)gridDim.x * gridDim.y * gridDim.z;
-      const unsigned long long b = blockIdx.x + (unsigned long long)gridDim.x * (blockIdx.y + (unsigned long long)gridDim.y * blockIdx.z);
-      on = (b == 0 || b == nb - 1);
-      if (on) t0 = flog_now();
-    }
-  }
-  __device__ __forceinline__ void done() {
-    if (on) { unsigned long long ts[2] = {t0, flog_now()}; flog_put(N, kind, s, jb, ts, 2); }
-  }
 };
 
 }  // namespace b200

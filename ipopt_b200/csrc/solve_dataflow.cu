@@ -101,7 +101,6 @@ struct DevSolve {
   const int2* subpair;         // work items of the subtree phase: (u0, u1) two subtrees walked side by side by the two halves
   int npair;                   //   of a CTA (their layouts fit the dynamic shared memory together), or (u0, -1) one subtree by the whole CTA
   int upper_max;               // fronts up to this order carry L11^T in the upper triangle of their pivot block
-  unsigned long long* tlog;    // optional (debug): 2 timestamps per top task, fwd then bwd; nullptr = off
 };
 
 __device__ __forceinline__ int ld_acquire(const int* p) {
@@ -946,7 +945,6 @@ __global__ void __launch_bounds__(64) k_linv_diag(DevSym S, DevNum N, const int*
   const int r0 = b * 64, nd = min(64, k - r0);
   const double* __restrict__ P = N.L + S.L_off[s];
   const int tid = threadIdx.x;
-  FlogScope fs(N, 10, s, b);
   for (int t = tid; t < 64 * 64; t += 64) {
     const int i = t & 63, q = t >> 6;
     Ls[i + q * LI_LD] = (i < nd && q < nd && i > q) ? P[(r0 + i) + (size_t)(r0 + q) * f] : 0.0;
@@ -977,7 +975,6 @@ __global__ void __launch_bounds__(64) k_linv_diag(DevSym S, DevNum N, const int*
     const int i = t & 63, q = t >> 6;
     E[i + (long long)q * K64] = Ls[i + q * LI_LD];
   }
-  fs.done();
 }
 
 // 64x64 tile per CTA of 128 threads, 8x4 register blocking (rows tx+8q, columns ty+16p), k-slabs of 16 prefetched
@@ -991,7 +988,6 @@ __global__ void __launch_bounds__(128) k_linv_gemm(DevSym S, DevNum N, const Lin
   __shared__ int s_last;
   const LinvItem it = items[blockIdx.x];
   const int s = it.s;
-  FlogScope fs(N, 10 + PHASE, s, it.ib);
   const int k = S.sn_start[s + 1] - S.sn_start[s];
   const long long f = k + (S.rows_ptr[s + 1] - S.rows_ptr[s]);
   const long long K64 = (long long)((k + 63) / 64) * 64;
@@ -1056,7 +1052,7 @@ __global__ void __launch_bounds__(128) k_linv_gemm(DevSym S, DevNum N, const Lin
     __syncthreads();
     if (tid == 0) s_last = (atomicAdd(part_cnt + it.slot, 1) == it.nch - 1) ? 1 : 0;
     __syncthreads();
-    if (!s_last) { fs.done(); return; }
+    if (!s_last) return;
     __threadfence();
     if (tid == 0) part_cnt[it.slot] = 0;          // ready for the next factorisation
     const double* __restrict__ base = part + (size_t)it.slot * 4096;
@@ -1077,7 +1073,6 @@ __global__ void __launch_bounds__(128) k_linv_gemm(DevSym S, DevNum N, const Lin
       if (PHASE == 1) { if (row < k && col < k) Wp[row + col * f] = acc[q][p]; }
       else Li[row + col * K64] = -acc[q][p];
     }
-  fs.done();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1104,8 +1099,6 @@ __device__ void solve_subtree(const DevSym& S, const DevNum& N, const DevSolve& 
                               unsigned long long* mbar, unsigned mphase, double* __restrict__ x, double* __restrict__ cbv,
                               const Team tm) {
   const int tid = tm.tid, warp = tid >> 5, NT = tm.nt;
-  unsigned long long t_a = 0, t_b = 0;
-  if (V.tlog && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_a));
   const SubDesc sd = V.subs[u];
   const int s0 = sd.s0, sR = sd.sR, nfront = sR - s0 + 1, nlv = sd.nlv;
   const int col0 = sd.col0, ncol = sd.ncol, nrt = sd.nrt, rroot = sd.rroot, ch00 = sd.ch00, nchi = sd.nchi;
@@ -1182,7 +1175,6 @@ __device__ void solve_subtree(const DevSym& S, const DevNum& N, const DevSolve& 
   io.gfd = V.fdesc; io.gcbv = cbv; io.grel = S.rel; io.grows = S.rows; io.gx = x;
   team_sync(tm);
   mbar_wait(mbar, mphase);
-  if (V.tlog && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_b));
   const int* lvl = meta;              // nlv + 1 offsets into the front list
   const int* nsm = meta + nlv + 1;    // nlv
   const int* fl = meta + 2 * nlv + 1; // nfront ids
@@ -1212,12 +1204,6 @@ __device__ void solve_subtree(const DevSym& S, const DevNum& N, const DevSolve& 
   }
   team_sync(tm);
   if (FWD && tid == 0) st_release(V.done_f + sR, epoch);
-  if (V.tlog && tid == 0) {   // debug: 4 records per subtree after the task records
-    unsigned long long t_c;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_c));
-    unsigned long long* rec = V.tlog + 2 * ((unsigned long long)V.ntasks_fwd + V.ntasks_bwd) + 4 * ((FWD ? 0 : (unsigned long long)V.nsub) + u);
-    rec[0] = t_a; rec[1] = t_b; rec[2] = t_c; rec[3] = ((unsigned long long)nfront << 32) | (unsigned)nlv;
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1270,8 +1256,8 @@ __device__ __forceinline__ void global_io(FrontIO& io, const DevSym& S, const De
 // ONE persistent kernel per sweep.  Work items are taken with an atomic ticket: forward = subtrees (largest first), then
 // the top tasks by level; backward = top tasks (levels descending), then the subtrees.  MULTI: (item, column) tickets over
 // M.nb columns.  Otherwise the ticket is the item and the column a compile-time 0 (no per-ticket division, the column view
-// is the identity), and the top tasks are recorded in V.tlog when it is set.  APPLY_D = false (forward only): the L
-// solve alone -- the pivot rows keep the values the fused sweep has before D^-1, in x (bigv for the big fronts).
+// is the identity).  APPLY_D = false (forward only): the L solve alone -- the pivot rows keep the values the fused sweep
+// has before D^-1, in x (bigv for the big fronts).
 // ------------------------------------------------------------------------------------------------
 template <bool FWD, bool MULTI, bool APPLY_D = true>
 __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, DevSolve V, MultiStride M, int epoch,
@@ -1323,8 +1309,6 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
     const SolveTask T = tasks[ti];
     FrontIO io;
     global_io(io, S, N, Vc, xc, cbvc);
-    unsigned long long t_start = 0;
-    if (!MULTI && V.tlog && threadIdx.x == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
     if (T.type == ST_SMALL) {
       const int w = threadIdx.x >> 5;
       if (w < T.blk) {
@@ -1361,12 +1345,6 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_solve(DevSym S, DevNum N, Dev
       big_bx(S, N, Vc, T, epoch, sm, &s_flag, xc);
     }
     __syncthreads();
-    if (!MULTI && V.tlog && threadIdx.x == 0) {
-      unsigned long long t_end;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_end));
-      unsigned long long* rec = V.tlog + 2 * ((FWD ? 0 : (unsigned long long)V.ntasks_fwd) + ti);
-      rec[0] = t_start; rec[1] = t_end;
-    }
   }
 }
 

@@ -89,14 +89,6 @@ void sort_entries(int n, std::vector<Ent>& a) {
 int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* vals,
             const AnalyseOptions& opt, Symbolic& S, std::string& err) {
   double t0 = now_s();
-  const bool lap_on = getenv("B200_SYMBOLIC_TIMES") != nullptr;
-  double t_lap = t0;
-  auto lap = [&](const char* what) {
-    if (!lap_on) return;
-    const double t = now_s();
-    fprintf(stderr, "[symbolic] %-28s %8.1f ms\n", what, (t - t_lap) * 1e3);
-    t_lap = t;
-  };
   S = Symbolic();
   S.n = n;
   S.nnz_in = nnz;
@@ -129,7 +121,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
   const int64_t nu = (int64_t)ur.size();
   S.nnz_u = nu;
 
-  lap("1 unique lower pattern");
   // ---- 2. symmetric adjacency (no diagonal) ---------------------------------------------------
   std::vector<int64_t> xadj(n + 1, 0);
   for (int64_t u = 0; u < nu; ++u) if (ur[u] != uc[u]) { xadj[ur[u] + 1]++; xadj[uc[u] + 1]++; }
@@ -146,7 +137,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     }
   }
 
-  lap("2 adjacency");
   // ---- 3. saddle pairing ----------------------------------------------------------------------
   std::vector<int> partner(n, -1);
   std::vector<char> saddle(n, 0);
@@ -218,7 +208,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     }
   }
 
-  lap("3 saddle pairing");
   // ---- 4. compressed graph --------------------------------------------------------------------
   std::vector<int> cnode(n, -1);
   std::vector<int> cfirst, csecond;  // members: primal first, saddle second (or -1)
@@ -257,13 +246,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
       std::vector<int64_t> mp(nc), mip(nc);
       int64_t mopt[40];
       METIS_SetDefaultOptions(mopt);
-      if (const char* e = getenv("B200_METIS_OPTS")) {   // "idx=value,idx=value" (experiments)
-        for (const char* p = e; *p;) {
-          int idx = atoi(p); while (*p && *p != '=') ++p; if (*p) ++p;
-          long val = atol(p); while (*p && *p != ',') ++p; if (*p) ++p;
-          if (idx >= 0 && idx < 40) mopt[idx] = val;
-        }
-      }
       int rc = METIS_NodeND(&nv, cx.data(), cadj.data(), vw.data(), mopt, mp.data(), mip.data());
       if (rc != 1) { err = "METIS_NodeND failed"; return -3; }
       for (int v = 0; v < nc; ++v) cperm[v] = (int)mp[v];  // new position v holds compressed node mp[v]
@@ -335,7 +317,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     }
   }
 
-  lap("4 compressed graph + ordering");
   // ---- 5. etree, postorder, relabel -----------------------------------------------------------
   std::vector<int> parent;
   etree_from_graph(n, xadj, adj, perm, iperm, parent);
@@ -353,7 +334,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
   std::vector<int> chead(n, -1), cnext(n, -1);
   for (int j = n - 1; j >= 0; --j) if (parent[j] >= 0) { cnext[j] = chead[parent[j]]; chead[parent[j]] = j; }
 
-  lap("5 etree/postorder/relabel");
   // ---- 6. column counts (pass 1) --------------------------------------------------------------
   // Skeleton-graph algorithm (Gilbert, Ng, Peyton 1994): entry (i, j), i > j, of the permuted matrix makes j a LEAF of the
   // row subtree of i iff j's first descendant lies beyond every leaf seen so far; every new leaf adds one to the count of j
@@ -412,7 +392,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     for (int j = 0; j < n; ++j) S.nnzL_true += cc[j];
   }
 
-  lap("6 column counts");
   // ---- 7. supernode partition -----------------------------------------------------------------
   std::vector<char> link(n, 0);  // link[j]: j and j+1 share a supernode
   if (n <= opt.dense_n) {
@@ -480,7 +459,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     for (int s = 0; s < nsn; ++s) if (S.sn_parent[s] >= 0) S.child_idx[pos[S.sn_parent[s]]++] = s;
   }
 
-  lap("7 supernode partition");
   // ---- 8. supernodal row structures (pass 2) --------------------------------------------------
   S.rows_ptr.assign(nsn + 1, 0);
   {
@@ -531,7 +509,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     }
   }
 
-  lap("8 row structures");
   // ---- 9. unique entries in final order, assembly maps ----------------------------------------
   {
     std::vector<Ent> k2((size_t)nu);
@@ -576,7 +553,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     for (int64_t e = 0; e < nnz; ++e) S.useg_src[pos[S.t2u[e]]++] = (int)e;
   }
 
-  lap("9 assembly maps");
   // ---- 10. offsets, levels, statistics ---------------------------------------------------------
   S.L_off.assign(nsn + 1, 0);
   S.cb_off.assign(nsn + 1, 0);
@@ -614,7 +590,6 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
 
   S.perm = perm;
   S.iperm = iperm;
-  lap("10 offsets/levels/stats");
   S.t_symbolic = now_s() - t0 - S.t_order;
   return 0;
 }
