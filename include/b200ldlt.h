@@ -122,6 +122,29 @@ int b200ldlt_solve_partial_device(b200ldlt_handle h, int job, int nrhs, double* 
  * 2 (first of a 2x2), 3 (second of a 2x2); dinv2[2p] = diagonal entry of D^-1, dinv2[2p+1] = off-diagonal entry
  * (p, p+1) of D^-1 when p opens a 2x2 pivot, else 0.  D^-1 is that of the scaled matrix S A S. */
 int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, double* dinv2);
+/* Sparse forward solve (cf. HSL_MA97 ma97_sparse_fwd_solve): job 1 for a right-hand side b with few non-zeros, at a cost
+ * that follows the non-zeros instead of the whole elimination tree.  bindex[0..nbi) are the distinct 0-based original
+ * variables where b is non-zero, b[i] the value at bindex[i] (compact: nbi values).  The non-zeros of L^-1 P^T S b lie in
+ * the REACH: the fronts on the tree paths from the fronts of those variables to the root.  On return *nxi is the number
+ * of pivot positions of the reach, xindex[0..nxi) those positions in ascending order (position p belongs to front s when
+ * sn_start[s] <= p < sn_start[s+1]) and x[i] the entry of job 1's vector at xindex[i]; every entry of job 1's vector
+ * outside xindex is zero.  The forward sweep runs job 1's own front routines over the lists of the full solve pruned to
+ * the fronts of the reach (and the fronts that share a work item with one), so x[i] equals job 1 on the dense b at
+ * that position as a value (they may differ in the sign of a zero), and repeated calls give the same bits.
+ * Device entry point: only the values are device memory -- d_b (nbi doubles) and d_x (room for n doubles); bindex,
+ * nxi and xindex are host memory in both entry points (the pruned work lists are built on the host from the pattern).
+ * Kernel launches (info.launches_solve): 2 + d + t, where d is the number of the B200_SOLVE_DIRECT bottom tree levels
+ * that hold a front of the reach solved by the direct kernel, and t = 1 when the reach has a front above those levels
+ * (always, unless the whole tree is made of direct fronts), else 0; nbi = 0 makes none.  info.ms_solve_gpu is the call's
+ * device time (host entry point: with its copies).  The first call after an analysis builds per-front indices into the
+ * solve's work lists, and pinned and device staging for the pruned lists (about 28 bytes per variable plus 40 per
+ * forward top task each), before its timing starts; a handle that never makes the call allocates none of it.
+ * FATAL_ERROR (message in last_error), with nothing written to nxi, xindex or x, for nbi < 0 or nbi > n, a NULL pointer
+ * with nbi > 0, an index out of range or repeated, without factors (also after SINGULAR) and on a sharded handle.
+ * nbi = 0 succeeds with *nxi = 0. */
+int b200ldlt_sparse_fwd_solve(b200ldlt_handle h, int nbi, const int* bindex, const double* b, int* nxi, int* xindex, double* x);
+int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bindex, const double* d_b, int* nxi, int* xindex,
+                                     double* d_x);
 
 /* ---- multiplication by the factors and alteration of D (cf. HSL_MA97 ma97_lmultiply / ma97_alter) --------------------
  * Same conventions as the partial solves (S A S = P L D L^T P^T, vectors in pivot order indexed by pivot position p):
@@ -167,7 +190,8 @@ int b200ldlt_set_pivtol(b200ldlt_handle h, double pivtol, double pivtolmax);
 int b200ldlt_get_info(b200ldlt_handle h, b200ldlt_info* info);
 /* Copy a named array of the symbolic analysis ("perm","sn_start","sn_parent","rows_ptr","rows","rel",
  * "L_off","cb_off","u_dst64","uent_ptr","t2u","sn_level","level_ptr","level_sn") as int64 into out (cap entries).
- * Returns the array length, or -1 for an unknown name. Runs the lazy analysis (pattern only) if needed. */
+ * Returns the array length, or -1 for an unknown name. Runs the lazy analysis (pattern only) if needed.
+ * "sparse_run_set": the fronts the last b200ldlt_sparse_fwd_solve swept, ascending (empty before the first one). */
 int64_t b200ldlt_symbolic_array(b200ldlt_handle h, const char* name, int64_t* out, int64_t cap);
 /* Force the symbolic phase now; vals may be NULL (no saddle pairing then). */
 int b200ldlt_analyse_now(b200ldlt_handle h, const double* vals);

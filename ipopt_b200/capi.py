@@ -57,7 +57,8 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_residual", "b200ldlt_set_pivtol",
             "b200ldlt_assemble_augsys_device", "b200ldlt_solve_refine_device",
             "b200ldlt_solve_partial", "b200ldlt_solve_partial_device", "b200ldlt_enquire_indef",
-            "b200ldlt_lmultiply", "b200ldlt_lmultiply_device", "b200ldlt_alter_d"]
+            "b200ldlt_lmultiply", "b200ldlt_lmultiply_device", "b200ldlt_alter_d",
+            "b200ldlt_sparse_fwd_solve", "b200ldlt_sparse_fwd_solve_device"]
 
 _lib = None
 
@@ -98,6 +99,8 @@ def load_library():
     L.b200ldlt_lmultiply.argtypes = [vp, C.c_int, C.c_int, dp, dp]
     L.b200ldlt_lmultiply_device.argtypes = [vp, C.c_int, C.c_int, vp, vp]
     L.b200ldlt_alter_d.argtypes = [vp, dp]
+    L.b200ldlt_sparse_fwd_solve.argtypes = [vp, C.c_int, ip, dp, ip, ip, dp]
+    L.b200ldlt_sparse_fwd_solve_device.argtypes = [vp, C.c_int, ip, vp, ip, ip, vp]
     L.b200ldlt_num_neg.argtypes = [vp]
     L.b200ldlt_increase_quality.argtypes = [vp]
     L.b200ldlt_get_info.argtypes = [vp, C.POINTER(Info)]
@@ -284,6 +287,31 @@ class B200Ldlt:
         d = np.ascontiguousarray(dinv, dtype=np.float64)
         assert d.size == 2 * self.dim
         return self._L.b200ldlt_alter_d(self._h, _dptr(d))
+
+    def sparse_fwd_solve(self, bindex, b):
+        """Job 1 (L^-1 P^T S b, pivot order) of a sparse b: bindex the distinct 0-based variables where b is non-zero, b
+        their values.  Returns (xindex, x): the pivot positions of the fronts b reaches, ascending, and job 1's vector
+        there (zero everywhere else).  Raises on a refusal."""
+        bi = np.ascontiguousarray(bindex, dtype=np.int32)
+        bv = np.ascontiguousarray(b, dtype=np.float64)
+        assert bv.shape == bi.shape
+        nxi = C.c_int(0)
+        xi, x = np.zeros(max(self.dim, 1), np.int32), np.zeros(max(self.dim, 1), np.float64)
+        if self._L.b200ldlt_sparse_fwd_solve(self._h, len(bi), _iptr(bi), _dptr(bv), C.byref(nxi), _iptr(xi),
+                                             _dptr(x)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return xi[:nxi.value].copy(), x[:nxi.value].copy()
+
+    def sparse_fwd_solve_device(self, bindex, d_b_ptr, d_x_ptr):
+        """The same with the values in device memory: d_b holds len(bindex) doubles, d_x receives the nxi values (room for
+        dim doubles).  Returns xindex; raises on a refusal."""
+        bi = np.ascontiguousarray(bindex, dtype=np.int32)
+        nxi = C.c_int(0)
+        xi = np.zeros(max(self.dim, 1), np.int32)
+        if self._L.b200ldlt_sparse_fwd_solve_device(self._h, len(bi), _iptr(bi), C.c_void_p(d_b_ptr), C.byref(nxi),
+                                                    _iptr(xi), C.c_void_p(d_x_ptr)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return xi[:nxi.value].copy()
 
     def device_ptr(self, name):
         """Device address of a named array of the handle (b200ldlt_device_ptr: "scale", "x", "cbv", ...), 0 if none."""

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -93,6 +94,34 @@ struct LmulPlan {
   DevBuf<double> d_scr;
   long long ld = 0;
   int width = 0;
+};
+
+// The sparse forward solve (b200ldlt_sparse_fwd_solve): host copies of the full plan's forward lists with per-front
+// indices into them, the marks of one call, and the staging of the pruned lists (pinned -> device, sized by the full
+// plan).  Built at the first sparse call after an analysis, before that call's timing starts; a handle that never makes
+// one allocates none of it.
+struct SparseFwdPlan {
+  std::vector<SolveTask> tf;                   // splan's forward top tasks, subtree items, bundles, direct-level lists
+  std::vector<int2> pairs;
+  std::vector<int> bundle;
+  std::vector<std::vector<int>> direct;
+  std::vector<int> dlev, didx;                 // by front: its direct level and index there, or -1
+  std::vector<int> item_of, sub_of;            // by front: the subtree item / the subtree that walks it, or -1
+  std::vector<int> task_ptr, task_idx;         // by front (CSR): its forward top tasks, ascending
+  std::vector<int> item_ptr, item_fr;          // by subtree item (CSR): the fronts its subtrees walk
+  std::vector<int> iperm, sn_of;               // variable -> permuted column; position -> front
+  std::vector<int> pos_bi;                     // position -> index into the compact b during a call, else -1
+  std::vector<unsigned> m_reach, m_run, m_fr, m_item, m_task;   // marks of the current call (== stamp)
+  std::vector<int> ord0, ord1;                 // per call: first / last slot of a run front in the pruned order
+  std::vector<int> last_run;                   // the run set of the last call, ascending (symbolic_array "sparse_run_set")
+  unsigned stamp = 0;
+  char* h_buf = nullptr;                       // pinned staging, the layout of d_buf up to the output slice
+  DevBuf<char> d_buf;
+  cudaEvent_t ev_staged = nullptr;             // the last copy out of h_buf
+  ~SparseFwdPlan() {
+    if (h_buf) cudaFreeHost(h_buf);
+    if (ev_staged) cudaEventDestroy(ev_staged);
+  }
 };
 
 struct LevelPlan {
@@ -196,6 +225,7 @@ struct Solver {
   DevBuf<long long> d_bigv_off;
   DevBuf<long long> d_piv_big;      // n : per pivot position, its index in bigv (pivots of big fronts) or -1 (partial solves)
   std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call after an analysis
+  std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve: built at its first call after an analysis
   DevBuf<double> d_alter;           // alter_d: the caller's 2n entries of D^-1 (allocated at the first call)
   DevBuf<int> d_alter_bad;
   DevBuf<double> d_linv;
@@ -747,6 +777,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   sv->rhs_cap = 0;
   sv->blk.reset();
   sv->lmul.reset();
+  sv->sfs.reset();
   if (sv->fgraph_exec) { cudaGraphExecDestroy(sv->fgraph_exec); sv->fgraph_exec = nullptr; }
   if (sv->fgraph) { cudaGraphDestroy(sv->fgraph); sv->fgraph = nullptr; }
   AnalyseOptions ao;
@@ -1240,16 +1271,25 @@ static DevSolve sweep_view(const Solver* sv, const SolvePlan& SP, const SweepSta
   return V;
 }
 
+// subsequences of a plan's forward lists, in their order, on the device (the sparse forward solve)
+struct PrunedLists {
+  const SolveTask* tf; int ntf;
+  const int2* subpair; int npair;
+  const int* direct; std::vector<int> direct_off, direct_cnt;   // direct level l: direct_cnt[l] fronts at direct + direct_off[l]
+};
+
 // one sweep of nb columns (nb <= W.width) over the fronts of a plan: the bottom levels one launch each, and ONE persistent
 // kernel (forward: bottom levels, then subtrees, then top tasks; backward: the reverse).  apply_d = false: a forward
-// sweep that leaves D^-1 out (partial solves)
-static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, bool fwd, bool apply_d = true) {
+// sweep that leaves D^-1 out (partial solves).  pruned (forward only): the sweep takes those lists instead of SP's
+static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, bool fwd, bool apply_d = true,
+                        const PrunedLists* pruned = nullptr) {
   cudaStream_t st = sv->stream;
-  const DevSolve V = sweep_view(sv, SP, W);
+  DevSolve V = sweep_view(sv, SP, W);
+  if (pruned) { V.tasks = pruned->tf; V.ntasks_fwd = pruned->ntf; V.subpair = pruned->subpair; V.npair = pruned->npair; }
   MultiStride M = W.M;
   M.nb = nb;
   const bool multi = nb > 1;
-  const long long nt = ((long long)(fwd ? SP.ntf : SP.ntb) + SP.npair) * nb;
+  const long long nt = ((long long)(fwd ? V.ntasks_fwd : V.ntasks_bwd) + V.npair) * nb;
   const int grid = (int)std::min<long long>(W.grid, nt);
   const int nd = (int)SP.direct_cnt.size();
   const auto k_direct = (fwd && !apply_d) ? (multi ? k_solve_direct<true, true, false> : k_solve_direct<true, false, false>)
@@ -1257,9 +1297,11 @@ static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, 
                               : (multi ? k_solve_direct<false, true> : k_solve_direct<false, false>);
   const auto k_sweep = sweep_kernel(fwd, multi, apply_d);
   auto direct = [&](int l) {
-    if (SP.direct_cnt[l] <= 0) return;
-    const unsigned g = cdiv(SP.direct_cnt[l] * nb, DF_THREADS / 32);
-    k_direct<<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, V, M, SP.d_direct[l]->p, SP.direct_cnt[l], sv->solve_epoch, W.d_x.p, W.d_cbv.p);
+    const int cnt = pruned ? pruned->direct_cnt[l] : SP.direct_cnt[l];
+    if (cnt <= 0) return;
+    const int* lst = pruned ? pruned->direct + pruned->direct_off[l] : SP.d_direct[l]->p;
+    const unsigned g = cdiv(cnt * nb, DF_THREADS / 32);
+    k_direct<<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, V, M, lst, cnt, sv->solve_epoch, W.d_x.p, W.d_cbv.p);
     ++sv->launches;
   };
   if (fwd) for (int l = 0; l < nd; ++l) direct(l);
@@ -1473,6 +1515,254 @@ static int enqueue_lmul_columns(Solver* sv, int trans, int nrhs, const double* d
     if (rc != B200LDLT_SUCCESS) return rc;
     c += w;
   }
+  return B200LDLT_SUCCESS;
+}
+
+// ---- sparse forward solve (b200ldlt_sparse_fwd_solve) --------------------------------------------------------------
+// Host copies of splan's forward lists and the per-front indices into them (SparseFwdPlan): at the first sparse call after
+// an analysis, before its timing starts.
+static int sfs_state(Solver* sv) {
+  if (sv->sfs) return B200LDLT_SUCCESS;
+  const Symbolic& S = sv->S;
+  const SolvePlan& SP = sv->splan;
+  const int n = sv->n, nsn = S.nsn;
+  cudaStream_t st = sv->stream;
+  std::unique_ptr<SparseFwdPlan> P(new SparseFwdPlan());
+  std::vector<SubDesc> subs(SP.nsub);
+  std::vector<int> meta(SP.d_sub_meta.n);
+  P->tf.resize(SP.ntf); P->pairs.resize(SP.npair); P->bundle.resize(SP.d_bundle.n);
+  if (SP.ntf) CU(cudaMemcpyAsync(P->tf.data(), SP.d_tf.p, SP.ntf * sizeof(SolveTask), cudaMemcpyDeviceToHost, st));
+  if (SP.npair) CU(cudaMemcpyAsync(P->pairs.data(), SP.d_subpair.p, SP.npair * sizeof(int2), cudaMemcpyDeviceToHost, st));
+  if (SP.nsub) CU(cudaMemcpyAsync(subs.data(), SP.d_subs.p, SP.nsub * sizeof(SubDesc), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(meta.data(), SP.d_sub_meta.p, meta.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(P->bundle.data(), SP.d_bundle.p, P->bundle.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+  P->direct.resize(SP.direct_cnt.size());
+  long long ndirect = 0;
+  for (size_t l = 0; l < SP.direct_cnt.size(); ++l) {
+    P->direct[l].resize(SP.direct_cnt[l]);
+    ndirect += SP.direct_cnt[l];
+    if (SP.direct_cnt[l]) CU(cudaMemcpyAsync(P->direct[l].data(), SP.d_direct[l]->p, SP.direct_cnt[l] * sizeof(int), cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaStreamSynchronize(st));
+  P->dlev.assign(nsn, -1); P->didx.assign(nsn, -1); P->item_of.assign(nsn, -1); P->sub_of.assign(nsn, -1);
+  for (size_t l = 0; l < P->direct.size(); ++l)
+    for (size_t i = 0; i < P->direct[l].size(); ++i) { const int s = P->direct[l][i]; P->dlev[s] = (int)l; P->didx[s] = (int)i; }
+  P->item_ptr.assign(1, 0);
+  for (int i = 0; i < SP.npair; ++i) {
+    for (const int u : {P->pairs[i].x, P->pairs[i].y}) {
+      if (u < 0) continue;
+      const SubDesc& d = subs[u];
+      for (int j = 0; j < d.nown; ++j) {
+        const int s = meta[d.moff + 2 * d.nlv + 1 + j];
+        P->item_fr.push_back(s); P->item_of[s] = i; P->sub_of[s] = u;
+      }
+    }
+    P->item_ptr.push_back((int)P->item_fr.size());
+  }
+  P->task_ptr.assign(nsn + 1, 0);
+  auto each_front = [&](const SolveTask& T, auto&& fn) {
+    if (T.type == ST_SMALL) { for (int w = 0; w < T.blk; ++w) fn(P->bundle[T.s + w]); }
+    else fn(T.s);
+  };
+  for (const SolveTask& T : P->tf) each_front(T, [&](int s) { P->task_ptr[s + 1]++; });
+  for (int s = 0; s < nsn; ++s) P->task_ptr[s + 1] += P->task_ptr[s];
+  P->task_idx.resize(P->task_ptr[nsn]);
+  {
+    std::vector<int> fill(P->task_ptr.begin(), P->task_ptr.end() - 1);
+    for (int j = 0; j < SP.ntf; ++j) each_front(P->tf[j], [&](int s) { P->task_idx[fill[s]++] = j; });
+  }
+  P->iperm.resize(n); P->sn_of.resize(n);
+  for (int i = 0; i < n; ++i) P->iperm[S.perm[i]] = i;
+  for (int s = 0; s < nsn; ++s) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) P->sn_of[p] = s;
+  P->pos_bi.assign(n, -1);
+  P->m_reach.assign(nsn, 0); P->m_run.assign(nsn, 0); P->m_fr.assign(nsn, 0);
+  P->m_item.assign(std::max(SP.npair, 1), 0); P->m_task.assign(std::max(SP.ntf, 1), 0);
+  P->ord0.assign(nsn, 0); P->ord1.assign(nsn, 0);
+  // staging: subtree items, b, top tasks, then the int lists (direct fronts, run-set positions and their b indices,
+  // output positions, frontier), and on the device the output slice
+  const size_t cap = 8 * (size_t)SP.npair + 8 * (size_t)n + sizeof(SolveTask) * (size_t)SP.ntf +
+                     4 * ((size_t)ndirect + 3 * (size_t)n + (size_t)nsn) + 8 * (size_t)n + 64;
+  CU(cudaHostAlloc((void**)&P->h_buf, cap, cudaHostAllocDefault));
+  CU(P->d_buf.alloc(cap));
+  CU(cudaEventCreateWithFlags(&P->ev_staged, cudaEventDisableTiming));
+  sv->sfs = std::move(P);
+  return B200LDLT_SUCCESS;
+}
+
+// one sparse call, as prepared on the host: counts, staging offsets (bytes) and the pruned lists on the device
+struct SfsCall {
+  int ncol = 0, nxi = 0, nfr = 0;
+  size_t o_b = 0, o_pos = 0, o_bi = 0, o_xi = 0, o_fr = 0, o_x = 0, staged = 0;
+  PrunedLists pl{};
+};
+
+static inline size_t align8(size_t b) { return (b + 7) & ~(size_t)7; }
+
+// Host part of a sparse forward solve.  The reach (the fronts on the tree paths from the fronts of b's variables to the
+// root) gives the run set R: the reach, the fronts walked by a subtree item that walks a reached front, and the fronts
+// of a bundle that holds one (items and bundles are kept whole).  The pruned lists take every entry of splan's forward
+// lists that belongs to a front of R, in list order.  F = the children of R outside R.  Before anything is launched, the
+// check that the pruned sweep cannot wait forever: every front of R owns work in the lists -- all of its top tasks, and
+// all chunks of each chunked block (the arrival counters count modulo the chunk count) -- and every child of a front of
+// R is in F or runs EARLIER in the pruned order (the same subtree walk counts: it is walked level by level).  Everything
+// the device needs goes to the pinned staging (b too when b_host).  FATAL_ERROR with a message, nothing written to the
+// caller and nothing launched, for a bad pattern or a failed check.
+static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_host, SfsCall& C) {
+  SparseFwdPlan& P = *sv->sfs;
+  const Symbolic& S = sv->S;
+  const int n = sv->n;
+  const int nd = (int)P.direct.size();
+  const unsigned m = ++P.stamp;
+  for (int i = 0; i < nbi; ++i) {
+    const int v = bindex[i];
+    const char* bad = (v < 0 || v >= n) ? "sparse_fwd_solve: index out of range" : (P.pos_bi[P.iperm[v]] >= 0) ? "sparse_fwd_solve: index appears twice" : nullptr;
+    if (bad) {
+      for (int j = 0; j < i; ++j) P.pos_bi[P.iperm[bindex[j]]] = -1;
+      sv->err = bad;
+      return B200LDLT_FATAL_ERROR;
+    }
+    P.pos_bi[P.iperm[v]] = i;
+  }
+  std::vector<int> reach;
+  for (int i = 0; i < nbi; ++i)
+    for (int s = P.sn_of[P.iperm[bindex[i]]]; s >= 0 && P.m_reach[s] != m; s = S.sn_parent[s]) { P.m_reach[s] = m; reach.push_back(s); }
+  std::sort(reach.begin(), reach.end());
+  std::vector<int> run(reach), items, tasks;
+  for (int s : reach) P.m_run[s] = m;
+  auto add = [&](int s) { if (P.m_run[s] != m) { P.m_run[s] = m; run.push_back(s); } };
+  for (size_t q = 0; q < run.size(); ++q) {
+    const int s = run[q], it = P.item_of[s];
+    if (it >= 0 && P.m_item[it] != m) {
+      P.m_item[it] = m; items.push_back(it);
+      for (int e = P.item_ptr[it]; e < P.item_ptr[it + 1]; ++e) add(P.item_fr[e]);
+    }
+    for (int e = P.task_ptr[s]; e < P.task_ptr[s + 1]; ++e) {
+      const int t = P.task_idx[e];
+      if (P.m_task[t] == m) continue;
+      P.m_task[t] = m; tasks.push_back(t);
+      const SolveTask& T = P.tf[t];
+      if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) add(P.bundle[T.s + w]);
+    }
+  }
+  std::sort(items.begin(), items.end());
+  std::sort(tasks.begin(), tasks.end());
+  std::vector<std::vector<int>> dl(nd);
+  for (int s : run) if (P.dlev[s] >= 0) dl[P.dlev[s]].push_back(P.didx[s]);
+  // staging layout
+  int ndir = 0, nrc = 0, nxi = 0;
+  for (auto& v : dl) { std::sort(v.begin(), v.end()); ndir += (int)v.size(); }
+  for (int s : run) nrc += S.sn_start[s + 1] - S.sn_start[s];
+  for (int s : reach) nxi += S.sn_start[s + 1] - S.sn_start[s];
+  char* h = P.h_buf;
+  const size_t o_tf = align8(8 * items.size()), o_b = o_tf + align8(sizeof(SolveTask) * tasks.size());
+  const size_t o_dir = o_b + align8(b_host ? 8 * (size_t)nbi : 0);
+  C.o_b = o_b; C.o_pos = o_dir + 4 * (size_t)ndir; C.o_bi = C.o_pos + 4 * (size_t)nrc; C.o_xi = C.o_bi + 4 * (size_t)nrc;
+  C.o_fr = C.o_xi + 4 * (size_t)nxi;
+  // (the previous call's copy out of the staging must be complete before it is rewritten)
+  if (cudaEventSynchronize(P.ev_staged) != cudaSuccess) {
+    for (int i = 0; i < nbi; ++i) P.pos_bi[P.iperm[bindex[i]]] = -1;
+    sv->err = "sparse_fwd_solve: staging copy failed";
+    return B200LDLT_FATAL_ERROR;
+  }
+  {
+    int* pos = reinterpret_cast<int*>(h + C.o_pos);
+    int* bi = reinterpret_cast<int*>(h + C.o_bi);
+    int* xi = reinterpret_cast<int*>(h + C.o_xi);
+    int j = 0;
+    for (int s : run) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p, ++j) { pos[j] = p; bi[j] = P.pos_bi[p]; }
+    j = 0;
+    for (int s : reach) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) xi[j++] = p;
+  }
+  for (int i = 0; i < nbi; ++i) P.pos_bi[P.iperm[bindex[i]]] = -1;
+  // pruned order: direct level l -> slot l, subtree item i -> nd + i, top task j -> nd + items + j
+  for (int s : run) { P.ord0[s] = INT_MAX; P.ord1[s] = -1; }
+  for (int l = 0; l < nd; ++l) for (int i : dl[l]) { const int s = P.direct[l][i]; P.ord0[s] = P.ord1[s] = l; }
+  for (size_t i = 0; i < items.size(); ++i)
+    for (int e = P.item_ptr[items[i]]; e < P.item_ptr[items[i] + 1]; ++e) P.ord0[P.item_fr[e]] = P.ord1[P.item_fr[e]] = nd + (int)i;
+  for (size_t j = 0; j < tasks.size(); ++j) {
+    const SolveTask& T = P.tf[tasks[j]];
+    const int o = nd + (int)(items.size() + j);
+    auto upd = [&](int s) { P.ord0[s] = std::min(P.ord0[s], o); P.ord1[s] = std::max(P.ord1[s], o); };
+    if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) upd(P.bundle[T.s + w]);
+    else upd(T.s);
+  }
+  std::vector<int> fr;
+  for (int s : run) {
+    bool ok = P.ord1[s] >= 0;
+    // all top tasks of the front are in the lists, each chunked block with all of its nq chunks, a big front with all
+    // of its FP and FC blocks
+    int nfp = 0, nfc = 0;
+    for (int e = P.task_ptr[s]; ok && e < P.task_ptr[s + 1]; ++e) {
+      const SolveTask& T = P.tf[P.task_idx[e]];
+      ok = P.m_task[P.task_idx[e]] == m;
+      if (ok && (T.type == ST_FP || T.type == ST_FC) && T.q == 0) {
+        ok = e + T.nq <= P.task_ptr[s + 1];
+        for (int q = 1; ok && q < T.nq; ++q) {
+          const SolveTask& U = P.tf[P.task_idx[e + q]];
+          ok = U.type == T.type && U.blk == T.blk && U.cidx == T.cidx && U.q == q && P.m_task[P.task_idx[e + q]] == m;
+        }
+        (T.type == ST_FP ? nfp : nfc) += 1;
+      }
+    }
+    if (ok && S.f(s) > DF_MIDMAX && P.dlev[s] < 0 && P.item_of[s] < 0)
+      ok = nfp == (S.k(s) + DF_BLK - 1) / DF_BLK && nfc == (S.r(s) + DF_BLK - 1) / DF_BLK;
+    for (int e = S.child_ptr[s]; ok && e < S.child_ptr[s + 1]; ++e) {
+      const int c = S.child_idx[e];
+      if (P.m_run[c] == m) ok = (P.sub_of[s] >= 0 && P.sub_of[c] == P.sub_of[s]) || P.ord1[c] < P.ord0[s];
+      else if (P.m_fr[c] != m) { P.m_fr[c] = m; fr.push_back(c); }
+    }
+    if (!ok) {
+      sv->err = "sparse_fwd_solve: the pruned sweep of front " + std::to_string(s) + " fails its dependency check (not launched)";
+      return B200LDLT_FATAL_ERROR;
+    }
+  }
+  P.last_run = run;
+  std::sort(P.last_run.begin(), P.last_run.end());
+  C.ncol = nrc; C.nxi = nxi; C.nfr = (int)fr.size();
+  C.staged = C.o_fr + 4 * fr.size();
+  C.o_x = align8(C.staged);
+  if (C.o_x + 8 * (size_t)n > P.d_buf.n) { sv->err = "sparse_fwd_solve: staging too small"; return B200LDLT_FATAL_ERROR; }
+  int2* hp = reinterpret_cast<int2*>(h);
+  for (size_t i = 0; i < items.size(); ++i) hp[i] = P.pairs[items[i]];
+  SolveTask* ht = reinterpret_cast<SolveTask*>(h + o_tf);
+  for (size_t j = 0; j < tasks.size(); ++j) ht[j] = P.tf[tasks[j]];
+  if (b_host) memcpy(h + o_b, b_host, 8 * (size_t)nbi);
+  int* hd = reinterpret_cast<int*>(h + o_dir);
+  C.pl.direct_off.assign(nd, 0); C.pl.direct_cnt.assign(nd, 0);
+  for (int l = 0, j = 0; l < nd; ++l) {
+    C.pl.direct_off[l] = j; C.pl.direct_cnt[l] = (int)dl[l].size();
+    for (int i : dl[l]) hd[j++] = P.direct[l][i];
+  }
+  std::copy(fr.begin(), fr.end(), reinterpret_cast<int*>(h + C.o_fr));
+  char* d = P.d_buf.p;
+  C.pl.subpair = reinterpret_cast<const int2*>(d); C.pl.npair = (int)items.size();
+  C.pl.tf = reinterpret_cast<const SolveTask*>(d + o_tf); C.pl.ntf = (int)tasks.size();
+  C.pl.direct = reinterpret_cast<const int*>(d + o_dir);
+  return B200LDLT_SUCCESS;
+}
+
+// Device part: the staged lists in, x = P^T S b on the run set and the frontier's update vectors / flags (k_sfs_in), the
+// forward sweep of job 1 over the pruned lists, the reached positions out (k_sfs_out).  Launches: 2 + the direct levels
+// that hold a front of the run set + 1 when the run set has a front outside them.
+static int sfs_enqueue(Solver* sv, const SfsCall& C, const double* d_b, double* d_out) {
+  SparseFwdPlan& P = *sv->sfs;
+  cudaStream_t st = sv->stream;
+  SweepState& W = sv->sweep;
+  const char* d = P.d_buf.p;
+  CU(cudaMemcpyAsync(P.d_buf.p, P.h_buf, C.staged, cudaMemcpyHostToDevice, st));
+  CU(cudaEventRecord(P.ev_staged, st));
+  sv->solve_epoch++;
+  k_sfs_in<<<cdiv(C.ncol, 256) + C.nfr, 256, 0, st>>>(C.ncol, reinterpret_cast<const int*>(d + C.o_pos),
+                                                      reinterpret_cast<const int*>(d + C.o_bi), sv->d_perm.p, sv->d_scale.p, d_b,
+                                                      W.d_x.p, reinterpret_cast<const int*>(d + C.o_fr), sv->d_rows_ptr.p,
+                                                      W.d_cbv.p, W.d_done_f.p, sv->solve_epoch);
+  ++sv->launches;
+  const int rc = launch_sweep(sv, sv->splan, W, 1, true, false, &C.pl);
+  if (rc != B200LDLT_SUCCESS) return rc;
+  k_sfs_out<<<cdiv(C.nxi, 256), 256, 0, st>>>(C.nxi, reinterpret_cast<const int*>(d + C.o_xi), sv->d_piv_big.p, W.d_x.p,
+                                             W.d_bigv.p, d_out);
+  ++sv->launches;
+  CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
 }
 
@@ -1729,6 +2019,38 @@ static bool factors_refused(Solver* sv, const char* what, int trans) {
   else return false;
   return true;
 }
+
+// b200ldlt_sparse_fwd_solve (host == true: b and x in host memory) / _device
+static int sparse_fwd(Solver* sv, int nbi, const int* bindex, const double* b, bool host, int* nxi, int* xindex, double* x) {
+  if (factors_refused(sv, "sparse_fwd_solve", 0)) return B200LDLT_FATAL_ERROR;
+  if (nbi < 0 || nbi > sv->n) { sv->err = "sparse_fwd_solve: nbi must be 0..n"; return B200LDLT_FATAL_ERROR; }
+  if (nbi > 0 && (!bindex || !b || !nxi || !xindex || !x)) { sv->err = "sparse_fwd_solve: NULL argument"; return B200LDLT_FATAL_ERROR; }
+  if (nbi == 0) {
+    if (nxi) *nxi = 0;
+    sv->info.launches_solve = 0;
+    sv->info.ms_solve_gpu = 0.0f;
+    return B200LDLT_SUCCESS;
+  }
+  CU(cudaSetDevice(sv->dev));
+  cudaStream_t st = sv->stream;
+  { const int rc = sfs_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
+  SfsCall C;
+  { const int rc = sfs_prepare(sv, nbi, bindex, host ? b : nullptr, C); if (rc != B200LDLT_SUCCESS) return rc; }
+  SparseFwdPlan& P = *sv->sfs;
+  double* d_x = host ? reinterpret_cast<double*>(P.d_buf.p + C.o_x) : x;
+  sv->launches = 0;
+  CU(cudaEventRecord(sv->ev0, st));
+  { const int rc = sfs_enqueue(sv, C, host ? reinterpret_cast<const double*>(P.d_buf.p + C.o_b) : b, d_x); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (host) CU(cudaMemcpyAsync(P.h_buf + C.o_x, d_x, (size_t)C.nxi * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(sv->ev1, st));
+  CU(cudaStreamSynchronize(st));
+  if (host) memcpy(x, P.h_buf + C.o_x, (size_t)C.nxi * sizeof(double));
+  memcpy(xindex, P.h_buf + C.o_xi, (size_t)C.nxi * sizeof(int));
+  *nxi = C.nxi;
+  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
+  sv->info.launches_solve = sv->launches;
+  return B200LDLT_SUCCESS;
+}
 }  // namespace b200
 
 extern "C" {
@@ -1834,6 +2156,19 @@ int b200ldlt_lmultiply(b200ldlt_handle h, int trans, int nrhs, const double* x, 
   cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
   sv->info.launches_solve = sv->launches;
   return B200LDLT_SUCCESS;
+}
+
+int b200ldlt_sparse_fwd_solve(b200ldlt_handle h, int nbi, const int* bindex, const double* b, int* nxi, int* xindex, double* x) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return sparse_fwd(sv, nbi, bindex, b, true, nxi, xindex, x);
+}
+
+int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bindex, const double* d_b, int* nxi, int* xindex,
+                                     double* d_x) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return sparse_fwd(sv, nbi, bindex, d_b, false, nxi, xindex, d_x);
 }
 
 int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2) {
@@ -2119,6 +2454,7 @@ int64_t b200ldlt_symbolic_array(b200ldlt_handle h, const char* name, int64_t* ou
   if (nm == "sn_level") RET(S.sn_level);
   if (nm == "level_ptr") RET(S.level_ptr);
   if (nm == "level_sn") RET(S.level_sn);
+  if (nm == "sparse_run_set") { static const std::vector<int> none; RET(sv->sfs ? sv->sfs->last_run : none); }
 #undef RET
   return -1;
 }

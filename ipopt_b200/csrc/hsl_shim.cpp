@@ -18,12 +18,13 @@
 //   scale[]                of ma97_factor_d / ma97_factor_solve_d: the equilibration factors of that factorisation;
 //   ma97_lmultiply_d       multiplication by S^-1 P L or its transpose (b200ldlt_lmultiply), hsl_ma97d.h:169-171;
 //   ma97_alter_d           writes D^-1 back in the layout ma97_enquire_indef_d returns (b200ldlt_alter_d);
-//   ma97_enquire_posdef_d  the diagonal of the Cholesky factor L D^1/2 when every pivot is a positive 1x1 pivot.
+//   ma97_enquire_posdef_d  the diagonal of the Cholesky factor L D^1/2 when every pivot is a positive 1x1 pivot;
+//   ma97_sparse_fwd_solve_d  job 1 of a sparse right-hand side, swept over the fronts it reaches only
+//                          (b200ldlt_sparse_fwd_solve), declared at hsl_ma97d.h:173-176.
 // Not provided: ma97_solve_fredholm_d (it needs the factors of a singular matrix, and the backend keeps none after
-// SINGULAR), ma97_sparse_fwd_solve_d (it needs a sweep pruned to the rows a sparse right-hand side reaches) and the
-// 64-bit variants.
-// The conventions of the inspection calls (enquire_indef / enquire_posdef / alter / lmultiply) are our reading of the
-// reference header; they have not been checked against the HSL user documentation.
+// SINGULAR) and the 64-bit variants.
+// The conventions of the inspection calls (enquire_indef / enquire_posdef / alter / lmultiply / sparse_fwd_solve) are our
+// reading of the reference header; they have not been checked against the HSL user documentation.
 #include <cuda_runtime_api.h>
 
 #include <cmath>
@@ -285,6 +286,38 @@ void ma97_enquire_posdef_d(void** akeep, void** fkeep, const ma97_control_d* con
     if (ty[p] != 1 || !(dinv2[2 * (size_t)p] > 0.0)) { fill_info(K, info); info->flag = -1; return; }
   for (int p = 0; p < K->n; ++p) d[p] = std::sqrt(1.0 / dinv2[2 * (size_t)p]);
   fill_info(K, info);
+  info->flag = 0;
+}
+
+// x = L^-1 P^T S b (job 1, pivot order) for a sparse b.  Our reading of the convention: b is a dense n-vector indexed by
+// variable, its entries b[bindex[i]]; x is a dense n-vector in pivot order, written whole (the solve at xindex[0..*nxi),
+// zeros elsewhere); bindex / xindex are 0- or 1-based as control->f_arrays says (as for ma97_analyse_d); order is ignored
+// (the shim's analyse takes no user ordering).  flag -1, with nothing written, for the refusals of
+// b200ldlt_sparse_fwd_solve (an index out of range or repeated, no factors).  Not checked against the HSL documentation.
+void ma97_sparse_fwd_solve_d(int nbi, const int bindex[], const double b[], const int order[], int* nxi, int xindex[],
+                             double x[], void** akeep, void** fkeep, const ma97_control_d* control, ma97_info_d* info) {
+  (void)fkeep; (void)order;
+  memset(info, 0, sizeof(*info));
+  Keep* K = akeep ? (Keep*)*akeep : nullptr;
+  if (!K || !K->h || !K->factored || nbi < 0 || nbi > K->n || !nxi || !xindex || !x || (nbi > 0 && (!bindex || !b))) {
+    info->flag = -1;
+    return;
+  }
+  const int base = control && control->f_arrays ? 1 : 0;
+  std::vector<int> bi(nbi), xi(K->n);
+  std::vector<double> bv(nbi), xv(K->n);
+  for (int i = 0; i < nbi; ++i) {
+    bi[i] = bindex[i] - base;
+    if (bi[i] < 0 || bi[i] >= K->n) { info->flag = -1; return; }
+    bv[i] = b[bi[i]];
+  }
+  int nx = 0;
+  const int st = b200ldlt_sparse_fwd_solve(K->h, nbi, bi.data(), bv.data(), &nx, xi.data(), xv.data());
+  fill_info(K, info);
+  if (st != B200LDLT_SUCCESS) { info->flag = -1; return; }
+  memset(x, 0, (size_t)K->n * sizeof(double));
+  for (int j = 0; j < nx; ++j) { x[xi[j]] = xv[j]; xindex[j] = xi[j] + base; }
+  *nxi = nx;
   info->flag = 0;
 }
 

@@ -73,6 +73,36 @@ __global__ void k_dinv(int n, const int* __restrict__ ptype, const double* __res
   if (q >= 0) big[c * ldbig + q] = y; else out[c * ldx + p] = y;
 }
 
+// Sparse forward solve (b200ldlt_sparse_fwd_solve): the single-column sweep state of a forward sweep pruned to a run set
+// R of fronts.  Blocks [0, cdiv(ncol, 256)): x at the ncol positions of R, the scaled entry of b where b has one
+// (bi[j] >= 0: its index into the compact b; the same single multiply as k_rhs_in) and 0 elsewhere.  Blocks after that:
+// frontier front fr[q] (a child of R outside R), its update vector zeroed and its forward flag set to this sweep's epoch,
+// so that its parent neither waits for it nor adds anything from it.
+__global__ void k_sfs_in(int ncol, const int* __restrict__ pos, const int* __restrict__ bi, const int* __restrict__ perm,
+                         const double* __restrict__ scale, const double* __restrict__ b, double* __restrict__ xp,
+                         const int* __restrict__ fr, const long long* __restrict__ rows_ptr, double* __restrict__ cbv,
+                         int* __restrict__ done_f, int epoch) {
+  const int nxb = (ncol + 255) / 256;
+  if ((int)blockIdx.x < nxb) {
+    const int j = blockIdx.x * 256 + threadIdx.x;
+    if (j < ncol) {
+      const int p = pos[j], q = bi[j];
+      xp[p] = q >= 0 ? scale[perm[p]] * b[q] : 0.0;
+    }
+    return;
+  }
+  const int c = fr[blockIdx.x - nxb];
+  const long long r0 = rows_ptr[c], r1 = rows_ptr[c + 1];
+  for (long long e = r0 + threadIdx.x; e < r1; e += blockDim.x) cbv[e] = 0.0;
+  if (threadIdx.x == 0) done_f[c] = epoch;
+}
+// out[i] = the sweep value at pivot position pos[i] (after a forward sweep without D; see k_piv_out)
+__global__ void k_sfs_out(int nx, const int* __restrict__ pos, const long long* __restrict__ piv_big,
+                          const double* __restrict__ xp, const double* __restrict__ big, double* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nx) { const int p = pos[i]; const long long q = piv_big[p]; out[i] = q >= 0 ? big[q] : xp[p]; }
+}
+
 // r = b - A x from the original triplets (tests / bench parity helper)
 __global__ void k_residual_init(int n, const double* __restrict__ b, double* __restrict__ r) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
