@@ -169,6 +169,46 @@ int b200ldlt_lmultiply_device(b200ldlt_handle h, int trans, int nrhs, const doub
  * call, which computes D afresh.  num_neg and b200ldlt_info keep describing the factorisation, not the altered D. */
 int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2);
 
+/* ---- singular matrices: zero pivots and the Fredholm alternative (cf. HSL_MA97 action, ma97_solve_fredholm) ----------
+ * A ZERO PIVOT is a 1x1 pivot that every threshold test rejected (it is forced) and whose whole remaining front column,
+ * diagonal included, is <= 1e-12 in the scaled matrix: rounding noise.  The factorisation replaces it by +-1.5e-8 (its L
+ * column is the noise over 1.5e-8, |l| <~ 7e-5), so with D_pp = 0 instead the factors are those of a singular matrix within
+ * about 1e-12 (scaled max norm) of S A S.  A LIFTED ZERO is a forced pivot with |d| <= tiny under a column that is NOT
+ * noise: its L column is that column over 1.5e-8, and D_pp = 0 would describe a matrix far from A.  Either makes the
+ * factor call return SINGULAR (info.num_tiny counts them).
+ * Keep mode (b200ldlt_set_singular_action(h, 1); default 0, from the next factor / refactor / factor_device call on; a
+ * sharded handle ignores it): a SINGULAR factorisation whose forced zeros are all zero pivots still returns SINGULAR -- the
+ * status describes the matrix -- but KEEPS its factors, with D^-1 = 0 at the zero pivots Z (D^+: D with its zero pivots
+ * left at zero, inverted elsewhere).  *num_neg and info.num_neg then leave the zero pivots out, info.num_tiny = |Z| =
+ * n - rank, and last_error says what happened.  Every solve, partial solve, sparse_fwd_solve, lmultiply, alter_d,
+ * enquire_indef (D^-1 = 0 at Z) and solve_refine_device work on kept factors unchanged; job 0 is then the D^+ solve.  A
+ * factorisation with a lifted zero keeps no factors in any mode (last_error names the pivot).  A non-singular
+ * factorisation is the same, bit for bit and launch for launch, in both modes.  keep must be 0 or 1. */
+int b200ldlt_set_singular_action(b200ldlt_handle h, int keep);
+/* *nzero = |Z| and, unless pos is NULL, pos[0..|Z|) = the pivot positions of Z in ascending order (0 for a factorisation
+ * without zero pivots).  FATAL_ERROR without factors. */
+int b200ldlt_enquire_zero_pivots(b200ldlt_handle h, int* nzero, int* pos);
+/* The Fredholm alternative for nrhs columns b_i.  x is n x 2 nrhs, column-major: on entry columns 0..nrhs-1 hold the b_i;
+ * on exit column i holds x_i and column nrhs + i holds f_i, and consistent[i] is 1 or 0.  With y = L^-1 P^T S b (job 1) and
+ * z = y on Z, 0 elsewhere:
+ *   consistent  iff  max_{p in Z} |y_p| <= tol * max_p |y_p|   (max-norms: exact, whatever the reduction order);
+ *   x = S P L^-T D^+ y   (job 4 after job 1 with D^+ = job 0 with D^+, bit for bit): A x = b - S^-1 P L z exactly in the
+ *                        factored matrix, so x solves A x = b when the column is consistent;
+ *   f = S P L^-T z       (job 3 on z): A f = S^-1 P L D z = 0 and b^T f = y^T z = sum_Z y_p^2 > 0 for an inconsistent
+ *                        column -- a certificate that b is not in the range of A.
+ * f is formed for every column whenever Z is non-empty; with Z empty x is job 0, f = 0 and every column is consistent.
+ * Z is that of the factorisation; D is read from D^-1 as it stands (alter_d may overwrite the zeros at Z).  Every column
+ * is bit-identical to a call on that column alone.  Kernel launches (info.launches_solve), D direct levels
+ * (B200_SOLVE_DIRECT, default 2): with the blocked state (B200_SOLVE_BLOCK >= 2), blocks of up to B200_SOLVE_BLOCK / 2
+ * columns (4 by default) with x and f through ONE backward sweep of twice the width: 5 + 2 D per block (9 by default);
+ * with B200_SOLVE_BLOCK = 1, two backward sweeps per column: 8 + 3 D per column (14); with Z empty, job 0's count.  The
+ * first call with Z non-empty allocates the blocked state as a blocked solve does.
+ * FATAL_ERROR (message in last_error), with nothing written, for nrhs < 0, tol < 0 or NaN, a NULL pointer with nrhs > 0,
+ * without factors (also after SINGULAR in the default mode and after a lifted zero) and on a sharded handle.
+ * Device entry point: the columns d_x are device memory, consistent host memory. */
+int b200ldlt_solve_fredholm(b200ldlt_handle h, int nrhs, double tol, double* x, int* consistent);
+int b200ldlt_solve_fredholm_device(b200ldlt_handle h, int nrhs, double tol, double* d_x, int* consistent);
+
 /* <-> NumberOfNegEVals() (hpp:207) */
 int b200ldlt_num_neg(b200ldlt_handle h);
 /* <-> IncreaseQuality() (hpp:220): pivtol <- min(pivtolmax, pivtol^0.75); returns 0 if already at max.

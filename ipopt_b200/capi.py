@@ -58,7 +58,8 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_assemble_augsys_device", "b200ldlt_solve_refine_device",
             "b200ldlt_solve_partial", "b200ldlt_solve_partial_device", "b200ldlt_enquire_indef",
             "b200ldlt_lmultiply", "b200ldlt_lmultiply_device", "b200ldlt_alter_d",
-            "b200ldlt_sparse_fwd_solve", "b200ldlt_sparse_fwd_solve_device"]
+            "b200ldlt_sparse_fwd_solve", "b200ldlt_sparse_fwd_solve_device", "b200ldlt_set_singular_action",
+            "b200ldlt_enquire_zero_pivots", "b200ldlt_solve_fredholm", "b200ldlt_solve_fredholm_device"]
 
 _lib = None
 
@@ -101,6 +102,10 @@ def load_library():
     L.b200ldlt_alter_d.argtypes = [vp, dp]
     L.b200ldlt_sparse_fwd_solve.argtypes = [vp, C.c_int, ip, dp, ip, ip, dp]
     L.b200ldlt_sparse_fwd_solve_device.argtypes = [vp, C.c_int, ip, vp, ip, ip, vp]
+    L.b200ldlt_set_singular_action.argtypes = [vp, C.c_int]
+    L.b200ldlt_enquire_zero_pivots.argtypes = [vp, ip, ip]
+    L.b200ldlt_solve_fredholm.argtypes = [vp, C.c_int, C.c_double, dp, ip]
+    L.b200ldlt_solve_fredholm_device.argtypes = [vp, C.c_int, C.c_double, vp, ip]
     L.b200ldlt_num_neg.argtypes = [vp]
     L.b200ldlt_increase_quality.argtypes = [vp]
     L.b200ldlt_get_info.argtypes = [vp, C.POINTER(Info)]
@@ -312,6 +317,42 @@ class B200Ldlt:
                                                     _iptr(xi), C.c_void_p(d_x_ptr)) != SYMSOLVER_SUCCESS:
             raise RuntimeError(self.last_error())
         return xi[:nxi.value].copy()
+
+    def set_singular_action(self, keep):
+        """keep = 1: a SINGULAR factorisation whose zero pivots are all rounding noise keeps its factors (D^+); 0 (the
+        default): it keeps none.  Takes effect from the next factor call; returns the status."""
+        return self._L.b200ldlt_set_singular_action(self._h, int(keep))
+
+    def enquire_zero_pivots(self):
+        """The pivot positions of the zero pivots of the kept factors, ascending.  Raises without factors."""
+        nz = C.c_int(0)
+        pos = np.zeros(max(self.dim, 1), np.int32)
+        if self._L.b200ldlt_enquire_zero_pivots(self._h, C.byref(nz), _iptr(pos)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return pos[:nz.value].copy()
+
+    def solve_fredholm(self, B, tol):
+        """Fredholm alternative for the columns of B (dim or dim x nrhs): returns (X, F, consistent) with X the D^+
+        solutions, F the null-space certificates (A F = 0, b^T f > 0 where inconsistent) and consistent a bool array.
+        Raises on a refusal."""
+        B = np.asarray(B, dtype=np.float64)
+        one = B.ndim == 1
+        Bm = B.reshape(self.dim, -1, order="F")
+        nrhs = Bm.shape[1]
+        x = np.zeros((self.dim, 2 * nrhs), order="F")
+        x[:, :nrhs] = Bm
+        cons = np.zeros(max(nrhs, 1), np.int32)
+        if self._L.b200ldlt_solve_fredholm(self._h, nrhs, float(tol), _dptr(x), _iptr(cons)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        X, F, c = x[:, :nrhs].copy(), x[:, nrhs:].copy(), cons[:nrhs].astype(bool)
+        return (X[:, 0], F[:, 0], c) if one else (X, F, c)
+
+    def solve_fredholm_device(self, d_x_ptr, nrhs, tol):
+        """The same on a device array of dim x 2 nrhs doubles (b's in the first nrhs columns; x and f on return).
+        Returns (status, consistent)."""
+        cons = np.zeros(max(int(nrhs), 1), np.int32)
+        st = self._L.b200ldlt_solve_fredholm_device(self._h, int(nrhs), float(tol), C.c_void_p(d_x_ptr), _iptr(cons))
+        return st, cons[:int(nrhs)].astype(bool)
 
     def device_ptr(self, name):
         """Device address of a named array of the handle (b200ldlt_device_ptr: "scale", "x", "cbv", ...), 0 if none."""

@@ -228,6 +228,14 @@ struct Solver {
   std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve: built at its first call after an analysis
   DevBuf<double> d_alter;           // alter_d: the caller's 2n entries of D^-1 (allocated at the first call)
   DevBuf<int> d_alter_bad;
+  // zero pivots (b200ldlt_set_singular_action): the factor kernels append every forced zero pivot to d_zlist; with
+  // keep_singular a factorisation whose zero pivots are all noise pivots keeps its factors, with dinv = 0 at zpos
+  bool keep_singular = false;
+  DevBuf<int> d_zlist, d_zpos;
+  DevBuf<unsigned char> d_zflag;    // n : 1 at the zero pivots of the kept factors
+  std::vector<int> zpos;            // the zero pivots of the kept factors, ascending (empty otherwise)
+  DevBuf<unsigned long long> d_fred_nrm;   // solve_fredholm: the two max-norms per column
+  DevBuf<double> d_fred_z;          // solve_fredholm without a blocked state: z of one column, pivot order
   DevBuf<double> d_linv;
   DevBuf<double> d_linv_part;       // partial tiles of the chunked k_linv_gemm items (one launch at a time uses it)
   DevBuf<int> d_linv_cnt;           // their arrival counters (self-resetting)
@@ -819,6 +827,8 @@ static int run_analysis(Solver* sv, const double* vals) {
   CU(sv->d_rhs.alloc(n)); CU(sv->d_res.alloc(n));
   CU(sv->d_ptype.alloc(n)); CU(sv->d_lperm.alloc(n)); CU(sv->d_bperm.alloc(n));
   CU(sv->d_counters.alloc(CNT_N));
+  CU(sv->d_zlist.alloc(n)); CU(sv->d_zflag.alloc(n));
+  sv->zpos.clear();
   CU(sv->d_colmax.alloc(n));
   CU(sv->d_rmax.alloc(n));
   CU(cudaMemsetAsync(sv->d_rmax.p, 0, n * sizeof(unsigned long long), st));
@@ -835,6 +845,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   N.L = sv->d_L.p; N.W = sv->d_W.p; N.CB = sv->d_CB.p; N.uval = sv->d_uval.p;
   N.dinv = sv->d_dinv.p; N.doff = sv->d_doff.p; N.ptype = sv->d_ptype.p;
   N.lperm = sv->d_lperm.p; N.bperm = sv->d_bperm.p; N.counters = sv->d_counters.p; N.colmax = sv->d_colmax.p;
+  N.zlist = sv->d_zlist.p;
 
   // inverse row maps of the children of the (factorisation-)big fronts, for the one-launch extend-add
   {
@@ -1162,6 +1173,12 @@ static int enqueue_linv(Solver* sv, const LinvPlan& LP, cudaStream_t st) {
   return B200LDLT_SUCCESS;
 }
 
+// keep mode: D^+ at the zero pivots zpos[0..nz) (dinv = 0; they are 1x1 pivots, doff is already 0) and their flags
+__global__ void k_zero_pivots(int nz, const int* __restrict__ zpos, double* __restrict__ dinv, unsigned char* __restrict__ zflag) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nz) { dinv[zpos[i]] = 0.0; zflag[zpos[i]] = 1; }
+}
+
 static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* num_neg) {
   cudaStream_t st = sv->stream;
   CU(cudaEventRecord(sv->ev1, st));
@@ -1178,12 +1195,44 @@ static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* n
   I.num_tiny = sv->h_counters[CNT_TINY];
   I.num_growth = sv->h_counters[CNT_GROWTH];
   I.num_2x2 = sv->h_counters[CNT_2X2];
+  // Factors of a matrix with a noise pivot (SINGULAR) are not offered to the solves, unless keep mode is on and every such
+  // pivot is a zero pivot (its whole column noise): D_pp = 0 then describes the matrix, so dinv[p] is set to 0 (D^+) and
+  // the pivot leaves the inertia.  A lifted zero (|pivot| <= tiny under a column that is not noise) never keeps factors.
+  // With num_forced > 0 the factors (and the inertia reported) are those of a matrix perturbed by <= 1e-8 |column| in the
+  // lifted pivots; the count is surfaced in b200ldlt_info and drives increase_quality (re-analysis with the current values).
+  sv->factored = (I.num_tiny == 0);
+  sv->zpos.clear();
+  if (I.num_tiny > 0) {
+    const int nz = std::min(sv->h_counters[CNT_ZLIST], sv->n);
+    std::vector<int> zl(nz);
+    CU(cudaMemcpy(zl.data(), sv->d_zlist.p, nz * sizeof(int), cudaMemcpyDeviceToHost));
+    std::sort(zl.begin(), zl.end());
+    int lifted = -1, zneg = 0;
+    for (int e : zl) {
+      if ((e & 2) && lifted < 0) lifted = e >> 2;
+      zneg += e & 1;
+    }
+    if (lifted >= 0) {
+      sv->err = "factor: SINGULAR with a lifted zero pivot (|pivot| <= tiny at pivot position " + std::to_string(lifted) +
+                ", whose column is not rounding noise): no factors kept";
+    } else {
+      sv->err = "factor: SINGULAR: " + std::to_string(nz) + " zero pivot(s)" +
+                (sv->keep_singular ? "; factors kept with D^+ (zero pivots left out of the inertia)" : "; no factors kept");
+      if (sv->keep_singular && !sv->shard.active && nz == I.num_tiny) {
+        for (int e : zl) sv->zpos.push_back(e >> 2);
+        CU(sv->d_zpos.upload(sv->zpos, st));
+        CU(cudaMemsetAsync(sv->d_zflag.p, 0, sv->n, st));
+        k_zero_pivots<<<cdiv(nz, 256), 256, 0, st>>>(nz, sv->d_zpos.p, sv->d_dinv.p, sv->d_zflag.p);
+        CU(cudaGetLastError());
+        CU(cudaStreamSynchronize(st));
+        I.launches_factor += 1;
+        I.num_neg -= zneg;
+        sv->factored = true;
+      }
+    }
+  }
   sv->num_neg = I.num_neg;
   if (num_neg) *num_neg = I.num_neg;
-  // Factors of a matrix with a noise pivot (SINGULAR) are not offered to the solves.  With num_forced > 0 the factors
-  // (and the inertia reported) are those of a matrix perturbed by <= 1e-8 |column| in the lifted pivots; the count is
-  // surfaced in b200ldlt_info and drives increase_quality (re-analysis with the current values).
-  sv->factored = (I.num_tiny == 0);
   if (sv->opt.verbose > 1)
     fprintf(stderr, "[b200ldlt] factor: %.3f ms, %d launches, neg=%d 2x2=%d forced=%d tiny=%d growth=%d (u=%g)\n", ms,
             sv->launches, I.num_neg, I.num_2x2, I.num_forced, I.num_tiny, I.num_growth, sv->pivtol);
@@ -1407,6 +1456,56 @@ static int enqueue_solve_columns(Solver* sv, double* d_rhs, int nrhs, bool block
     if (rc != B200LDLT_SUCCESS) return rc;
     c += w;
   }
+  return B200LDLT_SUCCESS;
+}
+
+// The Fredholm alternative (b200ldlt_solve_fredholm) with zero pivots Z: columns [0, nrhs) of d_x (leading dimension n)
+// hold the b's; on exit column i holds x_i = S P L^-T D^+ y_i and column nrhs + i holds f_i = S P L^-T z_i, where
+// y_i = L^-1 P^T S b_i and z_i is y_i on Z.  sv->d_fred_nrm receives max |y_i| and max_Z |y_i| per column.  x_i runs
+// job 1, then job 4 with D^+ (= job 0 with D^+, bit for bit); f_i runs job 3 on z_i.
+//   blocked (a state of width >= 2): blocks of w <= width / 2 columns, x and f through ONE backward sweep of 2w columns:
+//     k_rhs_in, forward sweep without D, k_fred, backward sweep, k_fred_out -- 5 + 2 D launches per block;
+//   otherwise column by column in the single-column state, z parked in sv->d_fred_z, two backward sweeps: k_rhs_in,
+//     forward, k_fred, backward, k_sol_out, k_piv_in, backward, k_sol_out -- 8 + 3 D launches per column.
+// Every column runs the arithmetic of a single-column call.
+static int enqueue_fredholm(Solver* sv, double* d_x, int nrhs, bool blocked) {
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  CU(cudaMemsetAsync(sv->d_fred_nrm.p, 0, 2 * (size_t)nrhs * sizeof(unsigned long long), st));
+  SweepState& W = blocked ? *sv->blk : sv->sweep;
+  const int cap = blocked ? W.width / 2 : 1;
+  const long long ldx = W.M.x, ldb = W.M.bigv;
+  for (int c = 0; c < nrhs;) {
+    const int w = std::min(cap, nrhs - c);
+    double* col = d_x + (size_t)c * n;
+    const dim3 g(cdiv(n, 256), w);
+    k_rhs_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, col, W.d_x.p, ldx); ++sv->launches;
+    sv->solve_epoch++;
+    int rc = launch_sweep(sv, sv->splan, W, w, true, false);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    k_fred<<<g, 256, 0, st>>>(n, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, sv->d_zflag.p, sv->d_piv_big.p, W.d_x.p, ldx,
+                              W.d_bigv.p, ldb, w, blocked ? nullptr : sv->d_fred_z.p, sv->d_fred_nrm.p + 2 * (size_t)c);
+    ++sv->launches;
+    sv->solve_epoch++;
+    if (blocked) {
+      rc = launch_sweep(sv, sv->splan, W, 2 * w, false);
+      if (rc != B200LDLT_SUCCESS) return rc;
+      k_fred_out<<<dim3(cdiv(n, 256), 2 * w), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, col, w, nrhs);
+      ++sv->launches;
+    } else {
+      rc = launch_sweep(sv, sv->splan, W, 1, false);
+      if (rc != B200LDLT_SUCCESS) return rc;
+      k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, col); ++sv->launches;
+      k_piv_in<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, sv->d_fred_z.p, W.d_x.p, ldx, W.d_bigv.p, ldb); ++sv->launches;
+      sv->solve_epoch++;
+      rc = launch_sweep(sv, sv->splan, W, 1, false);
+      if (rc != B200LDLT_SUCCESS) return rc;
+      k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, d_x + (size_t)(nrhs + c) * n);
+      ++sv->launches;
+    }
+    c += w;
+  }
+  CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
 }
 
@@ -2051,6 +2150,68 @@ static int sparse_fwd(Solver* sv, int nbi, const int* bindex, const double* b, b
   sv->info.launches_solve = sv->launches;
   return B200LDLT_SUCCESS;
 }
+
+// b200ldlt_solve_fredholm (host == true: x in host memory) / _device
+static int fredholm(Solver* sv, int nrhs, double tol, double* x, int* consistent, bool host) {
+  const char* why = nullptr;
+  if (nrhs < 0) why = "nrhs must be >= 0";
+  else if (!(tol >= 0.0)) why = "tol must be >= 0";
+  else if (nrhs > 0 && (!x || !consistent)) why = "NULL argument";
+  else if (!sv->factored) why = "no factors (factorise first; a SINGULAR factorisation keeps them only in keep mode, see b200ldlt_set_singular_action)";
+  else if (sv->shard.active) why = "not available on a sharded handle";
+  if (why) { sv->err = std::string("solve_fredholm: ") + why; return B200LDLT_FATAL_ERROR; }
+  if (nrhs == 0) { sv->info.launches_solve = 0; sv->info.ms_solve_gpu = 0.0f; return B200LDLT_SUCCESS; }
+  CU(cudaSetDevice(sv->dev));
+  cudaStream_t st = sv->stream;
+  const size_t n = sv->n;
+  if (sv->zpos.empty()) {
+    // no zero pivots: the solve itself, f = 0, every column consistent
+    int rc;
+    if (host) {
+      rc = solve_host_job(sv, 0, nrhs, x);
+      memset(x + n * nrhs, 0, n * nrhs * sizeof(double));
+    } else {
+      CU(cudaMemsetAsync(x + n * nrhs, 0, n * nrhs * sizeof(double), st));
+      rc = solve_device_job(sv, 0, nrhs, x);
+    }
+    if (rc != B200LDLT_SUCCESS) return rc;
+    for (int i = 0; i < nrhs; ++i) consistent[i] = 1;
+    return B200LDLT_SUCCESS;
+  }
+  const bool blocked = block_solve_state(sv);
+  if (sv->d_fred_nrm.n < 2 * (size_t)nrhs) CU(sv->d_fred_nrm.alloc(2 * (size_t)nrhs));
+  if (!blocked && sv->d_fred_z.n != n) CU(sv->d_fred_z.alloc(n));
+  const size_t total = n * 2 * (size_t)nrhs;
+  if (host && 2 * nrhs > sv->rhs_cap) {
+    if (sv->h_rhs) cudaFreeHost(sv->h_rhs);
+    sv->h_rhs = nullptr;
+    sv->rhs_cap = 0;
+    CU(cudaHostAlloc((void**)&sv->h_rhs, total * sizeof(double), cudaHostAllocDefault));
+    CU(sv->d_rhs.alloc(total));
+    sv->rhs_cap = 2 * nrhs;
+  }
+  std::vector<unsigned long long> nrm(2 * (size_t)nrhs);
+  double* d_x = host ? sv->d_rhs.p : x;
+  if (host) memcpy(sv->h_rhs, x, n * nrhs * sizeof(double));
+  sv->launches = 0;
+  CU(cudaEventRecord(sv->ev0, st));
+  if (host) CU(cudaMemcpyAsync(d_x, sv->h_rhs, n * nrhs * sizeof(double), cudaMemcpyHostToDevice, st));
+  { const int rc = enqueue_fredholm(sv, d_x, nrhs, blocked); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (host) CU(cudaMemcpyAsync(sv->h_rhs, d_x, total * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(nrm.data(), sv->d_fred_nrm.p, nrm.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(sv->ev1, st));
+  CU(cudaStreamSynchronize(st));
+  if (host) memcpy(x, sv->h_rhs, total * sizeof(double));
+  for (int i = 0; i < nrhs; ++i) {
+    double ymax, zmax;
+    memcpy(&ymax, &nrm[2 * (size_t)i], sizeof(double));
+    memcpy(&zmax, &nrm[2 * (size_t)i + 1], sizeof(double));
+    consistent[i] = zmax <= tol * ymax ? 1 : 0;
+  }
+  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
+  sv->info.launches_solve = sv->launches;
+  return B200LDLT_SUCCESS;
+}
 }  // namespace b200
 
 extern "C" {
@@ -2196,6 +2357,36 @@ int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2) {
   return B200LDLT_SUCCESS;
 }
 
+int b200ldlt_set_singular_action(b200ldlt_handle h, int keep) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  if (keep != 0 && keep != 1) { sv->err = "set_singular_action: keep must be 0 or 1"; return B200LDLT_FATAL_ERROR; }
+  sv->keep_singular = keep == 1;
+  return B200LDLT_SUCCESS;
+}
+
+int b200ldlt_enquire_zero_pivots(b200ldlt_handle h, int* nzero, int* pos) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  if (!nzero) { sv->err = "enquire_zero_pivots: NULL nzero"; return B200LDLT_FATAL_ERROR; }
+  if (!sv->factored) { sv->err = "enquire_zero_pivots: no factors (factorise first; a SINGULAR factorisation keeps them only in keep mode)"; return B200LDLT_FATAL_ERROR; }
+  *nzero = (int)sv->zpos.size();
+  if (pos) std::copy(sv->zpos.begin(), sv->zpos.end(), pos);
+  return B200LDLT_SUCCESS;
+}
+
+int b200ldlt_solve_fredholm(b200ldlt_handle h, int nrhs, double tol, double* x, int* consistent) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return fredholm(sv, nrhs, tol, x, consistent, true);
+}
+
+int b200ldlt_solve_fredholm_device(b200ldlt_handle h, int nrhs, double tol, double* d_x, int* consistent) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return fredholm(sv, nrhs, tol, d_x, consistent, false);
+}
+
 /* ---- multi-GPU elimination-tree sharding (SURVEY.md section 8e) -------------------------------------------
  * One process per GPU, each with its own handle and the SAME matrix.  After the (replicated, deterministic)
  * analysis, rank g factorises the subtrees it owns; the contribution blocks of the cut are moved to rank 0 by the
@@ -2266,6 +2457,7 @@ int b200ldlt_shard_factor_finish(b200ldlt_handle h, const int* counters_total, i
   sv->num_neg = I.num_neg;
   if (num_neg) *num_neg = I.num_neg;
   sv->factored = (I.num_tiny == 0);
+  sv->zpos.clear();
   if (I.num_tiny > 0) return B200LDLT_SINGULAR;
   if (check_inertia && I.num_neg != expected_neg) return B200LDLT_WRONG_INERTIA;
   return B200LDLT_SUCCESS;

@@ -130,7 +130,7 @@ __device__ void swap_sym(double* F, int ld, int f, int p, int q) {
 
 __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int* pt, double* cv1,
                                   double* cv2, volatile int* sh, double u, double tiny,
-                                  double* dinv, double* doff, int* ptype_g, int* counters) {
+                                  double* dinv, double* doff, int* ptype_g, int* counters, int* zlist, int pos0) {
   const int tid = threadIdx.x, nt = blockDim.x;
   const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;
   for (int t = tid; t < k; t += nt) lp[t] = t;
@@ -230,7 +230,7 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
       if (forced) {
         if (noise || !(fabs(d) > tiny)) {  // zero (or NaN) pivot: static perturbation, reported as SINGULAR
           d = (d < 0.0) ? -1.5e-8 : 1.5e-8;
-          if (tid == 0) ++c_tiny;
+          if (tid == 0) { ++c_tiny; zl_put(counters, zlist, pos0 + j, noise, d < 0.0); }
         } else {
           // static pivoting: lift the pivot to the threshold (see warp_ldlt32); cv2[j] holds max|column j|
           double offmax = 0.0;
@@ -368,6 +368,22 @@ __device__ __forceinline__ void wred_max_idx(double& v, int& idx) {
   }
 }
 
+// Zero pivots of the register pivoting routines (warp_ldlt32, cta_ldlt32s).  Their pivot loops run at the edge of the
+// register file, so the forced branch only sets bit t (pivot t is a zero pivot) or bit 32 + t (a lifted zero) of a mask,
+// and the entries are appended after the loop.  cta_ldlt32s keeps the mask in place of its count c_tiny and appends the
+// entries itself, at zl_pos0[0] (pivot position of its pivot 0, written by the kernel before the call).  warp_ldlt32 ORs
+// the bit into zl_mask[warp index] (cleared, with zl_pos0[warp index], by the kernel before the call), and its kernel
+// appends the entries at its end.  The sign comes from dinv_s.
+__shared__ int zl_pos0[4];
+__shared__ unsigned long long zl_mask[4];
+__device__ __forceinline__ void zl_append(int* counters, int* zlist, int pos0, unsigned long long zmask,
+                                          const double* dinv_s) {
+  for (unsigned m = (unsigned)zmask | (unsigned)(zmask >> 32); m; m &= m - 1) {
+    const int t = __ffs(m) - 1;
+    zl_put(counters, zlist, pos0 + t, (zmask >> t) & 1ull, dinv_s[t] < 0.0);
+  }
+}
+
 // TWO = true: fronts of order 33..64 with k <= 32.  The warp also carries rows 32..f-1 (lane -> row 32 + lane) of the
 // first 32 columns in b[]: they are never pivot candidates (all candidates are among rows 0..k-1 < 32), but they take part
 // in every threshold test, receive every update (so b[c], c < 32-k, ends as the Schur complement column k+c of row
@@ -495,7 +511,10 @@ __device__ void warp_ldlt32(double (&a)[32], double (&b)[32], const int f, const
     if (type == 1) {
       double dd = __shfl_sync(0xffffffffu, a[0], g0);
       if (forced) {
-        if (noise || !(fabs(dd) > tiny)) { dd = (dd < 0.0) ? -1.5e-8 : 1.5e-8; ++c_tiny; }
+        if (noise || !(fabs(dd) > tiny)) {
+          dd = (dd < 0.0) ? -1.5e-8 : 1.5e-8; ++c_tiny;
+          if (lane == 0) zl_mask[threadIdx.x >> 5] |= (noise ? 1ull : 1ull << 32) << t;
+        }
         else {
           // static pivoting: a pivot that fails the threshold test everywhere in its supernode is lifted to the
           // threshold (|l_ij| stays <= 1e8; the factors are those of a matrix perturbed by <= 1e-8 |column|,
@@ -645,7 +664,7 @@ __global__ void k_front_smem(DevSym S, DevNum N, const int* __restrict__ front_l
   }
 
   factor_front_smem(F, ld, f, k, lp, pt, cv1, cv2, sh, N.u, N.tiny, N.dinv + c0, N.doff + c0,
-                    N.ptype + c0, N.counters);
+                    N.ptype + c0, N.counters, N.zlist, c0);
 
   // write L panel (f x k, ld = f), unit diagonal.  The strictly-upper part of the k x k pivot block receives L11^T
   // (entry (i, t), i < t, = L[t][i]): the backward solve of the small fronts reads row t of L11 as the contiguous
@@ -724,6 +743,7 @@ __global__ void __launch_bounds__(128) k_front_warp(DevSym S, DevNum N, const in
   double a[32];
 #pragma unroll
   for (int c = 0; c < 32; ++c) a[c] = F[lane + c * ld];   // lanes >= f / columns >= f read zeros
+  if (lane == 0) { zl_pos0[threadIdx.x >> 5] = c0; zl_mask[threadIdx.x >> 5] = 0; }
   __syncwarp();
   warp_ldlt32<false>(a, a, f, k, N.u, N.tiny, F, order, pt, dinv_s, doff_s, colbuf, 0.0, N.counters);
   // L panel in pivot order
@@ -750,6 +770,8 @@ __global__ void __launch_bounds__(128) k_front_warp(DevSym S, DevNum N, const in
 #pragma unroll
   for (int c = 0; c < 32; ++c)
     if (lane >= k && lane < f && c <= lane - k) cbo[(lane - k) + (size_t)c * r] = a[c];
+  if (lane == 0 && zl_mask[threadIdx.x >> 5])
+    zl_append(N.counters, N.zlist, zl_pos0[threadIdx.x >> 5], zl_mask[threadIdx.x >> 5], dinv_s);
 }
 
 // --------------------------------------------------------------------------------------------
@@ -839,6 +861,7 @@ __global__ void __launch_bounds__(128, 2) k_front_warp2(DevSym S, DevNum N, cons
   double a[32], b[32];
 #pragma unroll
   for (int c = 0; c < 32; ++c) { a[c] = P0[lane + c * S2_LD]; b[c] = P0[32 + lane + c * S2_LD]; }   // rows >= f read zeros
+  if (lane == 0) { zl_pos0[threadIdx.x >> 5] = c0; zl_mask[threadIdx.x >> 5] = 0; }
   __syncwarp();     // every lane has its columns: the region becomes Lraw
   double* Lraw = P0;
   warp_ldlt32<true>(a, b, f, k, N.u, N.tiny, Lraw, order, pt, dinv_s, doff_s, colbuf, 0.0, N.counters, dpiv, dpb);
@@ -898,6 +921,8 @@ __global__ void __launch_bounds__(128, 2) k_front_warp2(DevSym S, DevNum N, cons
       if (j <= lane && lane < f1) cbo[(32 - k + lane) + (size_t)(32 - k + j) * r] = C22[lane + j * 33] - acc;
     }
   }
+  if (lane == 0 && zl_mask[threadIdx.x >> 5])
+    zl_append(N.counters, N.zlist, zl_pos0[threadIdx.x >> 5], zl_mask[threadIdx.x >> 5], dinv_s);
 }
 
 // --------------------------------------------------------------------------------------------
@@ -1029,13 +1054,14 @@ __device__ __forceinline__ double fast_rcp(const double d) {
 __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const double tiny,
                             double* __restrict__ As, double* __restrict__ Lraw, int* __restrict__ order, int* __restrict__ pt,
                             double* __restrict__ dinv_s, double* __restrict__ doff_s, const double* __restrict__ gext_s,
-                            int* counters) {
+                            int* counters, int* zlist) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   unsigned cand = (f >= 32) ? 0xffffffffu : ((1u << f) - 1u);
   unsigned parked = 0;
   int t = 0, progress = 0;
   bool forced = false;
-  int c_neg = 0, c_forced = 0, c_tiny = 0, c_2x2 = 0;
+  int c_neg = 0, c_forced = 0, c_2x2 = 0;
+  unsigned long long zmask = 0;   // zero pivots (see zl_append)
   int my_order = 0, my_pt = 1;
   double my_dinv = 0.0, my_doff = 0.0;
   const unsigned lbit = 1u << lane;
@@ -1104,7 +1130,7 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
       if (forced) {
         double dd = pa0;
         const bool noise = !(fmax(ajj, colmax_f) > 1e-12);
-        if (noise || !(fabs(dd) > tiny)) { dd = (dd < 0.0) ? -1.5e-8 : 1.5e-8; ++c_tiny; }
+        if (noise || !(fabs(dd) > tiny)) { dd = (dd < 0.0) ? -1.5e-8 : 1.5e-8; zmask |= (noise ? 1ull : 1ull << 32) << t; }
         else { dd = copysign(fmax(fabs(dd), 1e-8 * colmax_f), dd); ++c_forced; }
         apply1(a0, dd, 1.0 / dd, g0, pr0);
         continue;
@@ -1185,11 +1211,12 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
     if (lane == 0) {
       if (c_neg) atomicAdd(counters + CNT_NEG, c_neg);
       if (c_forced) atomicAdd(counters + CNT_FORCED, c_forced);
-      if (c_tiny) atomicAdd(counters + CNT_TINY, c_tiny);
+      if (zmask) atomicAdd(counters + CNT_TINY, __popcll(zmask));
       if (c_2x2) atomicAdd(counters + CNT_2X2, c_2x2);
     }
   }
   __syncthreads();
+  if (zmask && threadIdx.x == 0) zl_append(counters, zlist, zl_pos0[0], zmask, dinv_s);
 }
 
 // --------------------------------------------------------------------------------------------
@@ -1351,10 +1378,11 @@ __device__ void chain_role(const DevSym& S, const DevNum& N, const int s, const 
 #pragma unroll
   for (int q = 0; q < 8; ++q) { const int c = 8 * w + q; a[q] = (c <= lane) ? A2[lane * 33 + c] : A2[c * 33 + lane]; }
   if (w == 0) gext_s[lane] = gext;
+  if (tid == 0) zl_pos0[0] = c0 + o;
   __syncthreads();   // A2 becomes the full symmetric working copy of cta_ldlt32s: A2[c * 33 + i] = A[i][c]
 #pragma unroll
   for (int q = 0; q < 8; ++q) A2[(8 * w + q) * 33 + lane] = a[q];
-  cta_ldlt32s(a, nbn, N.u, N.tiny, A2, Ln, order, pt, dinv_s, doff_s, gext_s, N.counters);
+  cta_ldlt32s(a, nbn, N.u, N.tiny, A2, Ln, order, pt, dinv_s, doff_s, gext_s, N.counters, N.zlist);
   const int mine = (lane < nbn) ? order[lane] : 0;
 #pragma unroll
   for (int q = 0; q < 8; ++q) {

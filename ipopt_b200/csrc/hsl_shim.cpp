@@ -20,11 +20,13 @@
 //   ma97_alter_d           writes D^-1 back in the layout ma97_enquire_indef_d returns (b200ldlt_alter_d);
 //   ma97_enquire_posdef_d  the diagonal of the Cholesky factor L D^1/2 when every pivot is a positive 1x1 pivot;
 //   ma97_sparse_fwd_solve_d  job 1 of a sparse right-hand side, swept over the fronts it reaches only
-//                          (b200ldlt_sparse_fwd_solve), declared at hsl_ma97d.h:173-176.
-// Not provided: ma97_solve_fredholm_d (it needs the factors of a singular matrix, and the backend keeps none after
-// SINGULAR) and the 64-bit variants.
-// The conventions of the inspection calls (enquire_indef / enquire_posdef / alter / lmultiply / sparse_fwd_solve) are our
-// reading of the reference header; they have not been checked against the HSL user documentation.
+//                          (b200ldlt_sparse_fwd_solve), declared at hsl_ma97d.h:173-176;
+//   control->action        != 0 keeps the factors of a singular matrix whose zero pivots are all rounding noise
+//                          (b200ldlt_set_singular_action): flag 7 with factors, D^+ at the zero pivots;
+//   ma97_solve_fredholm_d  the Fredholm alternative on those factors (b200ldlt_solve_fredholm), hsl_ma97d.h:164-167.
+// Not provided: the 64-bit variants.
+// The conventions of the inspection calls (enquire_indef / enquire_posdef / alter / lmultiply / sparse_fwd_solve /
+// solve_fredholm) are our reading of the reference header; they have not been checked against the HSL user documentation.
 #include <cuda_runtime_api.h>
 
 #include <cmath>
@@ -187,10 +189,17 @@ void ma97_factor_d(int matrix_type, const int ptr[], const int row[], const doub
     K->u = control->u;
   }
   memcpy(b200ldlt_values_ptr(K->h), val, (size_t)K->nnz * sizeof(double));   // same order as the CSC entries
+  const bool keep = control && control->action;
+  b200ldlt_set_singular_action(K->h, keep ? 1 : 0);
   int neg = -1;
   const int st = b200ldlt_factor(K->h, 0, 0, &neg);
   fill_info(K, info);
-  if (st == B200LDLT_SINGULAR) { info->flag = (control && control->action) ? 7 : -7; K->factored = false; }
+  if (st == B200LDLT_SINGULAR) {
+    // action != 0: continue on singularity -- flag 7, with the factors (D^+) when they were kept (only zero pivots)
+    int nz = 0;
+    K->factored = keep && b200ldlt_enquire_zero_pivots(K->h, &nz, nullptr) == B200LDLT_SUCCESS;
+    info->flag = keep ? 7 : -7;
+  }
   else if (st != B200LDLT_SUCCESS) { info->flag = -1; K->factored = false; }
   else { info->flag = 0; K->factored = true; }
   if (K->factored && scale && !copy_scale(K, scale)) info->flag = -1;
@@ -324,10 +333,45 @@ void ma97_sparse_fwd_solve_d(int nbi, const int bindex[], const double b[], cons
 void ma97_factor_solve_d(int matrix_type, const int ptr[], const int row[], const double val[], int nrhs, double x[], int ldx,
                          void** akeep, void** fkeep, const ma97_control_d* control, ma97_info_d* info, double scale[]) {
   ma97_factor_d(matrix_type, ptr, row, val, akeep, fkeep, control, info, scale);
-  if (info->flag != 0) return;
+  if (info->flag != 0 && info->flag != 7) return;   // flag 7 comes with factors (kept D^+)
   ma97_info_d i2;
   ma97_solve_d(0, nrhs, x, ldx, akeep, fkeep, control, &i2);
   if (i2.flag != 0) info->flag = i2.flag;
+}
+
+// Fredholm alternative (b200ldlt_solve_fredholm) of the kept factors of a singular matrix.  Our reading of the convention:
+// x is ldx x 2 nrhs; on entry x(:, i) holds b_i, on exit the D^+ solution; flag_out[i] = 1 when column i is consistent
+// within control->consist_tol (max over the zero pivots of |L^-1 P^T S b| <= consist_tol * its max over all pivots),
+// else 0, and then x(:, nrhs + i) holds f_i with A f_i = 0 and b_i^T f_i > 0; for consistent columns x(:, nrhs + i) is
+// left untouched.  ldx != n: column by column, as ma97_solve_d does.  Neither this convention nor the scaling of
+// consist_tol has been checked against the HSL documentation; with MA97's default consist_tol (machine epsilon) only
+// columns whose components on the zero pivots are exactly zero count as consistent.
+void ma97_solve_fredholm_d(int nrhs, int flag_out[], double x[], int ldx, void** akeep, void** fkeep,
+                           const ma97_control_d* control, ma97_info_d* info) {
+  (void)fkeep;
+  memset(info, 0, sizeof(*info));
+  Keep* K = akeep ? (Keep*)*akeep : nullptr;
+  if (!K || !K->h || !K->factored || nrhs < 0 || ldx < K->n || (nrhs > 0 && (!x || !flag_out))) { info->flag = -1; return; }
+  if (nrhs == 0) return;
+  const double tol = control ? control->consist_tol : 2.220446049250313e-16;
+  const size_t n = (size_t)K->n;
+  const bool whole = ldx == K->n;
+  const int cols = whole ? nrhs : 1;
+  std::vector<double> buf(n * 2 * (size_t)cols);
+  std::vector<int> cons((size_t)cols);
+  int st = B200LDLT_SUCCESS;
+  for (int c0 = 0; c0 < nrhs && st == B200LDLT_SUCCESS; c0 += cols) {
+    for (int i = 0; i < cols; ++i) memcpy(buf.data() + i * n, x + (size_t)(c0 + i) * ldx, n * sizeof(double));
+    st = b200ldlt_solve_fredholm(K->h, cols, tol, buf.data(), cons.data());
+    if (st != B200LDLT_SUCCESS) break;
+    for (int i = 0; i < cols; ++i) {
+      memcpy(x + (size_t)(c0 + i) * ldx, buf.data() + i * n, n * sizeof(double));
+      flag_out[c0 + i] = cons[i];
+      if (!cons[i]) memcpy(x + (size_t)(nrhs + c0 + i) * ldx, buf.data() + (cols + i) * n, n * sizeof(double));
+    }
+  }
+  fill_info(K, info);
+  info->flag = (st == B200LDLT_SUCCESS) ? 0 : -1;
 }
 
 void ma97_free_akeep_d(void** akeep) {

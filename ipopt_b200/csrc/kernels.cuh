@@ -5,7 +5,16 @@
 namespace b200 {
 
 // counters[] layout
-enum { CNT_NEG = 0, CNT_FORCED = 1, CNT_TINY = 2, CNT_GROWTH = 3, CNT_2X2 = 4, CNT_N = 8 };
+// CNT_ZLIST: entries appended to DevNum::zlist (one per pivot counted in CNT_TINY)
+enum { CNT_NEG = 0, CNT_FORCED = 1, CNT_TINY = 2, CNT_GROWTH = 3, CNT_2X2 = 4, CNT_ZLIST = 5, CNT_N = 8 };
+
+// An entry of DevNum::zlist: a 1x1 pivot the forced branch replaced by +-1.5e-8 because it was zero.  zl_noise: its whole
+// column was rounding noise (a ZERO PIVOT: D_pp = 0 describes the matrix); otherwise |pivot| <= tiny under a column that
+// is not noise (a LIFTED ZERO).  zl_neg: the stored pivot is -1.5e-8 (counted in CNT_NEG).
+__device__ __forceinline__ int zl_entry(int pos, bool noise, bool neg) { return (pos << 2) | (noise ? 0 : 2) | (neg ? 1 : 0); }
+__device__ __forceinline__ void zl_put(int* counters, int* zlist, int pos, bool noise, bool neg) {
+  zlist[atomicAdd(counters + CNT_ZLIST, 1)] = zl_entry(pos, noise, neg);
+}
 
 struct DevSym {
   int n, nsn;
@@ -39,6 +48,7 @@ struct DevNum {
   int* bperm;       // n : block-local permutation of the last panel step (big fronts)
   double* colmax;   // n : big fronts only: max |entry| of a panel column BELOW its 32x32 diagonal block at panel start
   int* counters;    // CNT_N
+  int* zlist;       // n : the forced zero pivots, zl_entry encoded, in arrival order (count: counters[CNT_ZLIST])
   double u;         // pivot threshold
   double tiny;      // zero-pivot threshold (scaled matrix)
 };

@@ -73,6 +73,62 @@ __global__ void k_dinv(int n, const int* __restrict__ ptype, const double* __res
   if (q >= 0) big[c * ldbig + q] = y; else out[c * ldx + p] = y;
 }
 
+// Fredholm alternative (b200ldlt_solve_fredholm), between a forward sweep without D and the backward sweep, on the sweep
+// values (see k_piv_out) of column blockIdx.y = c holding y = L^-1 P^T S b.  In place, column c becomes D^+ y -- D^-1 from
+// dinv / doff through dinv_entry exactly as k_dinv rounds it, so the backward sweep gives job 0's bits; dinv = 0 at the
+// zero pivots makes it D^+ -- and z = y on the zero pivots (zflag[p] != 0, always 1x1 pivots), 0 elsewhere, goes to
+// column zcol + c of the sweep values (zout == nullptr) or to zout[c * n + p].  nrm[2c] / nrm[2c+1] (double bits,
+// atomicMax; zero-initialised) receive max_p |y_p| and max_Z |y_p|, NaN counted as infinity.  The thread of the first
+// pivot of a 2x2 block reads and writes both of its entries, so no thread reads what another writes.
+__global__ void k_fred(int n, const int* __restrict__ ptype, const double* __restrict__ dinv, const double* __restrict__ doff,
+                       const unsigned char* __restrict__ zflag, const long long* __restrict__ piv_big, double* __restrict__ xp,
+                       long long ldx, double* __restrict__ big, long long ldbig, int zcol, double* __restrict__ zout,
+                       unsigned long long* __restrict__ nrm) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long c = blockIdx.y;
+  const int ty = p < n ? ptype[p] : 3;
+  double ay = 0.0, az = 0.0;
+  // sweep value at position r (v) and where it lives; the outputs y (column c) and z (column zcol + c or zout)
+  auto get = [&](int r) { const long long q = piv_big[r]; return q >= 0 ? big[c * ldbig + q] : xp[c * ldx + r]; };
+  auto put = [&](int r, double y, double z) {
+    const long long q = piv_big[r];
+    if (q >= 0) { big[c * ldbig + q] = y; if (!zout) big[(zcol + c) * ldbig + q] = z; }
+    else { xp[c * ldx + r] = y; if (!zout) xp[(zcol + c) * ldx + r] = z; }
+    if (zout) zout[c * n + r] = z;
+  };
+  auto mag = [](double v) { return (v == v) ? fabs(v) : INFINITY; };
+  if (ty == 1) {
+    const double v = get(p);
+    ay = mag(v);
+    const bool zp = zflag[p] != 0;
+    if (zp) az = ay;
+    put(p, dinv_entry(1, v, 0.0, dinv[p], 0.0), zp ? v : 0.0);
+  } else if (ty == 2) {
+    const double v0 = get(p), v1 = get(p + 1);
+    ay = fmax(mag(v0), mag(v1));
+    put(p, dinv_entry(2, v0, v1, dinv[p], doff[p]), 0.0);
+    put(p + 1, dinv_entry(3, v1, v0, dinv[p + 1], doff[p]), 0.0);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ay = fmax(ay, __shfl_xor_sync(0xffffffffu, ay, o));
+    az = fmax(az, __shfl_xor_sync(0xffffffffu, az, o));
+  }
+  if ((threadIdx.x & 31) == 0) {
+    if (ay > 0.0) atomicMax(nrm + 2 * c, (unsigned long long)__double_as_longlong(ay));
+    if (az > 0.0) atomicMax(nrm + 2 * c + 1, (unsigned long long)__double_as_longlong(az));
+  }
+}
+// x[perm[i]] = scale[perm[i]] * xp[i] as k_sol_out, for the 2w columns of a Fredholm block: column c < w to x + c n, the
+// null-space columns c >= w to x + (fcol + c - w) n
+__global__ void k_fred_out(int n, const int* __restrict__ perm, const double* __restrict__ scale, const double* __restrict__ xp,
+                           long long ldx, double* __restrict__ x, int w, long long fcol) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long c = blockIdx.y;
+  const long long oc = c < w ? c : fcol + c - w;
+  if (i < n) { const int o = perm[i]; x[oc * n + o] = scale[o] * xp[c * ldx + i]; }
+}
+
 // Sparse forward solve (b200ldlt_sparse_fwd_solve): the single-column sweep state of a forward sweep pruned to a run set
 // R of fronts.  Blocks [0, cdiv(ncol, 256)): x at the ncol positions of R, the scaled entry of b where b has one
 // (bi[j] >= 0: its index into the compact b; the same single multiply as k_rhs_in) and 0 elsewhere.  Blocks after that:
