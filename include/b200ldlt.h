@@ -209,6 +209,28 @@ int b200ldlt_enquire_zero_pivots(b200ldlt_handle h, int* nzero, int* pos);
 int b200ldlt_solve_fredholm(b200ldlt_handle h, int nrhs, double tol, double* x, int* consistent);
 int b200ldlt_solve_fredholm_device(b200ldlt_handle h, int nrhs, double tol, double* d_x, int* consistent);
 
+/* ---- selected inversion: the diagonal of A^-1 and A^-1 on the pattern of A (cf. MUMPS entries of A^-1, PSelInv) --------
+ * M = S P L^-T D^-1 L^-1 P^T S, the matrix job 0 applies: A^-1 for a non-singular factorisation, the inverse of the
+ * perturbed matrix with info.num_forced > 0, the D^+ pseudo-inverse on kept singular factors, and the altered D after
+ * alter_d.  diag[i] = M_ii (n doubles, original order); vals[t] = M at (irn[t], jcn[t]) (nonzeros doubles, one per triplet
+ * given to b200ldlt_analyse, the order of values_ptr): either triangle, and duplicates read the same stored entry, so they
+ * are bit-equal, and the diagonal triplets equal diag bit for bit.  Either pointer may be NULL, not both.  Z = L^-T D^-1
+ * L^-1 is computed on the pattern of L by the supernodal Takahashi recurrences, from the root down the elimination tree,
+ * every entry as one fixed-order sum: the results are bit-reproducible, and both entry points give the same bits.
+ * Kernel launches (info.launches_solve; info.ms_solve_gpu is the call's device time, host entry point: with its copies):
+ *   2 + sum over tree levels l of ( g_l + s_l + m_l + 2 b_l + c_l )
+ * with, for the fronts of level l (order f = pivots k + rows r): g_l = 1 if one has r > 0, s_l = 1 if one has f <= 96,
+ * m_l = 1 if one has 96 < f <= 256, b_l = 1 if one has f > 96 and r > 0, c_l = 1 if one has f > 96; else 0.
+ * The first call after an analysis allocates the Z panels (nnz_L doubles: info.L_bytes), L11^-1 of the fronts of order
+ * 97..256, the work lists and the output staging, before its timing starts; a handle that never calls allocates none of
+ * it.  The call uses the contribution blocks and the W scratch of the factorisation as its own scratch (no factorisation
+ * reads them before writing them) and leaves the factors, D, the solves and the counters untouched.
+ * FATAL_ERROR (message in last_error), with nothing written, when both pointers are NULL, without factors (also after
+ * SINGULAR in the default mode and after a lifted zero) and on a sharded handle.
+ * Device entry point: d_diag and d_vals are device memory. */
+int b200ldlt_selected_inverse(b200ldlt_handle h, double* diag, double* vals);
+int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* d_vals);
+
 /* <-> NumberOfNegEVals() (hpp:207) */
 int b200ldlt_num_neg(b200ldlt_handle h);
 /* <-> IncreaseQuality() (hpp:220): pivtol <- min(pivtolmax, pivtol^0.75); returns 0 if already at max.
@@ -274,7 +296,8 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
 int b200ldlt_shard_setup(b200ldlt_handle h, int rank, int world);
 /* "owner" (per supernode: owning rank, -1 = top part on rank 0), "cut_roots", "top_fronts" */
 int64_t b200ldlt_shard_array(b200ldlt_handle h, const char* name, int64_t* out, int64_t cap);
-/* device arrays of the handle: "CB" (contribution blocks, offsets cb_off), "cbv" (update vectors, offsets rows_ptr),
+/* device arrays of the handle: "CB" (contribution blocks, offsets cb_off; after b200ldlt_selected_inverse it holds that
+ * call's scratch until the next factorisation), "cbv" (update vectors, offsets rows_ptr),
  * "x" (permuted solution vector), "counters" (8 ints), "vals" (triplet values), "scale" (the n equilibration factors
  * S of the last factor call, original order) */
 void* b200ldlt_device_ptr(b200ldlt_handle h, const char* name);

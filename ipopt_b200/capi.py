@@ -59,7 +59,8 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_solve_partial", "b200ldlt_solve_partial_device", "b200ldlt_enquire_indef",
             "b200ldlt_lmultiply", "b200ldlt_lmultiply_device", "b200ldlt_alter_d",
             "b200ldlt_sparse_fwd_solve", "b200ldlt_sparse_fwd_solve_device", "b200ldlt_set_singular_action",
-            "b200ldlt_enquire_zero_pivots", "b200ldlt_solve_fredholm", "b200ldlt_solve_fredholm_device"]
+            "b200ldlt_enquire_zero_pivots", "b200ldlt_solve_fredholm", "b200ldlt_solve_fredholm_device",
+            "b200ldlt_selected_inverse", "b200ldlt_selected_inverse_device"]
 
 _lib = None
 
@@ -106,6 +107,8 @@ def load_library():
     L.b200ldlt_enquire_zero_pivots.argtypes = [vp, ip, ip]
     L.b200ldlt_solve_fredholm.argtypes = [vp, C.c_int, C.c_double, dp, ip]
     L.b200ldlt_solve_fredholm_device.argtypes = [vp, C.c_int, C.c_double, vp, ip]
+    L.b200ldlt_selected_inverse.argtypes = [vp, dp, dp]
+    L.b200ldlt_selected_inverse_device.argtypes = [vp, vp, vp]
     L.b200ldlt_num_neg.argtypes = [vp]
     L.b200ldlt_increase_quality.argtypes = [vp]
     L.b200ldlt_get_info.argtypes = [vp, C.POINTER(Info)]
@@ -353,6 +356,21 @@ class B200Ldlt:
         cons = np.zeros(max(int(nrhs), 1), np.int32)
         st = self._L.b200ldlt_solve_fredholm_device(self._h, int(nrhs), float(tol), C.c_void_p(d_x_ptr), _iptr(cons))
         return st, cons[:int(nrhs)].astype(bool)
+
+    def selected_inverse(self, diag=True, pattern=True):
+        """Entries of M = A^-1 (b200ldlt_selected_inverse): (diag, vals) -- diag[i] = M_ii (dim doubles, original order),
+        vals[t] = M at triplet t of the analysed pattern (nonzeros doubles) -- each None when not asked for."""
+        d = np.zeros(self.dim) if diag else None
+        v = np.zeros(self.nonzeros) if pattern else None
+        if self._L.b200ldlt_selected_inverse(self._h, None if d is None else _dptr(d),
+                                             None if v is None else _dptr(v)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return d, v
+
+    def selected_inverse_device(self, d_diag_ptr, d_vals_ptr):
+        """The same into device arrays (pointers as ints, 0 = not wanted). Returns the status."""
+        return self._L.b200ldlt_selected_inverse_device(self._h, C.c_void_p(d_diag_ptr or None),
+                                                        C.c_void_p(d_vals_ptr or None))
 
     def device_ptr(self, name):
         """Device address of a named array of the handle (b200ldlt_device_ptr: "scale", "x", "cbv", ...), 0 if none."""

@@ -20,6 +20,7 @@
 #include "solve_dataflow.cu"
 #include "lmul_kernels.cu"
 #include "schur_tc.cu"
+#include "selinv_kernels.cu"
 #include "symbolic.hpp"
 
 namespace b200 {
@@ -124,6 +125,26 @@ struct SparseFwdPlan {
   }
 };
 
+// selected inversion (b200ldlt_selected_inverse, selinv_kernels.cu): per tree level the fronts of each launch and the tile
+// items of the fronts above SI_SMALL, the Z panels, the L11^-1 of the fronts of order (SI_SMALL, SI_MID] and the index
+// maps of the output.  Built at the first call after an analysis, before its timing starts; a handle that never makes
+// the call allocates none of it.
+struct SelInvPlan {
+  struct Level {
+    int g_off = 0, g_cnt = 0;      // k_si_gather items (32-row column segments of the G of the fronts with r > 0)
+    int s_off = 0, s_cnt = 0;      // fronts of order <= SI_SMALL (k_si_small), their largest f^2 + k^2 doubles in smem
+    int m_off = 0, m_cnt = 0;      // fronts of order (SI_SMALL, SI_MID] (k_si_linv)
+    size_t smem = 0;
+    int t_off[3] = {0, 0, 0}, t_cnt[3] = {0, 0, 0};   // k_si_tile<PASS> items
+  };
+  std::vector<Level> lev;
+  DevBuf<double> d_Z, d_E, d_diag, d_vals;   // Z (layout of L), L11^-1 (ld k), staging of the host entry point
+  DevBuf<int> d_fronts, d_iperm, d_sn_of, d_lpinv, d_t2u;
+  DevBuf<long long> d_eoff;
+  DevBuf<SiItem> d_items;
+  DevBuf<SiGather> d_gather;
+};
+
 struct LevelPlan {
   // big fronts of the level: [big_off, big_off+big_cnt) in front_list
   int big_off = 0, big_cnt = 0, big_kmax = 0, big_fmax = 0, big_rmax = 0, big_chmax = 0;
@@ -226,6 +247,7 @@ struct Solver {
   DevBuf<long long> d_piv_big;      // n : per pivot position, its index in bigv (pivots of big fronts) or -1 (partial solves)
   std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call after an analysis
   std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve: built at its first call after an analysis
+  std::unique_ptr<SelInvPlan> selinv;   // selected inversion: built at its first call after an analysis
   DevBuf<double> d_alter;           // alter_d: the caller's 2n entries of D^-1 (allocated at the first call)
   DevBuf<int> d_alter_bad;
   // zero pivots (b200ldlt_set_singular_action): the factor kernels append every forced zero pivot to d_zlist; with
@@ -786,6 +808,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   sv->blk.reset();
   sv->lmul.reset();
   sv->sfs.reset();
+  sv->selinv.reset();
   if (sv->fgraph_exec) { cudaGraphExecDestroy(sv->fgraph_exec); sv->fgraph_exec = nullptr; }
   if (sv->fgraph) { cudaGraphDestroy(sv->fgraph); sv->fgraph = nullptr; }
   AnalyseOptions ao;
@@ -2212,6 +2235,144 @@ static int fredholm(Solver* sv, int nrhs, double tol, double* x, int* consistent
   sv->info.launches_solve = sv->launches;
   return B200LDLT_SUCCESS;
 }
+
+// ---- selected inversion (b200ldlt_selected_inverse) ----------------------------------------------------------------
+static_assert(SI_MID == DF_MIDMAX && SI_MID == kSolveMidMax, "the fronts above SI_MID read the factorisation's L11^-1");
+
+static int selinv_state(Solver* sv) {
+  if (sv->selinv) return B200LDLT_SUCCESS;
+  const Symbolic& S = sv->S;
+  const int n = S.n, nsn = S.nsn;
+  cudaStream_t st = sv->stream;
+  std::unique_ptr<SelInvPlan> P(new SelInvPlan());
+  std::vector<long long> linv_off(nsn);
+  CU(cudaMemcpy(linv_off.data(), sv->d_linv_off.p, nsn * sizeof(long long), cudaMemcpyDeviceToHost));
+  std::vector<long long> eoff(nsn, -1);
+  long long etot = 0;
+  for (int s = 0; s < nsn; ++s)
+    if (S.f(s) > SI_SMALL && S.f(s) <= SI_MID) { eoff[s] = etot; etot += (long long)S.k(s) * S.k(s); }
+  CU(P->d_E.alloc(std::max<long long>(etot, 1)));
+  std::vector<int> fronts;
+  std::vector<SiItem> items;
+  std::vector<SiGather> gather;
+  P->lev.assign(S.nlevels, SelInvPlan::Level());
+  for (int l = 0; l < S.nlevels; ++l) {
+    SelInvPlan::Level& L = P->lev[l];
+    const int q0 = S.level_ptr[l], q1 = S.level_ptr[l + 1];
+    L.g_off = (int)gather.size();
+    for (int q = q0; q < q1; ++q) {
+      const int s = S.level_sn[q], r = S.r(s);
+      for (int b = 0; b < r; ++b)
+        for (int a0 = b; a0 < r; a0 += 32) gather.push_back(SiGather{s, b, a0});
+    }
+    L.g_cnt = (int)gather.size() - L.g_off;
+    L.s_off = (int)fronts.size();
+    for (int q = q0; q < q1; ++q) {
+      const int s = S.level_sn[q];
+      if (S.f(s) > SI_SMALL) continue;
+      fronts.push_back(s);
+      L.smem = std::max(L.smem, ((size_t)S.f(s) * S.f(s) + (size_t)S.k(s) * S.k(s)) * sizeof(double));
+    }
+    L.s_cnt = (int)fronts.size() - L.s_off;
+    L.m_off = (int)fronts.size();
+    for (int q = q0; q < q1; ++q) if (S.f(S.level_sn[q]) > SI_SMALL && S.f(S.level_sn[q]) <= SI_MID) fronts.push_back(S.level_sn[q]);
+    L.m_cnt = (int)fronts.size() - L.m_off;
+    for (int pass = 0; pass < 3; ++pass) {
+      L.t_off[pass] = (int)items.size();
+      for (int q = q0; q < q1; ++q) {
+        const int s = S.level_sn[q], k = S.k(s), r = S.r(s);
+        if (S.f(s) <= SI_SMALL) continue;
+        const bool big = S.f(s) > SI_MID;
+        const int ld_e = big ? (k + DF_BLK - 1) / DF_BLK * DF_BLK : k;
+        const double* E = big ? sv->d_linv.p + linv_off[s] : P->d_E.p + eoff[s];
+        const int nkb = (k + 63) / 64, nrb = (r + 63) / 64;
+        if (pass < 2) {
+          for (int ib = 0; ib < nrb; ++ib)
+            for (int jb = 0; jb < nkb; ++jb) items.push_back(SiItem{s, ib, jb, ld_e, E});
+        } else {
+          for (int ib = 0; ib < nkb; ++ib)
+            for (int jb = 0; jb <= ib; ++jb) items.push_back(SiItem{s, ib, jb, ld_e, E});
+        }
+      }
+      L.t_cnt[pass] = (int)items.size() - L.t_off[pass];
+    }
+  }
+  std::vector<int> iperm(n), sn_of(n);
+  for (int i = 0; i < n; ++i) iperm[S.perm[i]] = i;
+  for (int s = 0; s < nsn; ++s)
+    for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) sn_of[p] = s;
+  CU(P->d_fronts.upload(fronts, st));
+  CU(P->d_items.upload(items, st));
+  CU(P->d_gather.upload(gather, st));
+  CU(P->d_eoff.upload(eoff, st));
+  CU(P->d_iperm.upload(iperm, st));
+  CU(P->d_sn_of.upload(sn_of, st));
+  CU(P->d_t2u.upload(S.t2u, st));
+  CU(P->d_lpinv.alloc(n));
+  CU(P->d_Z.alloc(S.L_off[nsn]));
+  CU(cudaMemsetAsync(P->d_Z.p, 0, P->d_Z.n * sizeof(double), st));
+  CU(P->d_diag.alloc(n));
+  CU(P->d_vals.alloc(sv->nnz));
+  // a constant limit, as for the factor kernels: the attribute is per process, so a per-handle value would change it
+  // under the other handles
+  CU(cudaFuncSetAttribute(k_si_small, cudaFuncAttributeMaxDynamicSharedMemorySize, SI_SMALL_SMEM));
+  CU(cudaStreamSynchronize(st));
+  if (sv->opt.verbose)
+    fprintf(stderr, "[b200ldlt] selected inversion: %zu tile items, Z %.1f MB, L11^-1 (orders %d..%d) %.1f MB\n",
+            items.size(), 8e-6 * (double)S.L_off[nsn], SI_SMALL + 1, SI_MID, 8e-6 * (double)etot);
+  sv->selinv = std::move(P);
+  return B200LDLT_SUCCESS;
+}
+
+// top level first: per level gather, small fronts, L11^-1 of the middle fronts, the three tile passes; then the output
+static int enqueue_selinv(Solver* sv, double* d_diag, double* d_vals) {
+  const SelInvPlan& P = *sv->selinv;
+  const Symbolic& S = sv->S;
+  cudaStream_t st = sv->stream;
+  const int n = S.n;
+  int& L = sv->launches;
+  k_si_prep<<<cdiv(n, 256), 256, 0, st>>>(n, P.d_sn_of.p, sv->d_sn_start.p, sv->d_lperm.p, P.d_lpinv.p); ++L;
+  for (int l = S.nlevels - 1; l >= 0; --l) {
+    const SelInvPlan::Level& V = P.lev[l];
+    if (V.g_cnt) { k_si_gather<<<cdiv(V.g_cnt, 8), 256, 0, st>>>(sv->DS, P.d_Z.p, sv->d_CB.p, P.d_lpinv.p, P.d_gather.p + V.g_off, V.g_cnt); ++L; }
+    if (V.s_cnt) { k_si_small<<<V.s_cnt, 128, V.smem, st>>>(sv->DS, sv->DN, P.d_Z.p, P.d_fronts.p + V.s_off); ++L; }
+    if (V.m_cnt) { k_si_linv<<<V.m_cnt, 256, 0, st>>>(sv->DS, sv->DN, P.d_fronts.p + V.m_off, P.d_eoff.p, P.d_E.p); ++L; }
+    if (V.t_cnt[0]) { k_si_tile<0><<<V.t_cnt[0], 256, 0, st>>>(sv->DS, sv->DN, P.d_Z.p, P.d_items.p + V.t_off[0]); ++L; }
+    if (V.t_cnt[1]) { k_si_tile<1><<<V.t_cnt[1], 256, 0, st>>>(sv->DS, sv->DN, P.d_Z.p, P.d_items.p + V.t_off[1]); ++L; }
+    if (V.t_cnt[2]) { k_si_tile<2><<<V.t_cnt[2], 256, 0, st>>>(sv->DS, sv->DN, P.d_Z.p, P.d_items.p + V.t_off[2]); ++L; }
+  }
+  k_si_out<<<cdiv(std::max<long long>(n, sv->nnz), 256), 256, 0, st>>>(
+      n, sv->nnz, P.d_iperm.p, P.d_sn_of.p, sv->d_sn_start.p, sv->d_rows_ptr.p, sv->d_L_off.p, P.d_lpinv.p, P.d_Z.p,
+      sv->d_scale.p, sv->d_irn.p, sv->d_jcn.p, P.d_t2u.p, sv->d_u_dst64.p, d_diag, d_vals);
+  ++L;
+  CU(cudaGetLastError());
+  return B200LDLT_SUCCESS;
+}
+
+// b200ldlt_selected_inverse (host == true: diag and vals in host memory) / _device
+static int selected_inverse(Solver* sv, double* diag, double* vals, bool host) {
+  const char* why = nullptr;
+  if (!diag && !vals) why = "diag and vals are both NULL";
+  else if (!sv->factored) why = "no factors (factorise first; a SINGULAR factorisation keeps them only in keep mode, see b200ldlt_set_singular_action)";
+  else if (sv->shard.active) why = "not available on a sharded handle";
+  if (why) { sv->err = std::string("selected_inverse: ") + why; return B200LDLT_FATAL_ERROR; }
+  CU(cudaSetDevice(sv->dev));
+  cudaStream_t st = sv->stream;
+  { const int rc = selinv_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
+  SelInvPlan& P = *sv->selinv;
+  double* dd = diag ? (host ? P.d_diag.p : diag) : nullptr;
+  double* dv = vals ? (host ? P.d_vals.p : vals) : nullptr;
+  sv->launches = 0;
+  CU(cudaEventRecord(sv->ev0, st));
+  { const int rc = enqueue_selinv(sv, dd, dv); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (host && diag) CU(cudaMemcpyAsync(diag, dd, (size_t)sv->n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (host && vals) CU(cudaMemcpyAsync(vals, dv, (size_t)sv->nnz * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(sv->ev1, st));
+  CU(cudaStreamSynchronize(st));
+  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
+  sv->info.launches_solve = sv->launches;
+  return B200LDLT_SUCCESS;
+}
 }  // namespace b200
 
 extern "C" {
@@ -2385,6 +2546,18 @@ int b200ldlt_solve_fredholm_device(b200ldlt_handle h, int nrhs, double tol, doub
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
   return fredholm(sv, nrhs, tol, d_x, consistent, false);
+}
+
+int b200ldlt_selected_inverse(b200ldlt_handle h, double* diag, double* vals) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return selected_inverse(sv, diag, vals, true);
+}
+
+int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* d_vals) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return selected_inverse(sv, d_diag, d_vals, false);
 }
 
 /* ---- multi-GPU elimination-tree sharding (SURVEY.md section 8e) -------------------------------------------
