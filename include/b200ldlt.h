@@ -95,13 +95,26 @@ int b200ldlt_factor_device(b200ldlt_handle h, const double* d_vals, int check_in
  * nrhs > 1: the columns are solved in blocks of up to 8 (environment B200_SOLVE_BLOCK=n at b200ldlt_create caps the
  * width, 1 = one solve per column), one forward and one backward sweep per block; every column is bit-identical to a
  * solve of that column alone.  The first such call after an analysis allocates per-column device state for the full width
- * (before its timing starts); if that allocation fails, the columns are solved one by one.  info.launches_solve /
- * ms_solve_gpu describe the whole call. */
+ * (before its timing starts); if that allocation fails, the columns are solved one by one.  Refusals, timing and
+ * calls without columns: see the head of the next section. */
 int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs);
 /* Same with a device-resident rhs/solution. */
 int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs);
 
 /* ---- partial solves and factor inspection (cf. MA57 / HSL_MA97 job 1-4, Pardiso phases 331-333) ---------------------
+ * The calls that read the factors -- solve and the calls below -- share three rules:
+ *   refusals : FATAL_ERROR with "<call>: <reason>" in last_error and nothing written, first for the call's own
+ *              arguments (listed with each call), then without factors (never factorised, after a SINGULAR factorisation
+ *              outside keep mode, after a lifted zero) and on a sharded handle -- solve, enquire_indef and
+ *              enquire_zero_pivots accept a sharded handle;
+ *   timing   : info.launches_solve counts the call's kernel launches and info.ms_solve_gpu is its device time (host entry
+ *              point: with its copies); per-analysis state a call builds at its first use is built before its timing
+ *              starts (alter_d, enquire_indef and enquire_zero_pivots are not timed and leave both as they are);
+ *   no columns: nrhs <= 0 for solve, solve_partial and lmultiply, nrhs = 0 for solve_fredholm and nbi = 0 for
+ *              sparse_fwd_solve succeed, write nothing to the caller's arrays, launch nothing and set launches_solve and
+ *              ms_solve_gpu to 0.
+ * Host entry points copy through pinned staging owned by the handle, which grows to the largest call and is freed by
+ * the next analysis.
  * The factor call computes  S A S = P L D L^T P^T :  S the diagonal (power-of-two) equilibration of that call
  * (device_ptr "scale"), P the fill-reducing permutation composed with the pivoting inside the supernodes, L unit lower
  * triangular, D block diagonal with 1x1 and 2x2 blocks.  Intermediate vectors are indexed by PIVOT POSITION p = 0..n-1.
@@ -112,10 +125,9 @@ int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs);
  *   job 4 : x = S P L^-T D^-1 b             pivot -> original
  * job 3 . 2 . 1 = job 4 . 1 = job 0, bit for bit: the parts run the arithmetic of the full solve.  nrhs > 1 is blocked
  * like b200ldlt_solve, and every column is bit-identical to a partial solve of that column alone.  Kernel launches per
- * block (info.launches_solve; ms_solve_gpu as for job 0): job 1, 3, 4: 5 and job 2: 1 (job 0: 8) -- with the default
- * B200_SOLVE_DIRECT=2; in general job 1, 3, 4 take 3 + D and job 0 takes 4 + 2 D for D direct levels.
- * FATAL_ERROR (message in last_error) for a job outside 0..4, without factors (also after a SINGULAR factorisation) and
- * on a sharded handle.  With info.num_forced > 0, D holds the lifted pivots: the parts describe the perturbed matrix. */
+ * block: job 1, 3, 4: 5 and job 2: 1 (job 0: 8) -- with the default B200_SOLVE_DIRECT=2; in general job 1, 3, 4 take
+ * 3 + D and job 0 takes 4 + 2 D for D direct levels.  Refused: a job outside 0..4.  With info.num_forced > 0, D holds
+ * the lifted pivots: the parts describe the perturbed matrix. */
 int b200ldlt_solve_partial(b200ldlt_handle h, int job, int nrhs, double* rhs);
 int b200ldlt_solve_partial_device(b200ldlt_handle h, int job, int nrhs, double* d_rhs);
 /* Per pivot position p (any pointer may be NULL): pivot_var[p] = the 0-based original variable; pivot_type[p] = 1 (1x1),
@@ -133,15 +145,13 @@ int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, d
  * that position as a value (they may differ in the sign of a zero), and repeated calls give the same bits.
  * Device entry point: only the values are device memory -- d_b (nbi doubles) and d_x (room for n doubles); bindex,
  * nxi and xindex are host memory in both entry points (the pruned work lists are built on the host from the pattern).
- * Kernel launches (info.launches_solve): 2 + d + t, where d is the number of the B200_SOLVE_DIRECT bottom tree levels
- * that hold a front of the reach solved by the direct kernel, and t = 1 when the reach has a front above those levels
- * (always, unless the whole tree is made of direct fronts), else 0; nbi = 0 makes none.  info.ms_solve_gpu is the call's
- * device time (host entry point: with its copies).  The first call after an analysis builds per-front indices into the
+ * Kernel launches: 2 + d + t, where d is the number of the B200_SOLVE_DIRECT bottom tree levels that hold a front of
+ * the reach solved by the direct kernel, and t = 1 when the reach has a front above those levels (always, unless the
+ * whole tree is made of direct fronts), else 0.  The first call after an analysis builds per-front indices into the
  * solve's work lists, and pinned and device staging for the pruned lists (about 28 bytes per variable plus 40 per
- * forward top task each), before its timing starts; a handle that never makes the call allocates none of it.
- * FATAL_ERROR (message in last_error), with nothing written to nxi, xindex or x, for nbi < 0 or nbi > n, a NULL pointer
- * with nbi > 0, an index out of range or repeated, without factors (also after SINGULAR) and on a sharded handle.
- * nbi = 0 succeeds with *nxi = 0. */
+ * forward top task each); a handle that never makes the call allocates none of it.  Refused (nothing written to nxi,
+ * xindex or x): nbi < 0 or nbi > n, a NULL pointer with nbi > 0, an index out of range or repeated.  nbi = 0 sets
+ * *nxi = 0. */
 int b200ldlt_sparse_fwd_solve(b200ldlt_handle h, int nbi, const int* bindex, const double* b, int* nxi, int* xindex, double* x);
 int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bindex, const double* d_b, int* nxi, int* xindex,
                                      double* d_x);
@@ -154,19 +164,16 @@ int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bind
  * as the factorisation left it, so  lmultiply(0, D lmultiply(1, v))  =  A v  up to rounding (with
  * info.num_forced > 0: the perturbed matrix).  Results are bit-reproducible; nrhs > 1 runs in blocks of up to 8 columns
  * (B200_SOLVE_BLOCK, as for the solves), L streamed once per block, every column bit-identical to a call on that column
- * alone.  Kernel launches: 2 per block (trans 0: multiply + gather; trans 1: copy-in + multiply), in info.launches_solve;
- * info.ms_solve_gpu is the call's device time (host entry point: with its copies).  The first call after an analysis
- * builds the work lists and slot map (about 8 bytes per panel row and column chunk: 9 MB per column at MBndryCntrl1
- * N=400) before its timing starts; a handle that never multiplies allocates none of it.
- * FATAL_ERROR (message in last_error) for trans other than 0 / 1, without factors (also after SINGULAR) and on a sharded
- * handle. */
+ * alone.  Kernel launches: 2 per block (trans 0: multiply + gather; trans 1: copy-in + multiply).  The first call after
+ * an analysis builds the work lists and slot map (about 8 bytes per panel row and column chunk: 9 MB per column at
+ * MBndryCntrl1 N=400); a handle that never multiplies allocates none of it.  Refused: trans other than 0 / 1. */
 int b200ldlt_lmultiply(b200ldlt_handle h, int trans, int nrhs, const double* x, double* y);
 int b200ldlt_lmultiply_device(b200ldlt_handle h, int trans, int nrhs, const double* d_x, double* d_y);
 /* Replace D^-1 by the caller's, 2n doubles in the layout of enquire_indef (dinv2[2p] diagonal, dinv2[2p+1] off-diagonal
- * (p, p+1), host memory); the pivot types stay.  Refused with FATAL_ERROR -- and D left exactly as it was -- when an
- * entry is not finite or an off-diagonal entry is non-zero at a p that does not open a 2x2 pivot (also in the cases
- * lmultiply refuses).  Every later solve, partial solve and enquire_indef use the new D until the next factor or refactor
- * call, which computes D afresh.  num_neg and b200ldlt_info keep describing the factorisation, not the altered D. */
+ * (p, p+1), host memory); the pivot types stay.  Refused -- and D left exactly as it was -- for a NULL dinv2, and when
+ * an entry is not finite or an off-diagonal entry is non-zero at a p that does not open a 2x2 pivot.  Every later
+ * solve, partial solve and enquire_indef use the new D until the next factor or refactor call, which computes D afresh.
+ * num_neg and b200ldlt_info keep describing the factorisation, not the altered D. */
 int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2);
 
 /* ---- singular matrices: zero pivots and the Fredholm alternative (cf. HSL_MA97 action, ma97_solve_fredholm) ----------
@@ -186,7 +193,7 @@ int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2);
  * factorisation is the same, bit for bit and launch for launch, in both modes.  keep must be 0 or 1. */
 int b200ldlt_set_singular_action(b200ldlt_handle h, int keep);
 /* *nzero = |Z| and, unless pos is NULL, pos[0..|Z|) = the pivot positions of Z in ascending order (0 for a factorisation
- * without zero pivots).  FATAL_ERROR without factors. */
+ * without zero pivots).  Refused: a NULL nzero. */
 int b200ldlt_enquire_zero_pivots(b200ldlt_handle h, int* nzero, int* pos);
 /* The Fredholm alternative for nrhs columns b_i.  x is n x 2 nrhs, column-major: on entry columns 0..nrhs-1 hold the b_i;
  * on exit column i holds x_i and column nrhs + i holds f_i, and consistent[i] is 1 or 0.  With y = L^-1 P^T S b (job 1) and
@@ -198,14 +205,12 @@ int b200ldlt_enquire_zero_pivots(b200ldlt_handle h, int* nzero, int* pos);
  *                        column -- a certificate that b is not in the range of A.
  * f is formed for every column whenever Z is non-empty; with Z empty x is job 0, f = 0 and every column is consistent.
  * Z is that of the factorisation; D is read from D^-1 as it stands (alter_d may overwrite the zeros at Z).  Every column
- * is bit-identical to a call on that column alone.  Kernel launches (info.launches_solve), D direct levels
- * (B200_SOLVE_DIRECT, default 2): with the blocked state (B200_SOLVE_BLOCK >= 2), blocks of up to B200_SOLVE_BLOCK / 2
- * columns (4 by default) with x and f through ONE backward sweep of twice the width: 5 + 2 D per block (9 by default);
- * with B200_SOLVE_BLOCK = 1, two backward sweeps per column: 8 + 3 D per column (14); with Z empty, job 0's count.  The
- * first call with Z non-empty allocates the blocked state as a blocked solve does.
- * FATAL_ERROR (message in last_error), with nothing written, for nrhs < 0, tol < 0 or NaN, a NULL pointer with nrhs > 0,
- * without factors (also after SINGULAR in the default mode and after a lifted zero) and on a sharded handle.
- * Device entry point: the columns d_x are device memory, consistent host memory. */
+ * is bit-identical to a call on that column alone.  Kernel launches, D direct levels (B200_SOLVE_DIRECT, default 2):
+ * with the blocked state (B200_SOLVE_BLOCK >= 2), blocks of up to B200_SOLVE_BLOCK / 2 columns (4 by default) with x
+ * and f through ONE backward sweep of twice the width: 5 + 2 D per block (9 by default); with B200_SOLVE_BLOCK = 1, two
+ * backward sweeps per column: 8 + 3 D per column (14); with Z empty, job 0's count.  The first call with Z non-empty
+ * allocates the blocked state as a blocked solve does.  Refused: nrhs < 0, tol < 0 or NaN, a NULL pointer with
+ * nrhs > 0.  Device entry point: the columns d_x are device memory, consistent host memory. */
 int b200ldlt_solve_fredholm(b200ldlt_handle h, int nrhs, double tol, double* x, int* consistent);
 int b200ldlt_solve_fredholm_device(b200ldlt_handle h, int nrhs, double tol, double* d_x, int* consistent);
 
@@ -217,16 +222,13 @@ int b200ldlt_solve_fredholm_device(b200ldlt_handle h, int nrhs, double tol, doub
  * are bit-equal, and the diagonal triplets equal diag bit for bit.  Either pointer may be NULL, not both.  Z = L^-T D^-1
  * L^-1 is computed on the pattern of L by the supernodal Takahashi recurrences, from the root down the elimination tree,
  * every entry as one fixed-order sum: the results are bit-reproducible, and both entry points give the same bits.
- * Kernel launches (info.launches_solve; info.ms_solve_gpu is the call's device time, host entry point: with its copies):
- *   2 + sum over tree levels l of ( g_l + s_l + m_l + 2 b_l + c_l )
+ * Kernel launches:  2 + sum over tree levels l of ( g_l + s_l + m_l + 2 b_l + c_l )
  * with, for the fronts of level l (order f = pivots k + rows r): g_l = 1 if one has r > 0, s_l = 1 if one has f <= 96,
  * m_l = 1 if one has 96 < f <= 256, b_l = 1 if one has f > 96 and r > 0, c_l = 1 if one has f > 96; else 0.
  * The first call after an analysis allocates the Z panels (nnz_L doubles: info.L_bytes), L11^-1 of the fronts of order
- * 97..256, the work lists and the output staging, before its timing starts; a handle that never calls allocates none of
- * it.  The call uses the contribution blocks and the W scratch of the factorisation as its own scratch (no factorisation
- * reads them before writing them) and leaves the factors, D, the solves and the counters untouched.
- * FATAL_ERROR (message in last_error), with nothing written, when both pointers are NULL, without factors (also after
- * SINGULAR in the default mode and after a lifted zero) and on a sharded handle.
+ * 97..256, the work lists and the output staging; a handle that never calls allocates none of it.  The call uses the
+ * contribution blocks and the W scratch of the factorisation as its own scratch (no factorisation reads them before
+ * writing them) and leaves the factors, D, the solves and the counters untouched.  Refused: both pointers NULL.
  * Device entry point: d_diag and d_vals are device memory. */
 int b200ldlt_selected_inverse(b200ldlt_handle h, double* diag, double* vals);
 int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* d_vals);

@@ -31,11 +31,13 @@ struct DevBuf {
   size_t n = 0;
   ~DevBuf() { release(); }
   void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
+  // n is the size only once the memory is there: a failed allocation leaves the buffer released (p null, n 0)
   cudaError_t alloc(size_t count) {
     release();
-    n = count;
     if (count == 0) return cudaSuccess;
-    return cudaMalloc((void**)&p, count * sizeof(T));
+    const cudaError_t e = cudaMalloc((void**)&p, count * sizeof(T));
+    if (e == cudaSuccess) n = count; else p = nullptr;
+    return e;
   }
   template <class U>
   cudaError_t upload(const std::vector<U>& v, cudaStream_t st) {
@@ -200,13 +202,12 @@ struct Solver {
   size_t ev_next = 0;
   bool own_stream = false;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_zero = nullptr;
-  cudaEvent_t ev_chunk[4] = {nullptr, nullptr, nullptr, nullptr};   // D2H chunks of the host solve path
+  cudaEvent_t ev_chunk[4] = {nullptr, nullptr, nullptr, nullptr};   // D2H chunks of staged_call
 
   int n = 0, nnz = 0;
   std::vector<int> irn, jcn;
   double* h_vals = nullptr;      // pinned
-  double* h_rhs = nullptr;       // pinned staging (n * rhs_cap)
-  int rhs_cap = 0;
+  double* h_rhs = nullptr;       // pinned staging of the host entry points: d_rhs.n doubles, like d_rhs (staged_call)
   int* h_counters = nullptr;     // pinned
   bool analysed = false, factored = false, have_dev_vals = false;
   b200vec_ctx vec = nullptr;       // vector kernels on the handle's stream (device-side refinement)
@@ -305,6 +306,11 @@ struct Solver {
   cudaEvent_t next_event() {
     if (ev_next == ev_pool.size()) { cudaEvent_t e; cudaEventCreateWithFlags(&e, cudaEventDisableTiming); ev_pool.push_back(e); }
     return ev_pool[ev_next++];
+  }
+  void drop_staging() {
+    if (h_rhs) cudaFreeHost(h_rhs);
+    h_rhs = nullptr;
+    d_rhs.release();
   }
 };
 
@@ -803,8 +809,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   // a (re-)analysis invalidates the factors and every buffer sized by the old plan
   sv->factored = false;
   sv->reanalyse = false;
-  if (sv->h_rhs) { cudaFreeHost(sv->h_rhs); sv->h_rhs = nullptr; }
-  sv->rhs_cap = 0;
+  sv->drop_staging();
   sv->blk.reset();
   sv->lmul.reset();
   sv->sfs.reset();
@@ -847,7 +852,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   CU(sv->d_W.alloc(S.L_off[S.nsn]));
   CU(sv->d_CB.alloc(std::max<int64_t>(S.cb_off[S.nsn], 1)));
   CU(sv->d_dinv.alloc(n)); CU(sv->d_doff.alloc(n)); CU(sv->d_scale.alloc(n));
-  CU(sv->d_rhs.alloc(n)); CU(sv->d_res.alloc(n));
+  CU(sv->d_res.alloc(n));
   CU(sv->d_ptype.alloc(n)); CU(sv->d_lperm.alloc(n)); CU(sv->d_bperm.alloc(n));
   CU(sv->d_counters.alloc(CNT_N));
   CU(sv->d_zlist.alloc(n)); CU(sv->d_zflag.alloc(n));
@@ -2023,8 +2028,7 @@ int b200ldlt_analyse(b200ldlt_handle h, int dim, int nonzeros, const int* irn, c
   memset(sv->h_vals, 0, std::max<size_t>(nonzeros, 1) * sizeof(double));
   sv->analysed = false; sv->factored = false; sv->have_dev_vals = false;
   if (sv->amat) { b200vec_tmat_destroy(sv->amat); sv->amat = nullptr; }
-  if (sv->h_rhs) { cudaFreeHost(sv->h_rhs); sv->h_rhs = nullptr; }
-  sv->rhs_cap = 0;   // staging buffers are sized by dim: a new structure invalidates them
+  sv->drop_staging();
   return B200LDLT_SUCCESS;
 }
 
@@ -2058,181 +2062,165 @@ int b200ldlt_refactor(b200ldlt_handle h, int check_inertia, int expected_neg, in
 }  // extern "C"
 
 namespace b200 {
-// the solve (job 0) or one part of it (job 1..4) on device-resident columns
-static int solve_device_job(Solver* sv, int job, int nrhs, double* d_rhs) {
-  CU(cudaSetDevice(sv->dev));
+// ---- the calls that read the factors (include/b200ldlt.h, from the partial solves on) -------------------------------
+// The state check, after the call's own argument checks: FATAL_ERROR with "<call>: ..." in last_error without factors
+// and, unless sharded_ok, on a sharded handle; otherwise the handle's device is selected for what follows.
+static int factors_state(Solver* sv, const char* call, bool sharded_ok = false) {
+  if (!sv->factored)
+    sv->err = std::string(call) + ": no factors (factorise first; a SINGULAR factorisation keeps them only in keep mode, "
+                                  "see b200ldlt_set_singular_action)";
+  else if (sv->shard.active && !sharded_ok) sv->err = std::string(call) + ": not available on a sharded handle";
+  else { CU(cudaSetDevice(sv->dev)); return B200LDLT_SUCCESS; }
+  return B200LDLT_FATAL_ERROR;
+}
+
+// a call without columns: succeeds, launches nothing, writes nothing to the caller's arrays
+static int no_columns(Solver* sv) {
+  sv->info.launches_solve = 0;
+  sv->info.ms_solve_gpu = 0.0f;
+  return B200LDLT_SUCCESS;
+}
+
+// The timed part of a call: enqueue() between the events ev0 and ev1 with the launch count from 0, then drain() (host
+// work under the tail of the stream: the copy-out of staged_call) and the synchronise; info.ms_solve_gpu and
+// launches_solve then describe the call.  Lazy state is built by the caller before, outside the window.
+struct NoDrain { int operator()() const { return B200LDLT_SUCCESS; } };
+template <class Enqueue, class Drain = NoDrain>
+static int timed_call(Solver* sv, Enqueue&& enqueue, Drain&& drain = Drain()) {
   cudaStream_t st = sv->stream;
-  const bool blocked = nrhs > 1 && block_solve_state(sv);
   sv->launches = 0;
   CU(cudaEventRecord(sv->ev0, st));
-  {
-    int rc = enqueue_solve_columns(sv, d_rhs, nrhs, blocked, job);
-    if (rc != B200LDLT_SUCCESS) return rc;
-  }
+  { const int rc = enqueue(); if (rc != B200LDLT_SUCCESS) return rc; }
   CU(cudaEventRecord(sv->ev1, st));
+  { const int rc = drain(); if (rc != B200LDLT_SUCCESS) return rc; }
   CU(cudaStreamSynchronize(st));
   cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
   sv->info.launches_solve = sv->launches;
   return B200LDLT_SUCCESS;
 }
 
-// the same on host columns: staged through pinned memory in chunks (see b200ldlt_solve)
-static int solve_host_job(Solver* sv, int job, int nrhs, double* rhs) {
-  if (nrhs <= 0) return B200LDLT_SUCCESS;
-  CU(cudaSetDevice(sv->dev));
+// A timed call on host columns: nin doubles of `in` to the device staging, enqueue(its device address), nout doubles
+// back to `out` (which may be `in`), the copies inside the timed window.  Each way the copies run in at most four
+// chunks, so that the DMA of one chunk runs under the host copy of the next (the caller's array is pageable: Ipopt
+// allocates it per call, IpTSymLinearSolver.cpp:222-241).  The staging grows to the largest call and lasts until the
+// next analysis.
+template <class Enqueue>
+static int staged_call(Solver* sv, const double* in, size_t nin, double* out, size_t nout, Enqueue&& enqueue) {
+  const size_t need = std::max(nin, nout);
+  if (need > sv->d_rhs.n) {
+    sv->drop_staging();
+    CU(cudaHostAlloc((void**)&sv->h_rhs, need * sizeof(double), cudaHostAllocDefault));
+    CU(sv->d_rhs.alloc(need));   // (so d_rhs.n counts the doubles of both buffers, 0 when either is missing)
+  }
   cudaStream_t st = sv->stream;
-  const size_t n = sv->n;
-  if (nrhs > sv->rhs_cap) {
-    if (sv->h_rhs) cudaFreeHost(sv->h_rhs);
-    sv->h_rhs = nullptr;
-    CU(cudaHostAlloc((void**)&sv->h_rhs, n * nrhs * sizeof(double), cudaHostAllocDefault));
-    CU(sv->d_rhs.alloc(n * nrhs));
-    sv->rhs_cap = nrhs;
-  }
-  // Host rhs -> pinned staging -> device in chunks, so that the DMA of one chunk runs under the host copy of the next (the
-  // caller's array is pageable: Ipopt allocates it per call, IpTSymLinearSolver.cpp:222-241); same on the way back.
-  const size_t total = n * (size_t)nrhs;
-  const size_t chunk = std::max<size_t>((total + 3) / 4, 32768);
+  double* h = sv->h_rhs;
+  double* d = sv->d_rhs.p;
+  auto chunk = [](size_t total) { return std::max<size_t>((total + 3) / 4, 32768); };   // at most 4: ev_chunk
+  const size_t ci = chunk(nin), co = chunk(nout);
+  auto copy_out = [&]() -> int {
+    for (size_t o = 0, k = 0; o < nout; o += co, ++k) {
+      CU(cudaEventSynchronize(sv->ev_chunk[k]));
+      memcpy(out + o, h + o, std::min(co, nout - o) * sizeof(double));
+    }
+    return B200LDLT_SUCCESS;
+  };
+  return timed_call(sv, [&]() -> int {
+    for (size_t o = 0; o < nin; o += ci) {
+      const size_t m = std::min(ci, nin - o);
+      memcpy(h + o, in + o, m * sizeof(double));
+      CU(cudaMemcpyAsync(d + o, h + o, m * sizeof(double), cudaMemcpyHostToDevice, st));
+    }
+    { const int rc = enqueue(d); if (rc != B200LDLT_SUCCESS) return rc; }
+    for (size_t o = 0, k = 0; o < nout; o += co, ++k) {
+      CU(cudaMemcpyAsync(h + o, d + o, std::min(co, nout - o) * sizeof(double), cudaMemcpyDeviceToHost, st));
+      CU(cudaEventRecord(sv->ev_chunk[k], st));
+    }
+    return B200LDLT_SUCCESS;
+  }, copy_out);
+}
+
+// b200ldlt_solve (job 0) and b200ldlt_solve_partial (job 1..4) on nrhs columns of x, in place (host == true: x in host
+// memory) / _device
+static int solve_job(Solver* sv, int job, int nrhs, double* x, bool host) {
+  if (job < 0 || job > 4) { sv->err = "solve_partial: job must be 0..4"; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, job == 0 ? "solve" : "solve_partial", job == 0); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (nrhs <= 0) return no_columns(sv);
   const bool blocked = nrhs > 1 && block_solve_state(sv);
-  sv->launches = 0;
-  CU(cudaEventRecord(sv->ev0, st));
-  for (size_t o = 0; o < total; o += chunk) {
-    const size_t m = std::min(chunk, total - o);
-    memcpy(sv->h_rhs + o, rhs + o, m * sizeof(double));
-    CU(cudaMemcpyAsync(sv->d_rhs.p + o, sv->h_rhs + o, m * sizeof(double), cudaMemcpyHostToDevice, st));
-  }
-  {
-    int rc = enqueue_solve_columns(sv, sv->d_rhs.p, nrhs, blocked, job);
-    if (rc != B200LDLT_SUCCESS) return rc;
-  }
-  int nchunk = 0;
-  for (size_t o = 0; o < total; o += chunk, ++nchunk) {
-    const size_t m = std::min(chunk, total - o);
-    CU(cudaMemcpyAsync(sv->h_rhs + o, sv->d_rhs.p + o, m * sizeof(double), cudaMemcpyDeviceToHost, st));
-    if (nchunk < 4) CU(cudaEventRecord(sv->ev_chunk[nchunk], st));
-  }
-  CU(cudaEventRecord(sv->ev1, st));
-  nchunk = 0;
-  for (size_t o = 0; o < total; o += chunk, ++nchunk) {
-    const size_t m = std::min(chunk, total - o);
-    if (nchunk < 4) CU(cudaEventSynchronize(sv->ev_chunk[nchunk])); else CU(cudaStreamSynchronize(st));
-    memcpy(rhs + o, sv->h_rhs + o, m * sizeof(double));
-  }
-  CU(cudaStreamSynchronize(st));
-  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
-  sv->info.launches_solve = sv->launches;
-  return B200LDLT_SUCCESS;
+  auto enqueue = [&](double* d) { return enqueue_solve_columns(sv, d, nrhs, blocked, job); };
+  const size_t cnt = (size_t)sv->n * nrhs;
+  return host ? staged_call(sv, x, cnt, x, cnt, enqueue) : timed_call(sv, [&] { return enqueue(x); });
 }
 
-// job 1..4 are refused (FATAL_ERROR + last_error) out of range, without factors and on a sharded handle
-static bool partial_refused(Solver* sv, int job) {
-  if (job < 1 || job > 4) sv->err = "solve_partial: job must be 0..4";
-  else if (!sv->factored) sv->err = "solve_partial: no factors (factorise first; a SINGULAR factorisation leaves none)";
-  else if (sv->shard.active) sv->err = "solve_partial: not available on a sharded handle";
-  else return false;
-  return true;
-}
-
-// lmultiply / alter_d are refused in the same cases as the partial solves (alter_d passes trans = 0)
-static bool factors_refused(Solver* sv, const char* what, int trans) {
-  if (trans != 0 && trans != 1) sv->err = std::string(what) + ": trans must be 0 or 1";
-  else if (!sv->factored) sv->err = std::string(what) + ": no factors (factorise first; a SINGULAR factorisation leaves none)";
-  else if (sv->shard.active) sv->err = std::string(what) + ": not available on a sharded handle";
-  else return false;
-  return true;
+// b200ldlt_lmultiply (host == true: x and y in host memory) / _device
+static int lmultiply(Solver* sv, int trans, int nrhs, const double* x, double* y, bool host) {
+  if (trans != 0 && trans != 1) { sv->err = "lmultiply: trans must be 0 or 1"; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "lmultiply"); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (nrhs <= 0) return no_columns(sv);
+  { const int rc = lmul_state(sv, nrhs); if (rc != B200LDLT_SUCCESS) return rc; }
+  const size_t cnt = (size_t)sv->n * nrhs;
+  // host: in place in the staging (both kernel pairs allow it)
+  if (host) return staged_call(sv, x, cnt, y, cnt, [&](double* d) { return enqueue_lmul_columns(sv, trans, nrhs, d, d); });
+  return timed_call(sv, [&] { return enqueue_lmul_columns(sv, trans, nrhs, x, y); });
 }
 
 // b200ldlt_sparse_fwd_solve (host == true: b and x in host memory) / _device
 static int sparse_fwd(Solver* sv, int nbi, const int* bindex, const double* b, bool host, int* nxi, int* xindex, double* x) {
-  if (factors_refused(sv, "sparse_fwd_solve", 0)) return B200LDLT_FATAL_ERROR;
   if (nbi < 0 || nbi > sv->n) { sv->err = "sparse_fwd_solve: nbi must be 0..n"; return B200LDLT_FATAL_ERROR; }
   if (nbi > 0 && (!bindex || !b || !nxi || !xindex || !x)) { sv->err = "sparse_fwd_solve: NULL argument"; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "sparse_fwd_solve"); if (rc != B200LDLT_SUCCESS) return rc; }
   if (nbi == 0) {
     if (nxi) *nxi = 0;
-    sv->info.launches_solve = 0;
-    sv->info.ms_solve_gpu = 0.0f;
-    return B200LDLT_SUCCESS;
+    return no_columns(sv);
   }
-  CU(cudaSetDevice(sv->dev));
-  cudaStream_t st = sv->stream;
   { const int rc = sfs_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
   SfsCall C;
   { const int rc = sfs_prepare(sv, nbi, bindex, host ? b : nullptr, C); if (rc != B200LDLT_SUCCESS) return rc; }
   SparseFwdPlan& P = *sv->sfs;
+  const double* d_b = host ? reinterpret_cast<const double*>(P.d_buf.p + C.o_b) : b;
   double* d_x = host ? reinterpret_cast<double*>(P.d_buf.p + C.o_x) : x;
-  sv->launches = 0;
-  CU(cudaEventRecord(sv->ev0, st));
-  { const int rc = sfs_enqueue(sv, C, host ? reinterpret_cast<const double*>(P.d_buf.p + C.o_b) : b, d_x); if (rc != B200LDLT_SUCCESS) return rc; }
-  if (host) CU(cudaMemcpyAsync(P.h_buf + C.o_x, d_x, (size_t)C.nxi * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaEventRecord(sv->ev1, st));
-  CU(cudaStreamSynchronize(st));
+  const int rc = timed_call(sv, [&]() -> int {
+    { const int rc2 = sfs_enqueue(sv, C, d_b, d_x); if (rc2 != B200LDLT_SUCCESS) return rc2; }
+    if (host) CU(cudaMemcpyAsync(P.h_buf + C.o_x, d_x, (size_t)C.nxi * sizeof(double), cudaMemcpyDeviceToHost, sv->stream));
+    return B200LDLT_SUCCESS;
+  });
+  if (rc != B200LDLT_SUCCESS) return rc;
   if (host) memcpy(x, P.h_buf + C.o_x, (size_t)C.nxi * sizeof(double));
   memcpy(xindex, P.h_buf + C.o_xi, (size_t)C.nxi * sizeof(int));
   *nxi = C.nxi;
-  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
-  sv->info.launches_solve = sv->launches;
   return B200LDLT_SUCCESS;
 }
 
 // b200ldlt_solve_fredholm (host == true: x in host memory) / _device
 static int fredholm(Solver* sv, int nrhs, double tol, double* x, int* consistent, bool host) {
-  const char* why = nullptr;
-  if (nrhs < 0) why = "nrhs must be >= 0";
-  else if (!(tol >= 0.0)) why = "tol must be >= 0";
-  else if (nrhs > 0 && (!x || !consistent)) why = "NULL argument";
-  else if (!sv->factored) why = "no factors (factorise first; a SINGULAR factorisation keeps them only in keep mode, see b200ldlt_set_singular_action)";
-  else if (sv->shard.active) why = "not available on a sharded handle";
-  if (why) { sv->err = std::string("solve_fredholm: ") + why; return B200LDLT_FATAL_ERROR; }
-  if (nrhs == 0) { sv->info.launches_solve = 0; sv->info.ms_solve_gpu = 0.0f; return B200LDLT_SUCCESS; }
-  CU(cudaSetDevice(sv->dev));
-  cudaStream_t st = sv->stream;
-  const size_t n = sv->n;
-  if (sv->zpos.empty()) {
-    // no zero pivots: the solve itself, f = 0, every column consistent
-    int rc;
-    if (host) {
-      rc = solve_host_job(sv, 0, nrhs, x);
-      memset(x + n * nrhs, 0, n * nrhs * sizeof(double));
-    } else {
-      CU(cudaMemsetAsync(x + n * nrhs, 0, n * nrhs * sizeof(double), st));
-      rc = solve_device_job(sv, 0, nrhs, x);
-    }
-    if (rc != B200LDLT_SUCCESS) return rc;
-    for (int i = 0; i < nrhs; ++i) consistent[i] = 1;
-    return B200LDLT_SUCCESS;
-  }
-  const bool blocked = block_solve_state(sv);
-  if (sv->d_fred_nrm.n < 2 * (size_t)nrhs) CU(sv->d_fred_nrm.alloc(2 * (size_t)nrhs));
-  if (!blocked && sv->d_fred_z.n != n) CU(sv->d_fred_z.alloc(n));
-  const size_t total = n * 2 * (size_t)nrhs;
-  if (host && 2 * nrhs > sv->rhs_cap) {
-    if (sv->h_rhs) cudaFreeHost(sv->h_rhs);
-    sv->h_rhs = nullptr;
-    sv->rhs_cap = 0;
-    CU(cudaHostAlloc((void**)&sv->h_rhs, total * sizeof(double), cudaHostAllocDefault));
-    CU(sv->d_rhs.alloc(total));
-    sv->rhs_cap = 2 * nrhs;
-  }
+  const char* bad = nrhs < 0 ? "nrhs must be >= 0" : !(tol >= 0.0) ? "tol must be >= 0"
+                    : nrhs > 0 && (!x || !consistent) ? "NULL argument" : nullptr;
+  if (bad) { sv->err = std::string("solve_fredholm: ") + bad; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "solve_fredholm"); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (nrhs == 0) return no_columns(sv);
+  const size_t n = sv->n, nb = n * nrhs;
+  // no zero pivots: the solve itself, f = 0, every column consistent
+  const bool zero_pivots = !sv->zpos.empty();
+  const bool blocked = (zero_pivots || nrhs > 1) && block_solve_state(sv);
+  if (zero_pivots && sv->d_fred_nrm.n < 2 * (size_t)nrhs) CU(sv->d_fred_nrm.alloc(2 * (size_t)nrhs));
+  if (zero_pivots && !blocked && sv->d_fred_z.n != n) CU(sv->d_fred_z.alloc(n));
   std::vector<unsigned long long> nrm(2 * (size_t)nrhs);
-  double* d_x = host ? sv->d_rhs.p : x;
-  if (host) memcpy(sv->h_rhs, x, n * nrhs * sizeof(double));
-  sv->launches = 0;
-  CU(cudaEventRecord(sv->ev0, st));
-  if (host) CU(cudaMemcpyAsync(d_x, sv->h_rhs, n * nrhs * sizeof(double), cudaMemcpyHostToDevice, st));
-  { const int rc = enqueue_fredholm(sv, d_x, nrhs, blocked); if (rc != B200LDLT_SUCCESS) return rc; }
-  if (host) CU(cudaMemcpyAsync(sv->h_rhs, d_x, total * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(nrm.data(), sv->d_fred_nrm.p, nrm.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CU(cudaEventRecord(sv->ev1, st));
-  CU(cudaStreamSynchronize(st));
-  if (host) memcpy(x, sv->h_rhs, total * sizeof(double));
+  auto enqueue = [&](double* d) -> int {
+    if (!zero_pivots) {
+      CU(cudaMemsetAsync(d + nb, 0, nb * sizeof(double), sv->stream));
+      return enqueue_solve_columns(sv, d, nrhs, blocked);
+    }
+    { const int rc = enqueue_fredholm(sv, d, nrhs, blocked); if (rc != B200LDLT_SUCCESS) return rc; }
+    CU(cudaMemcpyAsync(nrm.data(), sv->d_fred_nrm.p, nrm.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, sv->stream));
+    return B200LDLT_SUCCESS;
+  };
+  const int rc = host ? staged_call(sv, x, nb, x, 2 * nb, enqueue) : timed_call(sv, [&] { return enqueue(x); });
+  if (rc != B200LDLT_SUCCESS) return rc;
   for (int i = 0; i < nrhs; ++i) {
     double ymax, zmax;
     memcpy(&ymax, &nrm[2 * (size_t)i], sizeof(double));
     memcpy(&zmax, &nrm[2 * (size_t)i + 1], sizeof(double));
-    consistent[i] = zmax <= tol * ymax ? 1 : 0;
+    consistent[i] = !zero_pivots || zmax <= tol * ymax ? 1 : 0;
   }
-  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
-  sv->info.launches_solve = sv->launches;
   return B200LDLT_SUCCESS;
 }
 
@@ -2351,27 +2339,18 @@ static int enqueue_selinv(Solver* sv, double* d_diag, double* d_vals) {
 
 // b200ldlt_selected_inverse (host == true: diag and vals in host memory) / _device
 static int selected_inverse(Solver* sv, double* diag, double* vals, bool host) {
-  const char* why = nullptr;
-  if (!diag && !vals) why = "diag and vals are both NULL";
-  else if (!sv->factored) why = "no factors (factorise first; a SINGULAR factorisation keeps them only in keep mode, see b200ldlt_set_singular_action)";
-  else if (sv->shard.active) why = "not available on a sharded handle";
-  if (why) { sv->err = std::string("selected_inverse: ") + why; return B200LDLT_FATAL_ERROR; }
-  CU(cudaSetDevice(sv->dev));
-  cudaStream_t st = sv->stream;
+  if (!diag && !vals) { sv->err = "selected_inverse: diag and vals are both NULL"; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "selected_inverse"); if (rc != B200LDLT_SUCCESS) return rc; }
   { const int rc = selinv_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
   SelInvPlan& P = *sv->selinv;
   double* dd = diag ? (host ? P.d_diag.p : diag) : nullptr;
   double* dv = vals ? (host ? P.d_vals.p : vals) : nullptr;
-  sv->launches = 0;
-  CU(cudaEventRecord(sv->ev0, st));
-  { const int rc = enqueue_selinv(sv, dd, dv); if (rc != B200LDLT_SUCCESS) return rc; }
-  if (host && diag) CU(cudaMemcpyAsync(diag, dd, (size_t)sv->n * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (host && vals) CU(cudaMemcpyAsync(vals, dv, (size_t)sv->nnz * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaEventRecord(sv->ev1, st));
-  CU(cudaStreamSynchronize(st));
-  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
-  sv->info.launches_solve = sv->launches;
-  return B200LDLT_SUCCESS;
+  return timed_call(sv, [&]() -> int {
+    { const int rc = enqueue_selinv(sv, dd, dv); if (rc != B200LDLT_SUCCESS) return rc; }
+    if (host && diag) CU(cudaMemcpyAsync(diag, dd, (size_t)sv->n * sizeof(double), cudaMemcpyDeviceToHost, sv->stream));
+    if (host && vals) CU(cudaMemcpyAsync(vals, dv, (size_t)sv->nnz * sizeof(double), cudaMemcpyDeviceToHost, sv->stream));
+    return B200LDLT_SUCCESS;
+  });
 }
 }  // namespace b200
 
@@ -2379,37 +2358,32 @@ extern "C" {
 
 int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs) {
   Solver* sv = (Solver*)h;
-  if (!sv || !sv->factored) { if (sv) sv->err = "solve before factor"; return B200LDLT_FATAL_ERROR; }
-  return solve_device_job(sv, 0, nrhs, d_rhs);
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return solve_job(sv, 0, nrhs, d_rhs, false);
 }
 
 int b200ldlt_solve(b200ldlt_handle h, int nrhs, double* rhs) {
   Solver* sv = (Solver*)h;
-  if (!sv || !sv->factored) { if (sv) sv->err = "solve before factor"; return B200LDLT_FATAL_ERROR; }
-  return solve_host_job(sv, 0, nrhs, rhs);
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return solve_job(sv, 0, nrhs, rhs, true);
 }
 
 int b200ldlt_solve_partial(b200ldlt_handle h, int job, int nrhs, double* rhs) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
-  if (job == 0) return b200ldlt_solve(h, nrhs, rhs);
-  if (partial_refused(sv, job)) return B200LDLT_FATAL_ERROR;
-  return solve_host_job(sv, job, nrhs, rhs);
+  return solve_job(sv, job, nrhs, rhs, true);
 }
 
 int b200ldlt_solve_partial_device(b200ldlt_handle h, int job, int nrhs, double* d_rhs) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
-  if (job == 0) return b200ldlt_solve_device(h, nrhs, d_rhs);
-  if (partial_refused(sv, job)) return B200LDLT_FATAL_ERROR;
-  return solve_device_job(sv, job, nrhs, d_rhs);
+  return solve_job(sv, job, nrhs, d_rhs, false);
 }
 
 int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, double* dinv2) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
-  if (!sv->factored) { sv->err = "enquire_indef: no factors (factorise first; a SINGULAR factorisation leaves none)"; return B200LDLT_FATAL_ERROR; }
-  CU(cudaSetDevice(sv->dev));
+  { const int rc = factors_state(sv, "enquire_indef", true); if (rc != B200LDLT_SUCCESS) return rc; }
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   std::vector<int> lperm(n), ptype(n);
@@ -2433,51 +2407,13 @@ int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, d
 int b200ldlt_lmultiply_device(b200ldlt_handle h, int trans, int nrhs, const double* d_x, double* d_y) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
-  if (factors_refused(sv, "lmultiply", trans)) return B200LDLT_FATAL_ERROR;
-  if (nrhs <= 0) return B200LDLT_SUCCESS;
-  CU(cudaSetDevice(sv->dev));
-  cudaStream_t st = sv->stream;
-  { const int rc = lmul_state(sv, nrhs); if (rc != B200LDLT_SUCCESS) return rc; }
-  sv->launches = 0;
-  CU(cudaEventRecord(sv->ev0, st));
-  { const int rc = enqueue_lmul_columns(sv, trans, nrhs, d_x, d_y); if (rc != B200LDLT_SUCCESS) return rc; }
-  CU(cudaEventRecord(sv->ev1, st));
-  CU(cudaStreamSynchronize(st));
-  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
-  sv->info.launches_solve = sv->launches;
-  return B200LDLT_SUCCESS;
+  return lmultiply(sv, trans, nrhs, d_x, d_y, false);
 }
 
 int b200ldlt_lmultiply(b200ldlt_handle h, int trans, int nrhs, const double* x, double* y) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
-  if (factors_refused(sv, "lmultiply", trans)) return B200LDLT_FATAL_ERROR;
-  if (nrhs <= 0) return B200LDLT_SUCCESS;
-  CU(cudaSetDevice(sv->dev));
-  cudaStream_t st = sv->stream;
-  const size_t n = sv->n, total = n * (size_t)nrhs;
-  if (nrhs > sv->rhs_cap) {
-    if (sv->h_rhs) cudaFreeHost(sv->h_rhs);
-    sv->h_rhs = nullptr;
-    sv->rhs_cap = 0;
-    CU(cudaHostAlloc((void**)&sv->h_rhs, total * sizeof(double), cudaHostAllocDefault));
-    CU(sv->d_rhs.alloc(total));
-    sv->rhs_cap = nrhs;
-  }
-  { const int rc = lmul_state(sv, nrhs); if (rc != B200LDLT_SUCCESS) return rc; }
-  // through the pinned staging of the solves, in place on the device (both kernel pairs allow it)
-  memcpy(sv->h_rhs, x, total * sizeof(double));
-  sv->launches = 0;
-  CU(cudaEventRecord(sv->ev0, st));
-  CU(cudaMemcpyAsync(sv->d_rhs.p, sv->h_rhs, total * sizeof(double), cudaMemcpyHostToDevice, st));
-  { const int rc = enqueue_lmul_columns(sv, trans, nrhs, sv->d_rhs.p, sv->d_rhs.p); if (rc != B200LDLT_SUCCESS) return rc; }
-  CU(cudaMemcpyAsync(sv->h_rhs, sv->d_rhs.p, total * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaEventRecord(sv->ev1, st));
-  CU(cudaStreamSynchronize(st));
-  memcpy(y, sv->h_rhs, total * sizeof(double));
-  cudaEventElapsedTime(&sv->info.ms_solve_gpu, sv->ev0, sv->ev1);
-  sv->info.launches_solve = sv->launches;
-  return B200LDLT_SUCCESS;
+  return lmultiply(sv, trans, nrhs, x, y, true);
 }
 
 int b200ldlt_sparse_fwd_solve(b200ldlt_handle h, int nbi, const int* bindex, const double* b, int* nxi, int* xindex, double* x) {
@@ -2496,9 +2432,8 @@ int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bind
 int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
-  if (factors_refused(sv, "alter_d", 0)) return B200LDLT_FATAL_ERROR;
   if (!dinv2) { sv->err = "alter_d: no entries"; return B200LDLT_FATAL_ERROR; }
-  CU(cudaSetDevice(sv->dev));
+  { const int rc = factors_state(sv, "alter_d"); if (rc != B200LDLT_SUCCESS) return rc; }
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   if (sv->d_alter.n != 2 * (size_t)n) CU(sv->d_alter.alloc(2 * (size_t)n));
@@ -2530,7 +2465,7 @@ int b200ldlt_enquire_zero_pivots(b200ldlt_handle h, int* nzero, int* pos) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
   if (!nzero) { sv->err = "enquire_zero_pivots: NULL nzero"; return B200LDLT_FATAL_ERROR; }
-  if (!sv->factored) { sv->err = "enquire_zero_pivots: no factors (factorise first; a SINGULAR factorisation keeps them only in keep mode)"; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "enquire_zero_pivots", true); if (rc != B200LDLT_SUCCESS) return rc; }
   *nzero = (int)sv->zpos.size();
   if (pos) std::copy(sv->zpos.begin(), sv->zpos.end(), pos);
   return B200LDLT_SUCCESS;
@@ -2728,7 +2663,7 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
     sv->amat = b200vec_tmat_create(sv->vec, n, n, sv->nnz, sv->irn.data(), sv->jcn.data(), 1);
     if (!sv->amat) { sv->err = "solve_refine: could not build the triplet operator"; return B200LDLT_FATAL_ERROR; }
   }
-  if ((int)sv->d_ref_b.n < n) { CU(sv->d_ref_b.alloc(n)); CU(sv->d_ref_r.alloc(n)); }
+  if ((int)sv->d_ref_b.n < n || (int)sv->d_ref_r.n < n) { CU(sv->d_ref_b.alloc(n)); CU(sv->d_ref_r.alloc(n)); }
   cudaStream_t st = sv->stream;
   CU(cudaMemcpyAsync(sv->d_ref_b.p, d_rhs, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
   sv->launches = 0;

@@ -114,6 +114,14 @@ void fill_info(Keep* K, ma97_info_d* info) {
   info->ordering = 3;                     // nested dissection (METIS)
 }
 
+// the start of the entry points on an analysed matrix: info cleared, then the Keep behind *akeep, or nullptr when there
+// is none or, with need_factors, it holds no factors (the caller then sets flag -1)
+Keep* keep_of(void** akeep, ma97_info_d* info, bool need_factors = true) {
+  memset(info, 0, sizeof(*info));
+  Keep* K = akeep ? (Keep*)*akeep : nullptr;
+  return K && K->h && (K->factored || !need_factors) ? K : nullptr;
+}
+
 // scale[] of the factor calls: the n equilibration factors of the factorisation just done (device_ptr "scale")
 bool copy_scale(Keep* K, double* scale) {
   const void* d = b200ldlt_device_ptr(K->h, "scale");
@@ -181,9 +189,8 @@ void ma97_analyse_d(int check, int n, const int ptr[], const int row[], double v
 void ma97_factor_d(int matrix_type, const int ptr[], const int row[], const double val[], void** akeep, void** fkeep,
                    const ma97_control_d* control, ma97_info_d* info, double scale[]) {
   (void)ptr; (void)row;
-  memset(info, 0, sizeof(*info));
-  Keep* K = akeep ? (Keep*)*akeep : nullptr;
-  if (!K || !K->h || !val || (matrix_type != 4 && matrix_type != 3)) { info->flag = -1; return; }
+  Keep* K = keep_of(akeep, info, false);
+  if (!K || !val || (matrix_type != 4 && matrix_type != 3)) { info->flag = -1; return; }
   if (control && control->u > 0.0 && control->u != K->u) {
     b200ldlt_set_pivtol(K->h, control->u, std::fmax(control->u, 1e-4));
     K->u = control->u;
@@ -211,9 +218,8 @@ void ma97_factor_d(int matrix_type, const int ptr[], const int row[], const doub
 void ma97_solve_d(int job, int nrhs, double x[], int ldx, void** akeep, void** fkeep, const ma97_control_d* control,
                   ma97_info_d* info) {
   (void)control; (void)fkeep;
-  memset(info, 0, sizeof(*info));
-  Keep* K = akeep ? (Keep*)*akeep : nullptr;
-  if (!K || !K->h || !K->factored || job < 0 || job > 4 || nrhs < 0) { info->flag = -1; return; }
+  Keep* K = keep_of(akeep, info);
+  if (!K || job < 0 || job > 4 || nrhs < 0) { info->flag = -1; return; }
   if (nrhs == 0) return;
   int st;
   if (ldx == K->n) st = b200ldlt_solve_partial(K->h, job, nrhs, x);
@@ -233,9 +239,8 @@ void ma97_solve_d(int job, int nrhs, double x[], int ldx, void** akeep, void** f
 void ma97_enquire_indef_d(void** akeep, void** fkeep, const ma97_control_d* control, ma97_info_d* info, int piv_order[],
                           double d[]) {
   (void)fkeep; (void)control;
-  memset(info, 0, sizeof(*info));
-  Keep* K = akeep ? (Keep*)*akeep : nullptr;
-  if (!K || !K->h || !K->factored) { info->flag = -1; return; }
+  Keep* K = keep_of(akeep, info);
+  if (!K) { info->flag = -1; return; }
   std::vector<int> var, ty;
   if (piv_order) { var.resize(K->n); ty.resize(K->n); }
   if (b200ldlt_enquire_indef(K->h, piv_order ? var.data() : nullptr, piv_order ? ty.data() : nullptr, d) != B200LDLT_SUCCESS) {
@@ -253,9 +258,8 @@ void ma97_enquire_indef_d(void** akeep, void** fkeep, const ma97_control_d* cont
 void ma97_lmultiply_d(int trans, int k, const double x[], int ldx, double y[], int ldy, void** akeep, void** fkeep,
                       const ma97_control_d* control, ma97_info_d* info) {
   (void)control; (void)fkeep;
-  memset(info, 0, sizeof(*info));
-  Keep* K = akeep ? (Keep*)*akeep : nullptr;
-  if (!K || !K->h || !K->factored || k < 0 || (trans != 0 && trans != 1) || ldx < K->n || ldy < K->n) { info->flag = -1; return; }
+  Keep* K = keep_of(akeep, info);
+  if (!K || k < 0 || (trans != 0 && trans != 1) || ldx < K->n || ldy < K->n) { info->flag = -1; return; }
   if (k == 0) return;
   int st;
   if (ldx == K->n && ldy == K->n) st = b200ldlt_lmultiply(K->h, trans, k, x, y);
@@ -273,9 +277,8 @@ void ma97_lmultiply_d(int trans, int k, const double x[], int ldx, double y[], i
 // non-finite entry or a non-zero off-diagonal entry where no 2x2 pivot opens.  Lasts until the next factorisation.
 void ma97_alter_d(const double d[], void** akeep, void** fkeep, const ma97_control_d* control, ma97_info_d* info) {
   (void)fkeep; (void)control;
-  memset(info, 0, sizeof(*info));
-  Keep* K = akeep ? (Keep*)*akeep : nullptr;
-  if (!K || !K->h || !K->factored || !d) { info->flag = -1; return; }
+  Keep* K = keep_of(akeep, info);
+  if (!K || !d) { info->flag = -1; return; }
   const int st = b200ldlt_alter_d(K->h, d);
   fill_info(K, info);
   info->flag = (st == B200LDLT_SUCCESS) ? 0 : -1;
@@ -285,9 +288,8 @@ void ma97_alter_d(const double d[], void** akeep, void** fkeep, const ma97_contr
 // every pivot is a positive 1x1 pivot (a positive-definite factorisation); otherwise flag -1 and d untouched.
 void ma97_enquire_posdef_d(void** akeep, void** fkeep, const ma97_control_d* control, ma97_info_d* info, double d[]) {
   (void)fkeep; (void)control;
-  memset(info, 0, sizeof(*info));
-  Keep* K = akeep ? (Keep*)*akeep : nullptr;
-  if (!K || !K->h || !K->factored || !d) { info->flag = -1; return; }
+  Keep* K = keep_of(akeep, info);
+  if (!K || !d) { info->flag = -1; return; }
   std::vector<int> ty(K->n);
   std::vector<double> dinv2(2 * (size_t)K->n);
   if (b200ldlt_enquire_indef(K->h, nullptr, ty.data(), dinv2.data()) != B200LDLT_SUCCESS) { info->flag = -1; return; }
@@ -306,12 +308,8 @@ void ma97_enquire_posdef_d(void** akeep, void** fkeep, const ma97_control_d* con
 void ma97_sparse_fwd_solve_d(int nbi, const int bindex[], const double b[], const int order[], int* nxi, int xindex[],
                              double x[], void** akeep, void** fkeep, const ma97_control_d* control, ma97_info_d* info) {
   (void)fkeep; (void)order;
-  memset(info, 0, sizeof(*info));
-  Keep* K = akeep ? (Keep*)*akeep : nullptr;
-  if (!K || !K->h || !K->factored || nbi < 0 || nbi > K->n || !nxi || !xindex || !x || (nbi > 0 && (!bindex || !b))) {
-    info->flag = -1;
-    return;
-  }
+  Keep* K = keep_of(akeep, info);
+  if (!K || nbi < 0 || nbi > K->n || !nxi || !xindex || !x || (nbi > 0 && (!bindex || !b))) { info->flag = -1; return; }
   const int base = control && control->f_arrays ? 1 : 0;
   std::vector<int> bi(nbi), xi(K->n);
   std::vector<double> bv(nbi), xv(K->n);
@@ -349,9 +347,8 @@ void ma97_factor_solve_d(int matrix_type, const int ptr[], const int row[], cons
 void ma97_solve_fredholm_d(int nrhs, int flag_out[], double x[], int ldx, void** akeep, void** fkeep,
                            const ma97_control_d* control, ma97_info_d* info) {
   (void)fkeep;
-  memset(info, 0, sizeof(*info));
-  Keep* K = akeep ? (Keep*)*akeep : nullptr;
-  if (!K || !K->h || !K->factored || nrhs < 0 || ldx < K->n || (nrhs > 0 && (!x || !flag_out))) { info->flag = -1; return; }
+  Keep* K = keep_of(akeep, info);
+  if (!K || nrhs < 0 || ldx < K->n || (nrhs > 0 && (!x || !flag_out))) { info->flag = -1; return; }
   if (nrhs == 0) return;
   const double tol = control ? control->consist_tol : 2.220446049250313e-16;
   const size_t n = (size_t)K->n;
