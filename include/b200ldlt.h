@@ -105,8 +105,9 @@ int b200ldlt_solve_device(b200ldlt_handle h, int nrhs, double* d_rhs);
  * The calls that read the factors -- solve and the calls below -- share three rules:
  *   refusals : FATAL_ERROR with "<call>: <reason>" in last_error and nothing written, first for the call's own
  *              arguments (listed with each call), then without factors (never factorised, after a SINGULAR factorisation
- *              outside keep mode, after a lifted zero) and on a sharded handle -- solve, enquire_indef and
- *              enquire_zero_pivots accept a sharded handle;
+ *              outside keep mode, after a lifted zero), on a sharded handle -- solve, enquire_indef and
+ *              enquire_zero_pivots accept a sharded handle -- and in Schur mode ("<call>: Schur mode", see
+ *              b200ldlt_set_schur; solve_refine_device too), where only the Schur calls read the factors;
  *   timing   : info.launches_solve counts the call's kernel launches and info.ms_solve_gpu is its device time (host entry
  *              point: with its copies); per-analysis state a call builds at its first use is built before its timing
  *              starts (alter_d, enquire_indef and enquire_zero_pivots are not timed and leave both as they are);
@@ -232,6 +233,46 @@ int b200ldlt_solve_fredholm_device(b200ldlt_handle h, int nrhs, double tol, doub
  * Device entry point: d_diag and d_vals are device memory. */
 int b200ldlt_selected_inverse(b200ldlt_handle h, double* diag, double* vals);
 int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* d_vals);
+
+/* ---- partial factorisation with an explicit Schur complement (cf. MUMPS ICNTL(19) / ICNTL(26), Pardiso iparm(36)) -----
+ * S = vars[0..m) are the caller's Schur variables (distinct 0-based original indices), E the other n - m.  In Schur mode
+ * the analysis orders E alone and places S last, in the caller's order, as one root front; the factor calls (factor,
+ * factor_device, refactor) eliminate E only and leave
+ *   S_c = A_SS - A_SE A_EE^-1 A_ES
+ * in a handle-owned device buffer of m x m doubles: unscaled (the equilibration factors are powers of two, so exactly),
+ * row / column i = vars[i], both triangles written from one, so S_c is bit-symmetric.  That root front is assembled by the
+ * big-front kernels and not factored.  *num_neg, info.num_neg and the inertia check (check_inertia, expected_neg)
+ * describe A_EE; by Haynsworth, inertia(A) = inertia(A_EE) + inertia(S_c).  Zero and lifted pivots inside E behave as
+ * outside Schur mode, except that a SINGULAR factorisation keeps neither factors nor S_c, whatever the keep mode (keep
+ * mode combined with Schur mode is not supported).  Pivots are never delayed from E into S.  Factor launches: those of
+ * the fronts of E, plus 4 (5 when some front of E is a child of the root): the root's zeroing, assembly and extend-add,
+ * the copy-out of S_c and the identity pivot block that replaces the root's factor state.
+ * Every other call that reads the factors is refused in Schur mode (see the rules of the partial solves). */
+/* Schur mode on vars[0..m) (m = 0: off).  Call it after b200ldlt_analyse, which clears Schur mode (a new pattern makes
+ * the indices meaningless); it invalidates the factors, and the next factor call re-analyses with S last.  The set
+ * persists through the re-analyses of increase_quality.  After m = 0 the handle's factors, solutions and launch counts
+ * are those of a handle that never called it, bit for bit.  Refused (FATAL_ERROR, "set_schur: <reason>", state
+ * unchanged): before b200ldlt_analyse, m < 0, m >= n, a NULL vars with m > 0, an index out of range or repeated, a
+ * sharded handle.  A handle in Schur mode refuses b200ldlt_shard_setup. */
+int b200ldlt_set_schur(b200ldlt_handle h, int m, const int* vars);
+/* S_c of the last Schur-mode factorisation, m x m column-major (host / device memory).  Not a launch: one copy.
+ * Refused: a NULL sc, a handle not in Schur mode ("<call>: not in Schur mode") or without its factors. */
+int b200ldlt_schur_complement(b200ldlt_handle h, double* sc);
+int b200ldlt_schur_complement_device(b200ldlt_handle h, double* d_sc);
+/* The reduced right-hand side  y = b_S - A_SE A_EE^-1 b_E  (b: n x nrhs, y: m x nrhs, column-major, row i = vars[i]).
+ * Job 1's forward sweep (the root's identity pivot block leaves the scaled y in the Schur positions), then one gather:
+ * 3 + D kernel launches per block (5 by default), D direct levels (B200_SOLVE_DIRECT). */
+int b200ldlt_schur_reduce(b200ldlt_handle h, int nrhs, const double* b, double* y);
+int b200ldlt_schur_reduce_device(b200ldlt_handle h, int nrhs, const double* d_b, double* d_y);
+/* The expansion of the caller's Schur solution xs (m x nrhs):  x_S = xs,  x_E = A_EE^-1 (b_E - A_ES xs)  (x: n x nrhs).
+ * With S_c xs = schur_reduce(b), A x = b.  Job 1's forward sweep on b, a kernel that writes the scaled xs into the
+ * Schur positions and applies D^-1 to E, then job 4's backward sweep, which leaves the Schur positions as they are, so
+ * x_E has job 0's arithmetic: 5 + 2 D launches per block (9 by default).  x may be b (in place).
+ * Both calls: blocks of up to B200_SOLVE_BLOCK columns like the other solves, every column bit-identical to a call on
+ * that column alone; nrhs = 0 is the no-columns case; refused for nrhs < 0, a NULL pointer with nrhs > 0, a handle not in
+ * Schur mode or without its factors. */
+int b200ldlt_schur_expand(b200ldlt_handle h, int nrhs, const double* b, const double* xs, double* x);
+int b200ldlt_schur_expand_device(b200ldlt_handle h, int nrhs, const double* d_b, const double* d_xs, double* d_x);
 
 /* <-> NumberOfNegEVals() (hpp:207) */
 int b200ldlt_num_neg(b200ldlt_handle h);

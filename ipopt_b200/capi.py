@@ -60,7 +60,9 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_lmultiply", "b200ldlt_lmultiply_device", "b200ldlt_alter_d",
             "b200ldlt_sparse_fwd_solve", "b200ldlt_sparse_fwd_solve_device", "b200ldlt_set_singular_action",
             "b200ldlt_enquire_zero_pivots", "b200ldlt_solve_fredholm", "b200ldlt_solve_fredholm_device",
-            "b200ldlt_selected_inverse", "b200ldlt_selected_inverse_device"]
+            "b200ldlt_selected_inverse", "b200ldlt_selected_inverse_device", "b200ldlt_set_schur",
+            "b200ldlt_schur_complement", "b200ldlt_schur_complement_device", "b200ldlt_schur_reduce",
+            "b200ldlt_schur_reduce_device", "b200ldlt_schur_expand", "b200ldlt_schur_expand_device"]
 
 _lib = None
 
@@ -109,6 +111,13 @@ def load_library():
     L.b200ldlt_solve_fredholm_device.argtypes = [vp, C.c_int, C.c_double, vp, ip]
     L.b200ldlt_selected_inverse.argtypes = [vp, dp, dp]
     L.b200ldlt_selected_inverse_device.argtypes = [vp, vp, vp]
+    L.b200ldlt_set_schur.argtypes = [vp, C.c_int, ip]
+    L.b200ldlt_schur_complement.argtypes = [vp, dp]
+    L.b200ldlt_schur_complement_device.argtypes = [vp, vp]
+    L.b200ldlt_schur_reduce.argtypes = [vp, C.c_int, dp, dp]
+    L.b200ldlt_schur_reduce_device.argtypes = [vp, C.c_int, vp, vp]
+    L.b200ldlt_schur_expand.argtypes = [vp, C.c_int, dp, dp, dp]
+    L.b200ldlt_schur_expand_device.argtypes = [vp, C.c_int, vp, vp, vp]
     L.b200ldlt_num_neg.argtypes = [vp]
     L.b200ldlt_increase_quality.argtypes = [vp]
     L.b200ldlt_get_info.argtypes = [vp, C.POINTER(Info)]
@@ -118,6 +127,9 @@ def load_library():
     L.b200ldlt_residual.argtypes = [vp, dp, dp, dp, dp, dp]
     L.b200ldlt_symbolic_create.argtypes = [C.c_int, C.c_int, ip, ip, dp, C.c_int, C.c_int, C.c_int, C.c_double]
     L.b200ldlt_symbolic_create.restype = vp
+    L.b200ldlt_symbolic_create_schur.argtypes = [C.c_int, C.c_int, ip, ip, dp, C.c_int, C.c_int, C.c_int, C.c_double,
+                                                 C.c_int, ip]
+    L.b200ldlt_symbolic_create_schur.restype = vp
     L.b200ldlt_symbolic_free.argtypes = [vp]
     L.b200ldlt_symbolic_free.restype = None
     L.b200ldlt_symbolic_get.argtypes = [vp, C.c_char_p, C.POINTER(C.c_longlong), C.c_longlong]
@@ -141,7 +153,9 @@ class SymbolicAnalysis:
     STATS = ["n", "nsn", "nlevels", "max_front", "max_k", "n_saddle", "n_pairs", "nnzL", "nnzL_true", "cb_total",
              "flops_panel", "flops_schur", "ms_order", "ms_symbolic"]
 
-    def __init__(self, dim, irn, jcn, vals=None, ordering=0, pair_saddle=1, leaf_k=0, relax_frac=-1.0):
+    def __init__(self, dim, irn, jcn, vals=None, ordering=0, pair_saddle=1, leaf_k=0, relax_frac=-1.0, schur=None):
+        """schur: the 0-based Schur variables, which become the last pivot positions in this order (one root
+        supernode); None or empty: the ordinary analysis."""
         L = load_library()
         irn = np.ascontiguousarray(irn, dtype=np.int32)
         jcn = np.ascontiguousarray(jcn, dtype=np.int32)
@@ -150,8 +164,9 @@ class SymbolicAnalysis:
             vals = np.ascontiguousarray(vals, dtype=np.float64)
             vp = _dptr(vals)
         self._L = L
-        self._h = L.b200ldlt_symbolic_create(int(dim), int(len(irn)), _iptr(irn), _iptr(jcn), vp, ordering,
-                                             pair_saddle, leaf_k, relax_frac)
+        sc = np.ascontiguousarray([] if schur is None else schur, dtype=np.int32)
+        self._h = L.b200ldlt_symbolic_create_schur(int(dim), int(len(irn)), _iptr(irn), _iptr(jcn), vp, ordering,
+                                                   pair_saddle, leaf_k, relax_frac, len(sc), _iptr(sc))
         if not self._h:
             raise RuntimeError("symbolic analysis failed")
 
@@ -201,6 +216,7 @@ class B200Ldlt:
         self.nonzeros = 0
         self._negevals = -1
         self._ia = self._ja = None
+        self._sc_m = 0
 
     # -- the 8 virtuals -------------------------------------------------------------------------
     def InitializeStructure(self, dim, nonzeros, ia, ja):
@@ -208,6 +224,7 @@ class B200Ldlt:
         self._ja = np.ascontiguousarray(ja, dtype=np.int32)
         assert len(self._ia) == nonzeros and len(self._ja) == nonzeros
         self.dim, self.nonzeros = int(dim), int(nonzeros)
+        self._sc_m = 0                   # (the analysis clears Schur mode)
         return self._L.b200ldlt_analyse(self._h, self.dim, self.nonzeros, _iptr(self._ia), _iptr(self._ja))
 
     def GetValuesArrayPtr(self):
@@ -371,6 +388,57 @@ class B200Ldlt:
         """The same into device arrays (pointers as ints, 0 = not wanted). Returns the status."""
         return self._L.b200ldlt_selected_inverse_device(self._h, C.c_void_p(d_diag_ptr or None),
                                                         C.c_void_p(d_vals_ptr or None))
+
+    def set_schur(self, vars):
+        """Schur mode on the 0-based variables vars (empty: off).  Takes effect at the next factor call, which re-analyses
+        with vars last and leaves their Schur complement.  Returns the status."""
+        v = np.ascontiguousarray(vars, dtype=np.int32)
+        st = self._L.b200ldlt_set_schur(self._h, len(v), _iptr(v) if len(v) else None)
+        if st == SYMSOLVER_SUCCESS:
+            self._sc_m = len(v)
+        return st
+
+    def schur_complement(self):
+        """S_c = A_SS - A_SE A_EE^-1 A_ES (m x m, row / column i = vars[i]) of the last factorisation.  Raises on a
+        refusal."""
+        m = self._sc_m
+        sc = np.zeros((m, m), order="F")
+        if self._L.b200ldlt_schur_complement(self._h, _dptr(sc)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return sc
+
+    def schur_complement_device(self, d_sc_ptr):
+        """The same into a device array of m x m doubles.  Returns the status."""
+        return self._L.b200ldlt_schur_complement_device(self._h, C.c_void_p(d_sc_ptr))
+
+    def schur_reduce(self, B):
+        """y = b_S - A_SE A_EE^-1 b_E for the columns of B (dim or dim x nrhs).  Raises on a refusal."""
+        B = np.asarray(B, dtype=np.float64)
+        Bm = np.asfortranarray(B.reshape(self.dim, -1, order="F"))
+        nrhs, m = Bm.shape[1], self._sc_m
+        y = np.zeros((m, nrhs), order="F")
+        if self._L.b200ldlt_schur_reduce(self._h, nrhs, _dptr(Bm), _dptr(y)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return y[:, 0] if B.ndim == 1 else y
+
+    def schur_reduce_device(self, d_b_ptr, d_y_ptr, nrhs=1):
+        return self._L.b200ldlt_schur_reduce_device(self._h, int(nrhs), C.c_void_p(d_b_ptr), C.c_void_p(d_y_ptr))
+
+    def schur_expand(self, B, XS):
+        """x with x_S = xs and x_E = A_EE^-1 (b_E - A_ES xs) for the columns of B (dim [x nrhs]) and XS (m [x nrhs]).
+        Raises on a refusal."""
+        B = np.asarray(B, dtype=np.float64)
+        Bm = np.asfortranarray(B.reshape(self.dim, -1, order="F"))
+        nrhs, m = Bm.shape[1], self._sc_m
+        Xs = np.asfortranarray(np.asarray(XS, dtype=np.float64).reshape(m, nrhs, order="F"))
+        x = np.zeros((self.dim, nrhs), order="F")
+        if self._L.b200ldlt_schur_expand(self._h, nrhs, _dptr(Bm), _dptr(Xs), _dptr(x)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return x[:, 0] if B.ndim == 1 else x
+
+    def schur_expand_device(self, d_b_ptr, d_xs_ptr, d_x_ptr, nrhs=1):
+        return self._L.b200ldlt_schur_expand_device(self._h, int(nrhs), C.c_void_p(d_b_ptr), C.c_void_p(d_xs_ptr),
+                                                    C.c_void_p(d_x_ptr))
 
     def device_ptr(self, name):
         """Device address of a named array of the handle (b200ldlt_device_ptr: "scale", "x", "cbv", ...), 0 if none."""

@@ -21,6 +21,7 @@
 #include "lmul_kernels.cu"
 #include "schur_tc.cu"
 #include "selinv_kernels.cu"
+#include "sc_kernels.cu"
 #include "symbolic.hpp"
 
 namespace b200 {
@@ -259,6 +260,14 @@ struct Solver {
   std::vector<int> zpos;            // the zero pivots of the kept factors, ascending (empty otherwise)
   DevBuf<unsigned long long> d_fred_nrm;   // solve_fredholm: the two max-norms per column
   DevBuf<double> d_fred_z;          // solve_fredholm without a blocked state: z of one column, pivot order
+  // Schur mode (b200ldlt_set_schur): the caller's Schur variables, given to every analysis until b200ldlt_analyse or
+  // set_schur(0) clears them.  An analysis with them makes supernode sc_root (the last one) their root front, which
+  // the factorisation assembles but does not factor; d_sc then holds S_c (m x m, column-major).
+  std::vector<int> sc_vars;
+  int sc_root = -1, sc_nch = 0;
+  long long sc_nent = 0, sc_linv_off = 0;   // its unique entries; its L11^-1 block in d_linv (order > 256)
+  DevBuf<int> d_sc_vars, d_sc_root;
+  DevBuf<double> d_sc;
   DevBuf<double> d_linv;
   DevBuf<double> d_linv_part;       // partial tiles of the chunked k_linv_gemm items (one launch at a time uses it)
   DevBuf<int> d_linv_cnt;           // their arrival counters (self-resetting)
@@ -821,11 +830,34 @@ static int run_analysis(Solver* sv, const double* vals) {
   ao.pair_saddle = sv->opt.pair_saddle;
   ao.leaf_k = sv->opt.leaf_k;
   ao.relax_frac = sv->opt.relax_frac;
+  ao.sc_vars = sv->sc_vars;
   std::string e;
   int rc = analyse(sv->n, sv->nnz, sv->irn.data(), sv->jcn.data(), vals, ao, sv->S, e);
   if (rc != 0) { sv->err = e; return B200LDLT_FATAL_ERROR; }
   Symbolic& S = sv->S;
   cudaStream_t st = sv->stream;
+  // Schur mode: the root front of S, factored by none of the plans below; assembled by the big-front kernels (one-entry
+  // front list d_sc_root), so its children get inverse row maps whatever its order
+  const int m = (int)sv->sc_vars.size();
+  sv->sc_root = -1;
+  if (m > 0) {
+    const int rt = S.nsn - 1;
+    if (S.sn_start[rt] != S.n - m || S.r(rt) != 0 || S.sn_parent[rt] != -1) {
+      sv->err = "internal: the Schur variables do not form the last root front";
+      return B200LDLT_FATAL_ERROR;
+    }
+    sv->sc_root = rt;
+    sv->sc_nch = S.child_ptr[rt + 1] - S.child_ptr[rt];
+    sv->sc_nent = S.uent_ptr[rt + 1] - S.uent_ptr[rt];
+    CU(sv->d_sc_vars.upload(sv->sc_vars, st));
+    CU(sv->d_sc_root.upload(std::vector<int>{rt}, st));
+    CU(sv->d_sc.alloc((size_t)m * m));
+  } else {
+    sv->d_sc_vars.release(); sv->d_sc_root.release(); sv->d_sc.release();
+  }
+  // the fronts the factorisation factors: all but the Schur root
+  std::vector<char> take_f(S.nsn, 1);
+  if (sv->sc_root >= 0) take_f[sv->sc_root] = 0;
   CU(sv->d_sn_start.upload(S.sn_start, st));
   CU(sv->d_sn_parent.upload(S.sn_parent, st));
   CU(sv->d_rows_ptr.upload(S.rows_ptr, st));
@@ -881,7 +913,7 @@ static int run_analysis(Solver* sv, const double* vals) {
     long long tot = 0;
     for (int c = 0; c < S.nsn; ++c) {
       const int p = S.sn_parent[c];
-      if (p >= 0 && S.f(p) > sv->opt.smem_front_max) { eoff[c] = tot; tot += S.f(p); }
+      if (p >= 0 && (S.f(p) > sv->opt.smem_front_max || p == sv->sc_root)) { eoff[c] = tot; tot += S.f(p); }
     }
     std::vector<int> einv((size_t)std::max<long long>(tot, 1), -1);
     for (int c = 0; c < S.nsn; ++c) if (eoff[c] >= 0) {
@@ -896,10 +928,7 @@ static int run_analysis(Solver* sv, const double* vals) {
 
   // ---- launch plan: per level, big fronts first then small ones by descending order --------
   std::vector<int> fl;
-  {
-    std::vector<char> take(S.nsn, 1);
-    build_level_plans(S, sv->opt.smem_front_max, take, fl, sv->plan, sv->schur, sv->tc_min_r, !sv->dbg.no_warp2);
-  }
+  build_level_plans(S, sv->opt.smem_front_max, take_f, fl, sv->plan, sv->schur, sv->tc_min_r, !sv->dbg.no_warp2);
   CU(sv->d_front_list.upload(fl, st));
   { int rc2 = upload_schur_lists(sv, sv->schur, st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
   CU(cudaFuncSetAttribute(k_tc_schur, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
@@ -928,17 +957,17 @@ static int run_analysis(Solver* sv, const double* vals) {
         const long long K64 = (long long)((S.k(s) + DF_BLK - 1) / DF_BLK) * DF_BLK;
         tot += K64 * K64;
       }
+      if (sv->sc_root >= 0) sv->sc_linv_off = std::max(linv_off[sv->sc_root], 0LL);
       CU(sv->d_linv_off.upload(linv_off, st));
       CU(sv->d_linv.alloc(std::max<long long>(tot, 1)));
       CU(cudaMemsetAsync(sv->d_linv.p, 0, sv->d_linv.n * sizeof(double), st));
-      std::vector<char> take(S.nsn, 1);
-      int rc2 = build_linv_plan(sv, S, take, sv->linv_plan, st);
+      int rc2 = build_linv_plan(sv, S, take_f, sv->linv_plan, st);
       if (rc2 != B200LDLT_SUCCESS) return rc2;
       sv->linv_level.clear();
       for (int l = 0; l < S.nlevels; ++l) {
         std::vector<char> tl(S.nsn, 0);
         bool any = false;
-        for (int q = 0; q < S.nsn; ++q) if (S.sn_level[q] == l && S.f(q) > kSolveMidMax) { tl[q] = 1; any = true; }
+        for (int q = 0; q < S.nsn; ++q) if (take_f[q] && S.sn_level[q] == l && S.f(q) > kSolveMidMax) { tl[q] = 1; any = true; }
         sv->linv_level.emplace_back(new LinvPlan());
         if (any) { rc2 = build_linv_plan(sv, S, tl, *sv->linv_level.back(), st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
       }
@@ -1174,6 +1203,22 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
       CU(cudaStreamWaitEvent(st, e, 0));
     }
   }
+  if (sv->sc_root >= 0) {
+    // Schur mode: the root front of S, once all of its children are done, through the big-front assembly (its panel
+    // is m x m, r = 0); S_c out of the assembled panel, then the identity pivot block in its place
+    const int m = (int)sv->sc_vars.size(), rt = sv->sc_root;
+    const long long mm = (long long)m * m;
+    const int* rl = sv->d_sc_root.p;
+    k_big_zero<<<dim3(std::min<unsigned>(cdiv(mm, 1024), 592), 1), 256, 0, st>>>(D, N, rl); ++L;
+    k_big_assemble<<<dim3(std::max(1u, std::min<unsigned>(cdiv(sv->sc_nent, 256), 64)), 1), 256, 0, st>>>(D, N, rl); ++L;
+    if (sv->sc_nch > 0) { k_big_extend_all<<<dim3(cdiv(m, 8), 1), 256, 0, st>>>(D, N, rl); ++L; }
+    double* P = sv->d_L.p + S.L_off[rt];
+    k_sc_out<<<cdiv(mm, 256), 256, 0, st>>>(m, P, sv->d_sc_vars.p, sv->d_scale.p, sv->d_sc.p); ++L;
+    const bool big = S.f(rt) > DF_MIDMAX;
+    const long long k64 = big ? (long long)((m + DF_BLK - 1) / DF_BLK) * DF_BLK : 0;
+    k_sc_identity<<<cdiv(std::max(mm, k64 * k64), 256), 256, 0, st>>>(m, n - m, k64, P, sv->d_lperm.p, sv->d_bperm.p,
+        sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, big ? sv->d_linv.p + sv->sc_linv_off : nullptr); ++L;
+  }
   if (linv_forked) {
     cudaEvent_t e = sv->next_event();
     CU(cudaEventRecord(e, sv->stream3));
@@ -1244,9 +1289,10 @@ static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* n
       sv->err = "factor: SINGULAR with a lifted zero pivot (|pivot| <= tiny at pivot position " + std::to_string(lifted) +
                 ", whose column is not rounding noise): no factors kept";
     } else {
+      const bool keep = sv->keep_singular && sv->sc_vars.empty();   // (Schur mode keeps no singular factors)
       sv->err = "factor: SINGULAR: " + std::to_string(nz) + " zero pivot(s)" +
-                (sv->keep_singular ? "; factors kept with D^+ (zero pivots left out of the inertia)" : "; no factors kept");
-      if (sv->keep_singular && !sv->shard.active && nz == I.num_tiny) {
+                (keep ? "; factors kept with D^+ (zero pivots left out of the inertia)" : "; no factors kept");
+      if (keep && !sv->shard.active && nz == I.num_tiny) {
         for (int e : zl) sv->zpos.push_back(e >> 2);
         CU(sv->d_zpos.upload(sv->zpos, st));
         CU(cudaMemsetAsync(sv->d_zflag.p, 0, sv->n, st));
@@ -2027,6 +2073,7 @@ int b200ldlt_analyse(b200ldlt_handle h, int dim, int nonzeros, const int* irn, c
   CU(cudaHostAlloc((void**)&sv->h_vals, std::max<size_t>(nonzeros, 1) * sizeof(double), cudaHostAllocDefault));
   memset(sv->h_vals, 0, std::max<size_t>(nonzeros, 1) * sizeof(double));
   sv->analysed = false; sv->factored = false; sv->have_dev_vals = false;
+  sv->sc_vars.clear();                // (a new pattern makes the Schur indices meaningless)
   if (sv->amat) { b200vec_tmat_destroy(sv->amat); sv->amat = nullptr; }
   sv->drop_staging();
   return B200LDLT_SUCCESS;
@@ -2065,11 +2112,13 @@ namespace b200 {
 // ---- the calls that read the factors (include/b200ldlt.h, from the partial solves on) -------------------------------
 // The state check, after the call's own argument checks: FATAL_ERROR with "<call>: ..." in last_error without factors
 // and, unless sharded_ok, on a sharded handle; otherwise the handle's device is selected for what follows.
-static int factors_state(Solver* sv, const char* call, bool sharded_ok = false) {
+static int factors_state(Solver* sv, const char* call, bool sharded_ok = false, bool schur_call = false) {
   if (!sv->factored)
     sv->err = std::string(call) + ": no factors (factorise first; a SINGULAR factorisation keeps them only in keep mode, "
                                   "see b200ldlt_set_singular_action)";
   else if (sv->shard.active && !sharded_ok) sv->err = std::string(call) + ": not available on a sharded handle";
+  else if (sv->sc_vars.empty() == schur_call)   // the Schur calls need Schur-mode factors, the others refuse them
+    sv->err = std::string(call) + (schur_call ? ": not in Schur mode" : ": Schur mode");
   else { CU(cudaSetDevice(sv->dev)); return B200LDLT_SUCCESS; }
   return B200LDLT_FATAL_ERROR;
 }
@@ -2222,6 +2271,75 @@ static int fredholm(Solver* sv, int nrhs, double tol, double* x, int* consistent
     consistent[i] = !zero_pivots || zmax <= tol * ymax ? 1 : 0;
   }
   return B200LDLT_SUCCESS;
+}
+
+// ---- Schur mode (b200ldlt_set_schur): S_c, reduce, expand ---------------------------------------------------------------
+// nrhs columns of d_b (leading dimension n).  Reduce (d_xs == nullptr): y = b_S - A_SE A_EE^-1 b_E to d_out (leading
+// dimension m).  Expand: x to d_out (leading dimension n), x_S = xs (d_xs, leading dimension m), x_E = A_EE^-1 (b_E -
+// A_ES xs).  Both start with job 1's forward sweep, which leaves the scaled reduced right-hand side in the Schur positions
+// (the root's pivot block is the identity); expand then writes the scaled xs there, applies D^-1 to E and runs job 4's
+// backward sweep, which passes the root's values through.  Blocks of up to B200_SOLVE_BLOCK columns (blocked: the result
+// of block_solve_state), each column with the arithmetic of a single-column call.  d_out may be d_b.
+static int enqueue_sc_columns(Solver* sv, int nrhs, const double* d_b, const double* d_xs, double* d_out, bool blocked) {
+  cudaStream_t st = sv->stream;
+  const int n = sv->n, m = (int)sv->sc_vars.size();
+  const int cap = blocked ? sv->blk->width : 1;
+  for (int c = 0; c < nrhs;) {
+    const int w = std::min(cap, nrhs - c);
+    SweepState& W = w == 1 ? sv->sweep : *sv->blk;
+    const long long ldx = W.M.x, ldb = W.M.bigv;
+    const dim3 g(cdiv(n, 256), w);
+    k_rhs_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_b + (size_t)c * n, W.d_x.p, ldx); ++sv->launches;
+    sv->solve_epoch++;
+    int rc = launch_sweep(sv, sv->splan, W, w, true, false);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    if (!d_xs) {
+      k_sc_reduce<<<dim3(cdiv(m, 256), w), 256, 0, st>>>(m, n - m, sv->d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb,
+                                                         sv->d_sc_vars.p, sv->d_scale.p, d_out + (size_t)c * m);
+      ++sv->launches;
+    } else {
+      k_sc_expand<<<g, 256, 0, st>>>(n, m, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, sv->d_piv_big.p, W.d_x.p, ldx,
+                                     W.d_bigv.p, ldb, sv->d_sc_vars.p, sv->d_scale.p, d_xs + (size_t)c * m);
+      ++sv->launches;
+      sv->solve_epoch++;
+      rc = launch_sweep(sv, sv->splan, W, w, false);
+      if (rc != B200LDLT_SUCCESS) return rc;
+      k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, d_out + (size_t)c * n); ++sv->launches;
+    }
+    c += w;
+  }
+  CU(cudaGetLastError());
+  return B200LDLT_SUCCESS;
+}
+
+// b200ldlt_schur_complement (host == true: sc in host memory) / _device
+static int schur_complement(Solver* sv, double* sc, bool host) {
+  if (!sc) { sv->err = "schur_complement: NULL argument"; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "schur_complement", false, true); if (rc != B200LDLT_SUCCESS) return rc; }
+  const size_t mm = sv->d_sc.n;
+  auto enqueue = [&](double* d) -> int {
+    CU(cudaMemcpyAsync(d, sv->d_sc.p, mm * sizeof(double), cudaMemcpyDeviceToDevice, sv->stream));
+    return B200LDLT_SUCCESS;
+  };
+  return host ? staged_call(sv, nullptr, 0, sc, mm, enqueue) : timed_call(sv, [&] { return enqueue(sc); });
+}
+
+// b200ldlt_schur_reduce (xs == nullptr) and b200ldlt_schur_expand (host == true: the arrays in host memory) / _device
+static int schur_solve(Solver* sv, const char* call, int nrhs, const double* b, const double* xs, double* out, bool host,
+                       bool expand) {
+  const char* bad = nrhs < 0 ? "nrhs must be >= 0" : nrhs > 0 && (!b || !out || (expand && !xs)) ? "NULL argument" : nullptr;
+  if (bad) { sv->err = std::string(call) + ": " + bad; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, call, false, true); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (nrhs == 0) return no_columns(sv);
+  const size_t n = sv->n, m = sv->sc_vars.size(), nb = n * nrhs, mb = m * nrhs;
+  const bool blocked = nrhs > 1 && block_solve_state(sv);
+  if (!host) return timed_call(sv, [&] { return enqueue_sc_columns(sv, nrhs, b, expand ? xs : nullptr, out, blocked); });
+  if (!expand)   // in place in the staging: y of a block lands below the b of the blocks after it
+    return staged_call(sv, b, nb, out, mb, [&](double* d) { return enqueue_sc_columns(sv, nrhs, d, nullptr, d, blocked); });
+  std::vector<double> in(nb + mb);   // b and xs side by side, one staged copy
+  std::copy(b, b + nb, in.begin());
+  std::copy(xs, xs + mb, in.begin() + nb);
+  return staged_call(sv, in.data(), nb + mb, out, nb, [&](double* d) { return enqueue_sc_columns(sv, nrhs, d, d + nb, d, blocked); });
 }
 
 // ---- selected inversion (b200ldlt_selected_inverse) ----------------------------------------------------------------
@@ -2495,6 +2613,63 @@ int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* 
   return selected_inverse(sv, d_diag, d_vals, false);
 }
 
+int b200ldlt_set_schur(b200ldlt_handle h, int m, const int* vars) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  const char* bad = sv->n <= 0 ? "analyse first" : m < 0 ? "m must be >= 0" : m >= sv->n ? "m must be < n"
+                    : m > 0 && !vars ? "NULL vars" : sv->shard.active ? "not available on a sharded handle" : nullptr;
+  if (!bad) {
+    std::vector<char> seen(sv->n, 0);
+    for (int i = 0; i < m && !bad; ++i) {
+      if (vars[i] < 0 || vars[i] >= sv->n) bad = "variable out of range";
+      else if (seen[vars[i]]) bad = "variable repeated";
+      else seen[vars[i]] = 1;
+    }
+  }
+  if (bad) { sv->err = std::string("set_schur: ") + bad; return B200LDLT_FATAL_ERROR; }
+  sv->sc_vars.assign(vars, vars + m);
+  // the factors no longer match the mode; the next factor call re-analyses (the ordering places S last)
+  sv->factored = false;
+  if (sv->analysed) sv->reanalyse = true;
+  return B200LDLT_SUCCESS;
+}
+
+int b200ldlt_schur_complement(b200ldlt_handle h, double* sc) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return schur_complement(sv, sc, true);
+}
+
+int b200ldlt_schur_complement_device(b200ldlt_handle h, double* d_sc) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return schur_complement(sv, d_sc, false);
+}
+
+int b200ldlt_schur_reduce(b200ldlt_handle h, int nrhs, const double* b, double* y) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return schur_solve(sv, "schur_reduce", nrhs, b, nullptr, y, true, false);
+}
+
+int b200ldlt_schur_reduce_device(b200ldlt_handle h, int nrhs, const double* d_b, double* d_y) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return schur_solve(sv, "schur_reduce", nrhs, d_b, nullptr, d_y, false, false);
+}
+
+int b200ldlt_schur_expand(b200ldlt_handle h, int nrhs, const double* b, const double* xs, double* x) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return schur_solve(sv, "schur_expand", nrhs, b, xs, x, true, true);
+}
+
+int b200ldlt_schur_expand_device(b200ldlt_handle h, int nrhs, const double* d_b, const double* d_xs, double* d_x) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return schur_solve(sv, "schur_expand", nrhs, d_b, d_xs, d_x, false, true);
+}
+
 /* ---- multi-GPU elimination-tree sharding (SURVEY.md section 8e) -------------------------------------------
  * One process per GPU, each with its own handle and the SAME matrix.  After the (replicated, deterministic)
  * analysis, rank g factorises the subtrees it owns; the contribution blocks of the cut are moved to rank 0 by the
@@ -2503,6 +2678,7 @@ int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* 
 int b200ldlt_shard_setup(b200ldlt_handle h, int rank, int world) {
   Solver* sv = (Solver*)h;
   if (!sv || !sv->analysed || world < 1 || rank < 0 || rank >= world) { if (sv) sv->err = "shard_setup: analyse first / bad rank"; return B200LDLT_FATAL_ERROR; }
+  if (!sv->sc_vars.empty()) { sv->err = "shard_setup: Schur mode"; return B200LDLT_FATAL_ERROR; }
   CU(cudaSetDevice(sv->dev));
   return shard_setup(sv, rank, world);
 }
@@ -2653,7 +2829,7 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
   Solver* sv = (Solver*)h;
   if (steps_done) *steps_done = 0;
   if (!sv || !sv->factored || !sv->have_dev_vals || !d_rhs) { if (sv) sv->err = "solve_refine: factor first (values on the device)"; return B200LDLT_FATAL_ERROR; }
-  CU(cudaSetDevice(sv->dev));
+  { const int rc = factors_state(sv, "solve_refine_device", true); if (rc != B200LDLT_SUCCESS) return rc; }
   const int n = sv->n;
   if (!sv->vec) {
     sv->vec = b200vec_create(sv->dev, (void*)sv->stream);

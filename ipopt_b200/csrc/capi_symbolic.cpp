@@ -12,16 +12,23 @@ struct SymHandle { Symbolic S; std::string err; };
 
 extern "C" {
 
-void* b200ldlt_symbolic_create(int dim, int nonzeros, const int* irn, const int* jcn, const double* vals,
-                               int ordering, int pair_saddle, int leaf_k, double relax_frac) {
+/* b200ldlt_symbolic_create with a Schur set: vars[0..m) (0-based) become the last m pivot positions, one root supernode */
+void* b200ldlt_symbolic_create_schur(int dim, int nonzeros, const int* irn, const int* jcn, const double* vals,
+                                     int ordering, int pair_saddle, int leaf_k, double relax_frac, int m, const int* vars) {
   SymHandle* h = new SymHandle();
   AnalyseOptions ao;
   ao.ordering = ordering; ao.pair_saddle = pair_saddle;
   if (leaf_k > 0) ao.leaf_k = leaf_k;
   if (relax_frac >= 0) ao.relax_frac = relax_frac;
+  if (m > 0 && vars) ao.sc_vars.assign(vars, vars + m);
   int rc = analyse(dim, nonzeros, irn, jcn, vals, ao, h->S, h->err);
   if (rc != 0) { fprintf(stderr, "[b200ldlt] symbolic analysis failed: %s\n", h->err.c_str()); delete h; return nullptr; }
   return h;
+}
+
+void* b200ldlt_symbolic_create(int dim, int nonzeros, const int* irn, const int* jcn, const double* vals,
+                               int ordering, int pair_saddle, int leaf_k, double relax_frac) {
+  return b200ldlt_symbolic_create_schur(dim, nonzeros, irn, jcn, vals, ordering, pair_saddle, leaf_k, relax_frac, 0, nullptr);
 }
 
 void b200ldlt_symbolic_free(void* p) { delete (SymHandle*)p; }

@@ -96,6 +96,15 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
   for (int64_t e = 0; e < nnz; ++e) {
     if (irn[e] < 1 || irn[e] > n || jcn[e] < 1 || jcn[e] > n) { err = "analyse: index out of range"; return -2; }
   }
+  // Schur variables: is_sc marks them; E (the rest) is ordered and eliminated, S follows in the caller's order
+  const std::vector<int>& sc = opt.sc_vars;
+  const int m = (int)sc.size();
+  std::vector<char> is_sc(n, 0);
+  if (m >= n) { err = "analyse: the Schur set must leave a variable to eliminate"; return -2; }
+  for (int v : sc) {
+    if (v < 0 || v >= n || is_sc[v]) { err = "analyse: Schur variable out of range or repeated"; return -2; }
+    is_sc[v] = 1;
+  }
 
   // ---- 1. unique lower pattern in ORIGINAL labels -------------------------------------------
   std::vector<Ent> keyed((size_t)nnz);
@@ -153,9 +162,9 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     }
     struct Cand { double w; int s, x; };
     std::vector<Cand> cand;
-    for (int i = 0; i < n; ++i) if (saddle[i])
+    for (int i = 0; i < n; ++i) if (saddle[i] && !is_sc[i])
       for (int64_t p = xadj[i]; p < xadj[i + 1]; ++p)
-        if (!saddle[adj[p]] && adjw[p] > 0.0) cand.push_back({adjw[p], i, adj[p]});
+        if (!saddle[adj[p]] && !is_sc[adj[p]] && adjw[p] > 0.0) cand.push_back({adjw[p], i, adj[p]});
     std::sort(cand.begin(), cand.end(), [](const Cand& a, const Cand& b) {
       if (a.w != b.w) return a.w > b.w;
       if (a.s != b.s) return a.s < b.s;
@@ -176,7 +185,7 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     std::vector<int> visit(n, -1), from_s(n, -1), depth(n, 0);
     std::vector<int> queue;
     for (int s0 = 0; s0 < n; ++s0) {
-      if (!saddle[s0] || partner[s0] >= 0) continue;
+      if (!saddle[s0] || partner[s0] >= 0 || is_sc[s0]) continue;
       queue.clear();
       queue.push_back(s0);
       depth[s0] = 1;
@@ -185,7 +194,7 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
         int sq = queue[qh];
         for (int64_t p = xadj[sq]; p < xadj[sq + 1]; ++p) {
           int x = adj[p];
-          if (saddle[x] || visit[x] == s0) continue;
+          if (saddle[x] || is_sc[x] || visit[x] == s0) continue;
           if (!(adjw[p] >= kMinFrac * rowmax[sq]) || !(adjw[p] > 0.0)) continue;
           visit[x] = s0;
           from_s[x] = sq;
@@ -212,7 +221,7 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
   std::vector<int> cnode(n, -1);
   std::vector<int> cfirst, csecond;  // members: primal first, saddle second (or -1)
   for (int i = 0; i < n; ++i) {
-    if (cnode[i] >= 0) continue;
+    if (cnode[i] >= 0 || is_sc[i]) continue;
     if (partner[i] < 0) { cnode[i] = (int)cfirst.size(); cfirst.push_back(i); csecond.push_back(-1); }
     else {
       int x = saddle[i] ? partner[i] : i, c = saddle[i] ? i : partner[i];
@@ -220,35 +229,37 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
       cfirst.push_back(x); csecond.push_back(c);
     }
   }
+  const int nce = (int)cfirst.size();    // the nodes of E: the ordering sees these only
+  for (int v : sc) { cnode[v] = (int)cfirst.size(); cfirst.push_back(v); csecond.push_back(-1); }
   const int nc = (int)cfirst.size();
   std::vector<int> cperm(nc);
   std::iota(cperm.begin(), cperm.end(), 0);
   double t_ord0 = now_s();
-  if (opt.ordering == 0 && n > opt.dense_n && nc > 2) {
-    std::vector<int64_t> cx(nc + 1, 0), cadj, vw(nc);
+  if (opt.ordering == 0 && n > opt.dense_n && nce > 2) {
+    std::vector<int64_t> cx(nce + 1, 0), cadj, vw(nce);
     std::vector<int> mark(nc, -1);
     cadj.reserve((size_t)xadj[n]);
-    for (int v = 0; v < nc; ++v) {
+    for (int v = 0; v < nce; ++v) {
       mark[v] = v;
       int mem[2] = {cfirst[v], csecond[v]};
       for (int m = 0; m < 2; ++m) {
         if (mem[m] < 0) continue;
         for (int64_t p = xadj[mem[m]]; p < xadj[mem[m] + 1]; ++p) {
           int w = cnode[adj[p]];
-          if (mark[w] != v) { mark[w] = v; cadj.push_back(w); }
+          if (w < nce && mark[w] != v) { mark[w] = v; cadj.push_back(w); }
         }
       }
       cx[v + 1] = (int64_t)cadj.size();
       vw[v] = csecond[v] >= 0 ? 2 : 1;
     }
     if (!cadj.empty()) {
-      int64_t nv = nc;
-      std::vector<int64_t> mp(nc), mip(nc);
+      int64_t nv = nce;
+      std::vector<int64_t> mp(nce), mip(nce);
       int64_t mopt[40];
       METIS_SetDefaultOptions(mopt);
       int rc = METIS_NodeND(&nv, cx.data(), cadj.data(), vw.data(), mopt, mp.data(), mip.data());
       if (rc != 1) { err = "METIS_NodeND failed"; return -3; }
-      for (int v = 0; v < nc; ++v) cperm[v] = (int)mp[v];  // new position v holds compressed node mp[v]
+      for (int v = 0; v < nce; ++v) cperm[v] = (int)mp[v];  // new position v holds compressed node mp[v]
     }
   }
   S.t_order = now_s() - t_ord0;
@@ -274,7 +285,7 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
       std::vector<int> shadow(partner);
       std::vector<int> visit(n, -1), from_s(n, -1), queue;
       for (int s0 = 0; s0 < n; ++s0) {
-        if (!saddle[s0] || partner[s0] >= 0) continue;
+        if (!saddle[s0] || partner[s0] >= 0 || is_sc[s0]) continue;
         queue.clear();
         queue.push_back(s0);
         int found_x = -1;
@@ -282,7 +293,7 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
           int sq = queue[qh];
           for (int64_t p = xadj[sq]; p < xadj[sq + 1]; ++p) {
             int x = adj[p];
-            if (saddle[x] || visit[x] == s0 || !(adjw[p] > 0.0)) continue;
+            if (saddle[x] || is_sc[x] || visit[x] == s0 || !(adjw[p] > 0.0)) continue;
             visit[x] = s0;
             from_s[x] = sq;
             if (shadow[x] < 0) { found_x = x; break; }
@@ -302,6 +313,7 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
           }
         }
         for (int64_t p = xadj[s0]; p < xadj[s0 + 1]; ++p) last = std::max(last, iperm[adj[p]]);
+        last = std::min(last, n - m - 1);   // never into the Schur block
         if (last > iperm[s0]) {
           // do not split the pair (primal at `last`, its saddle partner at last+1)
           const int xl = perm[last];
@@ -318,8 +330,28 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
   }
 
   // ---- 5. etree, postorder, relabel -----------------------------------------------------------
+  // The elimination tree, the column counts and the row structures see the path sc[0]-sc[1]-...-sc[m-1] as extra edges:
+  // S is then a chain at the top of the tree, which the postorder (roots ascending) keeps last and in order.  The
+  // numeric pattern (step 9) does not see them.
+  std::vector<int64_t> xadj_p;
+  std::vector<int> adj_p;
+  if (m > 1) {
+    std::vector<int> nxt(n, -1), prv(n, -1);
+    for (int i = 0; i + 1 < m; ++i) { nxt[sc[i]] = sc[i + 1]; prv[sc[i + 1]] = sc[i]; }
+    xadj_p.assign(n + 1, 0);
+    for (int i = 0; i < n; ++i) xadj_p[i + 1] = xadj_p[i] + (xadj[i + 1] - xadj[i]) + (nxt[i] >= 0) + (prv[i] >= 0);
+    adj_p.resize((size_t)xadj_p[n]);
+    for (int i = 0; i < n; ++i) {
+      int64_t q = xadj_p[i];
+      for (int64_t p = xadj[i]; p < xadj[i + 1]; ++p) adj_p[q++] = adj[p];
+      if (nxt[i] >= 0) adj_p[q++] = nxt[i];
+      if (prv[i] >= 0) adj_p[q++] = prv[i];
+    }
+  }
+  const std::vector<int64_t>& gx = m > 1 ? xadj_p : xadj;
+  const std::vector<int>& ga = m > 1 ? adj_p : adj;
   std::vector<int> parent;
-  etree_from_graph(n, xadj, adj, perm, iperm, parent);
+  etree_from_graph(n, gx, ga, perm, iperm, parent);
   {
     std::vector<int> post;
     postorder(n, parent, post);
@@ -327,7 +359,7 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     for (int t = 0; t < n; ++t) perm2[t] = perm[post[t]];
     perm.swap(perm2);
     for (int k = 0; k < n; ++k) iperm[perm[k]] = k;
-    etree_from_graph(n, xadj, adj, perm, iperm, parent);
+    etree_from_graph(n, gx, ga, perm, iperm, parent);
   }
 
   // children lists (ascending)
@@ -356,8 +388,8 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
     for (int j = 0; j < n; ++j) {
       if (parent[j] >= 0) delta[parent[j]]--;        // j is not a root: its parent's count loses the overlap
       const int old = perm[j];
-      for (int64_t p = xadj[old]; p < xadj[old + 1]; ++p) {
-        const int i = iperm[adj[p]];
+      for (int64_t p = gx[old]; p < gx[old + 1]; ++p) {
+        const int i = iperm[ga[p]];
         if (i <= j || first[j] <= maxfirst[i]) continue;
         maxfirst[i] = first[j];
         const int jprev = prevleaf[i];
@@ -376,8 +408,8 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
       for (int j = 0; j < n; ++j) {
         std::vector<int>& out = st[j];
         int old2 = perm[j];
-        for (int64_t p = xadj[old2]; p < xadj[old2 + 1]; ++p) {
-          int i = iperm[adj[p]];
+        for (int64_t p = gx[old2]; p < gx[old2 + 1]; ++p) {
+          int i = iperm[ga[p]];
           if (i > j && mark[i] != j) { mark[i] = j; out.push_back(i); }
         }
         for (int c = chead[j]; c >= 0; c = cnext[c]) {
@@ -394,8 +426,15 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
 
   // ---- 7. supernode partition -----------------------------------------------------------------
   std::vector<char> link(n, 0);  // link[j]: j and j+1 share a supernode
+  // the Schur block is one supernode of its own, whatever the merges below would do
+  auto sc_links = [&]() {
+    if (m == 0) return;
+    link[n - m - 1] = 0;
+    for (int j = n - m; j + 1 < n; ++j) link[j] = 1;
+  };
   if (n <= opt.dense_n) {
     for (int j = 0; j + 1 < n; ++j) link[j] = 1;
+    sc_links();
   } else {
     std::vector<int> sz(n, 1);
     for (int j = 0; j < n; ++j) if (parent[j] >= 0) sz[parent[j]] += sz[j];
@@ -410,6 +449,7 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
       int pc = iperm[i], px = iperm[partner[i]];
       if (pc == px + 1 && parent[px] == pc) link[px] = 1;
     }
+    sc_links();
     // relaxed amalgamation of a contiguous last child into its parent, cumulative criterion
     int gstart = 0;
     int64_t gtrue = 0;
@@ -422,7 +462,7 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
       for (int j = b; j <= e; ++j) ptrue += cc[j];
       gtrue += ptrue;
       // boundary after e
-      if (e + 1 < n && parent[e] == e + 1) {
+      if (e + 1 < n - m && parent[e] == e + 1) {
         int e2 = e + 1;
         while (e2 + 1 < n && link[e2]) ++e2;
         int64_t ntrue = 0;
@@ -469,8 +509,8 @@ int analyse(int n, int64_t nnz, const int* irn, const int* jcn, const double* va
       buf.clear();
       for (int j = a; j < e; ++j) {
         int old = perm[j];
-        for (int64_t p = xadj[old]; p < xadj[old + 1]; ++p) {
-          int i = iperm[adj[p]];
+        for (int64_t p = gx[old]; p < gx[old + 1]; ++p) {
+          int i = iperm[ga[p]];
           if (i >= e && mark[i] != s) { mark[i] = s; buf.push_back(i); }
         }
       }

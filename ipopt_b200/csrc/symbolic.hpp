@@ -9,7 +9,7 @@
 //
 // Pipeline: unique lower pattern -> saddle-row pairing (zero-diagonal constraint rows are
 // matched to a primal neighbour so a 2x2 pivot is always available inside a supernode) ->
-// compressed graph -> METIS nested dissection -> elimination tree -> postorder -> column
+// compressed graph -> METIS nested dissection (Schur variables, if any, appended) -> elimination tree -> postorder -> column
 // structures -> supernodes (leaf-subtree merge + fundamental + relaxed) -> assembly maps,
 // child->parent relative indices, level schedule.
 #pragma once
@@ -26,6 +26,10 @@ struct AnalyseOptions {
   double relax_frac = 0.05;    // relaxed amalgamation: tolerated fraction of explicit zeros
   int relax_small = 16;        // always merge a last child when merged k <= relax_small
   int dense_n = 48;            // n <= dense_n: a single dense front, natural order
+  // Schur variables (0-based original indices, distinct, fewer than n): the last sc_vars.size() pivot positions are
+  // sc_vars in this order and form one root supernode with r = 0.  They take no part in saddle pairing, the ordering
+  // sees the other variables only, and no supernode merges them with another variable.  Empty: the ordinary analysis.
+  std::vector<int> sc_vars;
 };
 
 struct Symbolic {
