@@ -63,6 +63,12 @@ struct LinvPlan {
 
 // triangular-solve work of a set of fronts (solve_dataflow.cu): subtrees for k_solve_sub + task lists for k_solve_top
 struct SolvePlan {
+  // host copies of the forward lists as uploaded, one-element placeholders included (the sparse forward solve prunes them)
+  std::vector<SolveTask> tf;
+  std::vector<int2> pairs;
+  std::vector<SubDesc> subs;
+  std::vector<int> meta, bundle;
+  std::vector<std::vector<int>> direct;
   DevBuf<SolveTask> d_tf, d_tb;
   DevBuf<int> d_bundle, d_sub_meta, d_ccnt, d_subrow;
   DevBuf<SubDesc> d_subs;
@@ -77,7 +83,7 @@ struct SolvePlan {
 
 // what the solve sweeps write, for `width` columns: column c of each array at its base + c * its stride in M.  The chunk
 // partials and counters belong to a plan (a counter counts modulo its task's nq, so plans must not share them): one column
-// uses those of the plan it sweeps, a block (width > 1) has its own copies of splan's in d_part / d_ccnt.
+// uses those of the plan it sweeps, a block (width > 1) has its own copies of the handle's in d_part / d_ccnt.
 struct SweepState {
   int width = 0;
   DevBuf<double> d_x, d_cbv, d_bigv, d_bigy, d_part;
@@ -100,15 +106,11 @@ struct LmulPlan {
   int width = 0;
 };
 
-// The sparse forward solve (b200ldlt_sparse_fwd_solve): host copies of the full plan's forward lists with per-front
-// indices into them, the marks of one call, and the staging of the pruned lists (pinned -> device, sized by the full
-// plan).  Built at the first sparse call after an analysis, before that call's timing starts; a handle that never makes
-// one allocates none of it.
+// The sparse forward solve (b200ldlt_sparse_fwd_solve): per-front indices into the host copies of the full plan's forward
+// lists, the marks of one call, and the staging of the pruned lists (pinned -> device, sized by the full plan).  Built at
+// the first sparse call after an analysis, before that call's timing starts; a handle that never makes one allocates
+// none of it.
 struct SparseFwdPlan {
-  std::vector<SolveTask> tf;                   // splan's forward top tasks, subtree items, bundles, direct-level lists
-  std::vector<int2> pairs;
-  std::vector<int> bundle;
-  std::vector<std::vector<int>> direct;
   std::vector<int> dlev, didx;                 // by front: its direct level and index there, or -1
   std::vector<int> item_of, sub_of;            // by front: the subtree item / the subtree that walks it, or -1
   std::vector<int> task_ptr, task_idx;         // by front (CSR): its forward top tasks, ascending
@@ -170,6 +172,18 @@ struct SchurLists {
   long long dig_bytes = 0, exp_ints = 0;   // scratch needed by the largest level
 };
 
+// what one set of fronts needs (build_front_plan): the factorisation's level plans, Schur lists and device front list,
+// the explicit L11^-1 work of the whole set and, when filled, the same work split by tree level (issued behind each
+// level's chain), and the triangular-solve plan
+struct FrontPlan {
+  std::vector<LevelPlan> levels;
+  SchurLists schur;
+  DevBuf<int> d_fl;
+  LinvPlan linv;
+  std::vector<std::unique_ptr<LinvPlan>> linv_level;
+  SolvePlan solve;
+};
+
 // environment switches for profiling / A-B runs, read ONCE at b200ldlt_create (never on the enqueue path)
 struct DebugSwitches {
   bool one_stream = false;        // B200_ONE_STREAM=1: big-front pipeline on a single stream
@@ -220,8 +234,7 @@ struct Solver {
   long long n_factor = 0;
   bool reanalysed_since_raise = false;
   Symbolic S;
-  std::vector<LevelPlan> plan;
-  SchurLists schur;
+  FrontPlan fronts;                  // factorisation: all fronts but the Schur root; solves: all fronts
   DevBuf<int8_t> d_tc_dig;           // digit scratch of the tensor-core Schur path (largest level)
   DevBuf<int> d_tc_exp;
   b200ldlt_info info;
@@ -229,7 +242,7 @@ struct Solver {
   double pivtol = 1e-8;
 
   // device
-  DevBuf<int> d_sn_start, d_sn_parent, d_rows, d_rel, d_child_ptr, d_child_idx, d_front_list, d_perm;
+  DevBuf<int> d_sn_start, d_sn_parent, d_rows, d_rel, d_child_ptr, d_child_idx, d_perm;
   DevBuf<int> d_useg_src, d_u_row, d_u_col, d_irn, d_jcn;
   DevBuf<long long> d_rows_ptr, d_uent_ptr, d_u_dst64, d_L_off, d_cb_off, d_useg_ptr;
   DevBuf<unsigned> d_u_dst;
@@ -272,11 +285,9 @@ struct Solver {
   DevBuf<double> d_linv_part;       // partial tiles of the chunked k_linv_gemm items (one launch at a time uses it)
   DevBuf<int> d_linv_cnt;           // their arrival counters (self-resetting)
   DevBuf<long long> d_linv_off, d_gmap_off;
+  std::vector<long long> linv_off;  // per supernode: its L11^-1 block in d_linv (order > 256), else -1
   DevBuf<FrontDesc> d_fdesc;
   DevBuf<int> d_gmap;
-  LinvPlan linv_plan;               // explicit inverses of the big fronts' pivot blocks (all fronts)
-  std::vector<std::unique_ptr<LinvPlan>> linv_level;   // the same work, split by tree level (issued behind each level's chain)
-  SolvePlan splan;                  // all fronts
   std::vector<char> solve_direct_front;   // per supernode: solved by k_solve_direct (see build_solve_tables)
   int solve_epoch = 0;
   int num_sms = 132;
@@ -284,11 +295,8 @@ struct Solver {
     bool active = false;
     int rank = 0, world = 1, nsub = 0;
     std::vector<int> owner, cut_roots, top_fronts;
-    std::vector<LevelPlan> plan[2];          // [0] my subtrees, [1] top part
-    SchurLists schur[2];
-    DevBuf<int> d_fl[2], d_mark_cut, d_mark_top;
-    SolvePlan splan[2];
-    LinvPlan linv_plan[2];
+    FrontPlan part[2];                       // [0] my subtrees, [1] top part
+    DevBuf<int> d_mark_cut, d_mark_top;
   } shard;
   cudaGraph_t fgraph = nullptr;
   cudaGraphExec_t fgraph_exec = nullptr;
@@ -679,7 +687,7 @@ static int build_solve_plan(Solver* sv, const Symbolic& S, const std::vector<cha
     }
   }
   // the bottom levels owned by k_solve_direct, one list per level
-  SP.d_direct.clear(); SP.direct_cnt.clear();
+  SP.d_direct.clear(); SP.direct_cnt.clear(); SP.direct.clear();
   long long ndirect = 0, direct_nnz = 0;
   for (int l = 0; l < S.nlevels && l < sv->dbg.solve_direct; ++l) {
     std::vector<int> lst;
@@ -692,6 +700,7 @@ static int build_solve_plan(Solver* sv, const Symbolic& S, const std::vector<cha
     SP.d_direct.emplace_back(new DevBuf<int>());
     if (lst.empty()) lst.push_back(0);
     CU(SP.d_direct.back()->upload(lst, st));
+    SP.direct.push_back(std::move(lst));
   }
   CU(SP.d_sub_Loff.upload(subLoff, st));
   if (sv->opt.verbose)
@@ -711,6 +720,8 @@ static int build_solve_plan(Solver* sv, const Symbolic& S, const std::vector<cha
   CU(SP.d_ccnt.alloc(std::max(ncidx, 1)));
   CU(cudaMemsetAsync(SP.d_ccnt.p, 0, SP.d_ccnt.n * sizeof(int), st));
   CU(SP.d_part.alloc(std::max<long long>(npart, 1) * 64));
+  SP.tf = std::move(tf); SP.pairs = std::move(pairs); SP.subs = std::move(subs);
+  SP.meta = std::move(meta); SP.bundle = std::move(bundle);
   return B200LDLT_SUCCESS;
 }
 
@@ -770,6 +781,23 @@ static int upload_schur_lists(Solver* sv, SchurLists& SL, cudaStream_t st) {
   if ((long long)sv->d_tc_dig.n < SL.dig_bytes) CU(sv->d_tc_dig.alloc(SL.dig_bytes));
   if ((long long)sv->d_tc_exp.n < SL.exp_ints) CU(sv->d_tc_exp.alloc(SL.exp_ints));
   return B200LDLT_SUCCESS;
+}
+
+// The plan of the fronts in take_factor (factorisation, L11^-1) and take_solve (triangular solves); FP.linv_level is left
+// empty.  Needs the solve tables (build_solve_tables).
+static int build_front_plan(Solver* sv, const std::vector<char>& take_factor, const std::vector<char>& take_solve,
+                            FrontPlan& FP) {
+  const Symbolic& S = sv->S;
+  cudaStream_t st = sv->stream;
+  std::vector<int> fl;
+  build_level_plans(S, sv->opt.smem_front_max, take_factor, fl, FP.levels, FP.schur, sv->tc_min_r, !sv->dbg.no_warp2);
+  if (fl.empty()) fl.push_back(0);
+  CU(FP.d_fl.upload(fl, st));
+  FP.linv_level.clear();
+  int rc = upload_schur_lists(sv, FP.schur, st);
+  if (rc == B200LDLT_SUCCESS) rc = build_linv_plan(sv, S, take_factor, FP.linv, st);
+  if (rc == B200LDLT_SUCCESS) rc = build_solve_plan(sv, S, take_solve, FP.solve, st);
+  return rc;
 }
 
 // the persistent sweep kernel for one column (multi = false) or a block of columns; apply_d = false: the forward sweep
@@ -926,11 +954,6 @@ static int run_analysis(Solver* sv, const double* vals) {
     D.einv_off = sv->d_einv_off.p; D.einv = sv->d_einv.p;
   }
 
-  // ---- launch plan: per level, big fronts first then small ones by descending order --------
-  std::vector<int> fl;
-  build_level_plans(S, sv->opt.smem_front_max, take_f, fl, sv->plan, sv->schur, sv->tc_min_r, !sv->dbg.no_warp2);
-  CU(sv->d_front_list.upload(fl, st));
-  { int rc2 = upload_schur_lists(sv, sv->schur, st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
   CU(cudaFuncSetAttribute(k_tc_schur, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
   CU(cudaFuncSetAttribute(k_big_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, CHAIN_SMEM));
   CU(cudaFuncSetAttribute(k_front_warp2, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * S2_SMEM_PER_WARP));
@@ -950,7 +973,8 @@ static int run_analysis(Solver* sv, const double* vals) {
     }
     // explicit inverses of the big fronts' pivot blocks (k_linv_*): K64 x K64 doubles per big front
     {
-      std::vector<long long> linv_off(S.nsn, -1);
+      std::vector<long long>& linv_off = sv->linv_off;
+      linv_off.assign(S.nsn, -1);
       long long tot = 0;
       for (int s = 0; s < S.nsn; ++s) if (S.f(s) > DF_MIDMAX) {
         linv_off[s] = tot;
@@ -961,16 +985,6 @@ static int run_analysis(Solver* sv, const double* vals) {
       CU(sv->d_linv_off.upload(linv_off, st));
       CU(sv->d_linv.alloc(std::max<long long>(tot, 1)));
       CU(cudaMemsetAsync(sv->d_linv.p, 0, sv->d_linv.n * sizeof(double), st));
-      int rc2 = build_linv_plan(sv, S, take_f, sv->linv_plan, st);
-      if (rc2 != B200LDLT_SUCCESS) return rc2;
-      sv->linv_level.clear();
-      for (int l = 0; l < S.nlevels; ++l) {
-        std::vector<char> tl(S.nsn, 0);
-        bool any = false;
-        for (int q = 0; q < S.nsn; ++q) if (take_f[q] && S.sn_level[q] == l && S.f(q) > kSolveMidMax) { tl[q] = 1; any = true; }
-        sv->linv_level.emplace_back(new LinvPlan());
-        if (any) { rc2 = build_linv_plan(sv, S, tl, *sv->linv_level.back(), st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
-      }
     }
     CU(sv->d_boff.upload(boff, st));
     CU(sv->d_bigv_off.upload(bigv_off, st));
@@ -986,12 +1000,16 @@ static int run_analysis(Solver* sv, const double* vals) {
                           std::max<long long>(bv, 1), 0};
     CU(alloc_sweep_state(sv, sv->sweep, one));
     sv->solve_epoch = 0;
-    {
-      int rc2 = build_solve_tables(sv, S, st);
-      if (rc2 != B200LDLT_SUCCESS) return rc2;
-      std::vector<char> take(S.nsn, 1);
-      rc2 = build_solve_plan(sv, S, take, sv->splan, st);
-      if (rc2 != B200LDLT_SUCCESS) return rc2;
+    int rc2 = build_solve_tables(sv, S, st);
+    if (rc2 == B200LDLT_SUCCESS) rc2 = build_front_plan(sv, take_f, std::vector<char>(S.nsn, 1), sv->fronts);
+    if (rc2 != B200LDLT_SUCCESS) return rc2;
+    // the L11^-1 work once more, split by tree level
+    for (int l = 0; l < S.nlevels; ++l) {
+      std::vector<char> tl(S.nsn, 0);
+      bool any = false;
+      for (int q = 0; q < S.nsn; ++q) if (take_f[q] && S.sn_level[q] == l && S.f(q) > kSolveMidMax) { tl[q] = 1; any = true; }
+      sv->fronts.linv_level.emplace_back(new LinvPlan());
+      if (any) { rc2 = build_linv_plan(sv, S, tl, *sv->fronts.linv_level.back(), st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
     }
     if (sv->opt.verbose)
       fprintf(stderr, "[b200ldlt] solve: %d big-front blocks, top grid %d x %d thr (%d CTAs per SM)\n",
@@ -1033,10 +1051,10 @@ static cudaError_t launch_pdl(bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-// enqueue the whole numeric factorisation of the values in d_vals
-static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nullptr, const int* fl_p = nullptr,
-                          bool prologue = true, const LinvPlan* linv_p = nullptr, const SchurLists* sl_p = nullptr) {
-  const SchurLists& SL = sl_p ? *sl_p : sv->schur;
+// enqueue the numeric factorisation of the fronts of FP from the values in d_vals; prologue: first the summing of
+// duplicates and the scaling
+static int enqueue_factor(Solver* sv, const FrontPlan& FP, bool prologue) {
+  const SchurLists& SL = FP.schur;
   Symbolic& S = sv->S;
   cudaStream_t st = sv->stream;
   DevSym& D = sv->DS;
@@ -1045,8 +1063,8 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
   N.tiny = sv->opt.tiny;
   const int n = S.n;
   const long long nu = S.nnz_u;
-  const int* fl = fl_p ? fl_p : sv->d_front_list.p;
-  const std::vector<LevelPlan>& plan = plan_p ? *plan_p : sv->plan;
+  const int* fl = FP.d_fl.p;
+  const std::vector<LevelPlan>& plan = FP.levels;
   int& L = sv->launches;
   if (prologue) {
   L = 0;
@@ -1174,14 +1192,14 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
         CU(cudaEventRecord(e, su));
         CU(cudaStreamWaitEvent(st, e, 0));
       }
-      if (!linv_p && !sv->dbg.one_stream && l < (int)sv->linv_level.size() && sv->linv_level[l]->ndiag > 0) {
+      if (!FP.linv_level.empty() && !sv->dbg.one_stream && FP.linv_level[l]->ndiag > 0) {
         // explicit L11 inverses of this level's fronts: behind the chain on their own stream, concurrent with the Schur
         // complements and the levels above (they only read the finished pivot blocks; k_linv_gemm<1> uses the top k x k
         // part of W as scratch, which nothing reads after the chain)
         cudaEvent_t e = sv->next_event();
         CU(cudaEventRecord(e, st));
         CU(cudaStreamWaitEvent(sv->stream3, e, 0));
-        int rc = enqueue_linv(sv, *sv->linv_level[l], sv->stream3);
+        int rc = enqueue_linv(sv, *FP.linv_level[l], sv->stream3);
         if (rc != B200LDLT_SUCCESS) return rc;
         linv_forked = true;
       }
@@ -1224,7 +1242,7 @@ static int enqueue_factor(Solver* sv, const std::vector<LevelPlan>* plan_p = nul
     CU(cudaEventRecord(e, sv->stream3));
     CU(cudaStreamWaitEvent(st, e, 0));
   } else {
-    int rc = enqueue_linv(sv, linv_p ? *linv_p : sv->linv_plan, st);
+    int rc = enqueue_linv(sv, FP.linv, st);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   CU(cudaGetLastError());
@@ -1353,7 +1371,7 @@ static int do_factor(Solver* sv, const double* d_vals_ext_in, bool from_host, in
       if (sv->fgraph_exec) { cudaGraphExecDestroy(sv->fgraph_exec); sv->fgraph_exec = nullptr; }
       if (sv->fgraph) { cudaGraphDestroy(sv->fgraph); sv->fgraph = nullptr; }
       CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      rc = enqueue_factor(sv);
+      rc = enqueue_factor(sv, sv->fronts, true);
       cudaError_t ce = cudaStreamEndCapture(st, &sv->fgraph);
       if (rc != B200LDLT_SUCCESS) return rc;
       CU(ce);
@@ -1364,7 +1382,7 @@ static int do_factor(Solver* sv, const double* d_vals_ext_in, bool from_host, in
     sv->launches = sv->fgraph_launches;
     CU(cudaGraphLaunch(sv->fgraph_exec, st));
   } else {
-    rc = enqueue_factor(sv);
+    rc = enqueue_factor(sv, sv->fronts, true);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   return finish_factor(sv, check_inertia, expected_neg, num_neg);
@@ -1439,37 +1457,60 @@ static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, 
   return B200LDLT_SUCCESS;
 }
 
-// nb columns of d_in (leading dimension n) -> d_out (in place when they are the same) by one forward and one backward
-// sweep over all fronts, nb <= W.width
-static int enqueue_solve(Solver* sv, SweepState& W, const double* d_in, double* d_out, int nb) {
-  cudaStream_t st = sv->stream;
+// The two stages every solve over the fronts of SP is built from, for nb <= W.width columns of leading dimension n.  Each
+// sweep waits on flags that its own fronts stamp with sv->solve_epoch, so each stage takes a new epoch: a flag left by
+// an earlier sweep never matches it.  (Backward work waits only on backward flags, so a backward stage may follow a
+// forward one under a new epoch.)
+// forward: x = P^T S d_in, then the forward sweep; apply_d = false leaves D^-1 out (L only)
+static int forward(Solver* sv, const SolvePlan& SP, SweepState& W, const double* d_in, int nb, bool apply_d = true) {
   const int n = sv->n;
-  const dim3 g(cdiv(n, 256), nb);
-  k_rhs_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_in, W.d_x.p, W.M.x); ++sv->launches;
+  k_rhs_in<<<dim3(cdiv(n, 256), nb), 256, 0, sv->stream>>>(n, sv->d_perm.p, sv->d_scale.p, d_in, W.d_x.p, W.M.x);
+  ++sv->launches;
   sv->solve_epoch++;
-  int rc = launch_sweep(sv, sv->splan, W, nb, true);
-  if (rc == B200LDLT_SUCCESS) rc = launch_sweep(sv, sv->splan, W, nb, false);
-  if (rc != B200LDLT_SUCCESS) return rc;
-  k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, W.M.x, d_out); ++sv->launches;
+  return launch_sweep(sv, SP, W, nb, true, apply_d);
+}
+
+// backward: the backward sweep, then d_out = S P x unless d_out is null
+static int backward(Solver* sv, const SolvePlan& SP, SweepState& W, double* d_out, int nb) {
+  sv->solve_epoch++;
+  const int rc = launch_sweep(sv, SP, W, nb, false);
+  if (rc != B200LDLT_SUCCESS || !d_out) return rc;
+  const int n = sv->n;
+  k_sol_out<<<dim3(cdiv(n, 256), nb), 256, 0, sv->stream>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, W.M.x, d_out);
+  ++sv->launches;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
 }
 
-// One part of the solve (job 1..4, include/b200ldlt.h) for nb columns of d_in -> d_out (leading dimension n, in place
-// when they are the same), nb <= W.width.  The parts are the pieces of enqueue_solve: job 1 is its first half with the
-// forward sweep leaving D^-1 out, copied out in pivot order; job 3 its second half, fed in pivot order; job 2 (and the
-// front of job 4) applies D^-1 through the helper the fused sweep uses.  So job 3 . 2 . 1 and job 4 . 1 reproduce
-// enqueue_solve bit for bit.  Launches: job 1, 3, 4: 2 + one sweep (the direct levels + 1); job 2: 1.
-static int enqueue_partial(Solver* sv, SweepState& W, int job, const double* d_in, double* d_out, int nb) {
+// columns [0, nrhs) in blocks of at most cap columns: block(c, w) for each, in order
+template <class Block>
+static int for_blocks(int nrhs, int cap, Block&& block) {
+  for (int c = 0; c < nrhs;) {
+    const int w = std::min(cap, nrhs - c);
+    const int rc = block(c, w);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    c += w;
+  }
+  return B200LDLT_SUCCESS;
+}
+
+// The solve (job 0) or one part of it (job 1..4, include/b200ldlt.h) for nb columns of d_in -> d_out (leading dimension
+// n, in place when they are the same), nb <= W.width.  Job 0 is forward then backward over all fronts; job 1 is its
+// forward stage leaving D^-1 out, copied out in pivot order; job 3 its backward stage, fed in pivot order; job 2 (and
+// the front of job 4) applies D^-1 through the helper the fused sweep uses.  So job 3 . 2 . 1 and job 4 . 1 reproduce
+// job 0 bit for bit.  Launches: job 0: 2 + two sweeps; job 1, 3, 4: 2 + one sweep (the direct levels + 1); job 2: 1.
+static int enqueue_solve(Solver* sv, SweepState& W, int job, const double* d_in, double* d_out, int nb) {
+  const SolvePlan& SP = sv->fronts.solve;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   const dim3 g(cdiv(n, 256), nb);
   const long long ldx = W.M.x, ldb = W.M.bigv;
-  int rc = B200LDLT_SUCCESS;
+  if (job == 0) {
+    const int rc = forward(sv, SP, W, d_in, nb);
+    return rc != B200LDLT_SUCCESS ? rc : backward(sv, SP, W, d_out, nb);
+  }
   if (job == 1) {
-    k_rhs_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_in, W.d_x.p, ldx); ++sv->launches;
-    sv->solve_epoch++;
-    rc = launch_sweep(sv, sv->splan, W, nb, true, false);
+    const int rc = forward(sv, SP, W, d_in, nb, false);
     if (rc != B200LDLT_SUCCESS) return rc;
     k_piv_out<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb, d_out); ++sv->launches;
   } else if (job == 2) {
@@ -1480,13 +1521,10 @@ static int enqueue_partial(Solver* sv, SweepState& W, int job, const double* d_i
     if (job == 3) k_piv_in<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, d_in, W.d_x.p, ldx, W.d_bigv.p, ldb);
     else k_dinv<<<g, 256, 0, st>>>(n, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, d_in, sv->d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb);
     ++sv->launches;
-    sv->solve_epoch++;
-    rc = launch_sweep(sv, sv->splan, W, nb, false);
-    if (rc != B200LDLT_SUCCESS) return rc;
-    k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, d_out); ++sv->launches;
+    return backward(sv, SP, W, d_out, nb);
   }
   CU(cudaGetLastError());
-  return rc;
+  return B200LDLT_SUCCESS;
 }
 
 // The sweep state of the blocked solve, B200_SOLVE_BLOCK columns wide: allocated once per analysis, at the first nrhs > 1
@@ -1500,8 +1538,8 @@ static bool block_solve_state(Solver* sv) {
   SweepState& B = *sv->blk;
   MultiStride M = sv->sweep.M;
   M.nb = nb;
-  M.nccnt = (int)sv->splan.d_ccnt.n;
-  M.part = (long long)sv->splan.d_part.n;
+  M.nccnt = (int)sv->fronts.solve.d_ccnt.n;
+  M.part = (long long)sv->fronts.solve.d_part.n;
   const cudaError_t e = alloc_sweep_state(sv, B, M);
   if (e != cudaSuccess) {
     if (sv->opt.verbose) fprintf(stderr, "[b200ldlt] blocked solve unavailable (%s): one solve per column\n", cudaGetErrorString(e));
@@ -1519,18 +1557,12 @@ static bool block_solve_state(Solver* sv) {
 
 // nrhs columns of d_rhs (leading dimension n), in place: blocks of up to B200_SOLVE_BLOCK columns through the blocked
 // state, single columns through the one-column state.  `blocked`: the result of block_solve_state, called by the entry
-// point before its timing starts.  job 0: the solve; 1..4: enqueue_partial.
+// point before its timing starts.  job: as in enqueue_solve.
 static int enqueue_solve_columns(Solver* sv, double* d_rhs, int nrhs, bool blocked, int job = 0) {
-  const int cap = blocked ? sv->blk->width : 1;
-  for (int c = 0; c < nrhs;) {
-    const int w = std::min(cap, nrhs - c);
+  return for_blocks(nrhs, blocked ? sv->blk->width : 1, [&](int c, int w) {
     double* col = d_rhs + (size_t)c * sv->n;
-    SweepState& W = w == 1 ? sv->sweep : *sv->blk;
-    const int rc = job == 0 ? enqueue_solve(sv, W, col, col, w) : enqueue_partial(sv, W, job, col, col, w);
-    if (rc != B200LDLT_SUCCESS) return rc;
-    c += w;
-  }
-  return B200LDLT_SUCCESS;
+    return enqueue_solve(sv, w == 1 ? sv->sweep : *sv->blk, job, col, col, w);
+  });
 }
 
 // The Fredholm alternative (b200ldlt_solve_fredholm) with zero pivots Z: columns [0, nrhs) of d_x (leading dimension n)
@@ -1546,39 +1578,30 @@ static int enqueue_fredholm(Solver* sv, double* d_x, int nrhs, bool blocked) {
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   CU(cudaMemsetAsync(sv->d_fred_nrm.p, 0, 2 * (size_t)nrhs * sizeof(unsigned long long), st));
+  const SolvePlan& SP = sv->fronts.solve;
   SweepState& W = blocked ? *sv->blk : sv->sweep;
-  const int cap = blocked ? W.width / 2 : 1;
   const long long ldx = W.M.x, ldb = W.M.bigv;
-  for (int c = 0; c < nrhs;) {
-    const int w = std::min(cap, nrhs - c);
+  const int rc = for_blocks(nrhs, blocked ? W.width / 2 : 1, [&](int c, int w) -> int {
     double* col = d_x + (size_t)c * n;
     const dim3 g(cdiv(n, 256), w);
-    k_rhs_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, col, W.d_x.p, ldx); ++sv->launches;
-    sv->solve_epoch++;
-    int rc = launch_sweep(sv, sv->splan, W, w, true, false);
-    if (rc != B200LDLT_SUCCESS) return rc;
+    int rc2 = forward(sv, SP, W, col, w, false);
+    if (rc2 != B200LDLT_SUCCESS) return rc2;
     k_fred<<<g, 256, 0, st>>>(n, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, sv->d_zflag.p, sv->d_piv_big.p, W.d_x.p, ldx,
                               W.d_bigv.p, ldb, w, blocked ? nullptr : sv->d_fred_z.p, sv->d_fred_nrm.p + 2 * (size_t)c);
     ++sv->launches;
-    sv->solve_epoch++;
     if (blocked) {
-      rc = launch_sweep(sv, sv->splan, W, 2 * w, false);
-      if (rc != B200LDLT_SUCCESS) return rc;
+      rc2 = backward(sv, SP, W, nullptr, 2 * w);
+      if (rc2 != B200LDLT_SUCCESS) return rc2;
       k_fred_out<<<dim3(cdiv(n, 256), 2 * w), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, col, w, nrhs);
       ++sv->launches;
-    } else {
-      rc = launch_sweep(sv, sv->splan, W, 1, false);
-      if (rc != B200LDLT_SUCCESS) return rc;
-      k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, col); ++sv->launches;
-      k_piv_in<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, sv->d_fred_z.p, W.d_x.p, ldx, W.d_bigv.p, ldb); ++sv->launches;
-      sv->solve_epoch++;
-      rc = launch_sweep(sv, sv->splan, W, 1, false);
-      if (rc != B200LDLT_SUCCESS) return rc;
-      k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, d_x + (size_t)(nrhs + c) * n);
-      ++sv->launches;
+      return B200LDLT_SUCCESS;
     }
-    c += w;
-  }
+    rc2 = backward(sv, SP, W, col, 1);
+    if (rc2 != B200LDLT_SUCCESS) return rc2;
+    k_piv_in<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, sv->d_fred_z.p, W.d_x.p, ldx, W.d_bigv.p, ldb); ++sv->launches;
+    return backward(sv, SP, W, d_x + (size_t)(nrhs + c) * n, 1);
+  });
+  if (rc != B200LDLT_SUCCESS) return rc;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
 }
@@ -1682,51 +1705,33 @@ static int enqueue_lmul(Solver* sv, int trans, const double* d_x, double* d_y, i
 
 // nrhs columns in blocks of up to B200_SOLVE_BLOCK (lmul_state called before)
 static int enqueue_lmul_columns(Solver* sv, int trans, int nrhs, const double* d_x, double* d_y) {
-  for (int c = 0; c < nrhs;) {
-    const int w = std::min(sv->lmul->width, nrhs - c);
-    const int rc = enqueue_lmul(sv, trans, d_x + (size_t)c * sv->n, d_y + (size_t)c * sv->n, w);
-    if (rc != B200LDLT_SUCCESS) return rc;
-    c += w;
-  }
-  return B200LDLT_SUCCESS;
+  return for_blocks(nrhs, sv->lmul->width, [&](int c, int w) {
+    return enqueue_lmul(sv, trans, d_x + (size_t)c * sv->n, d_y + (size_t)c * sv->n, w);
+  });
 }
 
 // ---- sparse forward solve (b200ldlt_sparse_fwd_solve) --------------------------------------------------------------
-// Host copies of splan's forward lists and the per-front indices into them (SparseFwdPlan): at the first sparse call after
-// an analysis, before its timing starts.
+// The per-front indices into the host copies of the handle's forward lists (SparseFwdPlan): at the first sparse call
+// after an analysis, before its timing starts.
 static int sfs_state(Solver* sv) {
   if (sv->sfs) return B200LDLT_SUCCESS;
   const Symbolic& S = sv->S;
-  const SolvePlan& SP = sv->splan;
+  const SolvePlan& SP = sv->fronts.solve;
   const int n = sv->n, nsn = S.nsn;
-  cudaStream_t st = sv->stream;
   std::unique_ptr<SparseFwdPlan> P(new SparseFwdPlan());
-  std::vector<SubDesc> subs(SP.nsub);
-  std::vector<int> meta(SP.d_sub_meta.n);
-  P->tf.resize(SP.ntf); P->pairs.resize(SP.npair); P->bundle.resize(SP.d_bundle.n);
-  if (SP.ntf) CU(cudaMemcpyAsync(P->tf.data(), SP.d_tf.p, SP.ntf * sizeof(SolveTask), cudaMemcpyDeviceToHost, st));
-  if (SP.npair) CU(cudaMemcpyAsync(P->pairs.data(), SP.d_subpair.p, SP.npair * sizeof(int2), cudaMemcpyDeviceToHost, st));
-  if (SP.nsub) CU(cudaMemcpyAsync(subs.data(), SP.d_subs.p, SP.nsub * sizeof(SubDesc), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(meta.data(), SP.d_sub_meta.p, meta.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(P->bundle.data(), SP.d_bundle.p, P->bundle.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
-  P->direct.resize(SP.direct_cnt.size());
+  P->dlev.assign(nsn, -1); P->didx.assign(nsn, -1); P->item_of.assign(nsn, -1); P->sub_of.assign(nsn, -1);
   long long ndirect = 0;
   for (size_t l = 0; l < SP.direct_cnt.size(); ++l) {
-    P->direct[l].resize(SP.direct_cnt[l]);
     ndirect += SP.direct_cnt[l];
-    if (SP.direct_cnt[l]) CU(cudaMemcpyAsync(P->direct[l].data(), SP.d_direct[l]->p, SP.direct_cnt[l] * sizeof(int), cudaMemcpyDeviceToHost, st));
+    for (int i = 0; i < SP.direct_cnt[l]; ++i) { const int s = SP.direct[l][i]; P->dlev[s] = (int)l; P->didx[s] = i; }
   }
-  CU(cudaStreamSynchronize(st));
-  P->dlev.assign(nsn, -1); P->didx.assign(nsn, -1); P->item_of.assign(nsn, -1); P->sub_of.assign(nsn, -1);
-  for (size_t l = 0; l < P->direct.size(); ++l)
-    for (size_t i = 0; i < P->direct[l].size(); ++i) { const int s = P->direct[l][i]; P->dlev[s] = (int)l; P->didx[s] = (int)i; }
   P->item_ptr.assign(1, 0);
   for (int i = 0; i < SP.npair; ++i) {
-    for (const int u : {P->pairs[i].x, P->pairs[i].y}) {
+    for (const int u : {SP.pairs[i].x, SP.pairs[i].y}) {
       if (u < 0) continue;
-      const SubDesc& d = subs[u];
+      const SubDesc& d = SP.subs[u];
       for (int j = 0; j < d.nown; ++j) {
-        const int s = meta[d.moff + 2 * d.nlv + 1 + j];
+        const int s = SP.meta[d.moff + 2 * d.nlv + 1 + j];
         P->item_fr.push_back(s); P->item_of[s] = i; P->sub_of[s] = u;
       }
     }
@@ -1734,15 +1739,15 @@ static int sfs_state(Solver* sv) {
   }
   P->task_ptr.assign(nsn + 1, 0);
   auto each_front = [&](const SolveTask& T, auto&& fn) {
-    if (T.type == ST_SMALL) { for (int w = 0; w < T.blk; ++w) fn(P->bundle[T.s + w]); }
+    if (T.type == ST_SMALL) { for (int w = 0; w < T.blk; ++w) fn(SP.bundle[T.s + w]); }
     else fn(T.s);
   };
-  for (const SolveTask& T : P->tf) each_front(T, [&](int s) { P->task_ptr[s + 1]++; });
+  for (int j = 0; j < SP.ntf; ++j) each_front(SP.tf[j], [&](int s) { P->task_ptr[s + 1]++; });
   for (int s = 0; s < nsn; ++s) P->task_ptr[s + 1] += P->task_ptr[s];
   P->task_idx.resize(P->task_ptr[nsn]);
   {
     std::vector<int> fill(P->task_ptr.begin(), P->task_ptr.end() - 1);
-    for (int j = 0; j < SP.ntf; ++j) each_front(P->tf[j], [&](int s) { P->task_idx[fill[s]++] = j; });
+    for (int j = 0; j < SP.ntf; ++j) each_front(SP.tf[j], [&](int s) { P->task_idx[fill[s]++] = j; });
   }
   P->iperm.resize(n); P->sn_of.resize(n);
   for (int i = 0; i < n; ++i) P->iperm[S.perm[i]] = i;
@@ -1773,7 +1778,7 @@ static inline size_t align8(size_t b) { return (b + 7) & ~(size_t)7; }
 
 // Host part of a sparse forward solve.  The reach (the fronts on the tree paths from the fronts of b's variables to the
 // root) gives the run set R: the reach, the fronts walked by a subtree item that walks a reached front, and the fronts
-// of a bundle that holds one (items and bundles are kept whole).  The pruned lists take every entry of splan's forward
+// of a bundle that holds one (items and bundles are kept whole).  The pruned lists take every entry of the handle's forward
 // lists that belongs to a front of R, in list order.  F = the children of R outside R.  Before anything is launched, the
 // check that the pruned sweep cannot wait forever: every front of R owns work in the lists -- all of its top tasks, and
 // all chunks of each chunked block (the arrival counters count modulo the chunk count) -- and every child of a front of
@@ -1782,9 +1787,10 @@ static inline size_t align8(size_t b) { return (b + 7) & ~(size_t)7; }
 // caller and nothing launched, for a bad pattern or a failed check.
 static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_host, SfsCall& C) {
   SparseFwdPlan& P = *sv->sfs;
+  const SolvePlan& SP = sv->fronts.solve;
   const Symbolic& S = sv->S;
   const int n = sv->n;
-  const int nd = (int)P.direct.size();
+  const int nd = (int)SP.direct_cnt.size();
   const unsigned m = ++P.stamp;
   for (int i = 0; i < nbi; ++i) {
     const int v = bindex[i];
@@ -1813,8 +1819,8 @@ static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_h
       const int t = P.task_idx[e];
       if (P.m_task[t] == m) continue;
       P.m_task[t] = m; tasks.push_back(t);
-      const SolveTask& T = P.tf[t];
-      if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) add(P.bundle[T.s + w]);
+      const SolveTask& T = SP.tf[t];
+      if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) add(SP.bundle[T.s + w]);
     }
   }
   std::sort(items.begin(), items.end());
@@ -1849,14 +1855,14 @@ static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_h
   for (int i = 0; i < nbi; ++i) P.pos_bi[P.iperm[bindex[i]]] = -1;
   // pruned order: direct level l -> slot l, subtree item i -> nd + i, top task j -> nd + items + j
   for (int s : run) { P.ord0[s] = INT_MAX; P.ord1[s] = -1; }
-  for (int l = 0; l < nd; ++l) for (int i : dl[l]) { const int s = P.direct[l][i]; P.ord0[s] = P.ord1[s] = l; }
+  for (int l = 0; l < nd; ++l) for (int i : dl[l]) { const int s = SP.direct[l][i]; P.ord0[s] = P.ord1[s] = l; }
   for (size_t i = 0; i < items.size(); ++i)
     for (int e = P.item_ptr[items[i]]; e < P.item_ptr[items[i] + 1]; ++e) P.ord0[P.item_fr[e]] = P.ord1[P.item_fr[e]] = nd + (int)i;
   for (size_t j = 0; j < tasks.size(); ++j) {
-    const SolveTask& T = P.tf[tasks[j]];
+    const SolveTask& T = SP.tf[tasks[j]];
     const int o = nd + (int)(items.size() + j);
     auto upd = [&](int s) { P.ord0[s] = std::min(P.ord0[s], o); P.ord1[s] = std::max(P.ord1[s], o); };
-    if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) upd(P.bundle[T.s + w]);
+    if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) upd(SP.bundle[T.s + w]);
     else upd(T.s);
   }
   std::vector<int> fr;
@@ -1866,12 +1872,12 @@ static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_h
     // of its FP and FC blocks
     int nfp = 0, nfc = 0;
     for (int e = P.task_ptr[s]; ok && e < P.task_ptr[s + 1]; ++e) {
-      const SolveTask& T = P.tf[P.task_idx[e]];
+      const SolveTask& T = SP.tf[P.task_idx[e]];
       ok = P.m_task[P.task_idx[e]] == m;
       if (ok && (T.type == ST_FP || T.type == ST_FC) && T.q == 0) {
         ok = e + T.nq <= P.task_ptr[s + 1];
         for (int q = 1; ok && q < T.nq; ++q) {
-          const SolveTask& U = P.tf[P.task_idx[e + q]];
+          const SolveTask& U = SP.tf[P.task_idx[e + q]];
           ok = U.type == T.type && U.blk == T.blk && U.cidx == T.cidx && U.q == q && P.m_task[P.task_idx[e + q]] == m;
         }
         (T.type == ST_FP ? nfp : nfc) += 1;
@@ -1896,15 +1902,15 @@ static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_h
   C.o_x = align8(C.staged);
   if (C.o_x + 8 * (size_t)n > P.d_buf.n) { sv->err = "sparse_fwd_solve: staging too small"; return B200LDLT_FATAL_ERROR; }
   int2* hp = reinterpret_cast<int2*>(h);
-  for (size_t i = 0; i < items.size(); ++i) hp[i] = P.pairs[items[i]];
+  for (size_t i = 0; i < items.size(); ++i) hp[i] = SP.pairs[items[i]];
   SolveTask* ht = reinterpret_cast<SolveTask*>(h + o_tf);
-  for (size_t j = 0; j < tasks.size(); ++j) ht[j] = P.tf[tasks[j]];
+  for (size_t j = 0; j < tasks.size(); ++j) ht[j] = SP.tf[tasks[j]];
   if (b_host) memcpy(h + o_b, b_host, 8 * (size_t)nbi);
   int* hd = reinterpret_cast<int*>(h + o_dir);
   C.pl.direct_off.assign(nd, 0); C.pl.direct_cnt.assign(nd, 0);
   for (int l = 0, j = 0; l < nd; ++l) {
     C.pl.direct_off[l] = j; C.pl.direct_cnt[l] = (int)dl[l].size();
-    for (int i : dl[l]) hd[j++] = P.direct[l][i];
+    for (int i : dl[l]) hd[j++] = SP.direct[l][i];
   }
   std::copy(fr.begin(), fr.end(), reinterpret_cast<int*>(h + C.o_fr));
   char* d = P.d_buf.p;
@@ -1930,7 +1936,7 @@ static int sfs_enqueue(Solver* sv, const SfsCall& C, const double* d_b, double* 
                                                       W.d_x.p, reinterpret_cast<const int*>(d + C.o_fr), sv->d_rows_ptr.p,
                                                       W.d_cbv.p, W.d_done_f.p, sv->solve_epoch);
   ++sv->launches;
-  const int rc = launch_sweep(sv, sv->splan, W, 1, true, false, &C.pl);
+  const int rc = launch_sweep(sv, sv->fronts.solve, W, 1, true, false, &C.pl);
   if (rc != B200LDLT_SUCCESS) return rc;
   k_sfs_out<<<cdiv(C.nxi, 256), 256, 0, st>>>(C.nxi, reinterpret_cast<const int*>(d + C.o_xi), sv->d_piv_big.p, W.d_x.p,
                                              W.d_bigv.p, d_out);
@@ -1958,13 +1964,8 @@ static int shard_setup(Solver* sv, int rank, int world) {
     }
   }
   for (int ph = 0; ph < 2; ++ph) {
-    std::vector<int> fl;
-    build_level_plans(S, sv->opt.smem_front_max, take[ph], fl, H.plan[ph], H.schur[ph], sv->tc_min_r, !sv->dbg.no_warp2);
-    { int rc2 = upload_schur_lists(sv, H.schur[ph], st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
-    { int rc2 = build_linv_plan(sv, S, take[ph], H.linv_plan[ph], st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
-    { int rc2 = build_solve_plan(sv, S, take[ph], H.splan[ph], st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
-    if (fl.empty()) fl.push_back(0);
-    CU(H.d_fl[ph].upload(fl, st));
+    const int rc = build_front_plan(sv, take[ph], take[ph], H.part[ph]);
+    if (rc != B200LDLT_SUCCESS) return rc;
   }
   if (mark_cut.empty()) mark_cut.push_back(0), H.d_mark_cut.n = 0;
   {
@@ -2282,32 +2283,26 @@ static int fredholm(Solver* sv, int nrhs, double tol, double* x, int* consistent
 // of block_solve_state), each column with the arithmetic of a single-column call.  d_out may be d_b.
 static int enqueue_sc_columns(Solver* sv, int nrhs, const double* d_b, const double* d_xs, double* d_out, bool blocked) {
   cudaStream_t st = sv->stream;
+  const SolvePlan& SP = sv->fronts.solve;
   const int n = sv->n, m = (int)sv->sc_vars.size();
-  const int cap = blocked ? sv->blk->width : 1;
-  for (int c = 0; c < nrhs;) {
-    const int w = std::min(cap, nrhs - c);
+  const int rc = for_blocks(nrhs, blocked ? sv->blk->width : 1, [&](int c, int w) -> int {
     SweepState& W = w == 1 ? sv->sweep : *sv->blk;
     const long long ldx = W.M.x, ldb = W.M.bigv;
-    const dim3 g(cdiv(n, 256), w);
-    k_rhs_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_b + (size_t)c * n, W.d_x.p, ldx); ++sv->launches;
-    sv->solve_epoch++;
-    int rc = launch_sweep(sv, sv->splan, W, w, true, false);
-    if (rc != B200LDLT_SUCCESS) return rc;
+    const int rc2 = forward(sv, SP, W, d_b + (size_t)c * n, w, false);
+    if (rc2 != B200LDLT_SUCCESS) return rc2;
     if (!d_xs) {
       k_sc_reduce<<<dim3(cdiv(m, 256), w), 256, 0, st>>>(m, n - m, sv->d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb,
                                                          sv->d_sc_vars.p, sv->d_scale.p, d_out + (size_t)c * m);
       ++sv->launches;
-    } else {
-      k_sc_expand<<<g, 256, 0, st>>>(n, m, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, sv->d_piv_big.p, W.d_x.p, ldx,
-                                     W.d_bigv.p, ldb, sv->d_sc_vars.p, sv->d_scale.p, d_xs + (size_t)c * m);
-      ++sv->launches;
-      sv->solve_epoch++;
-      rc = launch_sweep(sv, sv->splan, W, w, false);
-      if (rc != B200LDLT_SUCCESS) return rc;
-      k_sol_out<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, d_out + (size_t)c * n); ++sv->launches;
+      return B200LDLT_SUCCESS;
     }
-    c += w;
-  }
+    k_sc_expand<<<dim3(cdiv(n, 256), w), 256, 0, st>>>(n, m, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, sv->d_piv_big.p,
+                                                      W.d_x.p, ldx, W.d_bigv.p, ldb, sv->d_sc_vars.p, sv->d_scale.p,
+                                                      d_xs + (size_t)c * m);
+    ++sv->launches;
+    return backward(sv, SP, W, d_out + (size_t)c * n, w);
+  });
+  if (rc != B200LDLT_SUCCESS) return rc;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
 }
@@ -2351,8 +2346,6 @@ static int selinv_state(Solver* sv) {
   const int n = S.n, nsn = S.nsn;
   cudaStream_t st = sv->stream;
   std::unique_ptr<SelInvPlan> P(new SelInvPlan());
-  std::vector<long long> linv_off(nsn);
-  CU(cudaMemcpy(linv_off.data(), sv->d_linv_off.p, nsn * sizeof(long long), cudaMemcpyDeviceToHost));
   std::vector<long long> eoff(nsn, -1);
   long long etot = 0;
   for (int s = 0; s < nsn; ++s)
@@ -2390,7 +2383,7 @@ static int selinv_state(Solver* sv) {
         if (S.f(s) <= SI_SMALL) continue;
         const bool big = S.f(s) > SI_MID;
         const int ld_e = big ? (k + DF_BLK - 1) / DF_BLK * DF_BLK : k;
-        const double* E = big ? sv->d_linv.p + linv_off[s] : P->d_E.p + eoff[s];
+        const double* E = big ? sv->d_linv.p + sv->linv_off[s] : P->d_E.p + eoff[s];
         const int nkb = (k + 63) / 64, nrb = (r + 63) / 64;
         if (pass < 2) {
           for (int ib = 0; ib < nrb; ++ib)
@@ -2723,7 +2716,7 @@ int b200ldlt_shard_factor(b200ldlt_handle h, int phase, int from_host) {
     if (from_host) CU(cudaMemcpyAsync(sv->d_vals.p, sv->h_vals, sv->nnz * sizeof(double), cudaMemcpyHostToDevice, st));
     sv->have_dev_vals = true;
   }
-  return enqueue_factor(sv, &sv->shard.plan[phase], sv->shard.d_fl[phase].p, phase == 0, &sv->shard.linv_plan[phase], &sv->shard.schur[phase]);
+  return enqueue_factor(sv, sv->shard.part[phase], phase == 0);
 }
 
 /* counters_total: CNT_N ints already summed over the ranks (all-reduce of device_ptr("counters")) */
@@ -2757,18 +2750,17 @@ int b200ldlt_shard_solve(b200ldlt_handle h, int phase, double* d_rhs) {
   Solver::Shard& H = sv->shard;
   const int n = sv->n;
   int rc = B200LDLT_SUCCESS;
+  // (phases 1 and 2 run under phase 0's epoch: k_mark_flags stamps the cut roots and the top fronts with it)
   if (phase == 0) {
     sv->launches = 0;
-    k_rhs_in<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_rhs, sv->sweep.d_x.p, n);
-    sv->solve_epoch++;
-    rc = launch_sweep(sv, H.splan[0], sv->sweep, 1, true);
+    rc = forward(sv, H.part[0].solve, sv->sweep, d_rhs, 1);
   } else if (phase == 1) {
     if (H.d_mark_cut.n) k_mark_flags<<<cdiv((long long)H.d_mark_cut.n, 256), 256, 0, st>>>(sv->sweep.d_done_f.p, H.d_mark_cut.p, (int)H.d_mark_cut.n, sv->solve_epoch);
-    rc = launch_sweep(sv, H.splan[1], sv->sweep, 1, true);
-    if (rc == B200LDLT_SUCCESS) rc = launch_sweep(sv, H.splan[1], sv->sweep, 1, false);
+    rc = launch_sweep(sv, H.part[1].solve, sv->sweep, 1, true);
+    if (rc == B200LDLT_SUCCESS) rc = launch_sweep(sv, H.part[1].solve, sv->sweep, 1, false);
   } else if (phase == 2) {
     if (H.rank != 0 && H.d_mark_top.n) k_mark_flags<<<cdiv((long long)H.d_mark_top.n, 256), 256, 0, st>>>(sv->sweep.d_done_b.p, H.d_mark_top.p, (int)H.d_mark_top.n, sv->solve_epoch);
-    rc = launch_sweep(sv, H.splan[0], sv->sweep, 1, false);
+    rc = launch_sweep(sv, H.part[0].solve, sv->sweep, 1, false);
   } else if (phase == 3) {
     k_sol_out<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, sv->sweep.d_x.p, n, d_rhs);
   } else return B200LDLT_FATAL_ERROR;
@@ -2843,7 +2835,7 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
   cudaStream_t st = sv->stream;
   CU(cudaMemcpyAsync(sv->d_ref_b.p, d_rhs, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
   sv->launches = 0;
-  int rc = enqueue_solve(sv, sv->sweep, d_rhs, d_rhs, 1);
+  int rc = enqueue_solve(sv, sv->sweep, 0, d_rhs, d_rhs, 1);
   if (rc != B200LDLT_SUCCESS) return rc;
   b200vec vb{sv->d_ref_b.p, n, 0, 0.0}, vx{d_rhs, n, 0, 0.0}, vr{sv->d_ref_r.p, n, 0, 0.0};
   double nb = 0.0, ratio = 0.0;
@@ -2857,7 +2849,7 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
     if (b200vec_amax(sv->vec, &vr, &nr) || b200vec_amax(sv->vec, &vx, &nx)) { sv->err = b200vec_last_error(sv->vec); return B200LDLT_FATAL_ERROR; }
     ratio = (nb + nx == 0.0) ? nr : nr / (std::min(nx, 1e6 * nb) + nb);
     if (step >= max_steps || (step >= min_steps && ratio <= tol)) break;
-    rc = enqueue_solve(sv, sv->sweep, sv->d_ref_r.p, sv->d_ref_r.p, 1);     // d = A^-1 r
+    rc = enqueue_solve(sv, sv->sweep, 0, sv->d_ref_r.p, sv->d_ref_r.p, 1);     // d = A^-1 r
     if (rc != B200LDLT_SUCCESS) return rc;
     if (b200vec_axpy(sv->vec, 1.0, &vr, &vx)) { sv->err = b200vec_last_error(sv->vec); return B200LDLT_FATAL_ERROR; }
     ++step;
