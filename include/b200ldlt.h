@@ -274,6 +274,61 @@ int b200ldlt_schur_reduce_device(b200ldlt_handle h, int nrhs, const double* d_b,
 int b200ldlt_schur_expand(b200ldlt_handle h, int nrhs, const double* b, const double* xs, double* x);
 int b200ldlt_schur_expand_device(b200ldlt_handle h, int nrhs, const double* d_b, const double* d_xs, double* d_x);
 
+/* ---- error analysis and condition estimation (cf. MUMPS ICNTL(11) / RINFOG(4..11), LAPACK xSYCON) --------------------
+ * How far to trust a solution x of A x = b, per column, with componentwise measures (the rows of a KKT system differ in
+ * scale by orders of magnitude, so a normwise residual says little about the rows that matter).
+ *   A   the matrix of the last factor call: its values (device_ptr "vals", unscaled) with duplicate triplets summed in
+ *       triplet order, as the factorisation sums them, BEFORE absolute values are taken;
+ *   M   the operator job 0 applies (as for selected inversion): A^-1, the inverse of the perturbed matrix with
+ *       info.num_forced > 0, the matrix with the altered D after alter_d.
+ * For each column, with r = b - A x, s = |A| |x|, a_i = max_j |a_ij|, eps = 2^-52 and
+ * tau_i = 1000 n eps (a_i ||x||_inf + |b_i|):
+ *   I2 = { i : s_i + |b_i| <= tau_i },  I1 the other rows;
+ *   omega1 = max_{i in I1} |r_i| / (s_i + |b_i|),   omega2 = max_{i in I2} |r_i| / (s_i + a_i ||x||_inf)
+ *            (a term with r_i = 0 counts as 0; a zero denominator occurs only then), 0 for an empty set;
+ *   w1 = s + |b| on I1, 0 elsewhere;  w2 = s + a ||x||_inf on I2, 0 elsewhere;
+ *   cond_k = est || M diag(w_k) ||_inf / ||x||_inf = est || diag(w_k) M ||_1 / ||x||_inf (M is symmetric), estimated through
+ *            the products B v = w_k o (M v) and B^T v = M (w_k o v); an empty set gives cond_k = 0 and runs no estimator;
+ *   ferr   = omega1 cond1 + omega2 cond2, an estimated bound on ||x - x*||_inf / ||x||_inf (first order);
+ *   ||x||_inf = 0 runs no estimator: cond1 = cond2 = ferr = 0 if b = 0, +inf otherwise.
+ * The estimator is Higham's 1-norm estimator exactly as LAPACK dlacn2 runs it: start from x = e/n; sign(y) = +1 for
+ * y >= 0 (-0 included); j = the first index of max |z|; stop on a repeated sign vector, on est <= est_old, when
+ * z_jlast = |z_j| or after 5 iterations; finish with x_i = (-1)^i (1 + i/(n-1)) (i = 0..n-1) and the test 2 ||y||_1 / (3n)
+ * > est.  At most 11 products per estimator.
+ * cond = 0 (cheap, as MUMPS ICNTL(11) = 2): the norms, omega1, omega2 and n_i2 only; no solve runs, cond1 = cond2 = ferr
+ * = -1 ("not computed").  Kept singular factors (zero pivots, keep mode): omega1 and omega2 as usual, cond1 = cond2 =
+ * ferr = +inf, no estimator runs.
+ * Every column's struct is bit-identical to a call on that column alone, under any B200_SOLVE_BLOCK, between the two entry
+ * points and across calls: maxima are exact (atomicMax on bit patterns), |I2| an integer count and every sum (r, s, the
+ * row sums of |A|, ||y||_1) has a fixed order.  The call leaves the factors, D, the solves and their bits as they were.
+ * Kernel launches, with L0 = job 0's launches per block (4 + 2 D, 8 by default): cond = 0: 3 (the unique values, the row
+ * pass, the row classes); cond = 1: 3 + (2 + L0) T, where T is the number of estimator steps: each step is one input
+ * kernel, one job-0 solve of the block's unfinished estimators and one reduction kernel.  The two estimators of a column
+ * take two columns of the blocked solve state, so blocks of up to B200_SOLVE_BLOCK / 2 columns (4 by default) step in
+ * lockstep and T = the sum over the blocks of the largest product count of an estimator in the block; with
+ * B200_SOLVE_BLOCK = 1 (or without the blocked state) every estimator runs alone and T = the sum of nprod.
+ * The first call after an analysis builds |A| by rows (about 4 (n + 1 + 2 m) bytes, m the entries of both triangles,
+ * 2 nnz_unique - the diagonal ones) and its buffers: 8 (nnz_unique + n) bytes, 16 n bytes per right-hand side (grown to
+ * the largest call) and, with cond = 1, 9 n bytes per column of the solve state it uses.  b and x are n x nrhs,
+ * column-major, and are not modified; out is nrhs structs in host memory for both entry points.  Refused (nothing
+ * written to out): nrhs < 0, cond other than 0 or 1, a NULL pointer with nrhs > 0.  nrhs = 0 is the no-columns case. */
+typedef struct b200ldlt_errors {
+  double anorm;          /* ||A||_inf = max_i sum_j |a_ij|   (= ||A||_1, A symmetric)                                  */
+  double xnorm, rnorm;   /* ||x||_inf, ||r||_inf with r = b - A x                                                   */
+  double omega1, omega2; /* componentwise backward errors on I1 and I2 (Arioli, Demmel, Duff)                       */
+  double cond1, cond2;   /* estimated condition numbers for the two row sets                                        */
+  double ferr;           /* omega1 cond1 + omega2 cond2: estimated bound on ||x - x*||_inf / ||x||_inf               */
+  int n_i2;              /* |I2|                                                                                    */
+  int nprod;             /* products with M the column's estimators took (0 when cond == 0)                         */
+} b200ldlt_errors;
+int b200ldlt_error_analysis(b200ldlt_handle h, int nrhs, const double* b, const double* x, int cond, b200ldlt_errors* out);
+int b200ldlt_error_analysis_device(b200ldlt_handle h, int nrhs, const double* d_b, const double* d_x, int cond,
+                                   b200ldlt_errors* out);
+/* kappa1 = ||A||_1 est ||M||_1 (1 / LAPACK's rcond): one estimator with w = 1 through the single-column solve state.
+ * anorm1 (||A||_1), ainv1 (est ||M||_1) and nprod (products taken, <= 11) may be NULL.  Kept singular factors: kappa1 =
+ * ainv1 = +inf, no estimator runs.  Kernel launches: 2 + (2 + L0) nprod.  Refused: a NULL kappa1. */
+int b200ldlt_condest(b200ldlt_handle h, double* kappa1, double* anorm1, double* ainv1, int* nprod);
+
 /* <-> NumberOfNegEVals() (hpp:207) */
 int b200ldlt_num_neg(b200ldlt_handle h);
 /* <-> IncreaseQuality() (hpp:220): pivtol <- min(pivtolmax, pivtol^0.75); returns 0 if already at max.

@@ -50,6 +50,13 @@ class Info(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class Errors(C.Structure):
+    """b200ldlt_errors: the error analysis of one column (see include/b200ldlt.h for the definitions)"""
+    _fields_ = [("anorm", C.c_double), ("xnorm", C.c_double), ("rnorm", C.c_double), ("omega1", C.c_double),
+                ("omega2", C.c_double), ("cond1", C.c_double), ("cond2", C.c_double), ("ferr", C.c_double),
+                ("n_i2", C.c_int), ("nprod", C.c_int)]
+
+
 EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "b200ldlt_last_error",
             "b200ldlt_analyse", "b200ldlt_values_ptr", "b200ldlt_factor", "b200ldlt_factor_device",
             "b200ldlt_solve", "b200ldlt_solve_device", "b200ldlt_num_neg", "b200ldlt_increase_quality",
@@ -62,7 +69,8 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_enquire_zero_pivots", "b200ldlt_solve_fredholm", "b200ldlt_solve_fredholm_device",
             "b200ldlt_selected_inverse", "b200ldlt_selected_inverse_device", "b200ldlt_set_schur",
             "b200ldlt_schur_complement", "b200ldlt_schur_complement_device", "b200ldlt_schur_reduce",
-            "b200ldlt_schur_reduce_device", "b200ldlt_schur_expand", "b200ldlt_schur_expand_device"]
+            "b200ldlt_schur_reduce_device", "b200ldlt_schur_expand", "b200ldlt_schur_expand_device",
+            "b200ldlt_error_analysis", "b200ldlt_error_analysis_device", "b200ldlt_condest"]
 
 _lib = None
 
@@ -118,6 +126,9 @@ def load_library():
     L.b200ldlt_schur_reduce_device.argtypes = [vp, C.c_int, vp, vp]
     L.b200ldlt_schur_expand.argtypes = [vp, C.c_int, dp, dp, dp]
     L.b200ldlt_schur_expand_device.argtypes = [vp, C.c_int, vp, vp, vp]
+    L.b200ldlt_error_analysis.argtypes = [vp, C.c_int, dp, dp, C.c_int, C.POINTER(Errors)]
+    L.b200ldlt_error_analysis_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.POINTER(Errors)]
+    L.b200ldlt_condest.argtypes = [vp, dp, dp, dp, ip]
     L.b200ldlt_num_neg.argtypes = [vp]
     L.b200ldlt_increase_quality.argtypes = [vp]
     L.b200ldlt_get_info.argtypes = [vp, C.POINTER(Info)]
@@ -439,6 +450,42 @@ class B200Ldlt:
     def schur_expand_device(self, d_b_ptr, d_xs_ptr, d_x_ptr, nrhs=1):
         return self._L.b200ldlt_schur_expand_device(self._h, int(nrhs), C.c_void_p(d_b_ptr), C.c_void_p(d_xs_ptr),
                                                     C.c_void_p(d_x_ptr))
+
+    @staticmethod
+    def _errors_dict(out, one):
+        d = {k: np.array([getattr(o, k) for o in out], dtype=np.int32 if t is C.c_int else np.float64)
+             for k, t in Errors._fields_}
+        return {k: v[0] for k, v in d.items()} if one else d
+
+    def error_analysis(self, B, X, cond=True):
+        """Componentwise error analysis of the solutions X of A X = B (dim or dim x nrhs; b200ldlt_error_analysis): a dict
+        of per-column arrays (scalars for 1-D input) -- anorm, xnorm, rnorm, omega1, omega2, cond1, cond2, ferr, n_i2,
+        nprod.  cond=False: the norms and backward errors only (cond1 = cond2 = ferr = -1).  Raises on a refusal."""
+        B = np.asarray(B, dtype=np.float64)
+        one = B.ndim == 1
+        Bm = np.asfortranarray(B.reshape(self.dim, -1, order="F"))
+        Xm = np.asfortranarray(np.asarray(X, dtype=np.float64).reshape(self.dim, -1, order="F"))
+        assert Xm.shape == Bm.shape
+        nrhs = Bm.shape[1]
+        out = (Errors * max(nrhs, 1))()
+        if self._L.b200ldlt_error_analysis(self._h, nrhs, _dptr(Bm), _dptr(Xm), int(bool(cond)), out) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return self._errors_dict(out[:nrhs], one)
+
+    def error_analysis_device(self, d_b_ptr, d_x_ptr, nrhs=1, cond=True):
+        """The same on device arrays of dim x nrhs doubles.  Returns (status, dict of per-column arrays)."""
+        out = (Errors * max(int(nrhs), 1))()
+        st = self._L.b200ldlt_error_analysis_device(self._h, int(nrhs), C.c_void_p(d_b_ptr), C.c_void_p(d_x_ptr),
+                                                    int(cond), out)
+        return st, self._errors_dict(out[:int(nrhs)], False)
+
+    def condest(self):
+        """(kappa1, anorm1, ainv1, nprod): the 1-norm condition estimate ||A||_1 est||M||_1 (b200ldlt_condest).  Raises
+        on a refusal."""
+        k, a, m, p = C.c_double(), C.c_double(), C.c_double(), C.c_int()
+        if self._L.b200ldlt_condest(self._h, C.byref(k), C.byref(a), C.byref(m), C.byref(p)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return k.value, a.value, m.value, p.value
 
     def device_ptr(self, name):
         """Device address of a named array of the handle (b200ldlt_device_ptr: "scale", "x", "cbv", ...), 0 if none."""

@@ -22,6 +22,7 @@
 #include "schur_tc.cu"
 #include "selinv_kernels.cu"
 #include "sc_kernels.cu"
+#include "ea_kernels.cu"
 #include "symbolic.hpp"
 
 namespace b200 {
@@ -150,6 +151,23 @@ struct SelInvPlan {
   DevBuf<SiGather> d_gather;
 };
 
+// error analysis and condition estimation (b200ldlt_error_analysis / b200ldlt_condest, ea_kernels.cu): |A| by rows
+// (d_ptr / d_col / d_uid: both triangles of the unique entries, grouped by original row, columns ascending), the unique
+// values of the call (k_sum_dups of d_vals: d_uval is scaled in place by the factorisation) and the row maxima a_i; per
+// right-hand side r and s, overwritten by w1 and w2, and the reduced norms (grown to the largest call); the estimators'
+// input / product vectors and sign vectors (one column per estimator of a block) and the reduction scratch of
+// k_ea_post.  Built at the first call after an analysis, before its timing starts; a handle that never makes the calls
+// allocates none of it.
+struct EaPlan {
+  DevBuf<int> d_ptr, d_col, d_uid;
+  DevBuf<double> d_uval, d_amax, d_rs, d_v;
+  DevBuf<unsigned long long> d_nrm;
+  DevBuf<signed char> d_xi;
+  DevBuf<EaPart> d_part;
+  DevBuf<EaRes> d_res;
+  DevBuf<unsigned> d_cnt;
+};
+
 struct LevelPlan {
   // big fronts of the level: [big_off, big_off+big_cnt) in front_list
   int big_off = 0, big_cnt = 0, big_kmax = 0, big_fmax = 0, big_rmax = 0, big_chmax = 0;
@@ -263,6 +281,7 @@ struct Solver {
   std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call after an analysis
   std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve: built at its first call after an analysis
   std::unique_ptr<SelInvPlan> selinv;   // selected inversion: built at its first call after an analysis
+  std::unique_ptr<EaPlan> ea;       // error analysis / condest: built at the first such call after an analysis
   DevBuf<double> d_alter;           // alter_d: the caller's 2n entries of D^-1 (allocated at the first call)
   DevBuf<int> d_alter_bad;
   // zero pivots (b200ldlt_set_singular_action): the factor kernels append every forced zero pivot to d_zlist; with
@@ -851,6 +870,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   sv->lmul.reset();
   sv->sfs.reset();
   sv->selinv.reset();
+  sv->ea.reset();
   if (sv->fgraph_exec) { cudaGraphExecDestroy(sv->fgraph_exec); sv->fgraph_exec = nullptr; }
   if (sv->fgraph) { cudaGraphDestroy(sv->fgraph); sv->fgraph = nullptr; }
   AnalyseOptions ao;
@@ -2463,6 +2483,254 @@ static int selected_inverse(Solver* sv, double* diag, double* vals, bool host) {
     return B200LDLT_SUCCESS;
   });
 }
+
+// ---- error analysis and condition estimation (b200ldlt_error_analysis, b200ldlt_condest) -------------------------------
+// The call's state (EaPlan): |A| by rows from S.u_row / S.u_col at the first call after an analysis -- both triangles of
+// the unique entries by a counting sort on the column, then a stable one on the row, so each row's columns ascend --
+// and the buffers for nrhs right-hand sides and estimator blocks of `width` columns (0: no estimator), grown as needed.
+static int ea_state(Solver* sv, int nrhs, int width) {
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  if (!sv->ea) {
+    const Symbolic& S = sv->S;
+    std::unique_ptr<EaPlan> P(new EaPlan());
+    std::vector<int> er, ec, eu;
+    er.reserve(2 * S.nnz_u); ec.reserve(2 * S.nnz_u); eu.reserve(2 * S.nnz_u);
+    for (int64_t u = 0; u < S.nnz_u; ++u) {
+      er.push_back(S.u_row[u]); ec.push_back(S.u_col[u]); eu.push_back((int)u);
+      if (S.u_row[u] != S.u_col[u]) { er.push_back(S.u_col[u]); ec.push_back(S.u_row[u]); eu.push_back((int)u); }
+    }
+    const size_t m = er.size();
+    std::vector<int> cptr(n + 1, 0), rptr(n + 1, 0);
+    for (size_t e = 0; e < m; ++e) { cptr[ec[e] + 1]++; rptr[er[e] + 1]++; }
+    for (int i = 0; i < n; ++i) { cptr[i + 1] += cptr[i]; rptr[i + 1] += rptr[i]; }
+    std::vector<int> byc(m), col(m), uid(m);
+    std::vector<int> pos(cptr.begin(), cptr.end() - 1);
+    for (size_t e = 0; e < m; ++e) byc[pos[ec[e]]++] = (int)e;
+    pos.assign(rptr.begin(), rptr.end() - 1);
+    for (const int e : byc) { const int k = pos[er[e]]++; col[k] = ec[e]; uid[k] = eu[e]; }
+    CU(P->d_ptr.upload(rptr, st));
+    CU(P->d_col.upload(col, st));
+    CU(P->d_uid.upload(uid, st));
+    CU(P->d_uval.alloc(std::max<int64_t>(S.nnz_u, 1)));
+    CU(P->d_amax.alloc(n));
+    CU(P->d_res.alloc(MS_NB_MAX));
+    CU(P->d_part.alloc((size_t)MS_NB_MAX * ea_parts(n)));
+    CU(P->d_cnt.alloc(MS_NB_MAX));
+    CU(cudaMemsetAsync(P->d_cnt.p, 0, MS_NB_MAX * sizeof(unsigned), st));
+    CU(cudaStreamSynchronize(st));
+    sv->ea = std::move(P);
+  }
+  EaPlan& P = *sv->ea;
+  if (P.d_nrm.n < (size_t)EA_NRM * nrhs + 1) CU(P.d_nrm.alloc((size_t)EA_NRM * nrhs + 1));
+  if (P.d_rs.n < (size_t)2 * n * nrhs) CU(P.d_rs.alloc((size_t)2 * n * nrhs));
+  if (P.d_v.n < (size_t)n * width) { CU(P.d_v.alloc((size_t)n * width)); CU(P.d_xi.alloc((size_t)n * width)); }
+  return B200LDLT_SUCCESS;
+}
+
+// One run of Higham's 1-norm estimator, exactly as LAPACK dlacn2 runs it, for ||B||_1 with B v = w o (M v) and
+// B^T v = M (w o v) (w == nullptr: B = M).  jump is dlacn2's ISAVE(1) for the product in flight (0: finished).
+struct EaEst {
+  int xi = 0;                     // its column of the sign vectors
+  const double* w = nullptr;
+  int jump = 1, iter = 0, j = 0, nprod = 0;
+  double est = 0.0;
+};
+
+// dlacn2's decision after the product of T's step, from the reductions R of that product
+static void ea_decide(EaEst& T, const EaRes& R, int n) {
+  ++T.nprod;
+  const int jmax = R.jmax < n ? R.jmax : 0;   // (a product without a number in it: IDAMAX's 1)
+  switch (T.jump) {
+    case 1:                               // B x, x = e/n
+      T.est = R.l1;
+      T.jump = n == 1 ? 0 : 2;
+      break;
+    case 2:                               // B^T xi
+      T.j = jmax; T.iter = 2; T.jump = 3;
+      break;
+    case 3: {                             // B e_j: stop on a repeated sign vector or no increase
+      const double old = T.est;
+      T.est = R.l1;
+      T.jump = (R.changes == 0 || T.est <= old) ? 5 : 4;
+      break;
+    }
+    case 4:                               // B^T xi: continue while z[jlast] != max |z| and iter < 5
+      T.j = jmax;
+      if (R.zjl != R.zmax && T.iter < 5) { ++T.iter; T.jump = 3; } else T.jump = 5;
+      break;
+    default: {                            // B x, x the alternating vector
+      const double t = 2.0 * (R.l1 / (3.0 * (double)n));
+      if (t > T.est) T.est = t;
+      T.jump = 0;
+    }
+  }
+}
+
+// The estimators E[0..ne) in lockstep (ne <= W.width): per step, the inputs of the unfinished ones (k_ea_prep), ONE job-0
+// solve of that many columns through W, their reductions (k_ea_post), one D2H of them and dlacn2's decisions on the host.
+// Launches per step: 2 + job 0's.  Each column runs the arithmetic of a single-column solve, so an estimator's results do
+// not depend on the others of its block.
+static int run_estimators(Solver* sv, SweepState& W, EaEst* E, int ne) {
+  static const int kMode[6] = {0, 0, 2, 1, 2, 3};   // the input of each jump: e/n, xi, e_j, xi, alternating
+  EaPlan& P = *sv->ea;
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  for (;;) {
+    EaStep step;
+    EaEst* act[MS_NB_MAX];
+    int na = 0;
+    for (int e = 0; e < ne; ++e) {
+      EaEst& T = E[e];
+      if (!T.jump) continue;
+      const bool k2 = T.jump == 2 || T.jump == 4;
+      step.s[na] = EaSlot{k2 ? T.w : nullptr, k2 ? nullptr : T.w, T.xi, kMode[T.jump], T.j, T.j, k2 ? 2 : 1};
+      act[na++] = &T;
+    }
+    if (na == 0) return B200LDLT_SUCCESS;
+    k_ea_prep<<<dim3(cdiv(n, EA_THREADS), na), EA_THREADS, 0, st>>>(n, step, P.d_xi.p, P.d_v.p);
+    ++sv->launches;
+    { const int rc = enqueue_solve(sv, W, 0, P.d_v.p, P.d_v.p, na); if (rc != B200LDLT_SUCCESS) return rc; }
+    k_ea_post<<<dim3(ea_parts(n), na), EA_THREADS, 0, st>>>(n, step, P.d_v.p, P.d_xi.p, P.d_part.p, P.d_cnt.p, P.d_res.p);
+    ++sv->launches;
+    CU(cudaGetLastError());
+    EaRes R[MS_NB_MAX];
+    CU(cudaMemcpyAsync(R, P.d_res.p, na * sizeof(EaRes), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    for (int a = 0; a < na; ++a) ea_decide(*act[a], R[a], n);
+  }
+}
+
+// k_sum_dups into the call's unique values, then the row pass for nrhs columns of d_b / d_x (nrhs = 0: only ||A|| and
+// the row maxima) into P.d_nrm, which is cleared first
+static int enqueue_ea_rows(Solver* sv, int nrhs, const double* d_b, const double* d_x) {
+  EaPlan& P = *sv->ea;
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  const long long nu = sv->S.nnz_u;
+  CU(cudaMemsetAsync(P.d_nrm.p, 0, ((size_t)EA_NRM * nrhs + 1) * sizeof(unsigned long long), st));
+  k_sum_dups<<<cdiv(nu, 256), 256, 0, st>>>(nu, sv->d_useg_ptr.p, sv->d_useg_src.p, sv->d_vals.p, P.d_uval.p);
+  const unsigned g = std::min<unsigned>(cdiv(n, EA_WARPS), EA_ROW_CTAS);
+  k_ea_rows<<<dim3(g, std::max(nrhs, 1)), EA_THREADS, 0, st>>>(n, nrhs, P.d_ptr.p, P.d_col.p, P.d_uid.p, P.d_uval.p, d_b,
+                                                               d_x, P.d_rs.p, P.d_amax.p, P.d_nrm.p);
+  sv->launches += 2;
+  CU(cudaGetLastError());
+  return B200LDLT_SUCCESS;
+}
+
+static inline double ea_val(unsigned long long b) { double v; memcpy(&v, &b, sizeof(v)); return v; }
+
+// b200ldlt_error_analysis (host == true: b and x in host memory) / _device
+static int error_analysis(Solver* sv, int nrhs, const double* b, const double* x, int cond, b200ldlt_errors* out,
+                          bool host) {
+  const char* bad = nrhs < 0 ? "nrhs must be >= 0" : cond != 0 && cond != 1 ? "cond must be 0 or 1"
+                    : nrhs > 0 && (!b || !x || !out) ? "NULL argument" : nullptr;
+  if (bad) { sv->err = std::string("error_analysis: ") + bad; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "error_analysis"); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (nrhs == 0) return no_columns(sv);
+  const int n = sv->n;
+  const size_t nb = (size_t)n * nrhs;
+  // kept singular factors: M is no inverse of A, no estimator runs
+  const bool estimate = cond == 1 && sv->zpos.empty();
+  const bool blocked = estimate && block_solve_state(sv);
+  SweepState& W = blocked ? *sv->blk : sv->sweep;
+  { const int rc = ea_state(sv, nrhs, estimate ? W.width : 0); if (rc != B200LDLT_SUCCESS) return rc; }
+  EaPlan& P = *sv->ea;
+  cudaStream_t st = sv->stream;
+  std::vector<unsigned long long> nrm((size_t)EA_NRM * nrhs + 1);
+  auto at = [&](int c, int k) { return ea_val(nrm[(size_t)EA_NRM * c + k]); };
+  std::vector<double> est(2 * (size_t)nrhs, 0.0);
+  std::vector<int> nprod(nrhs, 0);
+  auto enqueue = [&](const double* d_b, const double* d_x) -> int {
+    { const int rc = enqueue_ea_rows(sv, nrhs, d_b, d_x); if (rc != B200LDLT_SUCCESS) return rc; }
+    k_ea_class<<<dim3(cdiv(n, EA_THREADS), nrhs), EA_THREADS, 0, st>>>(n, d_b, P.d_amax.p, P.d_rs.p, P.d_nrm.p);
+    ++sv->launches;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(nrm.data(), P.d_nrm.p, nrm.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    if (!estimate) return B200LDLT_SUCCESS;
+    CU(cudaStreamSynchronize(st));
+    // the estimators of cond1 (weights w1, on I1) and cond2 (w2, on I2) of each column with x != 0 and its set non-empty:
+    // blocked, those of up to width / 2 columns in lockstep, else one by one through the single-column state
+    return for_blocks(nrhs, blocked ? W.width / 2 : 1, [&](int c0, int w) -> int {
+      EaEst E[MS_NB_MAX];
+      int slot[MS_NB_MAX], ne = 0;
+      for (int c = c0; c < c0 + w; ++c) {
+        if (at(c, EA_X) == 0.0) continue;
+        const long long n2 = (long long)nrm[(size_t)EA_NRM * c + EA_NI2];
+        for (int k = 0; k < 2; ++k) {
+          if ((k == 0 ? n - n2 : n2) == 0) continue;
+          E[ne].xi = blocked ? ne : 0;
+          E[ne].w = P.d_rs.p + (size_t)(2 * c + k) * n;
+          slot[ne++] = 2 * c + k;
+        }
+      }
+      if (blocked) {
+        const int rc = run_estimators(sv, W, E, ne);
+        if (rc != B200LDLT_SUCCESS) return rc;
+      } else {
+        for (int e = 0; e < ne; ++e) { const int rc = run_estimators(sv, W, E + e, 1); if (rc != B200LDLT_SUCCESS) return rc; }
+      }
+      for (int e = 0; e < ne; ++e) { est[slot[e]] = E[e].est; nprod[slot[e] / 2] += E[e].nprod; }
+      return B200LDLT_SUCCESS;
+    });
+  };
+  int rc;
+  if (host) {
+    std::vector<double> in(2 * nb);
+    memcpy(in.data(), b, nb * sizeof(double));
+    memcpy(in.data() + nb, x, nb * sizeof(double));
+    rc = staged_call(sv, in.data(), 2 * nb, nullptr, 0, [&](double* d) { return enqueue(d, d + nb); });
+  } else {
+    rc = timed_call(sv, [&] { return enqueue(b, x); });
+  }
+  if (rc != B200LDLT_SUCCESS) return rc;
+  const double inf = INFINITY, anorm = ea_val(nrm[(size_t)EA_NRM * nrhs]);
+  for (int c = 0; c < nrhs; ++c) {
+    b200ldlt_errors& o = out[c];
+    o.anorm = anorm;
+    o.xnorm = at(c, EA_X);
+    o.rnorm = at(c, EA_R);
+    o.omega1 = at(c, EA_W1);
+    o.omega2 = at(c, EA_W2);
+    o.n_i2 = (int)nrm[(size_t)EA_NRM * c + EA_NI2];
+    o.nprod = nprod[c];
+    if (cond == 0) {
+      o.cond1 = o.cond2 = o.ferr = -1.0;
+    } else if (!sv->zpos.empty()) {
+      o.cond1 = o.cond2 = o.ferr = inf;
+    } else if (o.xnorm == 0.0) {
+      o.cond1 = o.cond2 = o.ferr = at(c, EA_B) == 0.0 ? 0.0 : inf;
+    } else {
+      o.cond1 = est[2 * (size_t)c] / o.xnorm;
+      o.cond2 = est[2 * (size_t)c + 1] / o.xnorm;
+      o.ferr = o.omega1 * o.cond1 + o.omega2 * o.cond2;
+    }
+  }
+  return B200LDLT_SUCCESS;
+}
+
+// b200ldlt_condest: ||A||_1 from the row pass, est ||M||_1 by one estimator through the single-column state
+static int condest(Solver* sv, double* kappa1, double* anorm1, double* ainv1, int* nprod) {
+  if (!kappa1) { sv->err = "condest: NULL kappa1"; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "condest"); if (rc != B200LDLT_SUCCESS) return rc; }
+  const bool estimate = sv->zpos.empty();
+  { const int rc = ea_state(sv, 0, estimate ? 1 : 0); if (rc != B200LDLT_SUCCESS) return rc; }
+  EaEst E;
+  unsigned long long an = 0;
+  const int rc = timed_call(sv, [&]() -> int {
+    { const int rc2 = enqueue_ea_rows(sv, 0, nullptr, nullptr); if (rc2 != B200LDLT_SUCCESS) return rc2; }
+    if (estimate) { const int rc2 = run_estimators(sv, sv->sweep, &E, 1); if (rc2 != B200LDLT_SUCCESS) return rc2; }
+    CU(cudaMemcpyAsync(&an, sv->ea->d_nrm.p, sizeof(an), cudaMemcpyDeviceToHost, sv->stream));
+    return B200LDLT_SUCCESS;
+  });
+  if (rc != B200LDLT_SUCCESS) return rc;
+  const double anorm = ea_val(an), ainv = estimate ? E.est : INFINITY;
+  *kappa1 = estimate ? anorm * ainv : INFINITY;
+  if (anorm1) *anorm1 = anorm;
+  if (ainv1) *ainv1 = ainv;
+  if (nprod) *nprod = E.nprod;
+  return B200LDLT_SUCCESS;
+}
 }  // namespace b200
 
 extern "C" {
@@ -2604,6 +2872,25 @@ int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* 
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
   return selected_inverse(sv, d_diag, d_vals, false);
+}
+
+int b200ldlt_error_analysis(b200ldlt_handle h, int nrhs, const double* b, const double* x, int cond, b200ldlt_errors* out) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return error_analysis(sv, nrhs, b, x, cond, out, true);
+}
+
+int b200ldlt_error_analysis_device(b200ldlt_handle h, int nrhs, const double* d_b, const double* d_x, int cond,
+                                   b200ldlt_errors* out) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return error_analysis(sv, nrhs, d_b, d_x, cond, out, false);
+}
+
+int b200ldlt_condest(b200ldlt_handle h, double* kappa1, double* anorm1, double* ainv1, int* nprod) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return condest(sv, kappa1, anorm1, ainv1, nprod);
 }
 
 int b200ldlt_set_schur(b200ldlt_handle h, int m, const int* vars) {
