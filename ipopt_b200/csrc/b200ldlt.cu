@@ -31,6 +31,9 @@ template <class T>
 struct DevBuf {
   T* p = nullptr;
   size_t n = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;              // one owner per allocation
+  DevBuf& operator=(const DevBuf&) = delete;
   ~DevBuf() { release(); }
   void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
   // n is the size only once the memory is there: a failed allocation leaves the buffer released (p null, n 0)
@@ -222,6 +225,79 @@ struct DebugSwitches {
   }
 };
 
+// Everything one analysis derives: the symbolic structure and its device copies, the factor and contribution-block
+// storage, the plans and sweep states, the per-call plans built at their first call, the shard plan, the captured
+// factorisation and the staging of the host entry points.  A new analysis replaces it whole and a failed one leaves
+// none, so nothing sized by an old analysis can outlive it.
+struct Analysis {
+  Symbolic S;
+  FrontPlan fronts;                  // factorisation: all fronts but the Schur root; solves: all fronts
+  bool factored = false;
+  DevBuf<int8_t> d_tc_dig;           // digit scratch of the tensor-core Schur path (largest level)
+  DevBuf<int> d_tc_exp;
+  DevBuf<int> d_sn_start, d_sn_parent, d_rows, d_rel, d_child_ptr, d_child_idx, d_perm;
+  DevBuf<int> d_useg_src, d_u_row, d_u_col, d_irn, d_jcn;
+  DevBuf<long long> d_rows_ptr, d_uent_ptr, d_u_dst64, d_L_off, d_cb_off, d_useg_ptr;
+  DevBuf<unsigned> d_u_dst;
+  DevBuf<double> d_uval, d_L, d_W, d_CB, d_dinv, d_doff, d_scale, d_res, d_colmax;
+  DevBuf<int> d_ptype, d_lperm, d_bperm, d_counters, d_einv;
+  DevBuf<long long> d_einv_off;
+  DevBuf<unsigned long long> d_rmax;
+  DevSym DS;
+  DevNum DN;
+  // solve (solve_dataflow.cu): per-front tables, sweep states + one plan per front set
+  SweepState sweep;                 // one column: every single-column solve (also the sharded one), device_ptr "x" / "cbv"
+  std::unique_ptr<SweepState> blk;  // blocked solve: B200_SOLVE_BLOCK columns, allocated at the first nrhs > 1 solve
+                                    // (width 0: the column loop)
+  DevBuf<int> d_boff;
+  DevBuf<long long> d_bigv_off;
+  DevBuf<long long> d_piv_big;      // n : per pivot position, its index in bigv (pivots of big fronts) or -1 (partial solves)
+  std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call
+  std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve: built at its first call
+  std::unique_ptr<SelInvPlan> selinv;   // selected inversion: built at its first call
+  std::unique_ptr<EaPlan> ea;       // error analysis / condest: built at the first such call
+  // zero pivots (b200ldlt_set_singular_action): the factor kernels append every forced zero pivot to d_zlist; with
+  // keep_singular a factorisation whose zero pivots are all noise pivots keeps its factors, with dinv = 0 at zpos
+  DevBuf<int> d_zlist, d_zpos;
+  DevBuf<unsigned char> d_zflag;    // n : 1 at the zero pivots of the kept factors
+  std::vector<int> zpos;            // the zero pivots of the kept factors, ascending (empty otherwise)
+  DevBuf<double> d_fred_z;          // solve_fredholm without a blocked state: z of one column, pivot order
+  // Schur mode: an analysis with the handle's Schur variables makes supernode sc_root (the last one) their root front,
+  // which the factorisation assembles but does not factor; d_sc then holds S_c (m x m, column-major)
+  int sc_root = -1, sc_nch = 0;
+  long long sc_nent = 0, sc_linv_off = 0;   // its unique entries; its L11^-1 block in d_linv (order > 256)
+  DevBuf<int> d_sc_vars, d_sc_root;
+  DevBuf<double> d_sc;
+  DevBuf<double> d_linv;
+  DevBuf<double> d_linv_part;       // partial tiles of the chunked k_linv_gemm items (one launch at a time uses it)
+  DevBuf<int> d_linv_cnt;           // their arrival counters (self-resetting)
+  DevBuf<long long> d_linv_off, d_gmap_off;
+  std::vector<long long> linv_off;  // per supernode: its L11^-1 block in d_linv (order > 256), else -1
+  DevBuf<FrontDesc> d_fdesc;
+  DevBuf<int> d_gmap;
+  std::vector<char> solve_direct_front;   // per supernode: solved by k_solve_direct (see build_solve_tables)
+  int solve_epoch = 0;
+  struct Shard {
+    bool active = false;
+    int rank = 0, world = 1, nsub = 0;
+    std::vector<int> owner, cut_roots, top_fronts;
+    FrontPlan part[2];                       // [0] my subtrees, [1] top part
+    DevBuf<int> d_mark_cut, d_mark_top;
+  } shard;
+  cudaGraph_t fgraph = nullptr;
+  cudaGraphExec_t fgraph_exec = nullptr;
+  double fgraph_u = -1.0;
+  int fgraph_launches = 0;
+  double* h_rhs = nullptr;          // pinned staging of the host entry points: d_rhs.n doubles, like d_rhs (staged_call)
+  DevBuf<double> d_rhs;
+
+  ~Analysis() {
+    if (fgraph_exec) cudaGraphExecDestroy(fgraph_exec);
+    if (fgraph) cudaGraphDestroy(fgraph);
+    if (h_rhs) cudaFreeHost(h_rhs);
+  }
+};
+
 struct Solver {
   b200ldlt_options opt;
   DebugSwitches dbg;
@@ -240,9 +316,9 @@ struct Solver {
   int n = 0, nnz = 0;
   std::vector<int> irn, jcn;
   double* h_vals = nullptr;      // pinned
-  double* h_rhs = nullptr;       // pinned staging of the host entry points: d_rhs.n doubles, like d_rhs (staged_call)
   int* h_counters = nullptr;     // pinned
-  bool analysed = false, factored = false, have_dev_vals = false;
+  DevBuf<double> d_vals;         // the values on the device (nnz): allocated at the first need, released with the pattern
+  bool have_dev_vals = false;
   b200vec_ctx vec = nullptr;       // vector kernels on the handle's stream (device-side refinement)
   b200vec_tmat amat = nullptr;     // the matrix as a symmetric triplet operator (residuals)
   DevBuf<double> d_ref_b, d_ref_r;
@@ -251,88 +327,29 @@ struct Solver {
   int n_reanalysed = 0;
   long long n_factor = 0;
   bool reanalysed_since_raise = false;
-  Symbolic S;
-  FrontPlan fronts;                  // factorisation: all fronts but the Schur root; solves: all fronts
-  DevBuf<int8_t> d_tc_dig;           // digit scratch of the tensor-core Schur path (largest level)
-  DevBuf<int> d_tc_exp;
+  std::unique_ptr<Analysis> an;    // null: not analysed (none yet, a new pattern, or the last analysis failed)
   b200ldlt_info info;
   int num_neg = 0;
   double pivtol = 1e-8;
-
-  // device
-  DevBuf<int> d_sn_start, d_sn_parent, d_rows, d_rel, d_child_ptr, d_child_idx, d_perm;
-  DevBuf<int> d_useg_src, d_u_row, d_u_col, d_irn, d_jcn;
-  DevBuf<long long> d_rows_ptr, d_uent_ptr, d_u_dst64, d_L_off, d_cb_off, d_useg_ptr;
-  DevBuf<unsigned> d_u_dst;
-  DevBuf<double> d_vals, d_uval, d_L, d_W, d_CB, d_dinv, d_doff, d_scale, d_rhs, d_res, d_colmax;
-  DevBuf<int> d_ptype, d_lperm, d_bperm, d_counters, d_einv;
-  DevBuf<long long> d_einv_off;
-  DevBuf<unsigned long long> d_rmax;
-  DevSym DS;
-  DevNum DN;
   int launches = 0;
-  // solve (solve_dataflow.cu): per-front tables, sweep states + one plan per front set
-  SweepState sweep;                 // one column: every single-column solve (also the sharded one), device_ptr "x" / "cbv"
-  std::unique_ptr<SweepState> blk;  // blocked solve: B200_SOLVE_BLOCK columns, allocated at the first nrhs > 1 solve after
-                                    // an analysis (width 0: the column loop)
-  DevBuf<int> d_boff;
-  DevBuf<long long> d_bigv_off;
-  DevBuf<long long> d_piv_big;      // n : per pivot position, its index in bigv (pivots of big fronts) or -1 (partial solves)
-  std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call after an analysis
-  std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve: built at its first call after an analysis
-  std::unique_ptr<SelInvPlan> selinv;   // selected inversion: built at its first call after an analysis
-  std::unique_ptr<EaPlan> ea;       // error analysis / condest: built at the first such call after an analysis
   DevBuf<double> d_alter;           // alter_d: the caller's 2n entries of D^-1 (allocated at the first call)
   DevBuf<int> d_alter_bad;
-  // zero pivots (b200ldlt_set_singular_action): the factor kernels append every forced zero pivot to d_zlist; with
-  // keep_singular a factorisation whose zero pivots are all noise pivots keeps its factors, with dinv = 0 at zpos
-  bool keep_singular = false;
-  DevBuf<int> d_zlist, d_zpos;
-  DevBuf<unsigned char> d_zflag;    // n : 1 at the zero pivots of the kept factors
-  std::vector<int> zpos;            // the zero pivots of the kept factors, ascending (empty otherwise)
+  bool keep_singular = false;       // b200ldlt_set_singular_action (see Analysis::zpos)
   DevBuf<unsigned long long> d_fred_nrm;   // solve_fredholm: the two max-norms per column
-  DevBuf<double> d_fred_z;          // solve_fredholm without a blocked state: z of one column, pivot order
   // Schur mode (b200ldlt_set_schur): the caller's Schur variables, given to every analysis until b200ldlt_analyse or
-  // set_schur(0) clears them.  An analysis with them makes supernode sc_root (the last one) their root front, which
-  // the factorisation assembles but does not factor; d_sc then holds S_c (m x m, column-major).
+  // set_schur(0) clears them
   std::vector<int> sc_vars;
-  int sc_root = -1, sc_nch = 0;
-  long long sc_nent = 0, sc_linv_off = 0;   // its unique entries; its L11^-1 block in d_linv (order > 256)
-  DevBuf<int> d_sc_vars, d_sc_root;
-  DevBuf<double> d_sc;
-  DevBuf<double> d_linv;
-  DevBuf<double> d_linv_part;       // partial tiles of the chunked k_linv_gemm items (one launch at a time uses it)
-  DevBuf<int> d_linv_cnt;           // their arrival counters (self-resetting)
-  DevBuf<long long> d_linv_off, d_gmap_off;
-  std::vector<long long> linv_off;  // per supernode: its L11^-1 block in d_linv (order > 256), else -1
-  DevBuf<FrontDesc> d_fdesc;
-  DevBuf<int> d_gmap;
-  std::vector<char> solve_direct_front;   // per supernode: solved by k_solve_direct (see build_solve_tables)
-  int solve_epoch = 0;
   int num_sms = 132;
-  struct Shard {
-    bool active = false;
-    int rank = 0, world = 1, nsub = 0;
-    std::vector<int> owner, cut_roots, top_fronts;
-    FrontPlan part[2];                       // [0] my subtrees, [1] top part
-    DevBuf<int> d_mark_cut, d_mark_top;
-  } shard;
-  cudaGraph_t fgraph = nullptr;
-  cudaGraphExec_t fgraph_exec = nullptr;
-  double fgraph_u = -1.0;
-  int fgraph_launches = 0;
 
   ~Solver() {
+    an.reset();   // (its graph and pinned buffers before the streams and events)
     if (amat) b200vec_tmat_destroy(amat);
     if (vec) b200vec_destroy(vec);
     if (h_vals) cudaFreeHost(h_vals);
-    if (h_rhs) cudaFreeHost(h_rhs);
     if (h_counters) cudaFreeHost(h_counters);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     for (cudaEvent_t e : ev_chunk) if (e) cudaEventDestroy(e);
-    if (fgraph_exec) cudaGraphExecDestroy(fgraph_exec);
-    if (fgraph) cudaGraphDestroy(fgraph);
     for (cudaEvent_t e : ev_pool) cudaEventDestroy(e);
     if (stream2) cudaStreamDestroy(stream2);
     if (stream3) cudaStreamDestroy(stream3);
@@ -342,11 +359,6 @@ struct Solver {
   cudaEvent_t next_event() {
     if (ev_next == ev_pool.size()) { cudaEvent_t e; cudaEventCreateWithFlags(&e, cudaEventDisableTiming); ev_pool.push_back(e); }
     return ev_pool[ev_next++];
-  }
-  void drop_staging() {
-    if (h_rhs) cudaFreeHost(h_rhs);
-    h_rhs = nullptr;
-    d_rhs.release();
   }
 };
 
@@ -463,7 +475,8 @@ static void build_level_plans(const Symbolic& S, int smax, const std::vector<cha
 
 static const int kSolveMidMax = 256;   // fronts above this order are "big" in the solve (block tasks + explicit L11 inverse)
 
-static int build_linv_plan(Solver* sv, const Symbolic& S, const std::vector<char>& take, LinvPlan& LP, cudaStream_t st) {
+static int build_linv_plan(Solver* sv, Analysis& A, const std::vector<char>& take, LinvPlan& LP, cudaStream_t st) {
+  const Symbolic& S = A.S;
   std::vector<int> pairs;
   int maxkb = 0;
   for (int s = 0; s < S.nsn; ++s) if (take[s] && S.f(s) > kSolveMidMax) {
@@ -512,11 +525,11 @@ static int build_linv_plan(Solver* sv, const Symbolic& S, const std::vector<char
     CU(LP.d_g.back()->upload(g1, st));
     CU(LP.d_g2.back()->upload(g2, st));
   }
-  if ((size_t)LP.part_tiles > sv->d_linv_cnt.n) {     // (analysis time: never inside a captured graph)
+  if ((size_t)LP.part_tiles > A.d_linv_cnt.n) {     // (analysis time: never inside a captured graph)
     CU(cudaStreamSynchronize(st));
-    CU(sv->d_linv_part.alloc((size_t)LP.part_tiles * 4096));
-    CU(sv->d_linv_cnt.alloc((size_t)LP.part_tiles));
-    CU(cudaMemset(sv->d_linv_cnt.p, 0, sv->d_linv_cnt.n * sizeof(int)));
+    CU(A.d_linv_part.alloc((size_t)LP.part_tiles * 4096));
+    CU(A.d_linv_cnt.alloc((size_t)LP.part_tiles));
+    CU(cudaMemset(A.d_linv_cnt.p, 0, A.d_linv_cnt.n * sizeof(int)));
   }
   return B200LDLT_SUCCESS;
 }
@@ -528,7 +541,8 @@ static int enqueue_linv(Solver* sv, const LinvPlan& LP, cudaStream_t st);
 //    fits the dynamic shared memory of k_solve_sub -> one CTA each, largest first.  Supernodes are numbered in postorder,
 //    so a subtree is the contiguous range [root - size + 1, root] and so are its panels, columns, row lists, child lists.
 //  * Everything else -> topologically sorted task lists for k_solve_top (forward: levels ascending; backward: descending).
-static int build_solve_plan(Solver* sv, const Symbolic& S, const std::vector<char>& take, SolvePlan& SP, cudaStream_t st) {
+static int build_solve_plan(Solver* sv, const Analysis& A, const std::vector<char>& take, SolvePlan& SP, cudaStream_t st) {
+  const Symbolic& S = A.S;
   const int nsn = S.nsn;
   std::vector<int> size(nsn, 1), ntaken(nsn, 0), subF(nsn, 0);
   for (int s = 0; s < nsn; ++s) {   // children precede parents
@@ -536,7 +550,7 @@ static int build_solve_plan(Solver* sv, const Symbolic& S, const std::vector<cha
     const int p = S.sn_parent[s];
     if (p >= 0) { size[p] += size[s]; ntaken[p] += ntaken[s]; subF[p] = std::max(subF[p], subF[s]); }
   }
-  const std::vector<char>& direct = sv->solve_direct_front;
+  const std::vector<char>& direct = A.solve_direct_front;
   // compact panel bytes of the fronts of [s0, s] that are walked inside a subtree (not owned by the direct kernel)
   std::vector<long long> ownL(nsn + 1, 0);   // prefix sums over supernodes
   std::vector<int> ownN(nsn + 1, 0);
@@ -745,15 +759,16 @@ static int build_solve_plan(Solver* sv, const Symbolic& S, const std::vector<cha
 }
 
 // per-front records shared by every solve plan: descriptors, gather maps of the big fronts, backward row addresses
-static int build_solve_tables(Solver* sv, const Symbolic& S, cudaStream_t st) {
+static int build_solve_tables(Solver* sv, Analysis& A, cudaStream_t st) {
+  const Symbolic& S = A.S;
   const int nsn = S.nsn;
   // fronts owned by k_solve_direct: on the lowest levels, order <= 64, all children of the same kind (children precede parents)
-  sv->solve_direct_front.assign(nsn, 0);
+  A.solve_direct_front.assign(nsn, 0);
   for (int s = 0; s < nsn; ++s) {
     if (S.sn_level[s] >= sv->dbg.solve_direct || S.f(s) > 64) continue;
     bool all = true;
-    for (int q = S.child_ptr[s]; q < S.child_ptr[s + 1]; ++q) all = all && sv->solve_direct_front[S.child_idx[q]];
-    sv->solve_direct_front[s] = all ? 1 : 0;
+    for (int q = S.child_ptr[s]; q < S.child_ptr[s + 1]; ++q) all = all && A.solve_direct_front[S.child_idx[q]];
+    A.solve_direct_front[s] = all ? 1 : 0;
   }
   std::vector<FrontDesc> fd(nsn);
   for (int s = 0; s < nsn; ++s) {
@@ -762,10 +777,10 @@ static int build_solve_tables(Solver* sv, const Symbolic& S, cudaStream_t st) {
     d.ch0 = S.child_ptr[s];
     const int nch = S.child_ptr[s + 1] - S.child_ptr[s];
     if (nch > 65535) { sv->err = "front with more than 65535 children"; return B200LDLT_FATAL_ERROR; }
-    d.nch = (unsigned short)nch; d.direct = (unsigned short)sv->solve_direct_front[s];
+    d.nch = (unsigned short)nch; d.direct = (unsigned short)A.solve_direct_front[s];
     d.L_off = S.L_off[s]; d.ro = S.rows_ptr[s];
   }
-  CU(sv->d_fdesc.upload(fd, st));
+  CU(A.d_fdesc.upload(fd, st));
   // gather maps of the big fronts: for child slot q and parent row j, the index into cbv (or -1)
   {
     std::vector<long long> goff(nsn, 0);
@@ -785,37 +800,37 @@ static int build_solve_tables(Solver* sv, const Symbolic& S, cudaStream_t st) {
         for (int j = 0; j < rc; ++j) dst[S.rel[ro + j]] = (int)(ro + j);
       }
     }
-    CU(sv->d_gmap_off.upload(goff, st));
-    CU(sv->d_gmap.upload(gm, st));
+    CU(A.d_gmap_off.upload(goff, st));
+    CU(A.d_gmap.upload(gm, st));
   }
   return B200LDLT_SUCCESS;
 }
 
-static int upload_schur_lists(Solver* sv, SchurLists& SL, cudaStream_t st) {
+static int upload_schur_lists(Solver* sv, Analysis& A, SchurLists& SL, cudaStream_t st) {
   std::vector<TcFront> f = SL.f; std::vector<TcTile> t = SL.t; std::vector<int> d = SL.dfl;
   if (f.empty()) f.push_back(TcFront{0, 0, 0, 0, 0});
   if (t.empty()) t.push_back(TcTile{0, 0, 0});
   if (d.empty()) d.push_back(0);
   CU(SL.d_f.upload(f, st)); CU(SL.d_t.upload(t, st)); CU(SL.d_dfl.upload(d, st));
-  if ((long long)sv->d_tc_dig.n < SL.dig_bytes) CU(sv->d_tc_dig.alloc(SL.dig_bytes));
-  if ((long long)sv->d_tc_exp.n < SL.exp_ints) CU(sv->d_tc_exp.alloc(SL.exp_ints));
+  if ((long long)A.d_tc_dig.n < SL.dig_bytes) CU(A.d_tc_dig.alloc(SL.dig_bytes));
+  if ((long long)A.d_tc_exp.n < SL.exp_ints) CU(A.d_tc_exp.alloc(SL.exp_ints));
   return B200LDLT_SUCCESS;
 }
 
 // The plan of the fronts in take_factor (factorisation, L11^-1) and take_solve (triangular solves); FP.linv_level is left
 // empty.  Needs the solve tables (build_solve_tables).
-static int build_front_plan(Solver* sv, const std::vector<char>& take_factor, const std::vector<char>& take_solve,
-                            FrontPlan& FP) {
-  const Symbolic& S = sv->S;
+static int build_front_plan(Solver* sv, Analysis& A, const std::vector<char>& take_factor,
+                            const std::vector<char>& take_solve, FrontPlan& FP) {
+  const Symbolic& S = A.S;
   cudaStream_t st = sv->stream;
   std::vector<int> fl;
   build_level_plans(S, sv->opt.smem_front_max, take_factor, fl, FP.levels, FP.schur, sv->tc_min_r, !sv->dbg.no_warp2);
   if (fl.empty()) fl.push_back(0);
   CU(FP.d_fl.upload(fl, st));
   FP.linv_level.clear();
-  int rc = upload_schur_lists(sv, FP.schur, st);
-  if (rc == B200LDLT_SUCCESS) rc = build_linv_plan(sv, S, take_factor, FP.linv, st);
-  if (rc == B200LDLT_SUCCESS) rc = build_solve_plan(sv, S, take_solve, FP.solve, st);
+  int rc = upload_schur_lists(sv, A, FP.schur, st);
+  if (rc == B200LDLT_SUCCESS) rc = build_linv_plan(sv, A, take_factor, FP.linv, st);
+  if (rc == B200LDLT_SUCCESS) rc = build_solve_plan(sv, A, take_solve, FP.solve, st);
   return rc;
 }
 
@@ -861,18 +876,13 @@ static cudaError_t alloc_sweep_state(Solver* sv, SweepState& W, const MultiStrid
   return cudaSuccess;
 }
 
+// A new analysis of the handle's pattern on vals.  The old one (and with it the factors) is released first, so its device
+// memory is free before the new one is allocated; the new one becomes the handle's only when all of it is built.
 static int run_analysis(Solver* sv, const double* vals) {
-  // a (re-)analysis invalidates the factors and every buffer sized by the old plan
-  sv->factored = false;
+  sv->an.reset();
   sv->reanalyse = false;
-  sv->drop_staging();
-  sv->blk.reset();
-  sv->lmul.reset();
-  sv->sfs.reset();
-  sv->selinv.reset();
-  sv->ea.reset();
-  if (sv->fgraph_exec) { cudaGraphExecDestroy(sv->fgraph_exec); sv->fgraph_exec = nullptr; }
-  if (sv->fgraph) { cudaGraphDestroy(sv->fgraph); sv->fgraph = nullptr; }
+  std::unique_ptr<Analysis> an(new Analysis());
+  Analysis& A = *an;
   AnalyseOptions ao;
   ao.ordering = sv->opt.ordering;
   ao.pair_saddle = sv->opt.pair_saddle;
@@ -880,80 +890,76 @@ static int run_analysis(Solver* sv, const double* vals) {
   ao.relax_frac = sv->opt.relax_frac;
   ao.sc_vars = sv->sc_vars;
   std::string e;
-  int rc = analyse(sv->n, sv->nnz, sv->irn.data(), sv->jcn.data(), vals, ao, sv->S, e);
+  int rc = analyse(sv->n, sv->nnz, sv->irn.data(), sv->jcn.data(), vals, ao, A.S, e);
   if (rc != 0) { sv->err = e; return B200LDLT_FATAL_ERROR; }
-  Symbolic& S = sv->S;
+  Symbolic& S = A.S;
   cudaStream_t st = sv->stream;
   // Schur mode: the root front of S, factored by none of the plans below; assembled by the big-front kernels (one-entry
   // front list d_sc_root), so its children get inverse row maps whatever its order
   const int m = (int)sv->sc_vars.size();
-  sv->sc_root = -1;
   if (m > 0) {
     const int rt = S.nsn - 1;
     if (S.sn_start[rt] != S.n - m || S.r(rt) != 0 || S.sn_parent[rt] != -1) {
       sv->err = "internal: the Schur variables do not form the last root front";
       return B200LDLT_FATAL_ERROR;
     }
-    sv->sc_root = rt;
-    sv->sc_nch = S.child_ptr[rt + 1] - S.child_ptr[rt];
-    sv->sc_nent = S.uent_ptr[rt + 1] - S.uent_ptr[rt];
-    CU(sv->d_sc_vars.upload(sv->sc_vars, st));
-    CU(sv->d_sc_root.upload(std::vector<int>{rt}, st));
-    CU(sv->d_sc.alloc((size_t)m * m));
-  } else {
-    sv->d_sc_vars.release(); sv->d_sc_root.release(); sv->d_sc.release();
+    A.sc_root = rt;
+    A.sc_nch = S.child_ptr[rt + 1] - S.child_ptr[rt];
+    A.sc_nent = S.uent_ptr[rt + 1] - S.uent_ptr[rt];
+    CU(A.d_sc_vars.upload(sv->sc_vars, st));
+    CU(A.d_sc_root.upload(std::vector<int>{rt}, st));
+    CU(A.d_sc.alloc((size_t)m * m));
   }
   // the fronts the factorisation factors: all but the Schur root
   std::vector<char> take_f(S.nsn, 1);
-  if (sv->sc_root >= 0) take_f[sv->sc_root] = 0;
-  CU(sv->d_sn_start.upload(S.sn_start, st));
-  CU(sv->d_sn_parent.upload(S.sn_parent, st));
-  CU(sv->d_rows_ptr.upload(S.rows_ptr, st));
-  CU(sv->d_rows.upload(S.rows, st));
-  CU(sv->d_rel.upload(S.rel, st));
-  CU(sv->d_child_ptr.upload(S.child_ptr, st));
-  CU(sv->d_child_idx.upload(S.child_idx, st));
-  CU(sv->d_uent_ptr.upload(S.uent_ptr, st));
-  CU(sv->d_u_dst.upload(S.u_dst, st));
-  CU(sv->d_u_dst64.upload(S.u_dst64, st));
-  CU(sv->d_L_off.upload(S.L_off, st));
-  CU(sv->d_cb_off.upload(S.cb_off, st));
-  CU(sv->d_useg_ptr.upload(S.useg_ptr, st));
-  CU(sv->d_useg_src.upload(S.useg_src, st));
-  CU(sv->d_u_row.upload(S.u_row, st));
-  CU(sv->d_u_col.upload(S.u_col, st));
-  CU(sv->d_perm.upload(S.perm, st));
-  CU(sv->d_irn.upload(sv->irn, st));
-  CU(sv->d_jcn.upload(sv->jcn, st));
+  if (A.sc_root >= 0) take_f[A.sc_root] = 0;
+  CU(A.d_sn_start.upload(S.sn_start, st));
+  CU(A.d_sn_parent.upload(S.sn_parent, st));
+  CU(A.d_rows_ptr.upload(S.rows_ptr, st));
+  CU(A.d_rows.upload(S.rows, st));
+  CU(A.d_rel.upload(S.rel, st));
+  CU(A.d_child_ptr.upload(S.child_ptr, st));
+  CU(A.d_child_idx.upload(S.child_idx, st));
+  CU(A.d_uent_ptr.upload(S.uent_ptr, st));
+  CU(A.d_u_dst.upload(S.u_dst, st));
+  CU(A.d_u_dst64.upload(S.u_dst64, st));
+  CU(A.d_L_off.upload(S.L_off, st));
+  CU(A.d_cb_off.upload(S.cb_off, st));
+  CU(A.d_useg_ptr.upload(S.useg_ptr, st));
+  CU(A.d_useg_src.upload(S.useg_src, st));
+  CU(A.d_u_row.upload(S.u_row, st));
+  CU(A.d_u_col.upload(S.u_col, st));
+  CU(A.d_perm.upload(S.perm, st));
+  CU(A.d_irn.upload(sv->irn, st));
+  CU(A.d_jcn.upload(sv->jcn, st));
   const int n = S.n;
-  CU(sv->d_vals.alloc(sv->nnz));
-  CU(sv->d_uval.alloc(S.nnz_u));
-  CU(sv->d_L.alloc(S.L_off[S.nsn]));
-  CU(sv->d_W.alloc(S.L_off[S.nsn]));
-  CU(sv->d_CB.alloc(std::max<int64_t>(S.cb_off[S.nsn], 1)));
-  CU(sv->d_dinv.alloc(n)); CU(sv->d_doff.alloc(n)); CU(sv->d_scale.alloc(n));
-  CU(sv->d_res.alloc(n));
-  CU(sv->d_ptype.alloc(n)); CU(sv->d_lperm.alloc(n)); CU(sv->d_bperm.alloc(n));
-  CU(sv->d_counters.alloc(CNT_N));
-  CU(sv->d_zlist.alloc(n)); CU(sv->d_zflag.alloc(n));
-  sv->zpos.clear();
-  CU(sv->d_colmax.alloc(n));
-  CU(sv->d_rmax.alloc(n));
-  CU(cudaMemsetAsync(sv->d_rmax.p, 0, n * sizeof(unsigned long long), st));
-  CU(cudaMemsetAsync(sv->d_L.p, 0, sv->d_L.n * sizeof(double), st));
+  if (!sv->d_vals.p) CU(sv->d_vals.alloc(sv->nnz));
+  CU(A.d_uval.alloc(S.nnz_u));
+  CU(A.d_L.alloc(S.L_off[S.nsn]));
+  CU(A.d_W.alloc(S.L_off[S.nsn]));
+  CU(A.d_CB.alloc(std::max<int64_t>(S.cb_off[S.nsn], 1)));
+  CU(A.d_dinv.alloc(n)); CU(A.d_doff.alloc(n)); CU(A.d_scale.alloc(n));
+  CU(A.d_res.alloc(n));
+  CU(A.d_ptype.alloc(n)); CU(A.d_lperm.alloc(n)); CU(A.d_bperm.alloc(n));
+  CU(A.d_counters.alloc(CNT_N));
+  CU(A.d_zlist.alloc(n)); CU(A.d_zflag.alloc(n));
+  CU(A.d_colmax.alloc(n));
+  CU(A.d_rmax.alloc(n));
+  CU(cudaMemsetAsync(A.d_rmax.p, 0, n * sizeof(unsigned long long), st));
+  CU(cudaMemsetAsync(A.d_L.p, 0, A.d_L.n * sizeof(double), st));
 
-  DevSym& D = sv->DS;
+  DevSym& D = A.DS;
   D.n = n; D.nsn = S.nsn;
-  D.sn_start = sv->d_sn_start.p; D.sn_parent = sv->d_sn_parent.p;
-  D.rows_ptr = sv->d_rows_ptr.p; D.rows = sv->d_rows.p; D.rel = sv->d_rel.p;
-  D.child_ptr = sv->d_child_ptr.p; D.child_idx = sv->d_child_idx.p;
-  D.uent_ptr = sv->d_uent_ptr.p; D.u_dst = sv->d_u_dst.p; D.u_dst64 = sv->d_u_dst64.p;
-  D.L_off = sv->d_L_off.p; D.cb_off = sv->d_cb_off.p;
-  DevNum& N = sv->DN;
-  N.L = sv->d_L.p; N.W = sv->d_W.p; N.CB = sv->d_CB.p; N.uval = sv->d_uval.p;
-  N.dinv = sv->d_dinv.p; N.doff = sv->d_doff.p; N.ptype = sv->d_ptype.p;
-  N.lperm = sv->d_lperm.p; N.bperm = sv->d_bperm.p; N.counters = sv->d_counters.p; N.colmax = sv->d_colmax.p;
-  N.zlist = sv->d_zlist.p;
+  D.sn_start = A.d_sn_start.p; D.sn_parent = A.d_sn_parent.p;
+  D.rows_ptr = A.d_rows_ptr.p; D.rows = A.d_rows.p; D.rel = A.d_rel.p;
+  D.child_ptr = A.d_child_ptr.p; D.child_idx = A.d_child_idx.p;
+  D.uent_ptr = A.d_uent_ptr.p; D.u_dst = A.d_u_dst.p; D.u_dst64 = A.d_u_dst64.p;
+  D.L_off = A.d_L_off.p; D.cb_off = A.d_cb_off.p;
+  DevNum& N = A.DN;
+  N.L = A.d_L.p; N.W = A.d_W.p; N.CB = A.d_CB.p; N.uval = A.d_uval.p;
+  N.dinv = A.d_dinv.p; N.doff = A.d_doff.p; N.ptype = A.d_ptype.p;
+  N.lperm = A.d_lperm.p; N.bperm = A.d_bperm.p; N.counters = A.d_counters.p; N.colmax = A.d_colmax.p;
+  N.zlist = A.d_zlist.p;
 
   // inverse row maps of the children of the (factorisation-)big fronts, for the one-launch extend-add
   {
@@ -961,7 +967,7 @@ static int run_analysis(Solver* sv, const double* vals) {
     long long tot = 0;
     for (int c = 0; c < S.nsn; ++c) {
       const int p = S.sn_parent[c];
-      if (p >= 0 && (S.f(p) > sv->opt.smem_front_max || p == sv->sc_root)) { eoff[c] = tot; tot += S.f(p); }
+      if (p >= 0 && (S.f(p) > sv->opt.smem_front_max || p == A.sc_root)) { eoff[c] = tot; tot += S.f(p); }
     }
     std::vector<int> einv((size_t)std::max<long long>(tot, 1), -1);
     for (int c = 0; c < S.nsn; ++c) if (eoff[c] >= 0) {
@@ -969,9 +975,9 @@ static int run_analysis(Solver* sv, const double* vals) {
       const int rc = S.r(c);
       for (int j = 0; j < rc; ++j) einv[(size_t)(eoff[c] + S.rel[ro + j])] = j;
     }
-    CU(sv->d_einv_off.upload(eoff, st));
-    CU(sv->d_einv.upload(einv, st));
-    D.einv_off = sv->d_einv_off.p; D.einv = sv->d_einv.p;
+    CU(A.d_einv_off.upload(eoff, st));
+    CU(A.d_einv.upload(einv, st));
+    D.einv_off = A.d_einv_off.p; D.einv = A.d_einv.p;
   }
 
   CU(cudaFuncSetAttribute(k_tc_schur, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
@@ -984,7 +990,6 @@ static int run_analysis(Solver* sv, const double* vals) {
   // ---- triangular solves: flags, scratch, explicit-inverse work lists, plan ------------------------------
   {
     std::vector<int> boff(S.nsn, 0);
-    sv->shard.active = false;
     std::vector<long long> bigv_off(S.nsn, 0);
     long long bv = 0; int bo = 0;
     for (int s = 0; s < S.nsn; ++s) if (S.f(s) > DF_MIDMAX) {
@@ -993,7 +998,7 @@ static int run_analysis(Solver* sv, const double* vals) {
     }
     // explicit inverses of the big fronts' pivot blocks (k_linv_*): K64 x K64 doubles per big front
     {
-      std::vector<long long>& linv_off = sv->linv_off;
+      std::vector<long long>& linv_off = A.linv_off;
       linv_off.assign(S.nsn, -1);
       long long tot = 0;
       for (int s = 0; s < S.nsn; ++s) if (S.f(s) > DF_MIDMAX) {
@@ -1001,39 +1006,38 @@ static int run_analysis(Solver* sv, const double* vals) {
         const long long K64 = (long long)((S.k(s) + DF_BLK - 1) / DF_BLK) * DF_BLK;
         tot += K64 * K64;
       }
-      if (sv->sc_root >= 0) sv->sc_linv_off = std::max(linv_off[sv->sc_root], 0LL);
-      CU(sv->d_linv_off.upload(linv_off, st));
-      CU(sv->d_linv.alloc(std::max<long long>(tot, 1)));
-      CU(cudaMemsetAsync(sv->d_linv.p, 0, sv->d_linv.n * sizeof(double), st));
+      if (A.sc_root >= 0) A.sc_linv_off = std::max(linv_off[A.sc_root], 0LL);
+      CU(A.d_linv_off.upload(linv_off, st));
+      CU(A.d_linv.alloc(std::max<long long>(tot, 1)));
+      CU(cudaMemsetAsync(A.d_linv.p, 0, A.d_linv.n * sizeof(double), st));
     }
-    CU(sv->d_boff.upload(boff, st));
-    CU(sv->d_bigv_off.upload(bigv_off, st));
+    CU(A.d_boff.upload(boff, st));
+    CU(A.d_bigv_off.upload(bigv_off, st));
     {
       // partial solves: where a pivot position's value lives between the sweeps (k_piv_out / k_piv_in)
       std::vector<long long> piv_big(n, -1);
       for (int s = 0; s < S.nsn; ++s) if (S.f(s) > DF_MIDMAX)
         for (int t = 0; t < S.k(s); ++t) piv_big[S.sn_start[s] + t] = bigv_off[s] + t;
-      CU(sv->d_piv_big.upload(piv_big, st));
+      CU(A.d_piv_big.upload(piv_big, st));
     }
     CU(cudaDeviceGetAttribute(&sv->num_sms, cudaDevAttrMultiProcessorCount, sv->dev));
     const MultiStride one{1, S.nsn, std::max(bo, 1), 0, n, (long long)std::max<size_t>(S.rows.size(), 1),
                           std::max<long long>(bv, 1), 0};
-    CU(alloc_sweep_state(sv, sv->sweep, one));
-    sv->solve_epoch = 0;
-    int rc2 = build_solve_tables(sv, S, st);
-    if (rc2 == B200LDLT_SUCCESS) rc2 = build_front_plan(sv, take_f, std::vector<char>(S.nsn, 1), sv->fronts);
+    CU(alloc_sweep_state(sv, A.sweep, one));
+    int rc2 = build_solve_tables(sv, A, st);
+    if (rc2 == B200LDLT_SUCCESS) rc2 = build_front_plan(sv, A, take_f, std::vector<char>(S.nsn, 1), A.fronts);
     if (rc2 != B200LDLT_SUCCESS) return rc2;
     // the L11^-1 work once more, split by tree level
     for (int l = 0; l < S.nlevels; ++l) {
       std::vector<char> tl(S.nsn, 0);
       bool any = false;
       for (int q = 0; q < S.nsn; ++q) if (take_f[q] && S.sn_level[q] == l && S.f(q) > kSolveMidMax) { tl[q] = 1; any = true; }
-      sv->fronts.linv_level.emplace_back(new LinvPlan());
-      if (any) { rc2 = build_linv_plan(sv, S, tl, *sv->fronts.linv_level.back(), st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
+      A.fronts.linv_level.emplace_back(new LinvPlan());
+      if (any) { rc2 = build_linv_plan(sv, A, tl, *A.fronts.linv_level.back(), st); if (rc2 != B200LDLT_SUCCESS) return rc2; }
     }
     if (sv->opt.verbose)
       fprintf(stderr, "[b200ldlt] solve: %d big-front blocks, top grid %d x %d thr (%d CTAs per SM)\n",
-              bo, sv->sweep.grid, DF_THREADS, sv->sweep.grid / sv->num_sms);
+              bo, A.sweep.grid, DF_THREADS, A.sweep.grid / sv->num_sms);
     CU(cudaStreamSynchronize(st));
   }
 
@@ -1042,7 +1046,7 @@ static int run_analysis(Solver* sv, const double* vals) {
   I.nsupernodes = S.nsn; I.nlevels = S.nlevels; I.max_front = S.max_front; I.max_pivots = S.max_k;
   I.n_saddle = S.n_saddle; I.n_pairs = S.n_pairs;
   I.nnz_L = S.nnzL; I.nnz_L_true = S.nnzL_true;
-  I.L_bytes = (int64_t)sv->d_L.n * 8; I.cb_bytes = (int64_t)sv->d_CB.n * 8;
+  I.L_bytes = (int64_t)A.d_L.n * 8; I.cb_bytes = (int64_t)A.d_CB.n * 8;
   I.flops_panel = S.flops_panel; I.flops_schur = S.flops_schur;
   I.t_order_s = S.t_order; I.t_symbolic_s = S.t_symbolic;
   if (sv->opt.verbose)
@@ -1052,7 +1056,7 @@ static int run_analysis(Solver* sv, const double* vals) {
             n, (long long)S.nnz_in, (long long)S.nnz_u, S.n_saddle, S.n_pairs, S.nsn, S.nlevels, S.max_front,
             S.max_k, (long long)S.nnzL, (long long)S.nnzL_true, S.flops_panel, S.flops_schur,
             S.cb_total * 8.0 / 1e6, S.t_order, S.t_symbolic);
-  sv->analysed = true;
+  sv->an = std::move(an);
   return B200LDLT_SUCCESS;
 }
 
@@ -1074,11 +1078,12 @@ static cudaError_t launch_pdl(bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 
 // enqueue the numeric factorisation of the fronts of FP from the values in d_vals; prologue: first the summing of
 // duplicates and the scaling
 static int enqueue_factor(Solver* sv, const FrontPlan& FP, bool prologue) {
+  Analysis& A = *sv->an;
   const SchurLists& SL = FP.schur;
-  Symbolic& S = sv->S;
+  Symbolic& S = A.S;
   cudaStream_t st = sv->stream;
-  DevSym& D = sv->DS;
-  DevNum& N = sv->DN;
+  DevSym& D = A.DS;
+  DevNum& N = A.DN;
   N.u = sv->pivtol;
   N.tiny = sv->opt.tiny;
   const int n = S.n;
@@ -1089,16 +1094,16 @@ static int enqueue_factor(Solver* sv, const FrontPlan& FP, bool prologue) {
   if (prologue) {
   L = 0;
   sv->ev_next = 0;
-  CU(cudaMemsetAsync(sv->d_counters.p, 0, CNT_N * sizeof(int), st));
-  CU(cudaMemsetAsync(sv->d_colmax.p, 0, (size_t)n * sizeof(double), st));
-  k_sum_dups<<<cdiv(nu, 256), 256, 0, st>>>(nu, sv->d_useg_ptr.p, sv->d_useg_src.p, sv->d_vals.p, sv->d_uval.p); ++L;
-  k_fill<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_scale.p, 1.0); ++L;
+  CU(cudaMemsetAsync(A.d_counters.p, 0, CNT_N * sizeof(int), st));
+  CU(cudaMemsetAsync(A.d_colmax.p, 0, (size_t)n * sizeof(double), st));
+  k_sum_dups<<<cdiv(nu, 256), 256, 0, st>>>(nu, A.d_useg_ptr.p, A.d_useg_src.p, sv->d_vals.p, A.d_uval.p); ++L;
+  k_fill<<<cdiv(n, 256), 256, 0, st>>>(n, A.d_scale.p, 1.0); ++L;
   for (int sw = 0; sw < sv->opt.scaling; ++sw) {
-    k_rowmax<<<cdiv(nu, 256), 256, 0, st>>>(nu, sv->d_u_row.p, sv->d_u_col.p, sv->d_uval.p, sv->d_scale.p, sv->d_rmax.p); ++L;
-    k_scale_update<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_scale.p, sv->d_rmax.p); ++L;
+    k_rowmax<<<cdiv(nu, 256), 256, 0, st>>>(nu, A.d_u_row.p, A.d_u_col.p, A.d_uval.p, A.d_scale.p, A.d_rmax.p); ++L;
+    k_scale_update<<<cdiv(n, 256), 256, 0, st>>>(n, A.d_scale.p, A.d_rmax.p); ++L;
   }
   if (sv->opt.scaling > 0) {
-    k_apply_scale<<<cdiv(nu, 256), 256, 0, st>>>(nu, sv->d_u_row.p, sv->d_u_col.p, sv->d_scale.p, sv->d_uval.p); ++L;
+    k_apply_scale<<<cdiv(nu, 256), 256, 0, st>>>(nu, A.d_u_row.p, A.d_u_col.p, A.d_scale.p, A.d_uval.p); ++L;
   }
   }  // prologue
   // storage of all big fronts of this plan is cleared up front on the third stream (idle until the first L11 inverse),
@@ -1227,9 +1232,9 @@ static int enqueue_factor(Solver* sv, const FrontPlan& FP, bool prologue) {
       // register-blocked DFMA tiles for the rest
       if (P.tc_t_cnt > 0) {
         const TcFront* tf = SL.d_f.p + P.tc_f_off;
-        k_tc_slice<<<dim3(cdiv(P.tc_rmax, 8), P.tc_f_cnt), 256, 0, st>>>(D, N, tf, 0, sv->d_tc_dig.p, sv->d_tc_exp.p); ++L;
-        k_tc_slice<<<dim3(cdiv(P.tc_rmax, 8), P.tc_f_cnt), 256, 0, st>>>(D, N, tf, 1, sv->d_tc_dig.p, sv->d_tc_exp.p); ++L;
-        k_tc_schur<<<P.tc_t_cnt, TC_THREADS, TC_SMEM_BYTES, st>>>(D, N, tf, SL.d_t.p + P.tc_t_off, sv->d_tc_dig.p, sv->d_tc_exp.p); ++L;
+        k_tc_slice<<<dim3(cdiv(P.tc_rmax, 8), P.tc_f_cnt), 256, 0, st>>>(D, N, tf, 0, A.d_tc_dig.p, A.d_tc_exp.p); ++L;
+        k_tc_slice<<<dim3(cdiv(P.tc_rmax, 8), P.tc_f_cnt), 256, 0, st>>>(D, N, tf, 1, A.d_tc_dig.p, A.d_tc_exp.p); ++L;
+        k_tc_schur<<<P.tc_t_cnt, TC_THREADS, TC_SMEM_BYTES, st>>>(D, N, tf, SL.d_t.p + P.tc_t_off, A.d_tc_dig.p, A.d_tc_exp.p); ++L;
       }
       if (!cb_panel && P.df_cnt > 0) {
         k_big_schur84<<<dim3(cdiv(P.df_rmax, TM), cdiv(P.df_rmax, TM), P.df_cnt), 128, 0, st>>>(D, N, SL.d_dfl.p + P.df_off); ++L;
@@ -1241,21 +1246,21 @@ static int enqueue_factor(Solver* sv, const FrontPlan& FP, bool prologue) {
       CU(cudaStreamWaitEvent(st, e, 0));
     }
   }
-  if (sv->sc_root >= 0) {
+  if (A.sc_root >= 0) {
     // Schur mode: the root front of S, once all of its children are done, through the big-front assembly (its panel
     // is m x m, r = 0); S_c out of the assembled panel, then the identity pivot block in its place
-    const int m = (int)sv->sc_vars.size(), rt = sv->sc_root;
+    const int m = (int)sv->sc_vars.size(), rt = A.sc_root;
     const long long mm = (long long)m * m;
-    const int* rl = sv->d_sc_root.p;
+    const int* rl = A.d_sc_root.p;
     k_big_zero<<<dim3(std::min<unsigned>(cdiv(mm, 1024), 592), 1), 256, 0, st>>>(D, N, rl); ++L;
-    k_big_assemble<<<dim3(std::max(1u, std::min<unsigned>(cdiv(sv->sc_nent, 256), 64)), 1), 256, 0, st>>>(D, N, rl); ++L;
-    if (sv->sc_nch > 0) { k_big_extend_all<<<dim3(cdiv(m, 8), 1), 256, 0, st>>>(D, N, rl); ++L; }
-    double* P = sv->d_L.p + S.L_off[rt];
-    k_sc_out<<<cdiv(mm, 256), 256, 0, st>>>(m, P, sv->d_sc_vars.p, sv->d_scale.p, sv->d_sc.p); ++L;
+    k_big_assemble<<<dim3(std::max(1u, std::min<unsigned>(cdiv(A.sc_nent, 256), 64)), 1), 256, 0, st>>>(D, N, rl); ++L;
+    if (A.sc_nch > 0) { k_big_extend_all<<<dim3(cdiv(m, 8), 1), 256, 0, st>>>(D, N, rl); ++L; }
+    double* P = A.d_L.p + S.L_off[rt];
+    k_sc_out<<<cdiv(mm, 256), 256, 0, st>>>(m, P, A.d_sc_vars.p, A.d_scale.p, A.d_sc.p); ++L;
     const bool big = S.f(rt) > DF_MIDMAX;
     const long long k64 = big ? (long long)((m + DF_BLK - 1) / DF_BLK) * DF_BLK : 0;
-    k_sc_identity<<<cdiv(std::max(mm, k64 * k64), 256), 256, 0, st>>>(m, n - m, k64, P, sv->d_lperm.p, sv->d_bperm.p,
-        sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, big ? sv->d_linv.p + sv->sc_linv_off : nullptr); ++L;
+    k_sc_identity<<<cdiv(std::max(mm, k64 * k64), 256), 256, 0, st>>>(m, n - m, k64, P, A.d_lperm.p, A.d_bperm.p,
+        A.d_ptype.p, A.d_dinv.p, A.d_doff.p, big ? A.d_linv.p + A.sc_linv_off : nullptr); ++L;
   }
   if (linv_forked) {
     cudaEvent_t e = sv->next_event();
@@ -1273,12 +1278,13 @@ static int enqueue_factor(Solver* sv, const FrontPlan& FP, bool prologue) {
 // 64x64 diagonal blocks in one launch, then two tile-GEMM launches per doubling level (all fronts and pairs batched)
 static int enqueue_linv(Solver* sv, const LinvPlan& LP, cudaStream_t st) {
   if (LP.ndiag <= 0) return B200LDLT_SUCCESS;
+  Analysis& A = *sv->an;
   int& L = sv->launches;
-  k_linv_diag<<<LP.ndiag, 64, 0, st>>>(sv->DS, sv->DN, LP.d_diag.p, sv->d_linv_off.p, sv->d_linv.p); ++L;
+  k_linv_diag<<<LP.ndiag, 64, 0, st>>>(A.DS, A.DN, LP.d_diag.p, A.d_linv_off.p, A.d_linv.p); ++L;
   for (size_t l = 0; l < LP.ng.size(); ++l) {
     if (LP.ng[l] <= 0) continue;
-    k_linv_gemm<1><<<LP.ng[l], 128, 0, st>>>(sv->DS, sv->DN, LP.d_g[l]->p, sv->d_linv_off.p, sv->d_linv.p, sv->d_linv_part.p, sv->d_linv_cnt.p); ++L;
-    k_linv_gemm<2><<<LP.ng2[l], 128, 0, st>>>(sv->DS, sv->DN, LP.d_g2[l]->p, sv->d_linv_off.p, sv->d_linv.p, sv->d_linv_part.p, sv->d_linv_cnt.p); ++L;
+    k_linv_gemm<1><<<LP.ng[l], 128, 0, st>>>(A.DS, A.DN, LP.d_g[l]->p, A.d_linv_off.p, A.d_linv.p, A.d_linv_part.p, A.d_linv_cnt.p); ++L;
+    k_linv_gemm<2><<<LP.ng2[l], 128, 0, st>>>(A.DS, A.DN, LP.d_g2[l]->p, A.d_linv_off.p, A.d_linv.p, A.d_linv_part.p, A.d_linv_cnt.p); ++L;
   }
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
@@ -1291,9 +1297,10 @@ __global__ void k_zero_pivots(int nz, const int* __restrict__ zpos, double* __re
 }
 
 static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* num_neg) {
+  Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
   CU(cudaEventRecord(sv->ev1, st));
-  CU(cudaMemcpyAsync(sv->h_counters, sv->d_counters.p, CNT_N * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(sv->h_counters, A.d_counters.p, CNT_N * sizeof(int), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   float ms = 0;
   cudaEventElapsedTime(&ms, sv->ev0, sv->ev1);
@@ -1311,12 +1318,12 @@ static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* n
   // the pivot leaves the inertia.  A lifted zero (|pivot| <= tiny under a column that is not noise) never keeps factors.
   // With num_forced > 0 the factors (and the inertia reported) are those of a matrix perturbed by <= 1e-8 |column| in the
   // lifted pivots; the count is surfaced in b200ldlt_info and drives increase_quality (re-analysis with the current values).
-  sv->factored = (I.num_tiny == 0);
-  sv->zpos.clear();
+  A.factored = (I.num_tiny == 0);
+  A.zpos.clear();
   if (I.num_tiny > 0) {
     const int nz = std::min(sv->h_counters[CNT_ZLIST], sv->n);
     std::vector<int> zl(nz);
-    CU(cudaMemcpy(zl.data(), sv->d_zlist.p, nz * sizeof(int), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(zl.data(), A.d_zlist.p, nz * sizeof(int), cudaMemcpyDeviceToHost));
     std::sort(zl.begin(), zl.end());
     int lifted = -1, zneg = 0;
     for (int e : zl) {
@@ -1330,16 +1337,16 @@ static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* n
       const bool keep = sv->keep_singular && sv->sc_vars.empty();   // (Schur mode keeps no singular factors)
       sv->err = "factor: SINGULAR: " + std::to_string(nz) + " zero pivot(s)" +
                 (keep ? "; factors kept with D^+ (zero pivots left out of the inertia)" : "; no factors kept");
-      if (keep && !sv->shard.active && nz == I.num_tiny) {
-        for (int e : zl) sv->zpos.push_back(e >> 2);
-        CU(sv->d_zpos.upload(sv->zpos, st));
-        CU(cudaMemsetAsync(sv->d_zflag.p, 0, sv->n, st));
-        k_zero_pivots<<<cdiv(nz, 256), 256, 0, st>>>(nz, sv->d_zpos.p, sv->d_dinv.p, sv->d_zflag.p);
+      if (keep && !A.shard.active && nz == I.num_tiny) {
+        for (int e : zl) A.zpos.push_back(e >> 2);
+        CU(A.d_zpos.upload(A.zpos, st));
+        CU(cudaMemsetAsync(A.d_zflag.p, 0, sv->n, st));
+        k_zero_pivots<<<cdiv(nz, 256), 256, 0, st>>>(nz, A.d_zpos.p, A.d_dinv.p, A.d_zflag.p);
         CU(cudaGetLastError());
         CU(cudaStreamSynchronize(st));
         I.launches_factor += 1;
         I.num_neg -= zneg;
-        sv->factored = true;
+        A.factored = true;
       }
     }
   }
@@ -1353,14 +1360,13 @@ static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* n
   return B200LDLT_SUCCESS;
 }
 
-static int do_factor(Solver* sv, const double* d_vals_ext_in, bool from_host, int check_inertia, int expected_neg,
+static int do_factor(Solver* sv, const double* d_vals_ext, bool from_host, int check_inertia, int expected_neg,
                      int* num_neg) {
-  const double* d_vals_ext = d_vals_ext_in;
   if (num_neg) *num_neg = -1;
   if (sv->n <= 0) { sv->err = "factor before analyse"; return B200LDLT_FATAL_ERROR; }
   CU(cudaSetDevice(sv->dev));
-  if (!sv->analysed || sv->reanalyse) {
-    if (sv->analysed) ++sv->n_reanalysed;
+  if (!sv->an || sv->reanalyse) {
+    if (sv->an) ++sv->n_reanalysed;
     std::vector<double> hv;
     const double* vals = sv->h_vals;
     if (!from_host && d_vals_ext) {
@@ -1370,12 +1376,8 @@ static int do_factor(Solver* sv, const double* d_vals_ext_in, bool from_host, in
     }
     int rc = run_analysis(sv, vals);
     if (rc != B200LDLT_SUCCESS) return rc;
-    if (!from_host && d_vals_ext) {
-      // the analysis re-allocated the device value array (d_vals_ext may have been that very array): restore it
-      CU(cudaMemcpy(sv->d_vals.p, hv.data(), sv->nnz * sizeof(double), cudaMemcpyHostToDevice));
-      d_vals_ext = sv->d_vals.p;
-    }
   }
+  Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
   CU(cudaEventRecord(sv->ev0, st));
   if (from_host)
@@ -1387,22 +1389,22 @@ static int do_factor(Solver* sv, const double* d_vals_ext_in, bool from_host, in
   int rc;
   if (sv->opt.use_graph == 1) {
     // the launch sequence is fixed by the symbolic structure: capture it once, replay it every factorisation
-    if (!sv->fgraph_exec || sv->fgraph_u != sv->pivtol) {
-      if (sv->fgraph_exec) { cudaGraphExecDestroy(sv->fgraph_exec); sv->fgraph_exec = nullptr; }
-      if (sv->fgraph) { cudaGraphDestroy(sv->fgraph); sv->fgraph = nullptr; }
+    if (!A.fgraph_exec || A.fgraph_u != sv->pivtol) {
+      if (A.fgraph_exec) { cudaGraphExecDestroy(A.fgraph_exec); A.fgraph_exec = nullptr; }
+      if (A.fgraph) { cudaGraphDestroy(A.fgraph); A.fgraph = nullptr; }
       CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      rc = enqueue_factor(sv, sv->fronts, true);
-      cudaError_t ce = cudaStreamEndCapture(st, &sv->fgraph);
+      rc = enqueue_factor(sv, A.fronts, true);
+      cudaError_t ce = cudaStreamEndCapture(st, &A.fgraph);
       if (rc != B200LDLT_SUCCESS) return rc;
       CU(ce);
-      CU(cudaGraphInstantiate(&sv->fgraph_exec, sv->fgraph, 0));
-      sv->fgraph_u = sv->pivtol;
-      sv->fgraph_launches = sv->launches;
+      CU(cudaGraphInstantiate(&A.fgraph_exec, A.fgraph, 0));
+      A.fgraph_u = sv->pivtol;
+      A.fgraph_launches = sv->launches;
     }
-    sv->launches = sv->fgraph_launches;
-    CU(cudaGraphLaunch(sv->fgraph_exec, st));
+    sv->launches = A.fgraph_launches;
+    CU(cudaGraphLaunch(A.fgraph_exec, st));
   } else {
-    rc = enqueue_factor(sv, sv->fronts, true);
+    rc = enqueue_factor(sv, A.fronts, true);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   return finish_factor(sv, check_inertia, expected_neg, num_neg);
@@ -1416,16 +1418,17 @@ __global__ void k_mark_flags(int* flags, const int* __restrict__ list, int n, in
 // the DevSolve of a sweep: the handle's per-front tables, the plan's work lists, the state's arrays (column 0; the
 // kernels find the other columns through MultiStride)
 static DevSolve sweep_view(const Solver* sv, const SolvePlan& SP, const SweepState& W) {
+  const Analysis& A = *sv->an;
   DevSolve V;
   V.tasks = SP.d_tf.p; V.tasks_bwd = SP.d_tb.p; V.ntasks_fwd = SP.ntf; V.ntasks_bwd = SP.ntb;
   V.bundle = SP.d_bundle.p;
   V.done_f = W.d_done_f.p; V.done_b = W.d_done_b.p;
   V.bflag_f = W.d_bflag_f.p; V.bflag_b = W.d_bflag_b.p; V.bcnt = W.d_bcnt.p; V.bcnt_b = W.d_bcnt_b.p;
-  V.boff = sv->d_boff.p; V.bigv_off = sv->d_bigv_off.p; V.bigv = W.d_bigv.p; V.bigy = W.d_bigy.p;
+  V.boff = A.d_boff.p; V.bigv_off = A.d_bigv_off.p; V.bigv = W.d_bigv.p; V.bigy = W.d_bigy.p;
   V.part = W.width > 1 ? W.d_part.p : SP.d_part.p; V.ccnt = W.width > 1 ? W.d_ccnt.p : SP.d_ccnt.p;
   V.ticket = W.d_ticket.p;
-  V.linv = sv->d_linv.p; V.linv_off = sv->d_linv_off.p;
-  V.fdesc = sv->d_fdesc.p; V.gmap = sv->d_gmap.p; V.gmap_off = sv->d_gmap_off.p;
+  V.linv = A.d_linv.p; V.linv_off = A.d_linv_off.p;
+  V.fdesc = A.d_fdesc.p; V.gmap = A.d_gmap.p; V.gmap_off = A.d_gmap_off.p;
   V.subs = SP.d_subs.p; V.sub_meta = SP.d_sub_meta.p; V.subrow = SP.d_subrow.p; V.nsub = SP.nsub;
   V.subpair = SP.d_subpair.p; V.npair = SP.npair; V.sub_Loff = SP.d_sub_Loff.p;
   V.upper_max = sv->opt.smem_front_max;
@@ -1444,6 +1447,7 @@ struct PrunedLists {
 // sweep that leaves D^-1 out (partial solves).  pruned (forward only): the sweep takes those lists instead of SP's
 static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, bool fwd, bool apply_d = true,
                         const PrunedLists* pruned = nullptr) {
+  Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
   DevSolve V = sweep_view(sv, SP, W);
   if (pruned) { V.tasks = pruned->tf; V.ntasks_fwd = pruned->ntf; V.subpair = pruned->subpair; V.npair = pruned->npair; }
@@ -1462,13 +1466,13 @@ static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, 
     if (cnt <= 0) return;
     const int* lst = pruned ? pruned->direct + pruned->direct_off[l] : SP.d_direct[l]->p;
     const unsigned g = cdiv(cnt * nb, DF_THREADS / 32);
-    k_direct<<<g, DF_THREADS, 0, st>>>(sv->DS, sv->DN, V, M, lst, cnt, sv->solve_epoch, W.d_x.p, W.d_cbv.p);
+    k_direct<<<g, DF_THREADS, 0, st>>>(A.DS, A.DN, V, M, lst, cnt, A.solve_epoch, W.d_x.p, W.d_cbv.p);
     ++sv->launches;
   };
   if (fwd) for (int l = 0; l < nd; ++l) direct(l);
   if (nt > 0) {
     unsigned long long& ticket = fwd ? W.ticket_f : W.ticket_b;
-    k_sweep<<<grid, DF_THREADS, DF_DYN_SMEM, st>>>(sv->DS, sv->DN, V, M, sv->solve_epoch, ticket, W.d_x.p, W.d_cbv.p);
+    k_sweep<<<grid, DF_THREADS, DF_DYN_SMEM, st>>>(A.DS, A.DN, V, M, A.solve_epoch, ticket, W.d_x.p, W.d_cbv.p);
     ticket += (unsigned long long)nt + grid;
     ++sv->launches;
   }
@@ -1478,25 +1482,27 @@ static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, 
 }
 
 // The two stages every solve over the fronts of SP is built from, for nb <= W.width columns of leading dimension n.  Each
-// sweep waits on flags that its own fronts stamp with sv->solve_epoch, so each stage takes a new epoch: a flag left by
+// sweep waits on flags that its own fronts stamp with A.solve_epoch, so each stage takes a new epoch: a flag left by
 // an earlier sweep never matches it.  (Backward work waits only on backward flags, so a backward stage may follow a
 // forward one under a new epoch.)
 // forward: x = P^T S d_in, then the forward sweep; apply_d = false leaves D^-1 out (L only)
 static int forward(Solver* sv, const SolvePlan& SP, SweepState& W, const double* d_in, int nb, bool apply_d = true) {
+  Analysis& A = *sv->an;
   const int n = sv->n;
-  k_rhs_in<<<dim3(cdiv(n, 256), nb), 256, 0, sv->stream>>>(n, sv->d_perm.p, sv->d_scale.p, d_in, W.d_x.p, W.M.x);
+  k_rhs_in<<<dim3(cdiv(n, 256), nb), 256, 0, sv->stream>>>(n, A.d_perm.p, A.d_scale.p, d_in, W.d_x.p, W.M.x);
   ++sv->launches;
-  sv->solve_epoch++;
+  A.solve_epoch++;
   return launch_sweep(sv, SP, W, nb, true, apply_d);
 }
 
 // backward: the backward sweep, then d_out = S P x unless d_out is null
 static int backward(Solver* sv, const SolvePlan& SP, SweepState& W, double* d_out, int nb) {
-  sv->solve_epoch++;
+  Analysis& A = *sv->an;
+  A.solve_epoch++;
   const int rc = launch_sweep(sv, SP, W, nb, false);
   if (rc != B200LDLT_SUCCESS || !d_out) return rc;
   const int n = sv->n;
-  k_sol_out<<<dim3(cdiv(n, 256), nb), 256, 0, sv->stream>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, W.M.x, d_out);
+  k_sol_out<<<dim3(cdiv(n, 256), nb), 256, 0, sv->stream>>>(n, A.d_perm.p, A.d_scale.p, W.d_x.p, W.M.x, d_out);
   ++sv->launches;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
@@ -1520,7 +1526,8 @@ static int for_blocks(int nrhs, int cap, Block&& block) {
 // the front of job 4) applies D^-1 through the helper the fused sweep uses.  So job 3 . 2 . 1 and job 4 . 1 reproduce
 // job 0 bit for bit.  Launches: job 0: 2 + two sweeps; job 1, 3, 4: 2 + one sweep (the direct levels + 1); job 2: 1.
 static int enqueue_solve(Solver* sv, SweepState& W, int job, const double* d_in, double* d_out, int nb) {
-  const SolvePlan& SP = sv->fronts.solve;
+  Analysis& A = *sv->an;
+  const SolvePlan& SP = A.fronts.solve;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   const dim3 g(cdiv(n, 256), nb);
@@ -1532,14 +1539,14 @@ static int enqueue_solve(Solver* sv, SweepState& W, int job, const double* d_in,
   if (job == 1) {
     const int rc = forward(sv, SP, W, d_in, nb, false);
     if (rc != B200LDLT_SUCCESS) return rc;
-    k_piv_out<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb, d_out); ++sv->launches;
+    k_piv_out<<<g, 256, 0, st>>>(n, A.d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb, d_out); ++sv->launches;
   } else if (job == 2) {
     // (through the sweep state's x: d_in and d_out may be the same array, and k_dinv reads partners from its input)
-    k_dinv<<<g, 256, 0, st>>>(n, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, d_in, nullptr, W.d_x.p, n, nullptr, 0); ++sv->launches;
+    k_dinv<<<g, 256, 0, st>>>(n, A.d_ptype.p, A.d_dinv.p, A.d_doff.p, d_in, nullptr, W.d_x.p, n, nullptr, 0); ++sv->launches;
     CU(cudaMemcpyAsync(d_out, W.d_x.p, (size_t)n * nb * sizeof(double), cudaMemcpyDeviceToDevice, st));
   } else {
-    if (job == 3) k_piv_in<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, d_in, W.d_x.p, ldx, W.d_bigv.p, ldb);
-    else k_dinv<<<g, 256, 0, st>>>(n, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, d_in, sv->d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb);
+    if (job == 3) k_piv_in<<<g, 256, 0, st>>>(n, A.d_piv_big.p, d_in, W.d_x.p, ldx, W.d_bigv.p, ldb);
+    else k_dinv<<<g, 256, 0, st>>>(n, A.d_ptype.p, A.d_dinv.p, A.d_doff.p, d_in, A.d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb);
     ++sv->launches;
     return backward(sv, SP, W, d_out, nb);
   }
@@ -1551,20 +1558,21 @@ static int enqueue_solve(Solver* sv, SweepState& W, int job, const double* d_in,
 // solve, before that solve's timing starts.  Returns false (and the columns are then solved one by one, as with
 // B200_SOLVE_BLOCK=1) when the device memory for it cannot be had.
 static bool block_solve_state(Solver* sv) {
-  if (sv->blk) return sv->blk->width > 1;
+  Analysis& A = *sv->an;
+  if (A.blk) return A.blk->width > 1;
   const int nb = sv->dbg.solve_block;
-  sv->blk.reset(new SweepState());   // width 0: not retried before the next analysis
+  A.blk.reset(new SweepState());   // width 0: not retried before the next analysis
   if (nb < 2) return false;
-  SweepState& B = *sv->blk;
-  MultiStride M = sv->sweep.M;
+  SweepState& B = *A.blk;
+  MultiStride M = A.sweep.M;
   M.nb = nb;
-  M.nccnt = (int)sv->fronts.solve.d_ccnt.n;
-  M.part = (long long)sv->fronts.solve.d_part.n;
+  M.nccnt = (int)A.fronts.solve.d_ccnt.n;
+  M.part = (long long)A.fronts.solve.d_part.n;
   const cudaError_t e = alloc_sweep_state(sv, B, M);
   if (e != cudaSuccess) {
     if (sv->opt.verbose) fprintf(stderr, "[b200ldlt] blocked solve unavailable (%s): one solve per column\n", cudaGetErrorString(e));
     cudaGetLastError();
-    sv->blk.reset(new SweepState());
+    A.blk.reset(new SweepState());
     return false;
   }
   if (sv->opt.verbose)
@@ -1579,9 +1587,10 @@ static bool block_solve_state(Solver* sv) {
 // state, single columns through the one-column state.  `blocked`: the result of block_solve_state, called by the entry
 // point before its timing starts.  job: as in enqueue_solve.
 static int enqueue_solve_columns(Solver* sv, double* d_rhs, int nrhs, bool blocked, int job = 0) {
-  return for_blocks(nrhs, blocked ? sv->blk->width : 1, [&](int c, int w) {
+  Analysis& A = *sv->an;
+  return for_blocks(nrhs, blocked ? A.blk->width : 1, [&](int c, int w) {
     double* col = d_rhs + (size_t)c * sv->n;
-    return enqueue_solve(sv, w == 1 ? sv->sweep : *sv->blk, job, col, col, w);
+    return enqueue_solve(sv, w == 1 ? A.sweep : *A.blk, job, col, col, w);
   });
 }
 
@@ -1591,34 +1600,35 @@ static int enqueue_solve_columns(Solver* sv, double* d_rhs, int nrhs, bool block
 // job 1, then job 4 with D^+ (= job 0 with D^+, bit for bit); f_i runs job 3 on z_i.
 //   blocked (a state of width >= 2): blocks of w <= width / 2 columns, x and f through ONE backward sweep of 2w columns:
 //     k_rhs_in, forward sweep without D, k_fred, backward sweep, k_fred_out -- 5 + 2 D launches per block;
-//   otherwise column by column in the single-column state, z parked in sv->d_fred_z, two backward sweeps: k_rhs_in,
+//   otherwise column by column in the single-column state, z parked in A.d_fred_z, two backward sweeps: k_rhs_in,
 //     forward, k_fred, backward, k_sol_out, k_piv_in, backward, k_sol_out -- 8 + 3 D launches per column.
 // Every column runs the arithmetic of a single-column call.
 static int enqueue_fredholm(Solver* sv, double* d_x, int nrhs, bool blocked) {
+  Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   CU(cudaMemsetAsync(sv->d_fred_nrm.p, 0, 2 * (size_t)nrhs * sizeof(unsigned long long), st));
-  const SolvePlan& SP = sv->fronts.solve;
-  SweepState& W = blocked ? *sv->blk : sv->sweep;
+  const SolvePlan& SP = A.fronts.solve;
+  SweepState& W = blocked ? *A.blk : A.sweep;
   const long long ldx = W.M.x, ldb = W.M.bigv;
   const int rc = for_blocks(nrhs, blocked ? W.width / 2 : 1, [&](int c, int w) -> int {
     double* col = d_x + (size_t)c * n;
     const dim3 g(cdiv(n, 256), w);
     int rc2 = forward(sv, SP, W, col, w, false);
     if (rc2 != B200LDLT_SUCCESS) return rc2;
-    k_fred<<<g, 256, 0, st>>>(n, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, sv->d_zflag.p, sv->d_piv_big.p, W.d_x.p, ldx,
-                              W.d_bigv.p, ldb, w, blocked ? nullptr : sv->d_fred_z.p, sv->d_fred_nrm.p + 2 * (size_t)c);
+    k_fred<<<g, 256, 0, st>>>(n, A.d_ptype.p, A.d_dinv.p, A.d_doff.p, A.d_zflag.p, A.d_piv_big.p, W.d_x.p, ldx,
+                              W.d_bigv.p, ldb, w, blocked ? nullptr : A.d_fred_z.p, sv->d_fred_nrm.p + 2 * (size_t)c);
     ++sv->launches;
     if (blocked) {
       rc2 = backward(sv, SP, W, nullptr, 2 * w);
       if (rc2 != B200LDLT_SUCCESS) return rc2;
-      k_fred_out<<<dim3(cdiv(n, 256), 2 * w), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, W.d_x.p, ldx, col, w, nrhs);
+      k_fred_out<<<dim3(cdiv(n, 256), 2 * w), 256, 0, st>>>(n, A.d_perm.p, A.d_scale.p, W.d_x.p, ldx, col, w, nrhs);
       ++sv->launches;
       return B200LDLT_SUCCESS;
     }
     rc2 = backward(sv, SP, W, col, 1);
     if (rc2 != B200LDLT_SUCCESS) return rc2;
-    k_piv_in<<<g, 256, 0, st>>>(n, sv->d_piv_big.p, sv->d_fred_z.p, W.d_x.p, ldx, W.d_bigv.p, ldb); ++sv->launches;
+    k_piv_in<<<g, 256, 0, st>>>(n, A.d_piv_big.p, A.d_fred_z.p, W.d_x.p, ldx, W.d_bigv.p, ldb); ++sv->launches;
     return backward(sv, SP, W, d_x + (size_t)(nrhs + c) * n, 1);
   });
   if (rc != B200LDLT_SUCCESS) return rc;
@@ -1632,7 +1642,7 @@ static int enqueue_fredholm(Solver* sv, double* d_x, int nrhs, bool blocked) {
 // contribution rows equal to q of its descendants (desc, by q: fronts ascending, then chunks).  All of it depends on the
 // analysis only.
 static int build_lmul_plan(Solver* sv, LmulPlan& M) {
-  const Symbolic& S = sv->S;
+  const Symbolic& S = sv->an->S;
   const int n = sv->n;
   cudaStream_t st = sv->stream;
   std::vector<LmulItem> itn;
@@ -1680,13 +1690,14 @@ static int build_lmul_plan(Solver* sv, LmulPlan& M) {
 // the multiply's state for calls of nrhs columns (before the call's timing starts): the map at the first call after an
 // analysis, the scratch for the widest block the call uses
 static int lmul_state(Solver* sv, int nrhs) {
-  if (!sv->lmul) {
+  Analysis& A = *sv->an;
+  if (!A.lmul) {
     std::unique_ptr<LmulPlan> M(new LmulPlan());
     const int rc = build_lmul_plan(sv, *M);
     if (rc != B200LDLT_SUCCESS) return rc;
-    sv->lmul = std::move(M);
+    A.lmul = std::move(M);
   }
-  LmulPlan& M = *sv->lmul;
+  LmulPlan& M = *A.lmul;
   const int w = std::min(nrhs, sv->dbg.solve_block);
   if (w > M.width) {
     M.width = 0;
@@ -1703,19 +1714,20 @@ static int enqueue_lmul(Solver* sv, int trans, const double* d_x, double* d_y, i
   static_assert(MS_NB_MAX == 8, "one instantiation per block width");
   static const KN kn[8] = {k_lmul_n<1>, k_lmul_n<2>, k_lmul_n<3>, k_lmul_n<4>, k_lmul_n<5>, k_lmul_n<6>, k_lmul_n<7>, k_lmul_n<8>};
   static const KT kt[8] = {k_lmul_t<1>, k_lmul_t<2>, k_lmul_t<3>, k_lmul_t<4>, k_lmul_t<5>, k_lmul_t<6>, k_lmul_t<7>, k_lmul_t<8>};
-  const LmulPlan& M = *sv->lmul;
+  const Analysis& A = *sv->an;
+  const LmulPlan& M = *A.lmul;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   const dim3 g(cdiv(n, 256), nb);
   if (trans == 0) {
     const int ni = (int)M.d_items_n.n;
-    kn[nb - 1]<<<cdiv(ni, 8), 256, 0, st>>>(sv->d_fdesc.p, sv->d_L.p, M.d_items_n.p, ni, d_x, n, M.d_scr.p, M.ld);
-    k_lmul_gather<<<g, 256, 0, st>>>(n, M.d_pcol0.p, sv->d_lperm.p, M.d_own_ptr.p, M.d_own.p, M.d_desc_ptr.p, M.d_desc.p,
-                                     sv->d_perm.p, sv->d_scale.p, M.d_scr.p, M.ld, d_y);
+    kn[nb - 1]<<<cdiv(ni, 8), 256, 0, st>>>(A.d_fdesc.p, A.d_L.p, M.d_items_n.p, ni, d_x, n, M.d_scr.p, M.ld);
+    k_lmul_gather<<<g, 256, 0, st>>>(n, M.d_pcol0.p, A.d_lperm.p, M.d_own_ptr.p, M.d_own.p, M.d_desc_ptr.p, M.d_desc.p,
+                                     A.d_perm.p, A.d_scale.p, M.d_scr.p, M.ld, d_y);
   } else {
     const int ni = (int)M.d_items_t.n;
-    k_lmul_in<<<g, 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, d_x, M.d_scr.p);
-    kt[nb - 1]<<<cdiv(ni, 8), 256, 0, st>>>(sv->d_fdesc.p, sv->d_L.p, M.d_items_t.p, ni, sv->d_lperm.p, sv->d_rows.p,
+    k_lmul_in<<<g, 256, 0, st>>>(n, A.d_perm.p, A.d_scale.p, d_x, M.d_scr.p);
+    kt[nb - 1]<<<cdiv(ni, 8), 256, 0, st>>>(A.d_fdesc.p, A.d_L.p, M.d_items_t.p, ni, A.d_lperm.p, A.d_rows.p,
                                             M.d_scr.p, n, d_y);
   }
   sv->launches += 2;
@@ -1725,7 +1737,7 @@ static int enqueue_lmul(Solver* sv, int trans, const double* d_x, double* d_y, i
 
 // nrhs columns in blocks of up to B200_SOLVE_BLOCK (lmul_state called before)
 static int enqueue_lmul_columns(Solver* sv, int trans, int nrhs, const double* d_x, double* d_y) {
-  return for_blocks(nrhs, sv->lmul->width, [&](int c, int w) {
+  return for_blocks(nrhs, sv->an->lmul->width, [&](int c, int w) {
     return enqueue_lmul(sv, trans, d_x + (size_t)c * sv->n, d_y + (size_t)c * sv->n, w);
   });
 }
@@ -1734,9 +1746,10 @@ static int enqueue_lmul_columns(Solver* sv, int trans, int nrhs, const double* d
 // The per-front indices into the host copies of the handle's forward lists (SparseFwdPlan): at the first sparse call
 // after an analysis, before its timing starts.
 static int sfs_state(Solver* sv) {
-  if (sv->sfs) return B200LDLT_SUCCESS;
-  const Symbolic& S = sv->S;
-  const SolvePlan& SP = sv->fronts.solve;
+  Analysis& A = *sv->an;
+  if (A.sfs) return B200LDLT_SUCCESS;
+  const Symbolic& S = A.S;
+  const SolvePlan& SP = A.fronts.solve;
   const int n = sv->n, nsn = S.nsn;
   std::unique_ptr<SparseFwdPlan> P(new SparseFwdPlan());
   P->dlev.assign(nsn, -1); P->didx.assign(nsn, -1); P->item_of.assign(nsn, -1); P->sub_of.assign(nsn, -1);
@@ -1783,7 +1796,7 @@ static int sfs_state(Solver* sv) {
   CU(cudaHostAlloc((void**)&P->h_buf, cap, cudaHostAllocDefault));
   CU(P->d_buf.alloc(cap));
   CU(cudaEventCreateWithFlags(&P->ev_staged, cudaEventDisableTiming));
-  sv->sfs = std::move(P);
+  A.sfs = std::move(P);
   return B200LDLT_SUCCESS;
 }
 
@@ -1806,9 +1819,10 @@ static inline size_t align8(size_t b) { return (b + 7) & ~(size_t)7; }
 // the device needs goes to the pinned staging (b too when b_host).  FATAL_ERROR with a message, nothing written to the
 // caller and nothing launched, for a bad pattern or a failed check.
 static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_host, SfsCall& C) {
-  SparseFwdPlan& P = *sv->sfs;
-  const SolvePlan& SP = sv->fronts.solve;
-  const Symbolic& S = sv->S;
+  Analysis& A = *sv->an;
+  SparseFwdPlan& P = *A.sfs;
+  const SolvePlan& SP = A.fronts.solve;
+  const Symbolic& S = A.S;
   const int n = sv->n;
   const int nd = (int)SP.direct_cnt.size();
   const unsigned m = ++P.stamp;
@@ -1944,21 +1958,22 @@ static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_h
 // forward sweep of job 1 over the pruned lists, the reached positions out (k_sfs_out).  Launches: 2 + the direct levels
 // that hold a front of the run set + 1 when the run set has a front outside them.
 static int sfs_enqueue(Solver* sv, const SfsCall& C, const double* d_b, double* d_out) {
-  SparseFwdPlan& P = *sv->sfs;
+  Analysis& A = *sv->an;
+  SparseFwdPlan& P = *A.sfs;
   cudaStream_t st = sv->stream;
-  SweepState& W = sv->sweep;
+  SweepState& W = A.sweep;
   const char* d = P.d_buf.p;
   CU(cudaMemcpyAsync(P.d_buf.p, P.h_buf, C.staged, cudaMemcpyHostToDevice, st));
   CU(cudaEventRecord(P.ev_staged, st));
-  sv->solve_epoch++;
+  A.solve_epoch++;
   k_sfs_in<<<cdiv(C.ncol, 256) + C.nfr, 256, 0, st>>>(C.ncol, reinterpret_cast<const int*>(d + C.o_pos),
-                                                      reinterpret_cast<const int*>(d + C.o_bi), sv->d_perm.p, sv->d_scale.p, d_b,
-                                                      W.d_x.p, reinterpret_cast<const int*>(d + C.o_fr), sv->d_rows_ptr.p,
-                                                      W.d_cbv.p, W.d_done_f.p, sv->solve_epoch);
+                                                      reinterpret_cast<const int*>(d + C.o_bi), A.d_perm.p, A.d_scale.p, d_b,
+                                                      W.d_x.p, reinterpret_cast<const int*>(d + C.o_fr), A.d_rows_ptr.p,
+                                                      W.d_cbv.p, W.d_done_f.p, A.solve_epoch);
   ++sv->launches;
-  const int rc = launch_sweep(sv, sv->fronts.solve, W, 1, true, false, &C.pl);
+  const int rc = launch_sweep(sv, A.fronts.solve, W, 1, true, false, &C.pl);
   if (rc != B200LDLT_SUCCESS) return rc;
-  k_sfs_out<<<cdiv(C.nxi, 256), 256, 0, st>>>(C.nxi, reinterpret_cast<const int*>(d + C.o_xi), sv->d_piv_big.p, W.d_x.p,
+  k_sfs_out<<<cdiv(C.nxi, 256), 256, 0, st>>>(C.nxi, reinterpret_cast<const int*>(d + C.o_xi), A.d_piv_big.p, W.d_x.p,
                                              W.d_bigv.p, d_out);
   ++sv->launches;
   CU(cudaGetLastError());
@@ -1966,9 +1981,10 @@ static int sfs_enqueue(Solver* sv, const SfsCall& C, const double* d_b, double* 
 }
 
 static int shard_setup(Solver* sv, int rank, int world) {
-  Symbolic& S = sv->S;
+  Analysis& A = *sv->an;
+  Symbolic& S = A.S;
   cudaStream_t st = sv->stream;
-  Solver::Shard& H = sv->shard;
+  Analysis::Shard& H = A.shard;
   H.rank = rank; H.world = world;
   H.nsub = shard_plan(S, world, H.owner);
   H.cut_roots.clear(); H.top_fronts.clear();
@@ -1984,7 +2000,7 @@ static int shard_setup(Solver* sv, int rank, int world) {
     }
   }
   for (int ph = 0; ph < 2; ++ph) {
-    const int rc = build_front_plan(sv, take[ph], take[ph], H.part[ph]);
+    const int rc = build_front_plan(sv, A, take[ph], take[ph], H.part[ph]);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   if (mark_cut.empty()) mark_cut.push_back(0), H.d_mark_cut.n = 0;
@@ -2093,10 +2109,11 @@ int b200ldlt_analyse(b200ldlt_handle h, int dim, int nonzeros, const int* irn, c
   if (sv->h_vals) { cudaFreeHost(sv->h_vals); sv->h_vals = nullptr; }
   CU(cudaHostAlloc((void**)&sv->h_vals, std::max<size_t>(nonzeros, 1) * sizeof(double), cudaHostAllocDefault));
   memset(sv->h_vals, 0, std::max<size_t>(nonzeros, 1) * sizeof(double));
-  sv->analysed = false; sv->factored = false; sv->have_dev_vals = false;
+  sv->an.reset();
+  sv->d_vals.release();
+  sv->have_dev_vals = false;
   sv->sc_vars.clear();                // (a new pattern makes the Schur indices meaningless)
   if (sv->amat) { b200vec_tmat_destroy(sv->amat); sv->amat = nullptr; }
-  sv->drop_staging();
   return B200LDLT_SUCCESS;
 }
 
@@ -2134,10 +2151,10 @@ namespace b200 {
 // The state check, after the call's own argument checks: FATAL_ERROR with "<call>: ..." in last_error without factors
 // and, unless sharded_ok, on a sharded handle; otherwise the handle's device is selected for what follows.
 static int factors_state(Solver* sv, const char* call, bool sharded_ok = false, bool schur_call = false) {
-  if (!sv->factored)
+  if (!sv->an || !sv->an->factored)
     sv->err = std::string(call) + ": no factors (factorise first; a SINGULAR factorisation keeps them only in keep mode, "
                                   "see b200ldlt_set_singular_action)";
-  else if (sv->shard.active && !sharded_ok) sv->err = std::string(call) + ": not available on a sharded handle";
+  else if (sv->an->shard.active && !sharded_ok) sv->err = std::string(call) + ": not available on a sharded handle";
   else if (sv->sc_vars.empty() == schur_call)   // the Schur calls need Schur-mode factors, the others refuse them
     sv->err = std::string(call) + (schur_call ? ": not in Schur mode" : ": Schur mode");
   else { CU(cudaSetDevice(sv->dev)); return B200LDLT_SUCCESS; }
@@ -2176,15 +2193,18 @@ static int timed_call(Solver* sv, Enqueue&& enqueue, Drain&& drain = Drain()) {
 // next analysis.
 template <class Enqueue>
 static int staged_call(Solver* sv, const double* in, size_t nin, double* out, size_t nout, Enqueue&& enqueue) {
+  Analysis& A = *sv->an;
   const size_t need = std::max(nin, nout);
-  if (need > sv->d_rhs.n) {
-    sv->drop_staging();
-    CU(cudaHostAlloc((void**)&sv->h_rhs, need * sizeof(double), cudaHostAllocDefault));
-    CU(sv->d_rhs.alloc(need));   // (so d_rhs.n counts the doubles of both buffers, 0 when either is missing)
+  if (need > A.d_rhs.n) {
+    A.d_rhs.release();
+    if (A.h_rhs) cudaFreeHost(A.h_rhs);
+    A.h_rhs = nullptr;
+    CU(cudaHostAlloc((void**)&A.h_rhs, need * sizeof(double), cudaHostAllocDefault));
+    CU(A.d_rhs.alloc(need));   // (so d_rhs.n counts the doubles of both buffers, 0 when either is missing)
   }
   cudaStream_t st = sv->stream;
-  double* h = sv->h_rhs;
-  double* d = sv->d_rhs.p;
+  double* h = A.h_rhs;
+  double* d = A.d_rhs.p;
   auto chunk = [](size_t total) { return std::max<size_t>((total + 3) / 4, 32768); };   // at most 4: ev_chunk
   const size_t ci = chunk(nin), co = chunk(nout);
   auto copy_out = [&]() -> int {
@@ -2245,7 +2265,7 @@ static int sparse_fwd(Solver* sv, int nbi, const int* bindex, const double* b, b
   { const int rc = sfs_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
   SfsCall C;
   { const int rc = sfs_prepare(sv, nbi, bindex, host ? b : nullptr, C); if (rc != B200LDLT_SUCCESS) return rc; }
-  SparseFwdPlan& P = *sv->sfs;
+  SparseFwdPlan& P = *sv->an->sfs;
   const double* d_b = host ? reinterpret_cast<const double*>(P.d_buf.p + C.o_b) : b;
   double* d_x = host ? reinterpret_cast<double*>(P.d_buf.p + C.o_x) : x;
   const int rc = timed_call(sv, [&]() -> int {
@@ -2267,12 +2287,13 @@ static int fredholm(Solver* sv, int nrhs, double tol, double* x, int* consistent
   if (bad) { sv->err = std::string("solve_fredholm: ") + bad; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "solve_fredholm"); if (rc != B200LDLT_SUCCESS) return rc; }
   if (nrhs == 0) return no_columns(sv);
+  Analysis& A = *sv->an;
   const size_t n = sv->n, nb = n * nrhs;
   // no zero pivots: the solve itself, f = 0, every column consistent
-  const bool zero_pivots = !sv->zpos.empty();
+  const bool zero_pivots = !A.zpos.empty();
   const bool blocked = (zero_pivots || nrhs > 1) && block_solve_state(sv);
   if (zero_pivots && sv->d_fred_nrm.n < 2 * (size_t)nrhs) CU(sv->d_fred_nrm.alloc(2 * (size_t)nrhs));
-  if (zero_pivots && !blocked && sv->d_fred_z.n != n) CU(sv->d_fred_z.alloc(n));
+  if (zero_pivots && !blocked && A.d_fred_z.n != n) CU(A.d_fred_z.alloc(n));
   std::vector<unsigned long long> nrm(2 * (size_t)nrhs);
   auto enqueue = [&](double* d) -> int {
     if (!zero_pivots) {
@@ -2302,22 +2323,23 @@ static int fredholm(Solver* sv, int nrhs, double tol, double* x, int* consistent
 // backward sweep, which passes the root's values through.  Blocks of up to B200_SOLVE_BLOCK columns (blocked: the result
 // of block_solve_state), each column with the arithmetic of a single-column call.  d_out may be d_b.
 static int enqueue_sc_columns(Solver* sv, int nrhs, const double* d_b, const double* d_xs, double* d_out, bool blocked) {
+  Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
-  const SolvePlan& SP = sv->fronts.solve;
+  const SolvePlan& SP = A.fronts.solve;
   const int n = sv->n, m = (int)sv->sc_vars.size();
-  const int rc = for_blocks(nrhs, blocked ? sv->blk->width : 1, [&](int c, int w) -> int {
-    SweepState& W = w == 1 ? sv->sweep : *sv->blk;
+  const int rc = for_blocks(nrhs, blocked ? A.blk->width : 1, [&](int c, int w) -> int {
+    SweepState& W = w == 1 ? A.sweep : *A.blk;
     const long long ldx = W.M.x, ldb = W.M.bigv;
     const int rc2 = forward(sv, SP, W, d_b + (size_t)c * n, w, false);
     if (rc2 != B200LDLT_SUCCESS) return rc2;
     if (!d_xs) {
-      k_sc_reduce<<<dim3(cdiv(m, 256), w), 256, 0, st>>>(m, n - m, sv->d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb,
-                                                         sv->d_sc_vars.p, sv->d_scale.p, d_out + (size_t)c * m);
+      k_sc_reduce<<<dim3(cdiv(m, 256), w), 256, 0, st>>>(m, n - m, A.d_piv_big.p, W.d_x.p, ldx, W.d_bigv.p, ldb,
+                                                         A.d_sc_vars.p, A.d_scale.p, d_out + (size_t)c * m);
       ++sv->launches;
       return B200LDLT_SUCCESS;
     }
-    k_sc_expand<<<dim3(cdiv(n, 256), w), 256, 0, st>>>(n, m, sv->d_ptype.p, sv->d_dinv.p, sv->d_doff.p, sv->d_piv_big.p,
-                                                      W.d_x.p, ldx, W.d_bigv.p, ldb, sv->d_sc_vars.p, sv->d_scale.p,
+    k_sc_expand<<<dim3(cdiv(n, 256), w), 256, 0, st>>>(n, m, A.d_ptype.p, A.d_dinv.p, A.d_doff.p, A.d_piv_big.p,
+                                                      W.d_x.p, ldx, W.d_bigv.p, ldb, A.d_sc_vars.p, A.d_scale.p,
                                                       d_xs + (size_t)c * m);
     ++sv->launches;
     return backward(sv, SP, W, d_out + (size_t)c * n, w);
@@ -2331,9 +2353,10 @@ static int enqueue_sc_columns(Solver* sv, int nrhs, const double* d_b, const dou
 static int schur_complement(Solver* sv, double* sc, bool host) {
   if (!sc) { sv->err = "schur_complement: NULL argument"; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "schur_complement", false, true); if (rc != B200LDLT_SUCCESS) return rc; }
-  const size_t mm = sv->d_sc.n;
+  const Analysis& A = *sv->an;
+  const size_t mm = A.d_sc.n;
   auto enqueue = [&](double* d) -> int {
-    CU(cudaMemcpyAsync(d, sv->d_sc.p, mm * sizeof(double), cudaMemcpyDeviceToDevice, sv->stream));
+    CU(cudaMemcpyAsync(d, A.d_sc.p, mm * sizeof(double), cudaMemcpyDeviceToDevice, sv->stream));
     return B200LDLT_SUCCESS;
   };
   return host ? staged_call(sv, nullptr, 0, sc, mm, enqueue) : timed_call(sv, [&] { return enqueue(sc); });
@@ -2361,8 +2384,9 @@ static int schur_solve(Solver* sv, const char* call, int nrhs, const double* b, 
 static_assert(SI_MID == DF_MIDMAX && SI_MID == kSolveMidMax, "the fronts above SI_MID read the factorisation's L11^-1");
 
 static int selinv_state(Solver* sv) {
-  if (sv->selinv) return B200LDLT_SUCCESS;
-  const Symbolic& S = sv->S;
+  Analysis& A = *sv->an;
+  if (A.selinv) return B200LDLT_SUCCESS;
+  const Symbolic& S = A.S;
   const int n = S.n, nsn = S.nsn;
   cudaStream_t st = sv->stream;
   std::unique_ptr<SelInvPlan> P(new SelInvPlan());
@@ -2403,7 +2427,7 @@ static int selinv_state(Solver* sv) {
         if (S.f(s) <= SI_SMALL) continue;
         const bool big = S.f(s) > SI_MID;
         const int ld_e = big ? (k + DF_BLK - 1) / DF_BLK * DF_BLK : k;
-        const double* E = big ? sv->d_linv.p + sv->linv_off[s] : P->d_E.p + eoff[s];
+        const double* E = big ? A.d_linv.p + A.linv_off[s] : P->d_E.p + eoff[s];
         const int nkb = (k + 63) / 64, nrb = (r + 63) / 64;
         if (pass < 2) {
           for (int ib = 0; ib < nrb; ++ib)
@@ -2439,30 +2463,31 @@ static int selinv_state(Solver* sv) {
   if (sv->opt.verbose)
     fprintf(stderr, "[b200ldlt] selected inversion: %zu tile items, Z %.1f MB, L11^-1 (orders %d..%d) %.1f MB\n",
             items.size(), 8e-6 * (double)S.L_off[nsn], SI_SMALL + 1, SI_MID, 8e-6 * (double)etot);
-  sv->selinv = std::move(P);
+  A.selinv = std::move(P);
   return B200LDLT_SUCCESS;
 }
 
 // top level first: per level gather, small fronts, L11^-1 of the middle fronts, the three tile passes; then the output
 static int enqueue_selinv(Solver* sv, double* d_diag, double* d_vals) {
-  const SelInvPlan& P = *sv->selinv;
-  const Symbolic& S = sv->S;
+  const Analysis& A = *sv->an;
+  const SelInvPlan& P = *A.selinv;
+  const Symbolic& S = A.S;
   cudaStream_t st = sv->stream;
   const int n = S.n;
   int& L = sv->launches;
-  k_si_prep<<<cdiv(n, 256), 256, 0, st>>>(n, P.d_sn_of.p, sv->d_sn_start.p, sv->d_lperm.p, P.d_lpinv.p); ++L;
+  k_si_prep<<<cdiv(n, 256), 256, 0, st>>>(n, P.d_sn_of.p, A.d_sn_start.p, A.d_lperm.p, P.d_lpinv.p); ++L;
   for (int l = S.nlevels - 1; l >= 0; --l) {
     const SelInvPlan::Level& V = P.lev[l];
-    if (V.g_cnt) { k_si_gather<<<cdiv(V.g_cnt, 8), 256, 0, st>>>(sv->DS, P.d_Z.p, sv->d_CB.p, P.d_lpinv.p, P.d_gather.p + V.g_off, V.g_cnt); ++L; }
-    if (V.s_cnt) { k_si_small<<<V.s_cnt, 128, V.smem, st>>>(sv->DS, sv->DN, P.d_Z.p, P.d_fronts.p + V.s_off); ++L; }
-    if (V.m_cnt) { k_si_linv<<<V.m_cnt, 256, 0, st>>>(sv->DS, sv->DN, P.d_fronts.p + V.m_off, P.d_eoff.p, P.d_E.p); ++L; }
-    if (V.t_cnt[0]) { k_si_tile<0><<<V.t_cnt[0], 256, 0, st>>>(sv->DS, sv->DN, P.d_Z.p, P.d_items.p + V.t_off[0]); ++L; }
-    if (V.t_cnt[1]) { k_si_tile<1><<<V.t_cnt[1], 256, 0, st>>>(sv->DS, sv->DN, P.d_Z.p, P.d_items.p + V.t_off[1]); ++L; }
-    if (V.t_cnt[2]) { k_si_tile<2><<<V.t_cnt[2], 256, 0, st>>>(sv->DS, sv->DN, P.d_Z.p, P.d_items.p + V.t_off[2]); ++L; }
+    if (V.g_cnt) { k_si_gather<<<cdiv(V.g_cnt, 8), 256, 0, st>>>(A.DS, P.d_Z.p, A.d_CB.p, P.d_lpinv.p, P.d_gather.p + V.g_off, V.g_cnt); ++L; }
+    if (V.s_cnt) { k_si_small<<<V.s_cnt, 128, V.smem, st>>>(A.DS, A.DN, P.d_Z.p, P.d_fronts.p + V.s_off); ++L; }
+    if (V.m_cnt) { k_si_linv<<<V.m_cnt, 256, 0, st>>>(A.DS, A.DN, P.d_fronts.p + V.m_off, P.d_eoff.p, P.d_E.p); ++L; }
+    if (V.t_cnt[0]) { k_si_tile<0><<<V.t_cnt[0], 256, 0, st>>>(A.DS, A.DN, P.d_Z.p, P.d_items.p + V.t_off[0]); ++L; }
+    if (V.t_cnt[1]) { k_si_tile<1><<<V.t_cnt[1], 256, 0, st>>>(A.DS, A.DN, P.d_Z.p, P.d_items.p + V.t_off[1]); ++L; }
+    if (V.t_cnt[2]) { k_si_tile<2><<<V.t_cnt[2], 256, 0, st>>>(A.DS, A.DN, P.d_Z.p, P.d_items.p + V.t_off[2]); ++L; }
   }
   k_si_out<<<cdiv(std::max<long long>(n, sv->nnz), 256), 256, 0, st>>>(
-      n, sv->nnz, P.d_iperm.p, P.d_sn_of.p, sv->d_sn_start.p, sv->d_rows_ptr.p, sv->d_L_off.p, P.d_lpinv.p, P.d_Z.p,
-      sv->d_scale.p, sv->d_irn.p, sv->d_jcn.p, P.d_t2u.p, sv->d_u_dst64.p, d_diag, d_vals);
+      n, sv->nnz, P.d_iperm.p, P.d_sn_of.p, A.d_sn_start.p, A.d_rows_ptr.p, A.d_L_off.p, P.d_lpinv.p, P.d_Z.p,
+      A.d_scale.p, A.d_irn.p, A.d_jcn.p, P.d_t2u.p, A.d_u_dst64.p, d_diag, d_vals);
   ++L;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
@@ -2473,7 +2498,7 @@ static int selected_inverse(Solver* sv, double* diag, double* vals, bool host) {
   if (!diag && !vals) { sv->err = "selected_inverse: diag and vals are both NULL"; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "selected_inverse"); if (rc != B200LDLT_SUCCESS) return rc; }
   { const int rc = selinv_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
-  SelInvPlan& P = *sv->selinv;
+  SelInvPlan& P = *sv->an->selinv;
   double* dd = diag ? (host ? P.d_diag.p : diag) : nullptr;
   double* dv = vals ? (host ? P.d_vals.p : vals) : nullptr;
   return timed_call(sv, [&]() -> int {
@@ -2489,10 +2514,11 @@ static int selected_inverse(Solver* sv, double* diag, double* vals, bool host) {
 // the unique entries by a counting sort on the column, then a stable one on the row, so each row's columns ascend --
 // and the buffers for nrhs right-hand sides and estimator blocks of `width` columns (0: no estimator), grown as needed.
 static int ea_state(Solver* sv, int nrhs, int width) {
+  Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
-  if (!sv->ea) {
-    const Symbolic& S = sv->S;
+  if (!A.ea) {
+    const Symbolic& S = A.S;
     std::unique_ptr<EaPlan> P(new EaPlan());
     std::vector<int> er, ec, eu;
     er.reserve(2 * S.nnz_u); ec.reserve(2 * S.nnz_u); eu.reserve(2 * S.nnz_u);
@@ -2519,9 +2545,9 @@ static int ea_state(Solver* sv, int nrhs, int width) {
     CU(P->d_cnt.alloc(MS_NB_MAX));
     CU(cudaMemsetAsync(P->d_cnt.p, 0, MS_NB_MAX * sizeof(unsigned), st));
     CU(cudaStreamSynchronize(st));
-    sv->ea = std::move(P);
+    A.ea = std::move(P);
   }
-  EaPlan& P = *sv->ea;
+  EaPlan& P = *A.ea;
   if (P.d_nrm.n < (size_t)EA_NRM * nrhs + 1) CU(P.d_nrm.alloc((size_t)EA_NRM * nrhs + 1));
   if (P.d_rs.n < (size_t)2 * n * nrhs) CU(P.d_rs.alloc((size_t)2 * n * nrhs));
   if (P.d_v.n < (size_t)n * width) { CU(P.d_v.alloc((size_t)n * width)); CU(P.d_xi.alloc((size_t)n * width)); }
@@ -2573,7 +2599,7 @@ static void ea_decide(EaEst& T, const EaRes& R, int n) {
 // not depend on the others of its block.
 static int run_estimators(Solver* sv, SweepState& W, EaEst* E, int ne) {
   static const int kMode[6] = {0, 0, 2, 1, 2, 3};   // the input of each jump: e/n, xi, e_j, xi, alternating
-  EaPlan& P = *sv->ea;
+  EaPlan& P = *sv->an->ea;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   for (;;) {
@@ -2604,12 +2630,13 @@ static int run_estimators(Solver* sv, SweepState& W, EaEst* E, int ne) {
 // k_sum_dups into the call's unique values, then the row pass for nrhs columns of d_b / d_x (nrhs = 0: only ||A|| and
 // the row maxima) into P.d_nrm, which is cleared first
 static int enqueue_ea_rows(Solver* sv, int nrhs, const double* d_b, const double* d_x) {
-  EaPlan& P = *sv->ea;
+  const Analysis& A = *sv->an;
+  EaPlan& P = *A.ea;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
-  const long long nu = sv->S.nnz_u;
+  const long long nu = A.S.nnz_u;
   CU(cudaMemsetAsync(P.d_nrm.p, 0, ((size_t)EA_NRM * nrhs + 1) * sizeof(unsigned long long), st));
-  k_sum_dups<<<cdiv(nu, 256), 256, 0, st>>>(nu, sv->d_useg_ptr.p, sv->d_useg_src.p, sv->d_vals.p, P.d_uval.p);
+  k_sum_dups<<<cdiv(nu, 256), 256, 0, st>>>(nu, A.d_useg_ptr.p, A.d_useg_src.p, sv->d_vals.p, P.d_uval.p);
   const unsigned g = std::min<unsigned>(cdiv(n, EA_WARPS), EA_ROW_CTAS);
   k_ea_rows<<<dim3(g, std::max(nrhs, 1)), EA_THREADS, 0, st>>>(n, nrhs, P.d_ptr.p, P.d_col.p, P.d_uid.p, P.d_uval.p, d_b,
                                                                d_x, P.d_rs.p, P.d_amax.p, P.d_nrm.p);
@@ -2628,14 +2655,15 @@ static int error_analysis(Solver* sv, int nrhs, const double* b, const double* x
   if (bad) { sv->err = std::string("error_analysis: ") + bad; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "error_analysis"); if (rc != B200LDLT_SUCCESS) return rc; }
   if (nrhs == 0) return no_columns(sv);
+  Analysis& A = *sv->an;
   const int n = sv->n;
   const size_t nb = (size_t)n * nrhs;
   // kept singular factors: M is no inverse of A, no estimator runs
-  const bool estimate = cond == 1 && sv->zpos.empty();
+  const bool estimate = cond == 1 && A.zpos.empty();
   const bool blocked = estimate && block_solve_state(sv);
-  SweepState& W = blocked ? *sv->blk : sv->sweep;
+  SweepState& W = blocked ? *A.blk : A.sweep;
   { const int rc = ea_state(sv, nrhs, estimate ? W.width : 0); if (rc != B200LDLT_SUCCESS) return rc; }
-  EaPlan& P = *sv->ea;
+  EaPlan& P = *A.ea;
   cudaStream_t st = sv->stream;
   std::vector<unsigned long long> nrm((size_t)EA_NRM * nrhs + 1);
   auto at = [&](int c, int k) { return ea_val(nrm[(size_t)EA_NRM * c + k]); };
@@ -2696,7 +2724,7 @@ static int error_analysis(Solver* sv, int nrhs, const double* b, const double* x
     o.nprod = nprod[c];
     if (cond == 0) {
       o.cond1 = o.cond2 = o.ferr = -1.0;
-    } else if (!sv->zpos.empty()) {
+    } else if (!A.zpos.empty()) {
       o.cond1 = o.cond2 = o.ferr = inf;
     } else if (o.xnorm == 0.0) {
       o.cond1 = o.cond2 = o.ferr = at(c, EA_B) == 0.0 ? 0.0 : inf;
@@ -2713,14 +2741,15 @@ static int error_analysis(Solver* sv, int nrhs, const double* b, const double* x
 static int condest(Solver* sv, double* kappa1, double* anorm1, double* ainv1, int* nprod) {
   if (!kappa1) { sv->err = "condest: NULL kappa1"; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "condest"); if (rc != B200LDLT_SUCCESS) return rc; }
-  const bool estimate = sv->zpos.empty();
+  Analysis& A = *sv->an;
+  const bool estimate = A.zpos.empty();
   { const int rc = ea_state(sv, 0, estimate ? 1 : 0); if (rc != B200LDLT_SUCCESS) return rc; }
   EaEst E;
   unsigned long long an = 0;
   const int rc = timed_call(sv, [&]() -> int {
     { const int rc2 = enqueue_ea_rows(sv, 0, nullptr, nullptr); if (rc2 != B200LDLT_SUCCESS) return rc2; }
-    if (estimate) { const int rc2 = run_estimators(sv, sv->sweep, &E, 1); if (rc2 != B200LDLT_SUCCESS) return rc2; }
-    CU(cudaMemcpyAsync(&an, sv->ea->d_nrm.p, sizeof(an), cudaMemcpyDeviceToHost, sv->stream));
+    if (estimate) { const int rc2 = run_estimators(sv, A.sweep, &E, 1); if (rc2 != B200LDLT_SUCCESS) return rc2; }
+    CU(cudaMemcpyAsync(&an, A.ea->d_nrm.p, sizeof(an), cudaMemcpyDeviceToHost, sv->stream));
     return B200LDLT_SUCCESS;
   });
   if (rc != B200LDLT_SUCCESS) return rc;
@@ -2763,16 +2792,17 @@ int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, d
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
   { const int rc = factors_state(sv, "enquire_indef", true); if (rc != B200LDLT_SUCCESS) return rc; }
+  const Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   std::vector<int> lperm(n), ptype(n);
   std::vector<double> dinv(n), doff(n);
-  CU(cudaMemcpyAsync(lperm.data(), sv->d_lperm.p, n * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(ptype.data(), sv->d_ptype.p, n * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(dinv.data(), sv->d_dinv.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(doff.data(), sv->d_doff.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(lperm.data(), A.d_lperm.p, n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(ptype.data(), A.d_ptype.p, n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(dinv.data(), A.d_dinv.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(doff.data(), A.d_doff.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  const Symbolic& S = sv->S;
+  const Symbolic& S = A.S;
   for (int s = 0; s < S.nsn; ++s)
     for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) {
       // pivot t of front s holds the front's local column lperm[p]: permuted column sn_start[s] + lperm[p]
@@ -2813,6 +2843,7 @@ int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2) {
   if (!sv) return B200LDLT_FATAL_ERROR;
   if (!dinv2) { sv->err = "alter_d: no entries"; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "alter_d"); if (rc != B200LDLT_SUCCESS) return rc; }
+  const Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
   if (sv->d_alter.n != 2 * (size_t)n) CU(sv->d_alter.alloc(2 * (size_t)n));
@@ -2820,8 +2851,8 @@ int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2) {
   int bad = 0;
   CU(cudaMemcpyAsync(sv->d_alter.p, dinv2, 2 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
   CU(cudaMemsetAsync(sv->d_alter_bad.p, 0, sizeof(int), st));
-  k_alter_check<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_ptype.p, sv->d_alter.p, sv->d_alter_bad.p);
-  k_alter<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_ptype.p, sv->d_alter.p, sv->d_alter_bad.p, sv->d_dinv.p, sv->d_doff.p);
+  k_alter_check<<<cdiv(n, 256), 256, 0, st>>>(n, A.d_ptype.p, sv->d_alter.p, sv->d_alter_bad.p);
+  k_alter<<<cdiv(n, 256), 256, 0, st>>>(n, A.d_ptype.p, sv->d_alter.p, sv->d_alter_bad.p, A.d_dinv.p, A.d_doff.p);
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(&bad, sv->d_alter_bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
@@ -2845,8 +2876,9 @@ int b200ldlt_enquire_zero_pivots(b200ldlt_handle h, int* nzero, int* pos) {
   if (!sv) return B200LDLT_FATAL_ERROR;
   if (!nzero) { sv->err = "enquire_zero_pivots: NULL nzero"; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "enquire_zero_pivots", true); if (rc != B200LDLT_SUCCESS) return rc; }
-  *nzero = (int)sv->zpos.size();
-  if (pos) std::copy(sv->zpos.begin(), sv->zpos.end(), pos);
+  const Analysis& A = *sv->an;
+  *nzero = (int)A.zpos.size();
+  if (pos) std::copy(A.zpos.begin(), A.zpos.end(), pos);
   return B200LDLT_SUCCESS;
 }
 
@@ -2897,7 +2929,7 @@ int b200ldlt_set_schur(b200ldlt_handle h, int m, const int* vars) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
   const char* bad = sv->n <= 0 ? "analyse first" : m < 0 ? "m must be >= 0" : m >= sv->n ? "m must be < n"
-                    : m > 0 && !vars ? "NULL vars" : sv->shard.active ? "not available on a sharded handle" : nullptr;
+                    : m > 0 && !vars ? "NULL vars" : sv->an && sv->an->shard.active ? "not available on a sharded handle" : nullptr;
   if (!bad) {
     std::vector<char> seen(sv->n, 0);
     for (int i = 0; i < m && !bad; ++i) {
@@ -2909,8 +2941,10 @@ int b200ldlt_set_schur(b200ldlt_handle h, int m, const int* vars) {
   if (bad) { sv->err = std::string("set_schur: ") + bad; return B200LDLT_FATAL_ERROR; }
   sv->sc_vars.assign(vars, vars + m);
   // the factors no longer match the mode; the next factor call re-analyses (the ordering places S last)
-  sv->factored = false;
-  if (sv->analysed) sv->reanalyse = true;
+  if (sv->an) {
+    sv->an->factored = false;
+    sv->reanalyse = true;
+  }
   return B200LDLT_SUCCESS;
 }
 
@@ -2957,7 +2991,7 @@ int b200ldlt_schur_expand_device(b200ldlt_handle h, int nrhs, const double* d_b,
  * the top part.  The solve mirrors it.  See ipopt_b200/sharded.py for the orchestration. */
 int b200ldlt_shard_setup(b200ldlt_handle h, int rank, int world) {
   Solver* sv = (Solver*)h;
-  if (!sv || !sv->analysed || world < 1 || rank < 0 || rank >= world) { if (sv) sv->err = "shard_setup: analyse first / bad rank"; return B200LDLT_FATAL_ERROR; }
+  if (!sv || !sv->an || world < 1 || rank < 0 || rank >= world) { if (sv) sv->err = "shard_setup: analyse first / bad rank"; return B200LDLT_FATAL_ERROR; }
   if (!sv->sc_vars.empty()) { sv->err = "shard_setup: Schur mode"; return B200LDLT_FATAL_ERROR; }
   CU(cudaSetDevice(sv->dev));
   return shard_setup(sv, rank, world);
@@ -2965,8 +2999,8 @@ int b200ldlt_shard_setup(b200ldlt_handle h, int rank, int world) {
 
 int64_t b200ldlt_shard_array(b200ldlt_handle h, const char* name, int64_t* out, int64_t cap) {
   Solver* sv = (Solver*)h;
-  if (!sv || !sv->shard.active || !name) return -1;
-  const Solver::Shard& H = sv->shard;
+  if (!sv || !sv->an || !sv->an->shard.active || !name) return -1;
+  const Analysis::Shard& H = sv->an->shard;
   std::string nm(name);
   const std::vector<int>* v = nullptr;
   if (nm == "owner") v = &H.owner;
@@ -2981,13 +3015,14 @@ void* b200ldlt_device_ptr(b200ldlt_handle h, const char* name) {
   Solver* sv = (Solver*)h;
   if (!sv || !name) return nullptr;
   std::string nm(name);
-  if (nm == "vals") return sv->d_vals.p;        // exists before the (lazy) analysis: assemble_augsys_device fills it
-  if (!sv->analysed) return nullptr;
-  if (nm == "CB") return sv->d_CB.p;
-  if (nm == "cbv") return sv->sweep.d_cbv.p;
-  if (nm == "x") return sv->sweep.d_x.p;
-  if (nm == "counters") return sv->d_counters.p;
-  if (nm == "scale") return sv->d_scale.p;
+  if (nm == "vals") return sv->d_vals.p;        // the handle's: assemble_augsys_device fills it before the (lazy) analysis
+  if (!sv->an) return nullptr;
+  const Analysis& A = *sv->an;
+  if (nm == "CB") return A.d_CB.p;
+  if (nm == "cbv") return A.sweep.d_cbv.p;
+  if (nm == "x") return A.sweep.d_x.p;
+  if (nm == "counters") return A.d_counters.p;
+  if (nm == "scale") return A.d_scale.p;
   return nullptr;
 }
 
@@ -2995,7 +3030,7 @@ void* b200ldlt_device_ptr(b200ldlt_handle h, const char* name) {
  * phase 1: the top part (only rank 0 has work).  Enqueues on the handle's stream and returns. */
 int b200ldlt_shard_factor(b200ldlt_handle h, int phase, int from_host) {
   Solver* sv = (Solver*)h;
-  if (!sv || !sv->shard.active || phase < 0 || phase > 1) { if (sv) sv->err = "shard_factor: shard_setup first"; return B200LDLT_FATAL_ERROR; }
+  if (!sv || !sv->an || !sv->an->shard.active || phase < 0 || phase > 1) { if (sv) sv->err = "shard_factor: shard_setup first"; return B200LDLT_FATAL_ERROR; }
   CU(cudaSetDevice(sv->dev));
   cudaStream_t st = sv->stream;
   if (phase == 0) {
@@ -3003,13 +3038,14 @@ int b200ldlt_shard_factor(b200ldlt_handle h, int phase, int from_host) {
     if (from_host) CU(cudaMemcpyAsync(sv->d_vals.p, sv->h_vals, sv->nnz * sizeof(double), cudaMemcpyHostToDevice, st));
     sv->have_dev_vals = true;
   }
-  return enqueue_factor(sv, sv->shard.part[phase], phase == 0);
+  return enqueue_factor(sv, sv->an->shard.part[phase], phase == 0);
 }
 
 /* counters_total: CNT_N ints already summed over the ranks (all-reduce of device_ptr("counters")) */
 int b200ldlt_shard_factor_finish(b200ldlt_handle h, const int* counters_total, int check_inertia, int expected_neg, int* num_neg) {
   Solver* sv = (Solver*)h;
-  if (!sv || !sv->shard.active || !counters_total) return B200LDLT_FATAL_ERROR;
+  if (!sv || !sv->an || !sv->an->shard.active || !counters_total) return B200LDLT_FATAL_ERROR;
+  Analysis& A = *sv->an;
   CU(cudaSetDevice(sv->dev));
   CU(cudaEventRecord(sv->ev1, sv->stream));
   CU(cudaStreamSynchronize(sv->stream));
@@ -3020,8 +3056,8 @@ int b200ldlt_shard_factor_finish(b200ldlt_handle h, const int* counters_total, i
   I.num_growth = counters_total[CNT_GROWTH]; I.num_2x2 = counters_total[CNT_2X2];
   sv->num_neg = I.num_neg;
   if (num_neg) *num_neg = I.num_neg;
-  sv->factored = (I.num_tiny == 0);
-  sv->zpos.clear();
+  A.factored = (I.num_tiny == 0);
+  A.zpos.clear();
   if (I.num_tiny > 0) return B200LDLT_SINGULAR;
   if (check_inertia && I.num_neg != expected_neg) return B200LDLT_WRONG_INERTIA;
   return B200LDLT_SUCCESS;
@@ -3031,25 +3067,26 @@ int b200ldlt_shard_factor_finish(b200ldlt_handle h, const int* counters_total, i
  * phase 2: backward sweep over my subtrees;  phase 3: un-permute/un-scale into d_rhs.  d_rhs: dim doubles on the device. */
 int b200ldlt_shard_solve(b200ldlt_handle h, int phase, double* d_rhs) {
   Solver* sv = (Solver*)h;
-  if (!sv || !sv->shard.active || !sv->factored) { if (sv) sv->err = "shard_solve: factor first"; return B200LDLT_FATAL_ERROR; }
+  if (!sv || !sv->an || !sv->an->shard.active || !sv->an->factored) { if (sv) sv->err = "shard_solve: factor first"; return B200LDLT_FATAL_ERROR; }
+  Analysis& A = *sv->an;
   CU(cudaSetDevice(sv->dev));
   cudaStream_t st = sv->stream;
-  Solver::Shard& H = sv->shard;
+  Analysis::Shard& H = A.shard;
   const int n = sv->n;
   int rc = B200LDLT_SUCCESS;
   // (phases 1 and 2 run under phase 0's epoch: k_mark_flags stamps the cut roots and the top fronts with it)
   if (phase == 0) {
     sv->launches = 0;
-    rc = forward(sv, H.part[0].solve, sv->sweep, d_rhs, 1);
+    rc = forward(sv, H.part[0].solve, A.sweep, d_rhs, 1);
   } else if (phase == 1) {
-    if (H.d_mark_cut.n) k_mark_flags<<<cdiv((long long)H.d_mark_cut.n, 256), 256, 0, st>>>(sv->sweep.d_done_f.p, H.d_mark_cut.p, (int)H.d_mark_cut.n, sv->solve_epoch);
-    rc = launch_sweep(sv, H.part[1].solve, sv->sweep, 1, true);
-    if (rc == B200LDLT_SUCCESS) rc = launch_sweep(sv, H.part[1].solve, sv->sweep, 1, false);
+    if (H.d_mark_cut.n) k_mark_flags<<<cdiv((long long)H.d_mark_cut.n, 256), 256, 0, st>>>(A.sweep.d_done_f.p, H.d_mark_cut.p, (int)H.d_mark_cut.n, A.solve_epoch);
+    rc = launch_sweep(sv, H.part[1].solve, A.sweep, 1, true);
+    if (rc == B200LDLT_SUCCESS) rc = launch_sweep(sv, H.part[1].solve, A.sweep, 1, false);
   } else if (phase == 2) {
-    if (H.rank != 0 && H.d_mark_top.n) k_mark_flags<<<cdiv((long long)H.d_mark_top.n, 256), 256, 0, st>>>(sv->sweep.d_done_b.p, H.d_mark_top.p, (int)H.d_mark_top.n, sv->solve_epoch);
-    rc = launch_sweep(sv, H.part[0].solve, sv->sweep, 1, false);
+    if (H.rank != 0 && H.d_mark_top.n) k_mark_flags<<<cdiv((long long)H.d_mark_top.n, 256), 256, 0, st>>>(A.sweep.d_done_b.p, H.d_mark_top.p, (int)H.d_mark_top.n, A.solve_epoch);
+    rc = launch_sweep(sv, H.part[0].solve, A.sweep, 1, false);
   } else if (phase == 3) {
-    k_sol_out<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_perm.p, sv->d_scale.p, sv->sweep.d_x.p, n, d_rhs);
+    k_sol_out<<<cdiv(n, 256), 256, 0, st>>>(n, A.d_perm.p, A.d_scale.p, A.sweep.d_x.p, n, d_rhs);
   } else return B200LDLT_FATAL_ERROR;
   CU(cudaGetLastError());
   return rc;
@@ -3081,7 +3118,7 @@ int b200ldlt_assemble_augsys_device(b200ldlt_handle h, const b200ldlt_augsys* a)
   const long long total = (long long)a->nnz_w + a->n_x + a->n_s + a->nnz_jc + a->n_c + a->nnz_jd + a->n_s + a->n_d;
   if (total != sv->nnz || a->n_x + a->n_s + a->n_c + a->n_d != sv->n) { sv->err = "assemble_augsys: block sizes do not match the analysed structure"; return B200LDLT_FATAL_ERROR; }
   CU(cudaSetDevice(sv->dev));
-  if (!sv->analysed && !sv->d_vals.p) CU(sv->d_vals.alloc(sv->nnz));   // (the lazy analysis re-allocates and keeps the contents: see do_factor)
+  if (!sv->d_vals.p) CU(sv->d_vals.alloc(sv->nnz));
   AugSegs A;
   long long off = 0;
   auto seg = [&](int q, const double* src, long long n, double scale, double add) { A.s[q] = AugSeg{src, off, n, scale, add}; off += n; };
@@ -3107,8 +3144,9 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
                                  int* steps_done, double* residual_ratio) {
   Solver* sv = (Solver*)h;
   if (steps_done) *steps_done = 0;
-  if (!sv || !sv->factored || !sv->have_dev_vals || !d_rhs) { if (sv) sv->err = "solve_refine: factor first (values on the device)"; return B200LDLT_FATAL_ERROR; }
+  if (!sv || !sv->an || !sv->an->factored || !sv->have_dev_vals || !d_rhs) { if (sv) sv->err = "solve_refine: factor first (values on the device)"; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "solve_refine_device", true); if (rc != B200LDLT_SUCCESS) return rc; }
+  Analysis& A = *sv->an;
   const int n = sv->n;
   if (!sv->vec) {
     sv->vec = b200vec_create(sv->dev, (void*)sv->stream);
@@ -3122,7 +3160,7 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
   cudaStream_t st = sv->stream;
   CU(cudaMemcpyAsync(sv->d_ref_b.p, d_rhs, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
   sv->launches = 0;
-  int rc = enqueue_solve(sv, sv->sweep, 0, d_rhs, d_rhs, 1);
+  int rc = enqueue_solve(sv, A.sweep, 0, d_rhs, d_rhs, 1);
   if (rc != B200LDLT_SUCCESS) return rc;
   b200vec vb{sv->d_ref_b.p, n, 0, 0.0}, vx{d_rhs, n, 0, 0.0}, vr{sv->d_ref_r.p, n, 0, 0.0};
   double nb = 0.0, ratio = 0.0;
@@ -3136,7 +3174,7 @@ int b200ldlt_solve_refine_device(b200ldlt_handle h, double* d_rhs, int min_steps
     if (b200vec_amax(sv->vec, &vr, &nr) || b200vec_amax(sv->vec, &vx, &nx)) { sv->err = b200vec_last_error(sv->vec); return B200LDLT_FATAL_ERROR; }
     ratio = (nb + nx == 0.0) ? nr : nr / (std::min(nx, 1e6 * nb) + nb);
     if (step >= max_steps || (step >= min_steps && ratio <= tol)) break;
-    rc = enqueue_solve(sv, sv->sweep, 0, sv->d_ref_r.p, sv->d_ref_r.p, 1);     // d = A^-1 r
+    rc = enqueue_solve(sv, A.sweep, 0, sv->d_ref_r.p, sv->d_ref_r.p, 1);     // d = A^-1 r
     if (rc != B200LDLT_SUCCESS) return rc;
     if (b200vec_axpy(sv->vec, 1.0, &vr, &vx)) { sv->err = b200vec_last_error(sv->vec); return B200LDLT_FATAL_ERROR; }
     ++step;
@@ -3155,7 +3193,7 @@ int b200ldlt_increase_quality(b200ldlt_handle h) {
   // The last factorisation lifted pivots (num_forced) or saw growth beyond 1/u: a larger threshold would only reject
   // more pivots inside the same supernodes.  The pairing / ordering were frozen on the values of the FIRST matrix; redo
   // the analysis on the current values instead (once per matrix: the second request raises the threshold as usual).
-  if ((sv->info.num_forced > 0 || sv->info.num_growth > 0) && sv->analysed && !sv->shard.active && !sv->reanalysed_since_raise) {
+  if ((sv->info.num_forced > 0 || sv->info.num_growth > 0) && sv->an && !sv->an->shard.active && !sv->reanalysed_since_raise) {
     sv->reanalyse = true;
     sv->reanalysed_since_raise = true;
     return 1;
@@ -3183,11 +3221,12 @@ int b200ldlt_get_info(b200ldlt_handle h, b200ldlt_info* info) {
 int64_t b200ldlt_symbolic_array(b200ldlt_handle h, const char* name, int64_t* out, int64_t cap) {
   Solver* sv = (Solver*)h;
   if (!sv || !name) return -1;
-  if (!sv->analysed) {
+  if (!sv->an) {
     if (sv->n <= 0) return -1;
     if (run_analysis(sv, nullptr) != B200LDLT_SUCCESS) return -1;
   }
-  const Symbolic& S = sv->S;
+  const Analysis& A = *sv->an;
+  const Symbolic& S = A.S;
   std::string nm(name);
 #define RET(vec)                                                        \
   do {                                                                  \
@@ -3209,7 +3248,7 @@ int64_t b200ldlt_symbolic_array(b200ldlt_handle h, const char* name, int64_t* ou
   if (nm == "sn_level") RET(S.sn_level);
   if (nm == "level_ptr") RET(S.level_ptr);
   if (nm == "level_sn") RET(S.level_sn);
-  if (nm == "sparse_run_set") { static const std::vector<int> none; RET(sv->sfs ? sv->sfs->last_run : none); }
+  if (nm == "sparse_run_set") { static const std::vector<int> none; RET(A.sfs ? A.sfs->last_run : none); }
 #undef RET
   return -1;
 }
@@ -3217,6 +3256,8 @@ int64_t b200ldlt_symbolic_array(b200ldlt_handle h, const char* name, int64_t* ou
 int b200ldlt_residual(b200ldlt_handle h, const double* x, const double* b, double* r_inf, double* x_inf, double* b_inf) {
   Solver* sv = (Solver*)h;
   if (!sv || !sv->have_dev_vals) { if (sv) sv->err = "residual: no matrix on the device"; return B200LDLT_FATAL_ERROR; }
+  if (!sv->an) { sv->err = "residual: no analysis (factorise first)"; return B200LDLT_FATAL_ERROR; }
+  const Analysis& A = *sv->an;
   CU(cudaSetDevice(sv->dev));
   cudaStream_t st = sv->stream;
   const int n = sv->n;
@@ -3226,9 +3267,9 @@ int b200ldlt_residual(b200ldlt_handle h, const double* x, const double* b, doubl
   CU(cudaMemcpyAsync(dx.p, x, n * sizeof(double), cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(db.p, b, n * sizeof(double), cudaMemcpyHostToDevice, st));
   CU(cudaMemsetAsync(dm.p, 0, 3 * sizeof(unsigned long long), st));
-  k_residual_init<<<cdiv(n, 256), 256, 0, st>>>(n, db.p, sv->d_res.p);
-  k_residual_acc<<<cdiv(sv->nnz, 256), 256, 0, st>>>(sv->nnz, sv->d_irn.p, sv->d_jcn.p, sv->d_vals.p, dx.p, sv->d_res.p);
-  k_absmax<<<cdiv(n, 256), 256, 0, st>>>(n, sv->d_res.p, dm.p);
+  k_residual_init<<<cdiv(n, 256), 256, 0, st>>>(n, db.p, A.d_res.p);
+  k_residual_acc<<<cdiv(sv->nnz, 256), 256, 0, st>>>(sv->nnz, A.d_irn.p, A.d_jcn.p, sv->d_vals.p, dx.p, A.d_res.p);
+  k_absmax<<<cdiv(n, 256), 256, 0, st>>>(n, A.d_res.p, dm.p);
   k_absmax<<<cdiv(n, 256), 256, 0, st>>>(n, dx.p, dm.p + 1);
   k_absmax<<<cdiv(n, 256), 256, 0, st>>>(n, db.p, dm.p + 2);
   unsigned long long hm[3];
