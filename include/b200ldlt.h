@@ -234,6 +234,40 @@ int b200ldlt_solve_fredholm_device(b200ldlt_handle h, int nrhs, double tol, doub
 int b200ldlt_selected_inverse(b200ldlt_handle h, double* diag, double* vals);
 int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* d_vals);
 
+/* ---- entries of A^-1 at chosen positions (cf. MUMPS ICNTL(30), sIPOPT's reduced Hessian) ------------------------------
+ * vals[t] = M(irow[t], jcol[t]) for t < nent, M as for selected inversion (A^-1, the perturbed matrix's inverse with
+ * info.num_forced > 0, D^+ on kept singular factors, the altered D after alter_d).  irow and jcol are 0-based original
+ * indices in host memory for both entry points; entries come in any order, repeats and both (i, j) and (j, i) allowed.
+ *   M_ij = y_i^T D^-1 y_j ,   y_k = L^-1 P^T S e_k   (job 1 of e_k = sparse_fwd_solve({k}, {1.0}))
+ * y_k is non-zero only on the reach of k, the path from its front to the root; fronts are numbered in postorder, so its
+ * positions ascend along the path, and y_i and y_j share exactly the path from the lowest common ancestor of their fronts
+ * to the root: a common SUFFIX of m positions.  Each entry is one dot over that suffix with D^-1 between (a 2x2 pivot
+ * never straddles a front); i and j in different trees of the forest give exactly +0.
+ * The columns (the distinct indices of irow and jcol) are sorted by pivot position and swept in blocks of up to
+ * B200_SOLVE_BLOCK columns (the blocked state of the solves, allocated as a blocked solve does; B200_SOLVE_BLOCK=1 or
+ * a failed allocation: one column per block), each block by job 1's forward sweep pruned to the union of its columns'
+ * reaches as in sparse_fwd_solve (the same run sets, work lists and dependency check, which refuses a sweep that could
+ * wait forever before anything is launched).
+ * Summation order, pinned (every operation rounded on its own, no FMA): with a = y_i and b = y_j on the suffix, the TERM
+ * at suffix offset o is d (a_o b_o) for a 1x1 pivot (d = D^-1 there), (d1 (a_o b_o) + d2 (a_o+1 b_o+1)) + e ((a_o b_o+1)
+ * + (a_o+1 b_o)) for a 2x2 pivot opening at o (d1, d2 its diagonal and e its off-diagonal entry of D^-1), none at the
+ * second position of a 2x2.  Partial sum l = 0..31 adds, from +0 in ascending o, the terms at o = l (mod 32); then
+ * s_l += s_(l xor k) for k = 16, 8, 4, 2, 1; the entry is s_0.  So (i, j) and (j, i) and repeats give the same bits,
+ * repeated calls and both entry points the same bits, and a float64 replay on y from sparse_fwd_solve and D^-1 from
+ * enquire_indef reproduces every entry; an entry equals the same entry requested alone, whatever B200_SOLVE_BLOCK, as a
+ * value (the y of a column swept in a block may differ from its y swept alone in the sign of a zero).
+ * Kernel launches: sum over blocks b of (1 + d_b + t_b + 1), plus 1, with d_b and t_b counted as for sparse_fwd_solve on
+ * the block's columns.  Memory: the first call after an analysis builds sparse_fwd_solve's per-front indices (not its
+ * staging) and two ints per front; each call needs 12 bytes per element of the y store (sum over the columns of the
+ * pivots on their paths to the root), 24 bytes per entry and per block its pruned lists, in pinned and device staging
+ * that grows to the largest call and is freed by the next analysis.  symbolic_array "inverse_run_set" returns the union
+ * of the run sets the last call swept.  The call leaves the factors, D, every later solve and "sparse_run_set" as they
+ * were.  Refused (nothing written): nent < 0, a NULL pointer with nent > 0, an index out of range, and (FATAL_ERROR with
+ * a message) a failed allocation of the staging or the y store.  nent = 0 is the no-columns case.
+ * Device entry point: d_vals (nent doubles) is device memory. */
+int b200ldlt_inverse_entries(b200ldlt_handle h, int nent, const int* irow, const int* jcol, double* vals);
+int b200ldlt_inverse_entries_device(b200ldlt_handle h, int nent, const int* irow, const int* jcol, double* d_vals);
+
 /* ---- partial factorisation with an explicit Schur complement (cf. MUMPS ICNTL(19) / ICNTL(26), Pardiso iparm(36)) -----
  * S = vars[0..m) are the caller's Schur variables (distinct 0-based original indices), E the other n - m.  In Schur mode
  * the analysis orders E alone and places S last, in the caller's order, as one root front; the factor calls (factor,
@@ -351,7 +385,8 @@ int b200ldlt_get_info(b200ldlt_handle h, b200ldlt_info* info);
 /* Copy a named array of the symbolic analysis ("perm","sn_start","sn_parent","rows_ptr","rows","rel",
  * "L_off","cb_off","u_dst64","uent_ptr","t2u","sn_level","level_ptr","level_sn") as int64 into out (cap entries).
  * Returns the array length, or -1 for an unknown name. Runs the lazy analysis (pattern only) if needed.
- * "sparse_run_set": the fronts the last b200ldlt_sparse_fwd_solve swept, ascending (empty before the first one). */
+ * "sparse_run_set": the fronts the last b200ldlt_sparse_fwd_solve swept, ascending (empty before the first one);
+ * "inverse_run_set": the union of the fronts the last b200ldlt_inverse_entries swept, ascending (empty before the first). */
 int64_t b200ldlt_symbolic_array(b200ldlt_handle h, const char* name, int64_t* out, int64_t cap);
 /* Force the symbolic phase now; vals may be NULL (no saddle pairing then). */
 int b200ldlt_analyse_now(b200ldlt_handle h, const double* vals);

@@ -70,7 +70,8 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_selected_inverse", "b200ldlt_selected_inverse_device", "b200ldlt_set_schur",
             "b200ldlt_schur_complement", "b200ldlt_schur_complement_device", "b200ldlt_schur_reduce",
             "b200ldlt_schur_reduce_device", "b200ldlt_schur_expand", "b200ldlt_schur_expand_device",
-            "b200ldlt_error_analysis", "b200ldlt_error_analysis_device", "b200ldlt_condest"]
+            "b200ldlt_error_analysis", "b200ldlt_error_analysis_device", "b200ldlt_condest",
+            "b200ldlt_inverse_entries", "b200ldlt_inverse_entries_device"]
 
 _lib = None
 
@@ -119,6 +120,8 @@ def load_library():
     L.b200ldlt_solve_fredholm_device.argtypes = [vp, C.c_int, C.c_double, vp, ip]
     L.b200ldlt_selected_inverse.argtypes = [vp, dp, dp]
     L.b200ldlt_selected_inverse_device.argtypes = [vp, vp, vp]
+    L.b200ldlt_inverse_entries.argtypes = [vp, C.c_int, ip, ip, dp]
+    L.b200ldlt_inverse_entries_device.argtypes = [vp, C.c_int, ip, ip, vp]
     L.b200ldlt_set_schur.argtypes = [vp, C.c_int, ip]
     L.b200ldlt_schur_complement.argtypes = [vp, dp]
     L.b200ldlt_schur_complement_device.argtypes = [vp, vp]
@@ -399,6 +402,24 @@ class B200Ldlt:
         """The same into device arrays (pointers as ints, 0 = not wanted). Returns the status."""
         return self._L.b200ldlt_selected_inverse_device(self._h, C.c_void_p(d_diag_ptr or None),
                                                         C.c_void_p(d_vals_ptr or None))
+
+    def inverse_entries(self, irow, jcol):
+        """Entries of M = A^-1 at chosen positions (b200ldlt_inverse_entries): vals[t] = M(irow[t], jcol[t]) for 0-based
+        original indices, as a numpy array.  Raises on a refusal."""
+        i = np.ascontiguousarray(irow, dtype=np.int32)
+        j = np.ascontiguousarray(jcol, dtype=np.int32)
+        assert i.shape == j.shape and i.ndim == 1
+        v = np.zeros(max(len(i), 1))
+        if self._L.b200ldlt_inverse_entries(self._h, len(i), _iptr(i), _iptr(j), _dptr(v)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return v[:len(i)].copy()
+
+    def inverse_entries_device(self, irow, jcol, d_vals_ptr):
+        """The same into a device array of len(irow) doubles (pointer as an int).  Returns the status."""
+        i = np.ascontiguousarray(irow, dtype=np.int32)
+        j = np.ascontiguousarray(jcol, dtype=np.int32)
+        assert i.shape == j.shape and i.ndim == 1
+        return self._L.b200ldlt_inverse_entries_device(self._h, len(i), _iptr(i), _iptr(j), C.c_void_p(d_vals_ptr))
 
     def set_schur(self, vars):
         """Schur mode on the 0-based variables vars (empty: off).  Takes effect at the next factor call, which re-analyses

@@ -110,10 +110,10 @@ struct LmulPlan {
   int width = 0;
 };
 
-// The sparse forward solve (b200ldlt_sparse_fwd_solve): per-front indices into the host copies of the full plan's forward
-// lists, the marks of one call, and the staging of the pruned lists (pinned -> device, sized by the full plan).  Built at
-// the first sparse call after an analysis, before that call's timing starts; a handle that never makes one allocates
-// none of it.
+// The pruned forward sweeps (b200ldlt_sparse_fwd_solve, b200ldlt_inverse_entries): per-front indices into the host copies
+// of the full plan's forward lists and the marks of one pruned sweep, built at the first such call after an analysis,
+// before that call's timing starts; and the staging of the sparse forward solve (pinned -> device, sized by the full
+// plan), allocated at its first call.  A handle that never makes either call allocates none of it.
 struct SparseFwdPlan {
   std::vector<int> dlev, didx;                 // by front: its direct level and index there, or -1
   std::vector<int> item_of, sub_of;            // by front: the subtree item / the subtree that walks it, or -1
@@ -129,6 +129,25 @@ struct SparseFwdPlan {
   DevBuf<char> d_buf;
   cudaEvent_t ev_staged = nullptr;             // the last copy out of h_buf
   ~SparseFwdPlan() {
+    if (h_buf) cudaFreeHost(h_buf);
+    if (ev_staged) cudaEventDestroy(ev_staged);
+  }
+};
+
+// Entries of A^-1 (b200ldlt_inverse_entries): per front its depth in the tree and the pivots on its path to the root;
+// the column of each variable during a call; the union of the run sets of the last call; the staging of a call (pinned
+// -> device: the entry list, the offsets and pivot positions of the y store, and per block its pruned lists, run-set
+// positions and column positions) and the values of the y store, both grown to the largest call.  Built at the first
+// call after an analysis, before its timing starts; a handle that never makes the call allocates none of it.
+struct InvPlan {
+  std::vector<int> depth, pathlen;             // by front
+  std::vector<int> col_of;                     // variable -> its column in the current call, else -1
+  std::vector<int> last_run;                   // symbolic_array "inverse_run_set"
+  char* h_buf = nullptr;
+  DevBuf<char> d_buf;
+  DevBuf<double> d_y;
+  cudaEvent_t ev_staged = nullptr;             // the last copy out of h_buf
+  ~InvPlan() {
     if (h_buf) cudaFreeHost(h_buf);
     if (ev_staged) cudaEventDestroy(ev_staged);
   }
@@ -253,7 +272,8 @@ struct Analysis {
   DevBuf<long long> d_bigv_off;
   DevBuf<long long> d_piv_big;      // n : per pivot position, its index in bigv (pivots of big fronts) or -1 (partial solves)
   std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call
-  std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve: built at its first call
+  std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve / inverse entries: built at the first such call
+  std::unique_ptr<InvPlan> inv;         // inverse entries: built at its first call
   std::unique_ptr<SelInvPlan> selinv;   // selected inversion: built at its first call
   std::unique_ptr<EaPlan> ea;       // error analysis / condest: built at the first such call
   // zero pivots (b200ldlt_set_singular_action): the factor kernels append every forced zero pivot to d_zlist; with
@@ -1742,61 +1762,70 @@ static int enqueue_lmul_columns(Solver* sv, int trans, int nrhs, const double* d
   });
 }
 
-// ---- sparse forward solve (b200ldlt_sparse_fwd_solve) --------------------------------------------------------------
-// The per-front indices into the host copies of the handle's forward lists (SparseFwdPlan): at the first sparse call
-// after an analysis, before its timing starts.
-static int sfs_state(Solver* sv) {
-  Analysis& A = *sv->an;
-  if (A.sfs) return B200LDLT_SUCCESS;
+// ---- pruned forward sweeps (b200ldlt_sparse_fwd_solve, b200ldlt_inverse_entries) -------------------------------------
+// The per-front indices into the host copies of the handle's forward lists and the marks of a pruned sweep.
+static void build_sfs_plan(const Analysis& A, int n, SparseFwdPlan& P) {
   const Symbolic& S = A.S;
   const SolvePlan& SP = A.fronts.solve;
-  const int n = sv->n, nsn = S.nsn;
-  std::unique_ptr<SparseFwdPlan> P(new SparseFwdPlan());
-  P->dlev.assign(nsn, -1); P->didx.assign(nsn, -1); P->item_of.assign(nsn, -1); P->sub_of.assign(nsn, -1);
-  long long ndirect = 0;
-  for (size_t l = 0; l < SP.direct_cnt.size(); ++l) {
-    ndirect += SP.direct_cnt[l];
-    for (int i = 0; i < SP.direct_cnt[l]; ++i) { const int s = SP.direct[l][i]; P->dlev[s] = (int)l; P->didx[s] = i; }
-  }
-  P->item_ptr.assign(1, 0);
+  const int nsn = S.nsn;
+  P.dlev.assign(nsn, -1); P.didx.assign(nsn, -1); P.item_of.assign(nsn, -1); P.sub_of.assign(nsn, -1);
+  for (size_t l = 0; l < SP.direct_cnt.size(); ++l)
+    for (int i = 0; i < SP.direct_cnt[l]; ++i) { const int s = SP.direct[l][i]; P.dlev[s] = (int)l; P.didx[s] = i; }
+  P.item_ptr.assign(1, 0);
   for (int i = 0; i < SP.npair; ++i) {
     for (const int u : {SP.pairs[i].x, SP.pairs[i].y}) {
       if (u < 0) continue;
       const SubDesc& d = SP.subs[u];
       for (int j = 0; j < d.nown; ++j) {
         const int s = SP.meta[d.moff + 2 * d.nlv + 1 + j];
-        P->item_fr.push_back(s); P->item_of[s] = i; P->sub_of[s] = u;
+        P.item_fr.push_back(s); P.item_of[s] = i; P.sub_of[s] = u;
       }
     }
-    P->item_ptr.push_back((int)P->item_fr.size());
+    P.item_ptr.push_back((int)P.item_fr.size());
   }
-  P->task_ptr.assign(nsn + 1, 0);
+  P.task_ptr.assign(nsn + 1, 0);
   auto each_front = [&](const SolveTask& T, auto&& fn) {
     if (T.type == ST_SMALL) { for (int w = 0; w < T.blk; ++w) fn(SP.bundle[T.s + w]); }
     else fn(T.s);
   };
-  for (int j = 0; j < SP.ntf; ++j) each_front(SP.tf[j], [&](int s) { P->task_ptr[s + 1]++; });
-  for (int s = 0; s < nsn; ++s) P->task_ptr[s + 1] += P->task_ptr[s];
-  P->task_idx.resize(P->task_ptr[nsn]);
+  for (int j = 0; j < SP.ntf; ++j) each_front(SP.tf[j], [&](int s) { P.task_ptr[s + 1]++; });
+  for (int s = 0; s < nsn; ++s) P.task_ptr[s + 1] += P.task_ptr[s];
+  P.task_idx.resize(P.task_ptr[nsn]);
   {
-    std::vector<int> fill(P->task_ptr.begin(), P->task_ptr.end() - 1);
-    for (int j = 0; j < SP.ntf; ++j) each_front(SP.tf[j], [&](int s) { P->task_idx[fill[s]++] = j; });
+    std::vector<int> fill(P.task_ptr.begin(), P.task_ptr.end() - 1);
+    for (int j = 0; j < SP.ntf; ++j) each_front(SP.tf[j], [&](int s) { P.task_idx[fill[s]++] = j; });
   }
-  P->iperm.resize(n); P->sn_of.resize(n);
-  for (int i = 0; i < n; ++i) P->iperm[S.perm[i]] = i;
-  for (int s = 0; s < nsn; ++s) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) P->sn_of[p] = s;
-  P->pos_bi.assign(n, -1);
-  P->m_reach.assign(nsn, 0); P->m_run.assign(nsn, 0); P->m_fr.assign(nsn, 0);
-  P->m_item.assign(std::max(SP.npair, 1), 0); P->m_task.assign(std::max(SP.ntf, 1), 0);
-  P->ord0.assign(nsn, 0); P->ord1.assign(nsn, 0);
-  // staging: subtree items, b, top tasks, then the int lists (direct fronts, run-set positions and their b indices,
-  // output positions, frontier), and on the device the output slice
+  P.iperm.resize(n); P.sn_of.resize(n);
+  for (int i = 0; i < n; ++i) P.iperm[S.perm[i]] = i;
+  for (int s = 0; s < nsn; ++s) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) P.sn_of[p] = s;
+  P.pos_bi.assign(n, -1);
+  P.m_reach.assign(nsn, 0); P.m_run.assign(nsn, 0); P.m_fr.assign(nsn, 0);
+  P.m_item.assign(std::max(SP.npair, 1), 0); P.m_task.assign(std::max(SP.ntf, 1), 0);
+  P.ord0.assign(nsn, 0); P.ord1.assign(nsn, 0);
+}
+
+// SparseFwdPlan at the first pruned call after an analysis, before its timing starts; with `staging` (the sparse
+// forward solve) also its staging.
+static int sfs_state(Solver* sv, bool staging) {
+  Analysis& A = *sv->an;
+  const int n = sv->n;
+  if (!A.sfs) {
+    std::unique_ptr<SparseFwdPlan> P(new SparseFwdPlan());
+    build_sfs_plan(A, n, *P);
+    A.sfs = std::move(P);
+  }
+  SparseFwdPlan& P = *A.sfs;
+  if (!staging || P.h_buf) return B200LDLT_SUCCESS;
+  const SolvePlan& SP = A.fronts.solve;
+  long long ndirect = 0;
+  for (const int c : SP.direct_cnt) ndirect += c;
+  // staging: subtree items, top tasks, direct fronts, frontier, b, run-set positions and their b indices, output
+  // positions, and on the device the output slice
   const size_t cap = 8 * (size_t)SP.npair + 8 * (size_t)n + sizeof(SolveTask) * (size_t)SP.ntf +
-                     4 * ((size_t)ndirect + 3 * (size_t)n + (size_t)nsn) + 8 * (size_t)n + 64;
-  CU(cudaHostAlloc((void**)&P->h_buf, cap, cudaHostAllocDefault));
-  CU(P->d_buf.alloc(cap));
-  CU(cudaEventCreateWithFlags(&P->ev_staged, cudaEventDisableTiming));
-  A.sfs = std::move(P);
+                     4 * ((size_t)ndirect + 3 * (size_t)n + (size_t)A.S.nsn) + 8 * (size_t)n + 64;
+  if (!P.ev_staged) CU(cudaEventCreateWithFlags(&P.ev_staged, cudaEventDisableTiming));
+  CU(P.d_buf.alloc(cap));
+  CU(cudaHostAlloc((void**)&P.h_buf, cap, cudaHostAllocDefault));
   return B200LDLT_SUCCESS;
 }
 
@@ -1809,38 +1838,37 @@ struct SfsCall {
 
 static inline size_t align8(size_t b) { return (b + 7) & ~(size_t)7; }
 
-// Host part of a sparse forward solve.  The reach (the fronts on the tree paths from the fronts of b's variables to the
-// root) gives the run set R: the reach, the fronts walked by a subtree item that walks a reached front, and the fronts
-// of a bundle that holds one (items and bundles are kept whole).  The pruned lists take every entry of the handle's forward
-// lists that belongs to a front of R, in list order.  F = the children of R outside R.  Before anything is launched, the
-// check that the pruned sweep cannot wait forever: every front of R owns work in the lists -- all of its top tasks, and
-// all chunks of each chunked block (the arrival counters count modulo the chunk count) -- and every child of a front of
-// R is in F or runs EARLIER in the pruned order (the same subtree walk counts: it is walked level by level).  Everything
-// the device needs goes to the pinned staging (b too when b_host).  FATAL_ERROR with a message, nothing written to the
-// caller and nothing launched, for a bad pattern or a failed check.
-static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_host, SfsCall& C) {
+// one pruned forward sweep as the host prepares it: the reach (ascending), the run set (the reach first), the subtree
+// items and top tasks it runs (ascending), per direct level the indices of its direct fronts (ascending), the frontier
+struct PrunedSweep {
+  std::vector<int> reach, run, items, tasks, fr;
+  std::vector<std::vector<int>> dl;
+};
+
+// Host part of a pruned forward sweep from the pivot positions seed[0..nseed).  The reach (the fronts on the tree paths
+// from the fronts of the seeds to the root) gives the run set R: the reach, the fronts walked by a subtree item that
+// walks a reached front, and the fronts of a bundle that holds one (items and bundles are kept whole).  The pruned lists
+// take every entry of the handle's forward lists that belongs to a front of R, in list order.  F = the children of R
+// outside R.  Then the check that the pruned sweep cannot wait forever, before anything is launched: every front of R
+// owns work in the lists -- all of its top tasks, and all chunks of each chunked block (the arrival counters count modulo
+// the chunk count) -- and every child of a front of R is in F or runs EARLIER in the pruned order (the same subtree walk
+// counts: it is walked level by level).  FATAL_ERROR with "<call>: ..." when the check fails.
+static int prune_forward(Solver* sv, const char* call, const int* seed, int nseed, PrunedSweep& R) {
   Analysis& A = *sv->an;
   SparseFwdPlan& P = *A.sfs;
   const SolvePlan& SP = A.fronts.solve;
   const Symbolic& S = A.S;
-  const int n = sv->n;
   const int nd = (int)SP.direct_cnt.size();
   const unsigned m = ++P.stamp;
-  for (int i = 0; i < nbi; ++i) {
-    const int v = bindex[i];
-    const char* bad = (v < 0 || v >= n) ? "sparse_fwd_solve: index out of range" : (P.pos_bi[P.iperm[v]] >= 0) ? "sparse_fwd_solve: index appears twice" : nullptr;
-    if (bad) {
-      for (int j = 0; j < i; ++j) P.pos_bi[P.iperm[bindex[j]]] = -1;
-      sv->err = bad;
-      return B200LDLT_FATAL_ERROR;
-    }
-    P.pos_bi[P.iperm[v]] = i;
-  }
-  std::vector<int> reach;
-  for (int i = 0; i < nbi; ++i)
-    for (int s = P.sn_of[P.iperm[bindex[i]]]; s >= 0 && P.m_reach[s] != m; s = S.sn_parent[s]) { P.m_reach[s] = m; reach.push_back(s); }
+  std::vector<int>& reach = R.reach;
+  std::vector<int>& run = R.run;
+  std::vector<int>& items = R.items;
+  std::vector<int>& tasks = R.tasks;
+  reach.clear(); items.clear(); tasks.clear(); R.fr.clear();
+  for (int i = 0; i < nseed; ++i)
+    for (int s = P.sn_of[seed[i]]; s >= 0 && P.m_reach[s] != m; s = S.sn_parent[s]) { P.m_reach[s] = m; reach.push_back(s); }
   std::sort(reach.begin(), reach.end());
-  std::vector<int> run(reach), items, tasks;
+  run = reach;
   for (int s : reach) P.m_run[s] = m;
   auto add = [&](int s) { if (P.m_run[s] != m) { P.m_run[s] = m; run.push_back(s); } };
   for (size_t q = 0; q < run.size(); ++q) {
@@ -1859,34 +1887,10 @@ static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_h
   }
   std::sort(items.begin(), items.end());
   std::sort(tasks.begin(), tasks.end());
-  std::vector<std::vector<int>> dl(nd);
+  std::vector<std::vector<int>>& dl = R.dl;
+  dl.assign(nd, std::vector<int>());
   for (int s : run) if (P.dlev[s] >= 0) dl[P.dlev[s]].push_back(P.didx[s]);
-  // staging layout
-  int ndir = 0, nrc = 0, nxi = 0;
-  for (auto& v : dl) { std::sort(v.begin(), v.end()); ndir += (int)v.size(); }
-  for (int s : run) nrc += S.sn_start[s + 1] - S.sn_start[s];
-  for (int s : reach) nxi += S.sn_start[s + 1] - S.sn_start[s];
-  char* h = P.h_buf;
-  const size_t o_tf = align8(8 * items.size()), o_b = o_tf + align8(sizeof(SolveTask) * tasks.size());
-  const size_t o_dir = o_b + align8(b_host ? 8 * (size_t)nbi : 0);
-  C.o_b = o_b; C.o_pos = o_dir + 4 * (size_t)ndir; C.o_bi = C.o_pos + 4 * (size_t)nrc; C.o_xi = C.o_bi + 4 * (size_t)nrc;
-  C.o_fr = C.o_xi + 4 * (size_t)nxi;
-  // (the previous call's copy out of the staging must be complete before it is rewritten)
-  if (cudaEventSynchronize(P.ev_staged) != cudaSuccess) {
-    for (int i = 0; i < nbi; ++i) P.pos_bi[P.iperm[bindex[i]]] = -1;
-    sv->err = "sparse_fwd_solve: staging copy failed";
-    return B200LDLT_FATAL_ERROR;
-  }
-  {
-    int* pos = reinterpret_cast<int*>(h + C.o_pos);
-    int* bi = reinterpret_cast<int*>(h + C.o_bi);
-    int* xi = reinterpret_cast<int*>(h + C.o_xi);
-    int j = 0;
-    for (int s : run) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p, ++j) { pos[j] = p; bi[j] = P.pos_bi[p]; }
-    j = 0;
-    for (int s : reach) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) xi[j++] = p;
-  }
-  for (int i = 0; i < nbi; ++i) P.pos_bi[P.iperm[bindex[i]]] = -1;
+  for (auto& v : dl) std::sort(v.begin(), v.end());
   // pruned order: direct level l -> slot l, subtree item i -> nd + i, top task j -> nd + items + j
   for (int s : run) { P.ord0[s] = INT_MAX; P.ord1[s] = -1; }
   for (int l = 0; l < nd; ++l) for (int i : dl[l]) { const int s = SP.direct[l][i]; P.ord0[s] = P.ord1[s] = l; }
@@ -1899,7 +1903,6 @@ static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_h
     if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) upd(SP.bundle[T.s + w]);
     else upd(T.s);
   }
-  std::vector<int> fr;
   for (int s : run) {
     bool ok = P.ord1[s] >= 0;
     // all top tasks of the front are in the lists, each chunked block with all of its nq chunks, a big front with all
@@ -1922,35 +1925,110 @@ static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_h
     for (int e = S.child_ptr[s]; ok && e < S.child_ptr[s + 1]; ++e) {
       const int c = S.child_idx[e];
       if (P.m_run[c] == m) ok = (P.sub_of[s] >= 0 && P.sub_of[c] == P.sub_of[s]) || P.ord1[c] < P.ord0[s];
-      else if (P.m_fr[c] != m) { P.m_fr[c] = m; fr.push_back(c); }
+      else if (P.m_fr[c] != m) { P.m_fr[c] = m; R.fr.push_back(c); }
     }
     if (!ok) {
-      sv->err = "sparse_fwd_solve: the pruned sweep of front " + std::to_string(s) + " fails its dependency check (not launched)";
+      sv->err = std::string(call) + ": the pruned sweep of front " + std::to_string(s) + " fails its dependency check (not launched)";
       return B200LDLT_FATAL_ERROR;
     }
   }
-  P.last_run = run;
-  std::sort(P.last_run.begin(), P.last_run.end());
-  C.ncol = nrc; C.nxi = nxi; C.nfr = (int)fr.size();
-  C.staged = C.o_fr + 4 * fr.size();
-  C.o_x = align8(C.staged);
-  if (C.o_x + 8 * (size_t)n > P.d_buf.n) { sv->err = "sparse_fwd_solve: staging too small"; return B200LDLT_FATAL_ERROR; }
-  int2* hp = reinterpret_cast<int2*>(h);
-  for (size_t i = 0; i < items.size(); ++i) hp[i] = SP.pairs[items[i]];
+  return B200LDLT_SUCCESS;
+}
+
+// bytes the pruned lists of R take in a staging (stage_pruned)
+static size_t pruned_bytes(const PrunedSweep& R) {
+  size_t ndir = 0;
+  for (auto& v : R.dl) ndir += v.size();
+  return align8(8 * R.items.size()) + align8(sizeof(SolveTask) * R.tasks.size()) + align8(4 * ndir) + align8(4 * R.fr.size());
+}
+
+// R's pruned lists to the staging h at offset o (8-aligned; the device copy of the staging is d): subtree items, top
+// tasks, direct fronts, frontier.  pl points into d; *o_fr receives the offset of the frontier.  Returns the end offset.
+static size_t stage_pruned(const SolvePlan& SP, const PrunedSweep& R, char* h, const char* d, size_t o, PrunedLists& pl,
+                           size_t* o_fr) {
+  const int nd = (int)SP.direct_cnt.size();
+  const size_t o_tf = o + align8(8 * R.items.size());
+  const size_t o_dir = o_tf + align8(sizeof(SolveTask) * R.tasks.size());
+  int2* hp = reinterpret_cast<int2*>(h + o);
+  for (size_t i = 0; i < R.items.size(); ++i) hp[i] = SP.pairs[R.items[i]];
   SolveTask* ht = reinterpret_cast<SolveTask*>(h + o_tf);
-  for (size_t j = 0; j < tasks.size(); ++j) ht[j] = SP.tf[tasks[j]];
-  if (b_host) memcpy(h + o_b, b_host, 8 * (size_t)nbi);
+  for (size_t j = 0; j < R.tasks.size(); ++j) ht[j] = SP.tf[R.tasks[j]];
   int* hd = reinterpret_cast<int*>(h + o_dir);
-  C.pl.direct_off.assign(nd, 0); C.pl.direct_cnt.assign(nd, 0);
-  for (int l = 0, j = 0; l < nd; ++l) {
-    C.pl.direct_off[l] = j; C.pl.direct_cnt[l] = (int)dl[l].size();
-    for (int i : dl[l]) hd[j++] = SP.direct[l][i];
+  pl.direct_off.assign(nd, 0); pl.direct_cnt.assign(nd, 0);
+  int j = 0;
+  for (int l = 0; l < nd; ++l) {
+    pl.direct_off[l] = j; pl.direct_cnt[l] = (int)R.dl[l].size();
+    for (int i : R.dl[l]) hd[j++] = SP.direct[l][i];
   }
-  std::copy(fr.begin(), fr.end(), reinterpret_cast<int*>(h + C.o_fr));
-  char* d = P.d_buf.p;
-  C.pl.subpair = reinterpret_cast<const int2*>(d); C.pl.npair = (int)items.size();
-  C.pl.tf = reinterpret_cast<const SolveTask*>(d + o_tf); C.pl.ntf = (int)tasks.size();
-  C.pl.direct = reinterpret_cast<const int*>(d + o_dir);
+  *o_fr = o_dir + align8(4 * (size_t)j);
+  std::copy(R.fr.begin(), R.fr.end(), reinterpret_cast<int*>(h + *o_fr));
+  pl.subpair = reinterpret_cast<const int2*>(d + o); pl.npair = (int)R.items.size();
+  pl.tf = reinterpret_cast<const SolveTask*>(d + o_tf); pl.ntf = (int)R.tasks.size();
+  pl.direct = reinterpret_cast<const int*>(d + o_dir);
+  return *o_fr + align8(4 * R.fr.size());
+}
+
+// Host part of a sparse forward solve: the pruned sweep of b's variables (prune_forward), and everything the device needs
+// in the pinned staging (b too when b_host).  FATAL_ERROR with a message, nothing written to the caller and nothing
+// launched, for a bad pattern or a failed check.
+static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_host, SfsCall& C) {
+  Analysis& A = *sv->an;
+  SparseFwdPlan& P = *A.sfs;
+  const SolvePlan& SP = A.fronts.solve;
+  const Symbolic& S = A.S;
+  const int n = sv->n;
+  std::vector<int> seed(nbi);
+  for (int i = 0; i < nbi; ++i) {
+    const int v = bindex[i];
+    const char* bad = (v < 0 || v >= n) ? "sparse_fwd_solve: index out of range" : (P.pos_bi[P.iperm[v]] >= 0) ? "sparse_fwd_solve: index appears twice" : nullptr;
+    if (bad) {
+      for (int j = 0; j < i; ++j) P.pos_bi[P.iperm[bindex[j]]] = -1;
+      sv->err = bad;
+      return B200LDLT_FATAL_ERROR;
+    }
+    P.pos_bi[P.iperm[v]] = i;
+    seed[i] = P.iperm[v];
+  }
+  PrunedSweep R;
+  int rc = prune_forward(sv, "sparse_fwd_solve", seed.data(), nbi, R);
+  int nrc = 0, nxi = 0;
+  for (int s : R.run) nrc += S.sn_start[s + 1] - S.sn_start[s];
+  for (int s : R.reach) nxi += S.sn_start[s + 1] - S.sn_start[s];
+  // staging layout: the pruned lists, b, run-set positions and their b indices, output positions; the output slice
+  C.o_b = pruned_bytes(R);
+  C.o_pos = C.o_b + (b_host ? 8 * (size_t)nbi : 0);
+  C.o_bi = C.o_pos + 4 * (size_t)nrc; C.o_xi = C.o_bi + 4 * (size_t)nrc;
+  C.staged = C.o_xi + 4 * (size_t)nxi;
+  C.o_x = align8(C.staged);
+  if (rc == B200LDLT_SUCCESS && C.o_x + 8 * (size_t)n > P.d_buf.n) {
+    sv->err = "sparse_fwd_solve: staging too small";
+    rc = B200LDLT_FATAL_ERROR;
+  }
+  // (the previous call's copy out of the staging must be complete before it is rewritten)
+  if (rc == B200LDLT_SUCCESS && cudaEventSynchronize(P.ev_staged) != cudaSuccess) {
+    sv->err = "sparse_fwd_solve: staging copy failed";
+    rc = B200LDLT_FATAL_ERROR;
+  }
+  if (rc != B200LDLT_SUCCESS) {
+    for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = -1;
+    return rc;
+  }
+  char* h = P.h_buf;
+  {
+    int* pos = reinterpret_cast<int*>(h + C.o_pos);
+    int* bi = reinterpret_cast<int*>(h + C.o_bi);
+    int* xi = reinterpret_cast<int*>(h + C.o_xi);
+    int j = 0;
+    for (int s : R.run) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p, ++j) { pos[j] = p; bi[j] = P.pos_bi[p]; }
+    j = 0;
+    for (int s : R.reach) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) xi[j++] = p;
+  }
+  for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = -1;
+  stage_pruned(SP, R, h, P.d_buf.p, 0, C.pl, &C.o_fr);
+  if (b_host) memcpy(h + C.o_b, b_host, 8 * (size_t)nbi);
+  P.last_run = R.run;
+  std::sort(P.last_run.begin(), P.last_run.end());
+  C.ncol = nrc; C.nxi = nxi; C.nfr = (int)R.fr.size();
   return B200LDLT_SUCCESS;
 }
 
@@ -1975,6 +2053,181 @@ static int sfs_enqueue(Solver* sv, const SfsCall& C, const double* d_b, double* 
   if (rc != B200LDLT_SUCCESS) return rc;
   k_sfs_out<<<cdiv(C.nxi, 256), 256, 0, st>>>(C.nxi, reinterpret_cast<const int*>(d + C.o_xi), A.d_piv_big.p, W.d_x.p,
                                              W.d_bigv.p, d_out);
+  ++sv->launches;
+  CU(cudaGetLastError());
+  return B200LDLT_SUCCESS;
+}
+
+// ---- entries of A^-1 (b200ldlt_inverse_entries) ---------------------------------------------------------------------
+// InvPlan at the first call after an analysis, before its timing starts.  Fronts are numbered in postorder (a parent
+// after its children), so one pass from the last front down gives every front's depth and path length.
+static int inv_state(Solver* sv) {
+  Analysis& A = *sv->an;
+  if (A.inv) return B200LDLT_SUCCESS;
+  const Symbolic& S = A.S;
+  std::unique_ptr<InvPlan> Q(new InvPlan());
+  Q->depth.assign(S.nsn, 0); Q->pathlen.assign(S.nsn, 0);
+  for (int s = S.nsn - 1; s >= 0; --s) {
+    const int p = S.sn_parent[s];
+    if (p >= 0 && p <= s) { sv->err = "inverse_entries: internal: the fronts are not in postorder"; return B200LDLT_FATAL_ERROR; }
+    Q->depth[s] = p >= 0 ? Q->depth[p] + 1 : 0;
+    Q->pathlen[s] = S.k(s) + (p >= 0 ? Q->pathlen[p] : 0);
+  }
+  Q->col_of.assign(sv->n, -1);
+  CU(cudaEventCreateWithFlags(&Q->ev_staged, cudaEventDisableTiming));
+  A.inv = std::move(Q);
+  return B200LDLT_SUCCESS;
+}
+
+// one block of unit columns: columns [c0, c0 + w) of the call, its run set's ncol positions and frontier of nfr fronts,
+// the longest reach of its columns, staging offsets (bytes) and the pruned lists on the device
+struct InvBlock {
+  int c0 = 0, w = 0, ncol = 0, nfr = 0, maxlen = 0;
+  size_t o_lst = 0, o_pos = 0, o_col = 0, o_fr = 0;
+  PrunedLists pl{};
+};
+// one call as prepared on the host: the entry list, the y store's offsets (ncols + 1) and positions, the blocks
+struct InvCall {
+  int nent = 0, ncols = 0;
+  size_t o_ent = 0, o_yoff = 0, o_ypos = 0, staged = 0;
+  std::vector<InvBlock> blk;
+};
+
+// Host part of b200ldlt_inverse_entries.  The columns are the distinct variables of irow and jcol, sorted by pivot
+// position (neighbours in the tree share fronts) and cut into blocks of `width`; each block is one pruned forward sweep
+// (prune_forward, its dependency check included) of its unit columns.  Column c keeps y_c = L^-1 P^T S e_c on its reach,
+// the path from its front to the root (ascending positions), at [yoff[c], yoff[c + 1]) of the y store.  Entry (i, j)
+// reads the common suffix of y_i and y_j: the path from the lowest common ancestor of their fronts to the root, pathlen
+// of that front long (0 in different trees of the forest).  Everything the device needs goes to the pinned staging, each
+// block in a region of its own, so one copy carries the call.  FATAL_ERROR with a message, nothing written and nothing
+// launched, for a failed check or allocation.
+static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, int width, InvCall& C) {
+  Analysis& A = *sv->an;
+  const SparseFwdPlan& P = *A.sfs;
+  InvPlan& Q = *A.inv;
+  const SolvePlan& SP = A.fronts.solve;
+  const Symbolic& S = A.S;
+  std::vector<int> cols;
+  for (int t = 0; t < nent; ++t)
+    for (const int v : {irow[t], jcol[t]})
+      if (Q.col_of[v] < 0) { Q.col_of[v] = 0; cols.push_back(v); }
+  std::sort(cols.begin(), cols.end(), [&](int a, int b) { return P.iperm[a] < P.iperm[b]; });
+  const int nc = (int)cols.size();
+  for (int c = 0; c < nc; ++c) Q.col_of[cols[c]] = c;
+  auto finish = [&](int rc) { for (const int v : cols) Q.col_of[v] = -1; return rc; };   // (col_of back to -1)
+  std::vector<long long> yoff(nc + 1, 0);
+  for (int c = 0; c < nc; ++c) yoff[c + 1] = yoff[c] + Q.pathlen[P.sn_of[P.iperm[cols[c]]]];
+  const long long ny = yoff[nc];
+  // the blocks, and the staging layout: entries, yoff, ypos, then per block its pruned lists, run-set positions and
+  // column positions
+  C.nent = nent; C.ncols = nc;
+  C.o_ent = 0;
+  C.o_yoff = align8(sizeof(InvEnt) * (size_t)nent);
+  C.o_ypos = C.o_yoff + 8 * (size_t)(nc + 1);
+  size_t o = align8(C.o_ypos + 4 * (size_t)ny);
+  std::vector<PrunedSweep> R((nc + width - 1) / width);
+  std::vector<int> seed(width), run_all;
+  C.blk.assign(R.size(), InvBlock());
+  for (size_t b = 0; b < R.size(); ++b) {
+    InvBlock& B = C.blk[b];
+    B.c0 = (int)b * width; B.w = std::min(width, nc - B.c0);
+    for (int c = 0; c < B.w; ++c) {
+      seed[c] = P.iperm[cols[B.c0 + c]];
+      B.maxlen = std::max(B.maxlen, (int)(yoff[B.c0 + c + 1] - yoff[B.c0 + c]));
+    }
+    const int rc = prune_forward(sv, "inverse_entries", seed.data(), B.w, R[b]);
+    if (rc != B200LDLT_SUCCESS) return finish(rc);
+    for (int s : R[b].run) B.ncol += S.sn_start[s + 1] - S.sn_start[s];
+    B.nfr = (int)R[b].fr.size();
+    run_all.insert(run_all.end(), R[b].run.begin(), R[b].run.end());
+    B.o_lst = o;
+    B.o_pos = o + pruned_bytes(R[b]);
+    B.o_col = B.o_pos + 4 * (size_t)B.ncol;
+    o = align8(B.o_col + 4 * (size_t)B.w);
+  }
+  C.staged = o;
+  // the staging and the y store, grown to this call (a failed allocation leaves them released)
+  if (C.staged > Q.d_buf.n) {
+    Q.d_buf.release();
+    if (Q.h_buf) cudaFreeHost(Q.h_buf);
+    Q.h_buf = nullptr;
+    if (Q.d_buf.alloc(C.staged) != cudaSuccess || cudaHostAlloc((void**)&Q.h_buf, C.staged, cudaHostAllocDefault) != cudaSuccess) {
+      cudaGetLastError();
+      Q.d_buf.release();
+      Q.h_buf = nullptr;
+      sv->err = "inverse_entries: cannot allocate the staging of " + std::to_string(C.staged) + " bytes";
+      return finish(B200LDLT_FATAL_ERROR);
+    }
+  }
+  if ((size_t)ny > Q.d_y.n && Q.d_y.alloc(ny) != cudaSuccess) {
+    cudaGetLastError();
+    sv->err = "inverse_entries: cannot allocate the y store of " + std::to_string(ny) + " doubles";
+    return finish(B200LDLT_FATAL_ERROR);
+  }
+  // (the previous call's copy out of the staging must be complete before it is rewritten)
+  if (cudaEventSynchronize(Q.ev_staged) != cudaSuccess) {
+    sv->err = "inverse_entries: staging copy failed";
+    return finish(B200LDLT_FATAL_ERROR);
+  }
+  char* h = Q.h_buf;
+  InvEnt* he = reinterpret_cast<InvEnt*>(h + C.o_ent);
+  for (int t = 0; t < nent; ++t) {
+    const int ci = Q.col_of[irow[t]], cj = Q.col_of[jcol[t]];
+    int a = P.sn_of[P.iperm[irow[t]]], b = P.sn_of[P.iperm[jcol[t]]];
+    while (Q.depth[a] > Q.depth[b]) a = S.sn_parent[a];
+    while (Q.depth[b] > Q.depth[a]) b = S.sn_parent[b];
+    while (a != b) { a = S.sn_parent[a]; b = S.sn_parent[b]; }   // (both -1 at once in different trees)
+    const int m = a >= 0 ? Q.pathlen[a] : 0;
+    he[t] = InvEnt{yoff[ci + 1] - m, yoff[cj + 1] - m, m, 0};
+  }
+  memcpy(h + C.o_yoff, yoff.data(), 8 * (size_t)(nc + 1));
+  int* yp = reinterpret_cast<int*>(h + C.o_ypos);
+  for (int c = 0; c < nc; ++c)
+    for (int s = P.sn_of[P.iperm[cols[c]]]; s >= 0; s = S.sn_parent[s])
+      for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *yp++ = p;
+  for (size_t b = 0; b < R.size(); ++b) {
+    InvBlock& B = C.blk[b];
+    stage_pruned(SP, R[b], h, Q.d_buf.p, B.o_lst, B.pl, &B.o_fr);
+    int* pos = reinterpret_cast<int*>(h + B.o_pos);
+    for (int s : R[b].run) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *pos++ = p;
+    int* cp = reinterpret_cast<int*>(h + B.o_col);
+    for (int c = 0; c < B.w; ++c) cp[c] = P.iperm[cols[B.c0 + c]];
+  }
+  std::sort(run_all.begin(), run_all.end());
+  run_all.erase(std::unique(run_all.begin(), run_all.end()), run_all.end());
+  Q.last_run = std::move(run_all);
+  return finish(B200LDLT_SUCCESS);
+}
+
+// Device part: the staging in, then per block k_inv_in, the forward sweep of job 1 over its pruned lists (block width
+// w: the blocked state, one column: the single-column state) and k_inv_out into the y store; then k_inv_dot to out.
+// Launches: sum over blocks of (2 + the direct levels that hold a front of the block's run set + 1 when the run set has
+// a front outside them), + 1.
+static int inv_enqueue(Solver* sv, const InvCall& C, double* out) {
+  Analysis& A = *sv->an;
+  InvPlan& Q = *A.inv;
+  cudaStream_t st = sv->stream;
+  const char* d = Q.d_buf.p;
+  const long long* yoff = reinterpret_cast<const long long*>(d + C.o_yoff);
+  const int* ypos = reinterpret_cast<const int*>(d + C.o_ypos);
+  CU(cudaMemcpyAsync(Q.d_buf.p, Q.h_buf, C.staged, cudaMemcpyHostToDevice, st));
+  CU(cudaEventRecord(Q.ev_staged, st));
+  for (const InvBlock& B : C.blk) {
+    SweepState& W = B.w == 1 ? A.sweep : *A.blk;
+    A.solve_epoch++;
+    k_inv_in<<<dim3(cdiv(B.ncol, 256) + B.nfr, B.w), 256, 0, st>>>(
+        B.ncol, reinterpret_cast<const int*>(d + B.o_pos), reinterpret_cast<const int*>(d + B.o_col), A.d_perm.p,
+        A.d_scale.p, W.d_x.p, W.M.x, reinterpret_cast<const int*>(d + B.o_fr), A.d_rows_ptr.p, W.d_cbv.p, W.M.cbv,
+        W.d_done_f.p, W.M.nsn, A.solve_epoch);
+    ++sv->launches;
+    const int rc = launch_sweep(sv, A.fronts.solve, W, B.w, true, false, &B.pl);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    k_inv_out<<<dim3(cdiv(B.maxlen, 256), B.w), 256, 0, st>>>(B.c0, yoff, ypos, A.d_piv_big.p, W.d_x.p, W.M.x,
+                                                              W.d_bigv.p, W.M.bigv, Q.d_y.p);
+    ++sv->launches;
+  }
+  k_inv_dot<<<cdiv(C.nent, 8), 256, 0, st>>>(C.nent, reinterpret_cast<const InvEnt*>(d + C.o_ent), Q.d_y.p, ypos,
+                                             A.d_ptype.p, A.d_dinv.p, A.d_doff.p, out);
   ++sv->launches;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
@@ -2262,7 +2515,7 @@ static int sparse_fwd(Solver* sv, int nbi, const int* bindex, const double* b, b
     if (nxi) *nxi = 0;
     return no_columns(sv);
   }
-  { const int rc = sfs_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
+  { const int rc = sfs_state(sv, true); if (rc != B200LDLT_SUCCESS) return rc; }
   SfsCall C;
   { const int rc = sfs_prepare(sv, nbi, bindex, host ? b : nullptr, C); if (rc != B200LDLT_SUCCESS) return rc; }
   SparseFwdPlan& P = *sv->an->sfs;
@@ -2278,6 +2531,25 @@ static int sparse_fwd(Solver* sv, int nbi, const int* bindex, const double* b, b
   memcpy(xindex, P.h_buf + C.o_xi, (size_t)C.nxi * sizeof(int));
   *nxi = C.nxi;
   return B200LDLT_SUCCESS;
+}
+
+// b200ldlt_inverse_entries (host == true: vals in host memory) / _device
+static int inverse_entries(Solver* sv, int nent, const int* irow, const int* jcol, double* vals, bool host) {
+  const char* bad = nent < 0 ? "nent must be >= 0" : nent > 0 && (!irow || !jcol || !vals) ? "NULL argument" : nullptr;
+  for (int t = 0; !bad && t < nent; ++t)
+    if (irow[t] < 0 || irow[t] >= sv->n || jcol[t] < 0 || jcol[t] >= sv->n) bad = "index out of range";
+  if (bad) { sv->err = std::string("inverse_entries: ") + bad; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "inverse_entries"); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (nent == 0) return no_columns(sv);
+  { const int rc = sfs_state(sv, false); if (rc != B200LDLT_SUCCESS) return rc; }
+  { const int rc = inv_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
+  bool several = false;
+  for (int t = 0; !several && t < nent; ++t) several = irow[t] != irow[0] || jcol[t] != irow[0];
+  const bool blocked = several && block_solve_state(sv);
+  InvCall C;
+  { const int rc = inv_prepare(sv, nent, irow, jcol, blocked ? sv->an->blk->width : 1, C); if (rc != B200LDLT_SUCCESS) return rc; }
+  auto enqueue = [&](double* d) { return inv_enqueue(sv, C, d); };
+  return host ? staged_call(sv, nullptr, 0, vals, (size_t)nent, enqueue) : timed_call(sv, [&] { return enqueue(vals); });
 }
 
 // b200ldlt_solve_fredholm (host == true: x in host memory) / _device
@@ -2838,6 +3110,18 @@ int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bind
   return sparse_fwd(sv, nbi, bindex, d_b, false, nxi, xindex, d_x);
 }
 
+int b200ldlt_inverse_entries(b200ldlt_handle h, int nent, const int* irow, const int* jcol, double* vals) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return inverse_entries(sv, nent, irow, jcol, vals, true);
+}
+
+int b200ldlt_inverse_entries_device(b200ldlt_handle h, int nent, const int* irow, const int* jcol, double* d_vals) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return inverse_entries(sv, nent, irow, jcol, d_vals, false);
+}
+
 int b200ldlt_alter_d(b200ldlt_handle h, const double* dinv2) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
@@ -3249,6 +3533,7 @@ int64_t b200ldlt_symbolic_array(b200ldlt_handle h, const char* name, int64_t* ou
   if (nm == "level_ptr") RET(S.level_ptr);
   if (nm == "level_sn") RET(S.level_sn);
   if (nm == "sparse_run_set") { static const std::vector<int> none; RET(A.sfs ? A.sfs->last_run : none); }
+  if (nm == "inverse_run_set") { static const std::vector<int> none; RET(A.inv ? A.inv->last_run : none); }
 #undef RET
   return -1;
 }

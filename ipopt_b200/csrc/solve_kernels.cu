@@ -159,6 +159,79 @@ __global__ void k_sfs_out(int nx, const int* __restrict__ pos, const long long* 
   if (i < nx) { const int p = pos[i]; const long long q = piv_big[p]; out[i] = q >= 0 ? big[q] : xp[p]; }
 }
 
+// Entries of A^-1 (b200ldlt_inverse_entries): the sparse forward solve of a block of unit columns, column blockIdx.y = c
+// of the sweep state (x: leading dimension ldx, update vectors ldcbv, forward flags ldf).  Blocks [0, cdiv(ncol, 256)):
+// x at the ncol positions of the block's run set, scale (scale * 1.0, the multiply of k_sfs_in) at colpos[c], the pivot
+// position of the column's variable, and 0 elsewhere.  Blocks after that: frontier front fr[q], the column's slice of its
+// update vector zeroed and its forward flag set to this sweep's epoch, as in k_sfs_in.
+__global__ void k_inv_in(int ncol, const int* __restrict__ pos, const int* __restrict__ colpos, const int* __restrict__ perm,
+                         const double* __restrict__ scale, double* __restrict__ xp, long long ldx, const int* __restrict__ fr,
+                         const long long* __restrict__ rows_ptr, double* __restrict__ cbv, long long ldcbv,
+                         int* __restrict__ done_f, long long ldf, int epoch) {
+  const long long c = blockIdx.y;
+  const int nxb = (ncol + 255) / 256;
+  if ((int)blockIdx.x < nxb) {
+    const int j = blockIdx.x * 256 + threadIdx.x;
+    if (j < ncol) { const int p = pos[j]; xp[c * ldx + p] = p == colpos[c] ? scale[perm[p]] : 0.0; }
+    return;
+  }
+  const int f = fr[blockIdx.x - nxb];
+  const long long r0 = rows_ptr[f], r1 = rows_ptr[f + 1];
+  for (long long e = r0 + threadIdx.x; e < r1; e += blockDim.x) cbv[c * ldcbv + e] = 0.0;
+  if (threadIdx.x == 0) done_f[c * ldf + f] = epoch;
+}
+// The y store: column c0 + blockIdx.y of the call keeps its reach at [yoff[c], yoff[c + 1]), ypos the pivot positions and
+// y the sweep values there (see k_piv_out), read from column blockIdx.y of the sweep state.
+__global__ void k_inv_out(int c0, const long long* __restrict__ yoff, const int* __restrict__ ypos,
+                          const long long* __restrict__ piv_big, const double* __restrict__ xp, long long ldx,
+                          const double* __restrict__ big, long long ldbig, double* __restrict__ y) {
+  const long long c = blockIdx.y;
+  const long long i = yoff[c0 + c] + blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i < yoff[c0 + c + 1]) {
+    const int p = ypos[i];
+    const long long q = piv_big[p];
+    y[i] = q >= 0 ? big[c * ldbig + q] : xp[c * ldx + p];
+  }
+}
+
+// one entry M_ij = y_i^T D^-1 y_j: the common suffix of the two columns in the y store, m elements at a (y_i) and b (y_j)
+struct InvEnt {
+  long long a, b;
+  int m, pad;
+};
+
+// One warp per entry.  Lane l sums, in ascending order from +0, the terms that start at suffix offsets o = l (mod 32):
+// d (a b) for a 1x1 pivot, (d1 (a1 b1) + d2 (a2 b2)) + o12 ((a1 b2) + (a2 b1)) for a 2x2 pivot at its first position,
+// nothing at its second; then s += shfl_xor(s, k) for k = 16, 8, 4, 2, 1.  Every operation is rounded on its own (no
+// FMA), and each term and each butterfly step is symmetric in its operands, so (i, j) and (j, i) give the same bits and
+// a float64 replay on the host reproduces them.
+__global__ void k_inv_dot(int nent, const InvEnt* __restrict__ ent, const double* __restrict__ y, const int* __restrict__ ypos,
+                          const int* __restrict__ ptype, const double* __restrict__ dinv, const double* __restrict__ doff,
+                          double* __restrict__ vals) {
+  const int t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int l = threadIdx.x & 31;
+  if (t >= nent) return;   // (the whole warp)
+  const InvEnt E = ent[t];
+  const double* ya = y + E.a;
+  const double* yb = y + E.b;
+  const int* pa = ypos + E.a;
+  double s = 0.0;
+  for (int o = l; o < E.m; o += 32) {
+    const int p = pa[o], ty = ptype[p];
+    if (ty == 1) {
+      s = __dadd_rn(s, __dmul_rn(dinv[p], __dmul_rn(ya[o], yb[o])));
+    } else if (ty == 2) {
+      const double a1 = ya[o], a2 = ya[o + 1], b1 = yb[o], b2 = yb[o + 1];
+      const double dd = __dadd_rn(__dmul_rn(dinv[p], __dmul_rn(a1, b1)), __dmul_rn(dinv[p + 1], __dmul_rn(a2, b2)));
+      const double od = __dmul_rn(doff[p], __dadd_rn(__dmul_rn(a1, b2), __dmul_rn(a2, b1)));
+      s = __dadd_rn(s, __dadd_rn(dd, od));
+    }
+  }
+#pragma unroll
+  for (int k = 16; k > 0; k >>= 1) s = __dadd_rn(s, __shfl_xor_sync(0xffffffffu, s, k));
+  if (l == 0) vals[t] = s;
+}
+
 // r = b - A x from the original triplets (tests / bench parity helper)
 __global__ void k_residual_init(int n, const double* __restrict__ b, double* __restrict__ r) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
