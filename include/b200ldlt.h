@@ -363,6 +363,67 @@ int b200ldlt_error_analysis_device(b200ldlt_handle h, int nrhs, const double* d_
  * ainv1 = +inf, no estimator runs.  Kernel launches: 2 + (2 + L0) nprod.  Refused: a NULL kappa1. */
 int b200ldlt_condest(b200ldlt_handle h, double* kappa1, double* anorm1, double* ainv1, int* nprod);
 
+/* ---- iterative refinement by the componentwise backward error (cf. MUMPS ICNTL(10) / CNTL(2), MA57 job 2..4, LAPACK
+ * xSYRFS / xSYRFSX) ------------------------------------------------------------------------------------------------------
+ * Solves A x = b for nrhs columns and refines each x until its componentwise backward error omega (Arioli, Demmel, Duff)
+ * is small, stops improving, or max_steps corrections are taken.  The residual is accumulated in double-double, so omega
+ * can fall to about eps even where cond(A) eps is large -- e.g. after lifted pivots (info.num_forced > 0), where job 0
+ * solves a perturbed matrix.  A, M, s = |A| |x|, a_i, tau_i, I1, I2, omega1 and omega2 are those of
+ * b200ldlt_error_analysis above, bit for bit given r; only r differs.
+ *   Iterates:  x_0 = job 0 on b (bit-identical to b200ldlt_solve);  x_{k+1} = x_k (+) d_k,  d_k = job 0 on r_k, one
+ *              rounded add (__dadd_rn) per entry.
+ *   Residual:  r_k = b - A x_k.  Row i is one warp over the row's entries of |A|'s row structure (both triangles of the
+ *              unique entries, columns ascending); lane l takes entries l, l + 32, ... in order.  Every operation below is
+ *              one correctly rounded IEEE operation (nothing is contracted); TwoSum(a, c) = (s, t) with s = a (+) c,
+ *              v = s (-) a, t = (a (-) (s (-) v)) (+) (c (-) v).
+ *                lane 0 starts from (h, l) = (b_i, 0), the other lanes from (0, 0);
+ *                per entry: p = (-a_ij) (*) x_j, e = fma(-a_ij, x_j, -p); (h, t) = TwoSum(h, p); l = l (+) (t (+) e);
+ *                then for o = 16, 8, 4, 2, 1 with (h', l') of lane l xor o: (h, t) = TwoSum(h, h'); l = (l (+) l') (+) t;
+ *                r_i = h (+) l (lane 0's).
+ *              Barring overflow and underflow, with m_i the entries of row i and E_i the exact residual:
+ *                |r_i - E_i| <= 2^-53 |E_i| + (m_i + 32)^2 2^-105 (|b_i| + sum_j |a_ij x_j|),
+ *              so each reported omega is within 2^-51 w + (m + 32)^2 2^-103 of the value w it has with exact residuals
+ *              (same s, classes and weights), m the longest row.
+ *   Omega:     omega_k = omega1 + omega2 of x_k (one rounded add).
+ *   Stopping:  on each iterate k = 0, 1, ..., in this order:
+ *                1. omega_k not finite: the result is the last iterate with a finite omega, status 3 (x_0 itself when
+ *                   k = 0, with its omega1 and omega2 as computed, so omega_first = +inf);
+ *                2. omega_k <= tol: x_k, status 0;
+ *                3. k >= 1 and omega_k > omega_{k-1} / 2: x_k if omega_k < omega_{k-1}, else x_{k-1}; status 1;
+ *                4. k = max_steps: x_k, status 2;
+ *              otherwise the column takes the next correction.  So the returned omega never exceeds omega_first, and
+ *              max_steps = 0 returns job 0 with its omega.  An inconsistent column (kept singular factors) ends by
+ *              stagnation.  A column with b = 0 returns x = 0 at k = 0, status 0.
+ *   Blocks:    columns run in blocks of up to B200_SOLVE_BLOCK (8 by default) in lockstep; each step solves only the
+ *              block's unfinished columns, packed into consecutive solve slots, and a finished column that returns
+ *              x_{k-1} gets it back from a copy.  Without the blocked state (B200_SOLVE_BLOCK = 1 or no memory for it)
+ *              the columns run one by one.  Every column's x and struct are bit-identical to a call on that column alone,
+ *              under any B200_SOLVE_BLOCK, between the two entry points and across calls.
+ * Kernel launches, with L0 = job 0's launches per block (4 + 2 D, 8 by default): 1 (the unique values) + per block
+ * E (L0 + 3) - 1, where E is the largest nres of the block's columns: x_0 (L0), per iterate the row pass and the row
+ * classes (2), per correction job 0 and the update kernel (L0 + 1).  One column: nres (L0 + 3).  Each iterate ends in one
+ * small D2H and a host decision, and the call synchronises per iterate.
+ * Memory: the state of b200ldlt_error_analysis (|A| by rows at the first call after an analysis, its 16 n bytes per
+ * column) for the block width, plus 16 n bytes per column of the block for the solve slots and the rollback copies
+ * (grown to the largest call, kept until the next analysis), and the blocked solve state if nrhs > 1 allocates it first.
+ * The host entry point stages 2 n nrhs doubles (x and a copy of b).
+ * b and x are n x nrhs, column-major; b is not modified and x may not be b; out is nrhs structs in host memory for both
+ * entry points.  Timing (info.ms_solve_gpu, launches_solve) and refusals follow the solve family: no factors, a sharded
+ * handle, Schur mode; and nrhs < 0, max_steps < 0, tol < 0 or NaN, a NULL pointer with nrhs > 0, x == b.  Nothing is
+ * written on a refusal; nrhs = 0 is the no-columns case.  The call leaves the factors, D, later solves and the results
+ * of b200ldlt_error_analysis as they were. */
+typedef struct b200ldlt_refined {
+  double omega_first;    /* omega1 + omega2 of x_0, the plain job-0 solution                                        */
+  double omega1, omega2; /* componentwise backward errors of the returned x                                         */
+  int steps;             /* corrections contained in the returned x                                                  */
+  int status;            /* 0 converged (omega <= tol), 1 stagnated, 2 max_steps reached, 3 non-finite omega          */
+  int nres;              /* residuals evaluated (iterates 0 .. nres - 1; steps + 1, or steps + 2 after a rollback)    */
+} b200ldlt_refined;
+int b200ldlt_solve_refined(b200ldlt_handle h, int nrhs, const double* b, double* x, int max_steps, double tol,
+                           b200ldlt_refined* out);
+int b200ldlt_solve_refined_device(b200ldlt_handle h, int nrhs, const double* d_b, double* d_x, int max_steps,
+                                  double tol, b200ldlt_refined* out);
+
 /* <-> NumberOfNegEVals() (hpp:207) */
 int b200ldlt_num_neg(b200ldlt_handle h);
 /* <-> IncreaseQuality() (hpp:220): pivtol <- min(pivtolmax, pivtol^0.75); returns 0 if already at max.

@@ -57,6 +57,12 @@ class Errors(C.Structure):
                 ("n_i2", C.c_int), ("nprod", C.c_int)]
 
 
+class Refined(C.Structure):
+    """b200ldlt_refined: the outcome of the refinement of one column (see include/b200ldlt.h)"""
+    _fields_ = [("omega_first", C.c_double), ("omega1", C.c_double), ("omega2", C.c_double), ("steps", C.c_int),
+                ("status", C.c_int), ("nres", C.c_int)]
+
+
 EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "b200ldlt_last_error",
             "b200ldlt_analyse", "b200ldlt_values_ptr", "b200ldlt_factor", "b200ldlt_factor_device",
             "b200ldlt_solve", "b200ldlt_solve_device", "b200ldlt_num_neg", "b200ldlt_increase_quality",
@@ -71,7 +77,8 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_schur_complement", "b200ldlt_schur_complement_device", "b200ldlt_schur_reduce",
             "b200ldlt_schur_reduce_device", "b200ldlt_schur_expand", "b200ldlt_schur_expand_device",
             "b200ldlt_error_analysis", "b200ldlt_error_analysis_device", "b200ldlt_condest",
-            "b200ldlt_inverse_entries", "b200ldlt_inverse_entries_device"]
+            "b200ldlt_inverse_entries", "b200ldlt_inverse_entries_device", "b200ldlt_solve_refined",
+            "b200ldlt_solve_refined_device"]
 
 _lib = None
 
@@ -132,6 +139,8 @@ def load_library():
     L.b200ldlt_error_analysis.argtypes = [vp, C.c_int, dp, dp, C.c_int, C.POINTER(Errors)]
     L.b200ldlt_error_analysis_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.POINTER(Errors)]
     L.b200ldlt_condest.argtypes = [vp, dp, dp, dp, ip]
+    L.b200ldlt_solve_refined.argtypes = [vp, C.c_int, dp, dp, C.c_int, C.c_double, C.POINTER(Refined)]
+    L.b200ldlt_solve_refined_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_double, C.POINTER(Refined)]
     L.b200ldlt_num_neg.argtypes = [vp]
     L.b200ldlt_increase_quality.argtypes = [vp]
     L.b200ldlt_get_info.argtypes = [vp, C.POINTER(Info)]
@@ -499,6 +508,32 @@ class B200Ldlt:
         st = self._L.b200ldlt_error_analysis_device(self._h, int(nrhs), C.c_void_p(d_b_ptr), C.c_void_p(d_x_ptr),
                                                     int(cond), out)
         return st, self._errors_dict(out[:int(nrhs)], False)
+
+    @staticmethod
+    def _refined_dict(out):
+        return {k: np.array([getattr(o, k) for o in out], dtype=np.int32 if t is C.c_int else np.float64)
+                for k, t in Refined._fields_}
+
+    def solve_refined(self, B, max_steps=10, tol=2.0 ** -52):
+        """Solve A X = B (dim or dim x nrhs) with iterative refinement until the componentwise backward error is <= tol,
+        stops improving or max_steps corrections are taken (b200ldlt_solve_refined).  Returns (X, dict of per-column
+        arrays: omega_first, omega1, omega2, steps, status, nres).  Raises on a refusal."""
+        B = np.asarray(B, dtype=np.float64)
+        Bm = np.asfortranarray(B.reshape(self.dim, -1, order="F"))
+        nrhs = Bm.shape[1]
+        X = np.zeros_like(Bm, order="F")
+        out = (Refined * max(nrhs, 1))()
+        if self._L.b200ldlt_solve_refined(self._h, nrhs, _dptr(Bm), _dptr(X), int(max_steps), float(tol),
+                                          out) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return X.reshape(B.shape, order="F"), self._refined_dict(out[:nrhs])
+
+    def solve_refined_device(self, d_b_ptr, d_x_ptr, nrhs=1, max_steps=10, tol=2.0 ** -52):
+        """The same on device arrays of dim x nrhs doubles (x written).  Returns (status, dict of per-column arrays)."""
+        out = (Refined * max(int(nrhs), 1))()
+        st = self._L.b200ldlt_solve_refined_device(self._h, int(nrhs), C.c_void_p(d_b_ptr), C.c_void_p(d_x_ptr),
+                                                   int(max_steps), float(tol), out)
+        return st, self._refined_dict(out[:int(nrhs)])
 
     def condest(self):
         """(kappa1, anorm1, ainv1, nprod): the 1-norm condition estimate ||A||_1 est||M||_1 (b200ldlt_condest).  Raises

@@ -178,11 +178,12 @@ struct SelInvPlan {
 // values of the call (k_sum_dups of d_vals: d_uval is scaled in place by the factorisation) and the row maxima a_i; per
 // right-hand side r and s, overwritten by w1 and w2, and the reduced norms (grown to the largest call); the estimators'
 // input / product vectors and sign vectors (one column per estimator of a block) and the reduction scratch of
-// k_ea_post.  Built at the first call after an analysis, before its timing starts; a handle that never makes the calls
+// k_ea_post; for the refinement (b200ldlt_solve_refined) the solve slots of a block (r, then d) and the rollback copies
+// of its x.  Built at the first call after an analysis, before its timing starts; a handle that never makes the calls
 // allocates none of it.
 struct EaPlan {
   DevBuf<int> d_ptr, d_col, d_uid;
-  DevBuf<double> d_uval, d_amax, d_rs, d_v;
+  DevBuf<double> d_uval, d_amax, d_rs, d_v, d_rf_d, d_rf_old;
   DevBuf<unsigned long long> d_nrm;
   DevBuf<signed char> d_xi;
   DevBuf<EaPart> d_part;
@@ -2443,11 +2444,12 @@ static int timed_call(Solver* sv, Enqueue&& enqueue, Drain&& drain = Drain()) {
 // back to `out` (which may be `in`), the copies inside the timed window.  Each way the copies run in at most four
 // chunks, so that the DMA of one chunk runs under the host copy of the next (the caller's array is pageable: Ipopt
 // allocates it per call, IpTSymLinearSolver.cpp:222-241).  The staging grows to the largest call and lasts until the
-// next analysis.
+// next analysis.  nwork: the staging holds at least that many doubles (device scratch of enqueue beyond in and out).
 template <class Enqueue>
-static int staged_call(Solver* sv, const double* in, size_t nin, double* out, size_t nout, Enqueue&& enqueue) {
+static int staged_call(Solver* sv, const double* in, size_t nin, double* out, size_t nout, Enqueue&& enqueue,
+                       size_t nwork = 0) {
   Analysis& A = *sv->an;
-  const size_t need = std::max(nin, nout);
+  const size_t need = std::max(std::max(nin, nout), nwork);
   if (need > A.d_rhs.n) {
     A.d_rhs.release();
     if (A.h_rhs) cudaFreeHost(A.h_rhs);
@@ -2910,8 +2912,9 @@ static int enqueue_ea_rows(Solver* sv, int nrhs, const double* d_b, const double
   CU(cudaMemsetAsync(P.d_nrm.p, 0, ((size_t)EA_NRM * nrhs + 1) * sizeof(unsigned long long), st));
   k_sum_dups<<<cdiv(nu, 256), 256, 0, st>>>(nu, A.d_useg_ptr.p, A.d_useg_src.p, sv->d_vals.p, P.d_uval.p);
   const unsigned g = std::min<unsigned>(cdiv(n, EA_WARPS), EA_ROW_CTAS);
-  k_ea_rows<<<dim3(g, std::max(nrhs, 1)), EA_THREADS, 0, st>>>(n, nrhs, P.d_ptr.p, P.d_col.p, P.d_uid.p, P.d_uval.p, d_b,
-                                                               d_x, P.d_rs.p, P.d_amax.p, P.d_nrm.p);
+  k_ea_rows<false><<<dim3(g, std::max(nrhs, 1)), EA_THREADS, 0, st>>>(n, nrhs, P.d_ptr.p, P.d_col.p, P.d_uid.p, P.d_uval.p,
+                                                                      d_b, d_x, P.d_rs.p, P.d_amax.p, P.d_nrm.p, RfCols{},
+                                                                      nullptr);
   sv->launches += 2;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
@@ -2943,7 +2946,8 @@ static int error_analysis(Solver* sv, int nrhs, const double* b, const double* x
   std::vector<int> nprod(nrhs, 0);
   auto enqueue = [&](const double* d_b, const double* d_x) -> int {
     { const int rc = enqueue_ea_rows(sv, nrhs, d_b, d_x); if (rc != B200LDLT_SUCCESS) return rc; }
-    k_ea_class<<<dim3(cdiv(n, EA_THREADS), nrhs), EA_THREADS, 0, st>>>(n, d_b, P.d_amax.p, P.d_rs.p, P.d_nrm.p);
+    k_ea_class<false><<<dim3(cdiv(n, EA_THREADS), nrhs), EA_THREADS, 0, st>>>(n, d_b, P.d_amax.p, P.d_rs.p, P.d_nrm.p,
+                                                                              RfCols{}, nullptr);
     ++sv->launches;
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(nrm.data(), P.d_nrm.p, nrm.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
@@ -3006,6 +3010,117 @@ static int error_analysis(Solver* sv, int nrhs, const double* b, const double* x
       o.ferr = o.omega1 * o.cond1 + o.omega2 * o.cond2;
     }
   }
+  return B200LDLT_SUCCESS;
+}
+
+// ---- iterative refinement (b200ldlt_solve_refined) -------------------------------------------------------------------
+// One column's state: the omegas of its last accepted iterate, its result fields and the residuals evaluated
+struct RfCol {
+  double first = 0.0, om1 = 0.0, om2 = 0.0;
+  int steps = 0, status = -1, nres = 0;
+};
+
+// The stopping rule of include/b200ldlt.h after the omegas of iterate k: 0 = go on to x_{k+1} (C now describes x_k),
+// 1 = x_k is the result, 2 = x_{k-1} is the result (C still describes it)
+static int rf_rule(RfCol& C, double om1, double om2, int k, int max_steps, double tol) {
+  const double om = om1 + om2, prev = C.om1 + C.om2;
+  C.nres = k + 1;
+  if (k == 0) C.first = om;
+  auto take = [&](int status) { C.om1 = om1; C.om2 = om2; C.steps = k; C.status = status; return status < 0 ? 0 : 1; };
+  auto back = [&](int status) { C.steps = k - 1; C.status = status; return 2; };
+  if (!std::isfinite(om)) return k == 0 ? take(3) : back(3);
+  if (om <= tol) return take(0);
+  if (k >= 1 && om > prev / 2) return om < prev ? take(1) : back(1);
+  if (k == max_steps) return take(2);
+  return take(-1);
+}
+
+// b200ldlt_solve_refined (host == true: b and x in host memory) / _device
+static int solve_refined(Solver* sv, int nrhs, const double* b, double* x, int max_steps, double tol,
+                         b200ldlt_refined* out, bool host) {
+  const char* bad = nrhs < 0 ? "nrhs must be >= 0" : max_steps < 0 ? "max_steps must be >= 0"
+                    : !(tol >= 0.0) ? "tol must be >= 0" : nrhs > 0 && (!b || !x || !out) ? "NULL argument"
+                    : nrhs > 0 && b == x ? "x must not be b" : nullptr;
+  if (bad) { sv->err = std::string("solve_refined: ") + bad; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "solve_refined"); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (nrhs == 0) return no_columns(sv);
+  Analysis& A = *sv->an;
+  const int n = sv->n;
+  const size_t nb = (size_t)n * nrhs;
+  const bool blocked = nrhs > 1 && block_solve_state(sv);
+  SweepState& W = blocked ? *A.blk : A.sweep;
+  const int width = blocked ? W.width : 1;
+  { const int rc = ea_state(sv, width, 0); if (rc != B200LDLT_SUCCESS) return rc; }
+  EaPlan& P = *A.ea;
+  if (P.d_rf_d.n < (size_t)n * width) { CU(P.d_rf_d.alloc((size_t)n * width)); CU(P.d_rf_old.alloc((size_t)n * width)); }
+  cudaStream_t st = sv->stream;
+  std::vector<RfCol> R(nrhs);
+  // x_held: d_x already holds b (the host staging)
+  auto enqueue = [&](const double* d_b, double* d_x, bool x_held) -> int {
+    const long long nu = A.S.nnz_u;
+    k_sum_dups<<<cdiv(nu, 256), 256, 0, st>>>(nu, A.d_useg_ptr.p, A.d_useg_src.p, sv->d_vals.p, P.d_uval.p);
+    ++sv->launches;
+    const unsigned g = std::min<unsigned>(cdiv(n, EA_WARPS), EA_ROW_CTAS);
+    return for_blocks(nrhs, width, [&](int c0, int w) -> int {
+      const double* bb = d_b + (size_t)c0 * n;
+      double* xb = d_x + (size_t)c0 * n;
+      if (!x_held) CU(cudaMemcpyAsync(xb, bb, (size_t)n * w * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      { const int rc = enqueue_solve(sv, W, 0, xb, xb, w); if (rc != B200LDLT_SUCCESS) return rc; }
+      RfCols act;
+      int na = w;
+      for (int s = 0; s < w; ++s) act.c[s] = s;
+      std::vector<unsigned long long> nrm((size_t)EA_NRM * w + 1);
+      for (int k = 0;; ++k) {
+        // r (double-double) of the unfinished columns into the slots, s and the omegas; one D2H of the maxima
+        CU(cudaMemsetAsync(P.d_nrm.p, 0, ((size_t)EA_NRM * na + 1) * sizeof(unsigned long long), st));
+        k_ea_rows<true><<<dim3(g, na), EA_THREADS, 0, st>>>(n, na, P.d_ptr.p, P.d_col.p, P.d_uid.p, P.d_uval.p, bb, xb,
+                                                            P.d_rs.p, P.d_amax.p, P.d_nrm.p, act, P.d_rf_d.p);
+        k_ea_class<true><<<dim3(cdiv(n, EA_THREADS), na), EA_THREADS, 0, st>>>(n, bb, P.d_amax.p, P.d_rs.p, P.d_nrm.p, act,
+                                                                               P.d_rf_d.p);
+        sv->launches += 2;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(nrm.data(), P.d_nrm.p, (size_t)EA_NRM * na * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        // the rule per column; a finished column that returns x_{k-1} gets it back, the others' r close up
+        RfCols next;
+        int nn = 0;
+        for (int s = 0; s < na; ++s) {
+          const int c = act.c[s];
+          const int v = rf_rule(R[c0 + c], ea_val(nrm[(size_t)EA_NRM * s + EA_W1]), ea_val(nrm[(size_t)EA_NRM * s + EA_W2]), k,
+                                max_steps, tol);
+          if (v == 2)
+            CU(cudaMemcpyAsync(xb + (size_t)c * n, P.d_rf_old.p + (size_t)c * n, (size_t)n * sizeof(double),
+                               cudaMemcpyDeviceToDevice, st));
+          if (v != 0) continue;
+          if (nn != s)
+            CU(cudaMemcpyAsync(P.d_rf_d.p + (size_t)nn * n, P.d_rf_d.p + (size_t)s * n, (size_t)n * sizeof(double),
+                               cudaMemcpyDeviceToDevice, st));
+          next.c[nn++] = c;
+        }
+        if (nn == 0) return B200LDLT_SUCCESS;
+        // d = job 0 on the slots, then x_{k+1} = x_k (+) d with x_k kept for a rollback
+        { const int rc = enqueue_solve(sv, W, 0, P.d_rf_d.p, P.d_rf_d.p, nn); if (rc != B200LDLT_SUCCESS) return rc; }
+        k_rf_update<<<dim3(cdiv(n, EA_THREADS), nn), EA_THREADS, 0, st>>>(n, next, P.d_rf_d.p, xb, P.d_rf_old.p);
+        ++sv->launches;
+        CU(cudaGetLastError());
+        act = next;
+        na = nn;
+      }
+    });
+  };
+  int rc;
+  if (host) {
+    // the staging holds x (b on entry, the refined x on exit) and then a copy of b
+    rc = staged_call(sv, b, nb, x, nb, [&](double* d) -> int {
+      CU(cudaMemcpyAsync(d + nb, d, nb * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      return enqueue(d + nb, d, true);
+    }, 2 * nb);
+  } else {
+    rc = timed_call(sv, [&] { return enqueue(b, x, false); });
+  }
+  if (rc != B200LDLT_SUCCESS) return rc;
+  for (int c = 0; c < nrhs; ++c)
+    out[c] = b200ldlt_refined{R[c].first, R[c].om1, R[c].om2, R[c].steps, R[c].status, R[c].nres};
   return B200LDLT_SUCCESS;
 }
 
@@ -3201,6 +3316,20 @@ int b200ldlt_error_analysis_device(b200ldlt_handle h, int nrhs, const double* d_
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
   return error_analysis(sv, nrhs, d_b, d_x, cond, out, false);
+}
+
+int b200ldlt_solve_refined(b200ldlt_handle h, int nrhs, const double* b, double* x, int max_steps, double tol,
+                           b200ldlt_refined* out) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return solve_refined(sv, nrhs, b, x, max_steps, tol, out, true);
+}
+
+int b200ldlt_solve_refined_device(b200ldlt_handle h, int nrhs, const double* d_b, double* d_x, int max_steps,
+                                  double tol, b200ldlt_refined* out) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return solve_refined(sv, nrhs, d_b, d_x, max_steps, tol, out, false);
 }
 
 int b200ldlt_condest(b200ldlt_handle h, double* kappa1, double* anorm1, double* ainv1, int* nprod) {

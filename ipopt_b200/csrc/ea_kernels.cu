@@ -6,6 +6,10 @@
 // estimator columns around one solve: prep builds each column's next input, post reduces each column's product to the
 // few numbers the host needs for dlacn2's decisions.
 //
+// k_ea_rows<true> / k_ea_class<true> / k_rf_update: one step of iterative refinement (b200ldlt_solve_refined) for the
+// unfinished columns of a block -- the residual in double-double straight into the solve's slots, s and the backward
+// errors as above, and after the solve of the slots x += d with x saved for a rollback.
+//
 // Every result is bit-reproducible: maxima are atomicMax on the bit patterns of non-negative doubles (exact, whatever the
 // order), |I2| an integer count, and every sum has a fixed order -- a row's entries by a fixed lane split and shuffle tree,
 // a vector's 1-norm by a fixed grid (a function of n only), a fixed tree in each CTA and the CTAs' partials in order.
@@ -66,46 +70,78 @@ __device__ __forceinline__ void ea_cta_max(double (&v)[NV], unsigned long long* 
   }
 }
 
+// The columns of a refinement step: slot s (blockIdx.y) holds column c[s] of b and x (counted from the block's first)
+struct RfCols { int c[MS_NB_MAX]; };
+
+// (s, t) with s + t = a + b exactly (Knuth's TwoSum, six rounded operations, no contraction)
+__device__ __forceinline__ void rf_two_sum(double a, double b, double& s, double& t) {
+  s = __dadd_rn(a, b);
+  const double bb = __dsub_rn(s, a);
+  t = __dadd_rn(__dsub_rn(a, __dsub_rn(s, bb)), __dsub_rn(b, bb));
+}
+
 // One warp per row i of |A| (grid-stride), column c = blockIdx.y of b / x (b == nullptr: only the A part).  The row's
 // entries (both triangles of the unique entries, columns ascending) are split over the lanes by position, each lane sums
 // its own in order, and a shuffle tree combines the lanes: a fixed order.
 //   r_i = b_i - sum_j a_ij x_j,  s_i = sum_j |a_ij| |x_j|  -> rs[2 c n + i], rs[(2 c + 1) n + i]
 //   max |x_i|, max |r_i|, max |b_i|  -> nrm (EA_X, EA_R, EA_B of column c)
 // and, for c = 0: amax[i] = max_j |a_ij| and max_i sum_j |a_ij| -> nrm[EA_NRM nrhs].
+// DD (refinement): slot c = blockIdx.y reads column cols.c[c] of b / x, and r is accumulated in double-double in the
+// order include/b200ldlt.h states and written to rout[c n + i] (s, the norms and the A part as above, by slot).
+template <bool DD>
 __global__ void __launch_bounds__(EA_THREADS) k_ea_rows(int n, int nrhs, const int* __restrict__ ptr,
                                                         const int* __restrict__ col, const int* __restrict__ uid,
                                                         const double* __restrict__ uval, const double* __restrict__ b,
                                                         const double* __restrict__ x, double* __restrict__ rs,
-                                                        double* __restrict__ amax, unsigned long long* __restrict__ nrm) {
+                                                        double* __restrict__ amax, unsigned long long* __restrict__ nrm,
+                                                        RfCols cols, double* __restrict__ rout) {
   const int lane = threadIdx.x & 31;
   const int c = blockIdx.y;
+  const size_t cc = DD ? (size_t)cols.c[c] : (size_t)c;
   const bool rhs = b != nullptr, mat = c == 0;
-  const double* xc = rhs ? x + (size_t)c * n : nullptr;
-  const double* bc = rhs ? b + (size_t)c * n : nullptr;
+  const double* xc = rhs ? x + cc * n : nullptr;
+  const double* bc = rhs ? b + cc * n : nullptr;
   double mx[4] = {0.0, 0.0, 0.0, 0.0};   // |x|, |r|, |b|, row sum of |A|
   const int nwarps = gridDim.x * EA_WARPS;
   for (int i = blockIdx.x * EA_WARPS + (threadIdx.x >> 5); i < n; i += nwarps) {
     double ax = 0.0, sx = 0.0, am = 0.0, as = 0.0;
+    double hi = 0.0, lo = 0.0;   // DD: this lane's (h, l)
+    if (DD && lane == 0) hi = bc[i];
     for (int e = ptr[i] + lane; e < ptr[i + 1]; e += 32) {
       const double a = uval[uid[e]];
       if (rhs) {
         const double xj = xc[col[e]];
-        ax += a * xj;
+        if (DD) {
+          const double na = -a, p = __dmul_rn(na, xj), q = __fma_rn(na, xj, -p);
+          double t;
+          rf_two_sum(hi, p, hi, t);
+          lo = __dadd_rn(lo, __dadd_rn(t, q));
+        } else {
+          ax += a * xj;
+        }
         sx += fabs(a) * fabs(xj);
       }
       if (mat) { am = fmax(am, fabs(a)); as += fabs(a); }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-      ax += __shfl_xor_sync(0xffffffffu, ax, o);
+      if (DD) {
+        const double h2 = __shfl_xor_sync(0xffffffffu, hi, o), l2 = __shfl_xor_sync(0xffffffffu, lo, o);
+        double t;
+        rf_two_sum(hi, h2, hi, t);
+        lo = __dadd_rn(__dadd_rn(lo, l2), t);
+      } else {
+        ax += __shfl_xor_sync(0xffffffffu, ax, o);
+      }
       sx += __shfl_xor_sync(0xffffffffu, sx, o);
       am = fmax(am, __shfl_xor_sync(0xffffffffu, am, o));
       as += __shfl_xor_sync(0xffffffffu, as, o);
     }
     if (lane == 0) {
       if (rhs) {
-        const double r = bc[i] - ax;
-        rs[(size_t)2 * c * n + i] = r;
+        const double r = DD ? __dadd_rn(hi, lo) : bc[i] - ax;
+        if (DD) rout[(size_t)c * n + i] = r;
+        else rs[(size_t)2 * c * n + i] = r;
         rs[(size_t)(2 * c + 1) * n + i] = sx;
         mx[0] = fmax(mx[0], ea_abs(xc[i]));
         mx[1] = fmax(mx[1], ea_abs(r));
@@ -123,10 +159,14 @@ __global__ void __launch_bounds__(EA_THREADS) k_ea_rows(int n, int nrhs, const i
 //   tau_i = ctau (a_i ||x|| + |b_i|), ctau = 1000 n 2^-52;  i in I2 iff s_i + |b_i| <= tau_i, else I1;
 //   omega1 = max_I1 |r_i| / (s_i + |b_i|),  omega2 = max_I2 |r_i| / (s_i + a_i ||x||)  (a term with r_i = 0 is 0);
 //   w1 = s_i + |b_i| on I1, w2 = s_i + a_i ||x|| on I2, 0 elsewhere;  |I2| counted.
+// RF (refinement): slot c reads column cols.c[c] of b and its r from rin[c n + i]; rs keeps s, no weights are written.
+template <bool RF>
 __global__ void __launch_bounds__(EA_THREADS) k_ea_class(int n, const double* __restrict__ b, const double* __restrict__ amax,
-                                                         double* __restrict__ rs, unsigned long long* __restrict__ nrm) {
+                                                         double* __restrict__ rs, unsigned long long* __restrict__ nrm,
+                                                         RfCols cols, const double* __restrict__ rin) {
   const int i = blockIdx.x * EA_THREADS + threadIdx.x;
   const int c = blockIdx.y;
+  const size_t cc = RF ? (size_t)cols.c[c] : (size_t)c;
   unsigned long long* base = nrm + (size_t)EA_NRM * c;
   const double xn = __longlong_as_double((long long)base[EA_X]);
   const double ctau = 1000.0 * (double)n * 0x1p-52;
@@ -135,7 +175,8 @@ __global__ void __launch_bounds__(EA_THREADS) k_ea_class(int n, const double* __
   if (i < n) {
     double* r_w1 = rs + (size_t)2 * c * n;
     double* s_w2 = rs + (size_t)(2 * c + 1) * n;
-    const double r = r_w1[i], s = s_w2[i], ab = fabs(b[(size_t)c * n + i]), ax = amax[i] * xn;
+    const double r = RF ? rin[(size_t)c * n + i] : r_w1[i];
+    const double s = s_w2[i], ab = fabs(b[cc * n + i]), ax = amax[i] * xn;
     const double tau = ctau * (ax + ab);
     double w1 = 0.0, w2 = 0.0;
     if (s + ab <= tau) {
@@ -146,13 +187,27 @@ __global__ void __launch_bounds__(EA_THREADS) k_ea_class(int n, const double* __
       w1 = s + ab;
       if (r != 0.0) om[0] = ea_abs(r / w1);
     }
-    r_w1[i] = w1;
-    s_w2[i] = w2;
+    if (!RF) {
+      r_w1[i] = w1;
+      s_w2[i] = w2;
+    }
   }
   const unsigned cnt = __syncthreads_count(in2);
   unsigned long long* const dst[2] = {base + EA_W1, base + EA_W2};
   ea_cta_max<2>(om, dst);
   if (threadIdx.x == 0 && cnt) atomicAdd(base + EA_NI2, (unsigned long long)cnt);
+}
+
+// The update of a refinement step: slot s = blockIdx.y holds the correction d of column c = cols.c[s] (counted from the
+// block's first); xold[c n + i] = x[c n + i], then x[c n + i] = x[c n + i] (+) d[s n + i], one rounded add.
+__global__ void __launch_bounds__(EA_THREADS) k_rf_update(int n, RfCols cols, const double* __restrict__ d,
+                                                          double* __restrict__ x, double* __restrict__ xold) {
+  const int i = blockIdx.x * EA_THREADS + threadIdx.x;
+  if (i >= n) return;
+  const size_t c = (size_t)cols.c[blockIdx.y];
+  const double v = x[c * n + i];
+  xold[c * n + i] = v;
+  x[c * n + i] = __dadd_rn(v, d[(size_t)blockIdx.y * n + i]);
 }
 
 // The input of estimator column s = blockIdx.y of a step: v[s n + i] = (its mode's vector)_i * pre_i
