@@ -157,6 +157,49 @@ int b200ldlt_sparse_fwd_solve(b200ldlt_handle h, int nbi, const int* bindex, con
 int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bindex, const double* d_b, int* nxi, int* xindex,
                                      double* d_x);
 
+/* ---- sparse solve: chosen entries of A^-1 b for a sparse b (cf. Pardiso iparm(31), MUMPS ICNTL(20)) -------------------
+ * nrhs columns b_c that share one pattern, and the entries of x_c = M b_c at chosen variables; M as for selected inversion
+ * below (A^-1, the perturbed matrix's inverse with info.num_forced > 0, D^+ on kept singular factors, the altered D after
+ * alter_d): the operator of job 0.  Column c of b is compact: b[c*nbi + i] is its value at variable bindex[i], and it is
+ * zero elsewhere.  On return x[c*nxs + i] is entry xsel[i] of x_c.  The indices are 0-based original variables in host
+ * memory for both entry points; bindex entries are distinct, xsel entries may repeat and come in any order.
+ *   bindex == NULL (nbi = n): b is dense (b[c*n + v] at variable v); the forward stage is job 0's;
+ *   xsel == NULL (nxs = n):   every entry (x[c*n + v]); the backward stage and the output are job 0's;
+ *   both NULL:                the call IS b200ldlt_solve on b: the same launches and the same bits.
+ * x_c = S P L^-T D^-1 L^-1 P^T S b_c.  L^-1 P^T S b_c is non-zero only on the REACH of bindex (sparse_fwd_solve), and the
+ * entries at xsel need L^-T only on the reach of xsel: the fronts on the tree paths from their fronts to the root.  The
+ * forward sweep runs job 0's front routines (D^-1 applied as the fused sweep applies it) over the run set R_f of bindex
+ * -- the work lists of the full solve pruned to the reach and the fronts that share a work item with one, as in
+ * sparse_fwd_solve -- and the backward sweep runs job 0's over the run set R_b of xsel, pruned the same way over the
+ * backward lists.  The fronts of R_b outside R_f start the backward sweep from zero.  Both run sets are built once per
+ * call and shared by every column, with a check that refuses, before anything is launched, a pruned sweep that could
+ * wait forever.
+ * Values: every returned entry equals job 0 on the dense b as a value (the two may differ in the sign of a zero, as
+ * sparse_fwd_solve allows).  Repeated calls, both entry points and any B200_SOLVE_BLOCK give the same bits, and every
+ * column is bit-identical to a call on that column alone.
+ * Kernel launches per block of up to B200_SOLVE_BLOCK columns (blocked as b200ldlt_solve is):
+ *   1 (input) + d_f + t_f + 1 (between the sweeps) + d_b + t_b + 1 (output)
+ * with d_f and t_f counted as for sparse_fwd_solve on the reach of bindex (d_f: the B200_SOLVE_DIRECT bottom levels that
+ * hold a direct front of R_f, t_f = 1 when R_f has a front above them), d_b and t_b the same counts for R_b; a dense b
+ * gives d_f = D and t_f = 1, a full selection d_b = D and t_b = 1 (D = the direct levels that hold any front).  With both
+ * NULL: job 0's 4 + 2 D.  nbi = 0 is a zero b: d_f = t_f = 0.
+ * Memory: the first call after an analysis builds sparse_fwd_solve's per-front indices (not its staging) and a host copy
+ * of the backward top tasks indexed by front, before its timing starts; each call stages its pruned lists and position
+ * lists (4 bytes per position of R_f twice, per zeroed position and per selected entry) in pinned and device staging
+ * that grows to the largest call and is freed by the next analysis; a handle that never makes the call allocates none
+ * of it.  symbolic_array "sparse_solve_fwd_run_set" and "sparse_solve_bwd_run_set" return the run sets of the last call
+ * (every front for a dense b / a full selection), ascending; the call leaves "sparse_run_set", "inverse_run_set", the
+ * factors, D and every later solve as they were.
+ * Refused (FATAL_ERROR with "sparse_solve: <reason>", nothing written to x): nrhs < 0, nbi < 0 or nbi > n, nxs < 0; a
+ * NULL b with nrhs, nbi > 0 or a NULL x with nrhs, nxs > 0; a NULL bindex with nbi != n or a NULL xsel with nxs != n; an
+ * index out of range or a repeated bindex entry; the failed dependency check; a failed staging allocation.
+ * nrhs = 0 or nxs = 0 is the no-columns case.  Device entry point: d_b (nrhs*nbi doubles) and d_x (nrhs*nxs) are
+ * device memory. */
+int b200ldlt_sparse_solve(b200ldlt_handle h, int nrhs, int nbi, const int* bindex, const double* b, int nxs, const int* xsel,
+                          double* x);
+int b200ldlt_sparse_solve_device(b200ldlt_handle h, int nrhs, int nbi, const int* bindex, const double* d_b, int nxs,
+                                 const int* xsel, double* d_x);
+
 /* ---- multiplication by the factors and alteration of D (cf. HSL_MA97 ma97_lmultiply / ma97_alter) --------------------
  * Same conventions as the partial solves (S A S = P L D L^T P^T, vectors in pivot order indexed by pivot position p):
  *   trans = 0 :  y = S^-1 P L x        x in pivot order, y in original order   (the inverse of job 1)

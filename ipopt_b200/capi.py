@@ -78,7 +78,7 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_schur_reduce_device", "b200ldlt_schur_expand", "b200ldlt_schur_expand_device",
             "b200ldlt_error_analysis", "b200ldlt_error_analysis_device", "b200ldlt_condest",
             "b200ldlt_inverse_entries", "b200ldlt_inverse_entries_device", "b200ldlt_solve_refined",
-            "b200ldlt_solve_refined_device"]
+            "b200ldlt_solve_refined_device", "b200ldlt_sparse_solve", "b200ldlt_sparse_solve_device"]
 
 _lib = None
 
@@ -121,6 +121,8 @@ def load_library():
     L.b200ldlt_alter_d.argtypes = [vp, dp]
     L.b200ldlt_sparse_fwd_solve.argtypes = [vp, C.c_int, ip, dp, ip, ip, dp]
     L.b200ldlt_sparse_fwd_solve_device.argtypes = [vp, C.c_int, ip, vp, ip, ip, vp]
+    L.b200ldlt_sparse_solve.argtypes = [vp, C.c_int, C.c_int, ip, dp, C.c_int, ip, dp]
+    L.b200ldlt_sparse_solve_device.argtypes = [vp, C.c_int, C.c_int, ip, vp, C.c_int, ip, vp]
     L.b200ldlt_set_singular_action.argtypes = [vp, C.c_int]
     L.b200ldlt_enquire_zero_pivots.argtypes = [vp, ip, ip]
     L.b200ldlt_solve_fredholm.argtypes = [vp, C.c_int, C.c_double, dp, ip]
@@ -360,6 +362,36 @@ class B200Ldlt:
                                                     _iptr(xi), C.c_void_p(d_x_ptr)) != SYMSOLVER_SUCCESS:
             raise RuntimeError(self.last_error())
         return xi[:nxi.value].copy()
+
+    def sparse_solve(self, bindex, B, xsel):
+        """Chosen entries of A^-1 b for sparse b's that share one pattern (b200ldlt_sparse_solve): B is nrhs x nbi (or a
+        vector of nbi), row c the values of column c at the 0-based variables bindex; returns the nrhs x nxs entries of
+        the solutions at the variables xsel (a vector for a vector B).  bindex = None: B is dense (nrhs x dim); xsel =
+        None: every entry.  Raises on a refusal."""
+        B = np.asarray(B, dtype=np.float64)
+        one = B.ndim == 1
+        nbi = self.dim if bindex is None else len(bindex)
+        Bm = np.ascontiguousarray(B.reshape(1 if one else B.shape[0], nbi))
+        nrhs = Bm.shape[0]
+        bi = None if bindex is None else np.ascontiguousarray(bindex, dtype=np.int32)
+        xs = None if xsel is None else np.ascontiguousarray(xsel, dtype=np.int32)
+        nxs = self.dim if xs is None else len(xs)
+        X = np.zeros((nrhs, nxs))
+        if self._L.b200ldlt_sparse_solve(self._h, nrhs, nbi, None if bi is None else _iptr(bi), _dptr(Bm), nxs,
+                                         None if xs is None else _iptr(xs), _dptr(X)) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return X[0] if one else X
+
+    def sparse_solve_device(self, bindex, d_b_ptr, xsel, d_x_ptr, nrhs=1):
+        """The same with the values in device memory: d_b holds nrhs x nbi doubles (column c at c nbi), d_x receives
+        nrhs x nxs (pointers as ints).  Returns the status."""
+        bi = None if bindex is None else np.ascontiguousarray(bindex, dtype=np.int32)
+        xs = None if xsel is None else np.ascontiguousarray(xsel, dtype=np.int32)
+        nbi = self.dim if bi is None else len(bi)
+        nxs = self.dim if xs is None else len(xs)
+        return self._L.b200ldlt_sparse_solve_device(self._h, int(nrhs), nbi, None if bi is None else _iptr(bi),
+                                                    C.c_void_p(d_b_ptr), nxs, None if xs is None else _iptr(xs),
+                                                    C.c_void_p(d_x_ptr))
 
     def set_singular_action(self, keep):
         """keep = 1: a SINGULAR factorisation whose zero pivots are all rounding noise keeps its factors (D^+); 0 (the

@@ -11,6 +11,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <iterator>
 #include <string>
 #include <memory>
 #include <vector>
@@ -153,6 +154,24 @@ struct InvPlan {
   }
 };
 
+// The sparse solve (b200ldlt_sparse_solve): the host copy of the backward top tasks (SolvePlan::d_tb, copied back once)
+// and per front its entries there, the marks of a pruned backward sweep, the run sets of the last call, and the staging
+// of a call (pinned -> device: its pruned lists and position lists), grown to the largest call.  Built at the first call
+// after an analysis, before its timing starts; a handle that never makes the call allocates none of it.
+struct SparseSolvePlan {
+  std::vector<SolveTask> tb;
+  std::vector<int> task_ptr, task_idx;         // by front (CSR): its backward top tasks, ascending
+  std::vector<unsigned> m_task;
+  std::vector<int> last_fwd, last_bwd;         // symbolic_array "sparse_solve_fwd_run_set" / "sparse_solve_bwd_run_set"
+  char* h_buf = nullptr;
+  DevBuf<char> d_buf;
+  cudaEvent_t ev_staged = nullptr;             // the last copy out of h_buf
+  ~SparseSolvePlan() {
+    if (h_buf) cudaFreeHost(h_buf);
+    if (ev_staged) cudaEventDestroy(ev_staged);
+  }
+};
+
 // selected inversion (b200ldlt_selected_inverse, selinv_kernels.cu): per tree level the fronts of each launch and the tile
 // items of the fronts above SI_SMALL, the Z panels, the L11^-1 of the fronts of order (SI_SMALL, SI_MID] and the index
 // maps of the output.  Built at the first call after an analysis, before its timing starts; a handle that never makes
@@ -275,6 +294,7 @@ struct Analysis {
   std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call
   std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve / inverse entries: built at the first such call
   std::unique_ptr<InvPlan> inv;         // inverse entries: built at its first call
+  std::unique_ptr<SparseSolvePlan> sps; // sparse solve: built at its first call
   std::unique_ptr<SelInvPlan> selinv;   // selected inversion: built at its first call
   std::unique_ptr<EaPlan> ea;       // error analysis / condest: built at the first such call
   // zero pivots (b200ldlt_set_singular_action): the factor kernels append every forced zero pivot to d_zlist; with
@@ -1456,22 +1476,27 @@ static DevSolve sweep_view(const Solver* sv, const SolvePlan& SP, const SweepSta
   return V;
 }
 
-// subsequences of a plan's forward lists, in their order, on the device (the sparse forward solve)
+// subsequences of a plan's lists, in their order, on the device (the pruned sweeps): the top tasks of the sweep's
+// direction (forward or backward list), the subtree items, the direct fronts of each level
 struct PrunedLists {
-  const SolveTask* tf; int ntf;
+  const SolveTask* tasks; int ntasks;
   const int2* subpair; int npair;
   const int* direct; std::vector<int> direct_off, direct_cnt;   // direct level l: direct_cnt[l] fronts at direct + direct_off[l]
 };
 
 // one sweep of nb columns (nb <= W.width) over the fronts of a plan: the bottom levels one launch each, and ONE persistent
 // kernel (forward: bottom levels, then subtrees, then top tasks; backward: the reverse).  apply_d = false: a forward
-// sweep that leaves D^-1 out (partial solves).  pruned (forward only): the sweep takes those lists instead of SP's
+// sweep that leaves D^-1 out (partial solves).  pruned: the sweep takes those lists instead of SP's
 static int launch_sweep(Solver* sv, const SolvePlan& SP, SweepState& W, int nb, bool fwd, bool apply_d = true,
                         const PrunedLists* pruned = nullptr) {
   Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
   DevSolve V = sweep_view(sv, SP, W);
-  if (pruned) { V.tasks = pruned->tf; V.ntasks_fwd = pruned->ntf; V.subpair = pruned->subpair; V.npair = pruned->npair; }
+  if (pruned) {
+    if (fwd) { V.tasks = pruned->tasks; V.ntasks_fwd = pruned->ntasks; }
+    else { V.tasks_bwd = pruned->tasks; V.ntasks_bwd = pruned->ntasks; }
+    V.subpair = pruned->subpair; V.npair = pruned->npair;
+  }
   MultiStride M = W.M;
   M.nb = nb;
   const bool multi = nb > 1;
@@ -1764,6 +1789,21 @@ static int enqueue_lmul_columns(Solver* sv, int trans, int nrhs, const double* d
 }
 
 // ---- pruned forward sweeps (b200ldlt_sparse_fwd_solve, b200ldlt_inverse_entries) -------------------------------------
+// the top tasks T[0..nt) by front (CSR, ascending): a bundle's entry under each of its fronts
+static void index_tasks(const SolvePlan& SP, const std::vector<SolveTask>& T, int nt, int nsn, std::vector<int>& ptr,
+                        std::vector<int>& idx) {
+  ptr.assign(nsn + 1, 0);
+  auto each_front = [&](const SolveTask& K, auto&& fn) {
+    if (K.type == ST_SMALL) { for (int w = 0; w < K.blk; ++w) fn(SP.bundle[K.s + w]); }
+    else fn(K.s);
+  };
+  for (int j = 0; j < nt; ++j) each_front(T[j], [&](int s) { ptr[s + 1]++; });
+  for (int s = 0; s < nsn; ++s) ptr[s + 1] += ptr[s];
+  idx.resize(ptr[nsn]);
+  std::vector<int> fill(ptr.begin(), ptr.end() - 1);
+  for (int j = 0; j < nt; ++j) each_front(T[j], [&](int s) { idx[fill[s]++] = j; });
+}
+
 // The per-front indices into the host copies of the handle's forward lists and the marks of a pruned sweep.
 static void build_sfs_plan(const Analysis& A, int n, SparseFwdPlan& P) {
   const Symbolic& S = A.S;
@@ -1784,18 +1824,7 @@ static void build_sfs_plan(const Analysis& A, int n, SparseFwdPlan& P) {
     }
     P.item_ptr.push_back((int)P.item_fr.size());
   }
-  P.task_ptr.assign(nsn + 1, 0);
-  auto each_front = [&](const SolveTask& T, auto&& fn) {
-    if (T.type == ST_SMALL) { for (int w = 0; w < T.blk; ++w) fn(SP.bundle[T.s + w]); }
-    else fn(T.s);
-  };
-  for (int j = 0; j < SP.ntf; ++j) each_front(SP.tf[j], [&](int s) { P.task_ptr[s + 1]++; });
-  for (int s = 0; s < nsn; ++s) P.task_ptr[s + 1] += P.task_ptr[s];
-  P.task_idx.resize(P.task_ptr[nsn]);
-  {
-    std::vector<int> fill(P.task_ptr.begin(), P.task_ptr.end() - 1);
-    for (int j = 0; j < SP.ntf; ++j) each_front(SP.tf[j], [&](int s) { P.task_idx[fill[s]++] = j; });
-  }
+  index_tasks(SP, SP.tf, SP.ntf, nsn, P.task_ptr, P.task_idx);
   P.iperm.resize(n); P.sn_of.resize(n);
   for (int i = 0; i < n; ++i) P.iperm[S.perm[i]] = i;
   for (int s = 0; s < nsn; ++s) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) P.sn_of[p] = s;
@@ -1846,21 +1875,12 @@ struct PrunedSweep {
   std::vector<std::vector<int>> dl;
 };
 
-// Host part of a pruned forward sweep from the pivot positions seed[0..nseed).  The reach (the fronts on the tree paths
-// from the fronts of the seeds to the root) gives the run set R: the reach, the fronts walked by a subtree item that
-// walks a reached front, and the fronts of a bundle that holds one (items and bundles are kept whole).  The pruned lists
-// take every entry of the handle's forward lists that belongs to a front of R, in list order.  F = the children of R
-// outside R.  Then the check that the pruned sweep cannot wait forever, before anything is launched: every front of R
-// owns work in the lists -- all of its top tasks, and all chunks of each chunked block (the arrival counters count modulo
-// the chunk count) -- and every child of a front of R is in F or runs EARLIER in the pruned order (the same subtree walk
-// counts: it is walked level by level).  FATAL_ERROR with "<call>: ..." when the check fails.
-static int prune_forward(Solver* sv, const char* call, const int* seed, int nseed, PrunedSweep& R) {
-  Analysis& A = *sv->an;
-  SparseFwdPlan& P = *A.sfs;
-  const SolvePlan& SP = A.fronts.solve;
-  const Symbolic& S = A.S;
+// The run set of a pruned sweep, with stamp m: R's reach, run set, subtree items, top tasks and direct fronts (R.fr
+// cleared).  T is the sweep's top-task list, tptr / tidx its entries by front (CSR), mtask its marks.
+static void collect_run_set(SparseFwdPlan& P, const SolvePlan& SP, const Symbolic& S, const std::vector<SolveTask>& T,
+                            const std::vector<int>& tptr, const std::vector<int>& tidx, std::vector<unsigned>& mtask,
+                            unsigned m, const int* seed, int nseed, PrunedSweep& R) {
   const int nd = (int)SP.direct_cnt.size();
-  const unsigned m = ++P.stamp;
   std::vector<int>& reach = R.reach;
   std::vector<int>& run = R.run;
   std::vector<int>& items = R.items;
@@ -1878,12 +1898,11 @@ static int prune_forward(Solver* sv, const char* call, const int* seed, int nsee
       P.m_item[it] = m; items.push_back(it);
       for (int e = P.item_ptr[it]; e < P.item_ptr[it + 1]; ++e) add(P.item_fr[e]);
     }
-    for (int e = P.task_ptr[s]; e < P.task_ptr[s + 1]; ++e) {
-      const int t = P.task_idx[e];
-      if (P.m_task[t] == m) continue;
-      P.m_task[t] = m; tasks.push_back(t);
-      const SolveTask& T = SP.tf[t];
-      if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) add(SP.bundle[T.s + w]);
+    for (int e = tptr[s]; e < tptr[s + 1]; ++e) {
+      const int t = tidx[e];
+      if (mtask[t] == m) continue;
+      mtask[t] = m; tasks.push_back(t);
+      if (T[t].type == ST_SMALL) for (int w = 0; w < T[t].blk; ++w) add(SP.bundle[T[t].s + w]);
     }
   }
   std::sort(items.begin(), items.end());
@@ -1892,6 +1911,28 @@ static int prune_forward(Solver* sv, const char* call, const int* seed, int nsee
   dl.assign(nd, std::vector<int>());
   for (int s : run) if (P.dlev[s] >= 0) dl[P.dlev[s]].push_back(P.didx[s]);
   for (auto& v : dl) std::sort(v.begin(), v.end());
+}
+
+// Host part of a pruned forward sweep from the pivot positions seed[0..nseed).  The reach (the fronts on the tree paths
+// from the fronts of the seeds to the root) gives the run set R: the reach, the fronts walked by a subtree item that
+// walks a reached front, and the fronts of a bundle that holds one (items and bundles are kept whole).  The pruned lists
+// take every entry of the handle's forward lists that belongs to a front of R, in list order.  F = the children of R
+// outside R.  Then the check that the pruned sweep cannot wait forever, before anything is launched: every front of R
+// owns work in the lists -- all of its top tasks, and all chunks of each chunked block (the arrival counters count modulo
+// the chunk count) -- and every child of a front of R is in F or runs EARLIER in the pruned order (the same subtree walk
+// counts: it is walked level by level).  FATAL_ERROR with "<call>: ..." when the check fails.
+static int prune_forward(Solver* sv, const char* call, const int* seed, int nseed, PrunedSweep& R) {
+  Analysis& A = *sv->an;
+  SparseFwdPlan& P = *A.sfs;
+  const SolvePlan& SP = A.fronts.solve;
+  const Symbolic& S = A.S;
+  const int nd = (int)SP.direct_cnt.size();
+  const unsigned m = ++P.stamp;
+  collect_run_set(P, SP, S, SP.tf, P.task_ptr, P.task_idx, P.m_task, m, seed, nseed, R);
+  const std::vector<int>& run = R.run;
+  const std::vector<int>& items = R.items;
+  const std::vector<int>& tasks = R.tasks;
+  const std::vector<std::vector<int>>& dl = R.dl;
   // pruned order: direct level l -> slot l, subtree item i -> nd + i, top task j -> nd + items + j
   for (int s : run) { P.ord0[s] = INT_MAX; P.ord1[s] = -1; }
   for (int l = 0; l < nd; ++l) for (int i : dl[l]) { const int s = SP.direct[l][i]; P.ord0[s] = P.ord1[s] = l; }
@@ -1944,16 +1985,16 @@ static size_t pruned_bytes(const PrunedSweep& R) {
 }
 
 // R's pruned lists to the staging h at offset o (8-aligned; the device copy of the staging is d): subtree items, top
-// tasks, direct fronts, frontier.  pl points into d; *o_fr receives the offset of the frontier.  Returns the end offset.
-static size_t stage_pruned(const SolvePlan& SP, const PrunedSweep& R, char* h, const char* d, size_t o, PrunedLists& pl,
-                           size_t* o_fr) {
+// tasks (entries of T, the sweep's list), direct fronts, frontier.  pl points into d; *o_fr receives the offset of the frontier.  Returns the end offset.
+static size_t stage_pruned(const SolvePlan& SP, const std::vector<SolveTask>& T, const PrunedSweep& R, char* h, const char* d,
+                           size_t o, PrunedLists& pl, size_t* o_fr) {
   const int nd = (int)SP.direct_cnt.size();
   const size_t o_tf = o + align8(8 * R.items.size());
   const size_t o_dir = o_tf + align8(sizeof(SolveTask) * R.tasks.size());
   int2* hp = reinterpret_cast<int2*>(h + o);
   for (size_t i = 0; i < R.items.size(); ++i) hp[i] = SP.pairs[R.items[i]];
   SolveTask* ht = reinterpret_cast<SolveTask*>(h + o_tf);
-  for (size_t j = 0; j < R.tasks.size(); ++j) ht[j] = SP.tf[R.tasks[j]];
+  for (size_t j = 0; j < R.tasks.size(); ++j) ht[j] = T[R.tasks[j]];
   int* hd = reinterpret_cast<int*>(h + o_dir);
   pl.direct_off.assign(nd, 0); pl.direct_cnt.assign(nd, 0);
   int j = 0;
@@ -1964,7 +2005,7 @@ static size_t stage_pruned(const SolvePlan& SP, const PrunedSweep& R, char* h, c
   *o_fr = o_dir + align8(4 * (size_t)j);
   std::copy(R.fr.begin(), R.fr.end(), reinterpret_cast<int*>(h + *o_fr));
   pl.subpair = reinterpret_cast<const int2*>(d + o); pl.npair = (int)R.items.size();
-  pl.tf = reinterpret_cast<const SolveTask*>(d + o_tf); pl.ntf = (int)R.tasks.size();
+  pl.tasks = reinterpret_cast<const SolveTask*>(d + o_tf); pl.ntasks = (int)R.tasks.size();
   pl.direct = reinterpret_cast<const int*>(d + o_dir);
   return *o_fr + align8(4 * R.fr.size());
 }
@@ -2025,7 +2066,7 @@ static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_h
     for (int s : R.reach) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) xi[j++] = p;
   }
   for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = -1;
-  stage_pruned(SP, R, h, P.d_buf.p, 0, C.pl, &C.o_fr);
+  stage_pruned(SP, SP.tf, R, h, P.d_buf.p, 0, C.pl, &C.o_fr);
   if (b_host) memcpy(h + C.o_b, b_host, 8 * (size_t)nbi);
   P.last_run = R.run;
   std::sort(P.last_run.begin(), P.last_run.end());
@@ -2188,7 +2229,7 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
       for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *yp++ = p;
   for (size_t b = 0; b < R.size(); ++b) {
     InvBlock& B = C.blk[b];
-    stage_pruned(SP, R[b], h, Q.d_buf.p, B.o_lst, B.pl, &B.o_fr);
+    stage_pruned(SP, SP.tf, R[b], h, Q.d_buf.p, B.o_lst, B.pl, &B.o_fr);
     int* pos = reinterpret_cast<int*>(h + B.o_pos);
     for (int s : R[b].run) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *pos++ = p;
     int* cp = reinterpret_cast<int*>(h + B.o_col);
@@ -2232,6 +2273,245 @@ static int inv_enqueue(Solver* sv, const InvCall& C, double* out) {
   ++sv->launches;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
+}
+
+// ---- sparse solve (b200ldlt_sparse_solve) ---------------------------------------------------------------------------
+// SparseSolvePlan, and sparse_fwd_solve's per-front indices (not its staging), at the first call after an analysis,
+// before its timing starts.  The analysis keeps the backward top tasks on the device only: they are copied back here,
+// once, and indexed by front.
+static int sps_state(Solver* sv) {
+  { const int rc = sfs_state(sv, false); if (rc != B200LDLT_SUCCESS) return rc; }
+  Analysis& A = *sv->an;
+  if (A.sps) return B200LDLT_SUCCESS;
+  const SolvePlan& SP = A.fronts.solve;
+  std::unique_ptr<SparseSolvePlan> Q(new SparseSolvePlan());
+  Q->tb.resize(SP.ntb);
+  if (SP.ntb > 0) {
+    CU(cudaMemcpyAsync(Q->tb.data(), SP.d_tb.p, sizeof(SolveTask) * (size_t)SP.ntb, cudaMemcpyDeviceToHost, sv->stream));
+    CU(cudaStreamSynchronize(sv->stream));
+  }
+  index_tasks(SP, Q->tb, SP.ntb, A.S.nsn, Q->task_ptr, Q->task_idx);
+  Q->m_task.assign(std::max(SP.ntb, 1), 0);
+  CU(cudaEventCreateWithFlags(&Q->ev_staged, cudaEventDisableTiming));
+  A.sps = std::move(Q);
+  return B200LDLT_SUCCESS;
+}
+
+// Host part of a pruned backward sweep from the pivot positions seed[0..nseed) of the selected variables.  The reach (the
+// fronts on the tree paths from their fronts to the root) is ancestor-closed; the run set R_b adds the fronts walked by
+// a subtree item that walks a reached front and the fronts of a backward bundle that holds one (collect_run_set over
+// the backward list).  The frontier F_b (R.fr) = the parents of R_b outside R_b: only item-mates and bundle-mates have
+// one.  Their backward flags are stamped, so those mates read stale x at ancestor positions; their outputs are never
+// returned and nothing in the reach reads them.  Then the mirror of prune_forward's check, before anything is launched:
+// every front of R_b owns all of its backward top tasks -- each chunked block with all of its chunks, a big front with
+// all of its BT and BX blocks (bcnt_b and the chunk counters count modulo) -- and the parent of every front of R_b is a
+// root, in F_b, or runs EARLIER in the pruned backward order: top tasks, then subtree items (the same subtree walk
+// counts: it is walked from its root down), then the direct levels from the top down.  FATAL_ERROR with
+// "sparse_solve: ..." when the check fails.
+static int prune_backward(Solver* sv, const int* seed, int nseed, PrunedSweep& R) {
+  Analysis& A = *sv->an;
+  SparseFwdPlan& P = *A.sfs;
+  SparseSolvePlan& Q = *A.sps;
+  const SolvePlan& SP = A.fronts.solve;
+  const Symbolic& S = A.S;
+  const int nd = (int)SP.direct_cnt.size();
+  const unsigned m = ++P.stamp;
+  collect_run_set(P, SP, S, Q.tb, Q.task_ptr, Q.task_idx, Q.m_task, m, seed, nseed, R);
+  // pruned backward order: top task j -> slot j, subtree item i -> tasks + i, direct level l -> tasks + items + nd - 1 - l
+  const int nt = (int)R.tasks.size(), ni = (int)R.items.size();
+  for (int s : R.run) { P.ord0[s] = INT_MAX; P.ord1[s] = -1; }
+  auto upd = [&](int s, int o) { P.ord0[s] = std::min(P.ord0[s], o); P.ord1[s] = std::max(P.ord1[s], o); };
+  for (int j = 0; j < nt; ++j) {
+    const SolveTask& T = Q.tb[R.tasks[j]];
+    if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) upd(SP.bundle[T.s + w], j);
+    else upd(T.s, j);
+  }
+  for (int i = 0; i < ni; ++i)
+    for (int e = P.item_ptr[R.items[i]]; e < P.item_ptr[R.items[i] + 1]; ++e) upd(P.item_fr[e], nt + i);
+  for (int l = 0; l < nd; ++l) for (int i : R.dl[l]) upd(SP.direct[l][i], nt + ni + nd - 1 - l);
+  for (int s : R.run) {
+    bool ok = P.ord1[s] >= 0;
+    int nbt = 0, nbx = 0;
+    for (int e = Q.task_ptr[s]; ok && e < Q.task_ptr[s + 1]; ++e) {
+      const SolveTask& T = Q.tb[Q.task_idx[e]];
+      ok = Q.m_task[Q.task_idx[e]] == m;
+      if (ok && (T.type == ST_BT || T.type == ST_BX) && T.q == 0) {
+        ok = e + T.nq <= Q.task_ptr[s + 1];
+        for (int q = 1; ok && q < T.nq; ++q) {
+          const SolveTask& U = Q.tb[Q.task_idx[e + q]];
+          ok = U.type == T.type && U.blk == T.blk && U.cidx == T.cidx && U.q == q && Q.m_task[Q.task_idx[e + q]] == m;
+        }
+        (T.type == ST_BT ? nbt : nbx) += 1;
+      }
+    }
+    if (ok && S.f(s) > DF_MIDMAX && P.dlev[s] < 0 && P.item_of[s] < 0)
+      ok = nbt == (S.k(s) + DF_BLK - 1) / DF_BLK && nbx == (S.k(s) + DF_BLK - 1) / DF_BLK;
+    const int p = S.sn_parent[s];
+    if (ok && p >= 0) {
+      if (P.m_run[p] == m) ok = (P.sub_of[s] >= 0 && P.sub_of[p] == P.sub_of[s]) || P.ord1[p] < P.ord0[s];
+      else if (P.m_fr[p] != m) { P.m_fr[p] = m; R.fr.push_back(p); }
+    }
+    if (!ok) {
+      sv->err = "sparse_solve: the pruned backward sweep of front " + std::to_string(s) + " fails its dependency check (not launched)";
+      return B200LDLT_FATAL_ERROR;
+    }
+  }
+  return B200LDLT_SUCCESS;
+}
+
+// one sparse solve as prepared on the host: dense b (bindex NULL) / every entry (xsel NULL); the forward run set's
+// ncol positions and frontier of nfr fronts; the nz positions to zero and the nfb fronts of F_b between the sweeps; the
+// staging offsets (bytes) and the pruned lists on the device
+struct SpsCall {
+  bool dense_b = false, all_x = false;
+  int nbi = 0, nxs = 0, ncol = 0, nfr = 0, nz = 0, nfb = 0;
+  size_t o_pos = 0, o_bi = 0, o_ffr = 0, o_z = 0, o_fb = 0, o_xpos = 0, staged = 0;
+  PrunedLists plf{}, plb{};
+};
+
+// Host part of b200ldlt_sparse_solve (arguments already checked): one pruned forward sweep for the pattern of b
+// (prune_forward) and one pruned backward sweep for the selection (prune_backward), shared by every block of columns;
+// the positions to zero between the sweeps (R_b \ R_f with a sparse b; with a full selection everything outside R_f);
+// the output positions; all of it in the pinned staging, grown to this call.  FATAL_ERROR with a message, nothing
+// written and nothing launched, for a failed check or allocation.
+static int sps_prepare(Solver* sv, int nbi, const int* bindex, int nxs, const int* xsel, SpsCall& C) {
+  Analysis& A = *sv->an;
+  SparseFwdPlan& P = *A.sfs;
+  SparseSolvePlan& Q = *A.sps;
+  const SolvePlan& SP = A.fronts.solve;
+  const Symbolic& S = A.S;
+  const int nsn = S.nsn;
+  C.dense_b = !bindex; C.all_x = !xsel; C.nbi = nbi; C.nxs = nxs;
+  std::vector<int> all;
+  if (C.dense_b || C.all_x) { all.resize(nsn); for (int s = 0; s < nsn; ++s) all[s] = s; }
+  if (C.dense_b && C.all_x) {   // job 0 itself
+    Q.last_fwd = all; Q.last_bwd = all;
+    return B200LDLT_SUCCESS;
+  }
+  PrunedSweep Rf, Rb;
+  std::vector<int> seed;
+  if (!C.dense_b) {
+    seed.resize(nbi);
+    for (int i = 0; i < nbi; ++i) seed[i] = P.iperm[bindex[i]];
+    const int rc = prune_forward(sv, "sparse_solve", seed.data(), nbi, Rf);
+    if (rc != B200LDLT_SUCCESS) return rc;
+  }
+  if (!C.all_x) {
+    std::vector<int> sb(nxs);
+    for (int i = 0; i < nxs; ++i) sb[i] = P.iperm[xsel[i]];
+    const int rc = prune_backward(sv, sb.data(), nxs, Rb);
+    if (rc != B200LDLT_SUCCESS) return rc;
+  }
+  std::vector<int> runf = C.dense_b ? all : Rf.run, runb = C.all_x ? all : Rb.run;
+  std::sort(runf.begin(), runf.end());
+  std::sort(runb.begin(), runb.end());
+  std::vector<int> zf;   // fronts whose forward result is zeroed between the sweeps
+  if (!C.dense_b) std::set_difference(runb.begin(), runb.end(), runf.begin(), runf.end(), std::back_inserter(zf));
+  if (!C.dense_b) for (int s : runf) C.ncol += S.sn_start[s + 1] - S.sn_start[s];
+  for (int s : zf) C.nz += S.sn_start[s + 1] - S.sn_start[s];
+  C.nfr = (int)Rf.fr.size(); C.nfb = (int)Rb.fr.size();
+  // staging layout: forward pruned lists, backward pruned lists, run-set positions and their b indices, zeroed
+  // positions, output positions
+  C.o_pos = pruned_bytes(Rf) + pruned_bytes(Rb);
+  C.o_bi = C.o_pos + 4 * (size_t)C.ncol;
+  C.o_z = C.o_bi + 4 * (size_t)C.ncol;
+  C.o_xpos = C.o_z + 4 * (size_t)C.nz;
+  C.staged = align8(C.o_xpos + (C.all_x ? 0 : 4 * (size_t)nxs));
+  if (C.staged > Q.d_buf.n) {
+    Q.d_buf.release();
+    if (Q.h_buf) cudaFreeHost(Q.h_buf);
+    Q.h_buf = nullptr;
+    if (Q.d_buf.alloc(C.staged) != cudaSuccess || cudaHostAlloc((void**)&Q.h_buf, C.staged, cudaHostAllocDefault) != cudaSuccess) {
+      cudaGetLastError();
+      Q.d_buf.release();
+      Q.h_buf = nullptr;
+      sv->err = "sparse_solve: cannot allocate the staging of " + std::to_string(C.staged) + " bytes";
+      return B200LDLT_FATAL_ERROR;
+    }
+  }
+  // (the previous call's copy out of the staging must be complete before it is rewritten)
+  if (cudaEventSynchronize(Q.ev_staged) != cudaSuccess) {
+    sv->err = "sparse_solve: staging copy failed";
+    return B200LDLT_FATAL_ERROR;
+  }
+  char* h = Q.h_buf;
+  const char* d = Q.d_buf.p;
+  size_t o = 0;
+  if (!C.dense_b) o = stage_pruned(SP, SP.tf, Rf, h, d, o, C.plf, &C.o_ffr);
+  if (!C.all_x) {
+    stage_pruned(SP, Q.tb, Rb, h, d, o, C.plb, &C.o_fb);
+    int* xp = reinterpret_cast<int*>(h + C.o_xpos);
+    for (int i = 0; i < nxs; ++i) xp[i] = P.iperm[xsel[i]];
+  }
+  if (!C.dense_b) {
+    for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = i;
+    int* pos = reinterpret_cast<int*>(h + C.o_pos);
+    int* bi = reinterpret_cast<int*>(h + C.o_bi);
+    int j = 0;
+    for (int s : runf) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p, ++j) { pos[j] = p; bi[j] = P.pos_bi[p]; }
+    for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = -1;
+  }
+  int* zp = reinterpret_cast<int*>(h + C.o_z);
+  for (int s : zf) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *zp++ = p;
+  Q.last_fwd = std::move(runf);
+  Q.last_bwd = std::move(runb);
+  return B200LDLT_SUCCESS;
+}
+
+// Device part: the staging in, then per block of w columns (the blocked state, or the single-column state for w = 1):
+// the forward stage -- dense b: job 0's (k_rhs_in and the full sweep); sparse b: k_sps_in and job 0's forward sweep
+// (D^-1 applied, the rounding of the fused sweep) over the pruned lists -- then under the backward epoch k_sps_mid, the
+// backward sweep (pruned to R_b unless every entry is selected) and the output (k_sol_out for every entry, k_sps_out
+// for a selection).  Launches per block: 1 + d_f + t_f + 1 + d_b + t_b + 1; with a dense b and every entry selected the
+// block is job 0 itself (enqueue_solve): 4 + 2 D.
+static int sps_enqueue(Solver* sv, const SpsCall& C, int nrhs, bool blocked, const double* d_b, double* d_x) {
+  Analysis& A = *sv->an;
+  SparseSolvePlan& Q = *A.sps;
+  const SolvePlan& SP = A.fronts.solve;
+  cudaStream_t st = sv->stream;
+  const int n = sv->n;
+  const char* d = Q.d_buf.p;
+  const bool job0 = C.dense_b && C.all_x;
+  if (!job0) {
+    CU(cudaMemcpyAsync(Q.d_buf.p, Q.h_buf, C.staged, cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(Q.ev_staged, st));
+  }
+  return for_blocks(nrhs, blocked ? A.blk->width : 1, [&](int c, int w) -> int {
+    SweepState& W = w == 1 ? A.sweep : *A.blk;
+    const double* b = d_b + (size_t)c * C.nbi;
+    double* x = d_x + (size_t)c * C.nxs;
+    if (job0) return enqueue_solve(sv, W, 0, b, x, w);
+    int rc;
+    if (C.dense_b) {
+      rc = forward(sv, SP, W, b, w);
+    } else {
+      A.solve_epoch++;
+      const unsigned g = std::max(1u, cdiv(C.ncol, 256) + (unsigned)C.nfr);
+      k_sps_in<<<dim3(g, w), 256, 0, st>>>(C.ncol, reinterpret_cast<const int*>(d + C.o_pos),
+                                           reinterpret_cast<const int*>(d + C.o_bi), A.d_perm.p, A.d_scale.p, b, C.nbi,
+                                           W.d_x.p, W.M.x, C.nfr, reinterpret_cast<const int*>(d + C.o_ffr), A.d_rows_ptr.p,
+                                           W.d_cbv.p, W.M.cbv, W.d_done_f.p, W.M.nsn, A.solve_epoch);
+      ++sv->launches;
+      rc = launch_sweep(sv, SP, W, w, true, true, &C.plf);
+    }
+    if (rc != B200LDLT_SUCCESS) return rc;
+    A.solve_epoch++;
+    const unsigned g = std::max(1u, cdiv(C.nz, 256) + cdiv(C.nfb, 256));
+    k_sps_mid<<<dim3(g, w), 256, 0, st>>>(C.nz, reinterpret_cast<const int*>(d + C.o_z), A.d_piv_big.p, W.d_x.p, W.M.x,
+                                          W.d_bigv.p, W.M.bigv, C.nfb, reinterpret_cast<const int*>(d + C.o_fb),
+                                          W.d_done_b.p, W.M.nsn, A.solve_epoch);
+    ++sv->launches;
+    rc = launch_sweep(sv, SP, W, w, false, true, C.all_x ? nullptr : &C.plb);
+    if (rc != B200LDLT_SUCCESS) return rc;
+    if (C.all_x)
+      k_sol_out<<<dim3(cdiv(n, 256), w), 256, 0, st>>>(n, A.d_perm.p, A.d_scale.p, W.d_x.p, W.M.x, x);
+    else
+      k_sps_out<<<dim3(cdiv(C.nxs, 256), w), 256, 0, st>>>(C.nxs, reinterpret_cast<const int*>(d + C.o_xpos), A.d_perm.p,
+                                                            A.d_scale.p, W.d_x.p, W.M.x, x);
+    ++sv->launches;
+    CU(cudaGetLastError());
+    return B200LDLT_SUCCESS;
+  });
 }
 
 static int shard_setup(Solver* sv, int rank, int world) {
@@ -2445,11 +2725,12 @@ static int timed_call(Solver* sv, Enqueue&& enqueue, Drain&& drain = Drain()) {
 // chunks, so that the DMA of one chunk runs under the host copy of the next (the caller's array is pageable: Ipopt
 // allocates it per call, IpTSymLinearSolver.cpp:222-241).  The staging grows to the largest call and lasts until the
 // next analysis.  nwork: the staging holds at least that many doubles (device scratch of enqueue beyond in and out).
+// in_off: `in` is staged at that many doubles from the start (out always at the start).
 template <class Enqueue>
 static int staged_call(Solver* sv, const double* in, size_t nin, double* out, size_t nout, Enqueue&& enqueue,
-                       size_t nwork = 0) {
+                       size_t nwork = 0, size_t in_off = 0) {
   Analysis& A = *sv->an;
-  const size_t need = std::max(std::max(nin, nout), nwork);
+  const size_t need = std::max(std::max(in_off + nin, nout), nwork);
   if (need > A.d_rhs.n) {
     A.d_rhs.release();
     if (A.h_rhs) cudaFreeHost(A.h_rhs);
@@ -2472,8 +2753,8 @@ static int staged_call(Solver* sv, const double* in, size_t nin, double* out, si
   return timed_call(sv, [&]() -> int {
     for (size_t o = 0; o < nin; o += ci) {
       const size_t m = std::min(ci, nin - o);
-      memcpy(h + o, in + o, m * sizeof(double));
-      CU(cudaMemcpyAsync(d + o, h + o, m * sizeof(double), cudaMemcpyHostToDevice, st));
+      memcpy(h + in_off + o, in + o, m * sizeof(double));
+      CU(cudaMemcpyAsync(d + in_off + o, h + in_off + o, m * sizeof(double), cudaMemcpyHostToDevice, st));
     }
     { const int rc = enqueue(d); if (rc != B200LDLT_SUCCESS) return rc; }
     for (size_t o = 0, k = 0; o < nout; o += co, ++k) {
@@ -2552,6 +2833,36 @@ static int inverse_entries(Solver* sv, int nent, const int* irow, const int* jco
   { const int rc = inv_prepare(sv, nent, irow, jcol, blocked ? sv->an->blk->width : 1, C); if (rc != B200LDLT_SUCCESS) return rc; }
   auto enqueue = [&](double* d) { return inv_enqueue(sv, C, d); };
   return host ? staged_call(sv, nullptr, 0, vals, (size_t)nent, enqueue) : timed_call(sv, [&] { return enqueue(vals); });
+}
+
+// b200ldlt_sparse_solve (host == true: b and x in host memory) / _device
+static int sparse_solve(Solver* sv, int nrhs, int nbi, const int* bindex, const double* b, int nxs, const int* xsel,
+                        double* x, bool host) {
+  const int n = sv->n;
+  const char* bad = nrhs < 0 ? "nrhs must be >= 0" : (nbi < 0 || nbi > n) ? "nbi must be 0..n" : nxs < 0 ? "nxs must be >= 0"
+                  : ((!b && nrhs > 0 && nbi > 0) || (!x && nrhs > 0 && nxs > 0)) ? "NULL argument"
+                  : (!bindex && nbi != n) ? "a NULL bindex needs nbi = n" : (!xsel && nxs != n) ? "a NULL xsel needs nxs = n"
+                  : nullptr;
+  if (!bad && bindex) {
+    std::vector<int> v(nbi);
+    if (nbi > 0) memcpy(v.data(), bindex, sizeof(int) * (size_t)nbi);
+    std::sort(v.begin(), v.end());
+    if (nbi > 0 && (v.front() < 0 || v.back() >= n)) bad = "index out of range";
+    else if (std::adjacent_find(v.begin(), v.end()) != v.end()) bad = "bindex entry appears twice";
+  }
+  for (int i = 0; !bad && xsel && i < nxs; ++i)
+    if (xsel[i] < 0 || xsel[i] >= n) bad = "index out of range";
+  if (bad) { sv->err = std::string("sparse_solve: ") + bad; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "sparse_solve"); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (nrhs == 0 || nxs == 0) return no_columns(sv);
+  { const int rc = sps_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
+  const bool blocked = nrhs > 1 && block_solve_state(sv);
+  SpsCall C;
+  { const int rc = sps_prepare(sv, nbi, bindex, nxs, xsel, C); if (rc != B200LDLT_SUCCESS) return rc; }
+  const size_t nin = (size_t)nrhs * nbi, nout = (size_t)nrhs * nxs;
+  // host: x at the start of the staging, b after it
+  if (host) return staged_call(sv, b, nin, x, nout, [&](double* d) { return sps_enqueue(sv, C, nrhs, blocked, d + nout, d); }, 0, nout);
+  return timed_call(sv, [&] { return sps_enqueue(sv, C, nrhs, blocked, b, x); });
 }
 
 // b200ldlt_solve_fredholm (host == true: x in host memory) / _device
@@ -3225,6 +3536,20 @@ int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bind
   return sparse_fwd(sv, nbi, bindex, d_b, false, nxi, xindex, d_x);
 }
 
+int b200ldlt_sparse_solve(b200ldlt_handle h, int nrhs, int nbi, const int* bindex, const double* b, int nxs, const int* xsel,
+                          double* x) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return sparse_solve(sv, nrhs, nbi, bindex, b, nxs, xsel, x, true);
+}
+
+int b200ldlt_sparse_solve_device(b200ldlt_handle h, int nrhs, int nbi, const int* bindex, const double* d_b, int nxs,
+                                 const int* xsel, double* d_x) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return sparse_solve(sv, nrhs, nbi, bindex, d_b, nxs, xsel, d_x, false);
+}
+
 int b200ldlt_inverse_entries(b200ldlt_handle h, int nent, const int* irow, const int* jcol, double* vals) {
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
@@ -3663,6 +3988,8 @@ int64_t b200ldlt_symbolic_array(b200ldlt_handle h, const char* name, int64_t* ou
   if (nm == "level_sn") RET(S.level_sn);
   if (nm == "sparse_run_set") { static const std::vector<int> none; RET(A.sfs ? A.sfs->last_run : none); }
   if (nm == "inverse_run_set") { static const std::vector<int> none; RET(A.inv ? A.inv->last_run : none); }
+  if (nm == "sparse_solve_fwd_run_set") { static const std::vector<int> none; RET(A.sps ? A.sps->last_fwd : none); }
+  if (nm == "sparse_solve_bwd_run_set") { static const std::vector<int> none; RET(A.sps ? A.sps->last_bwd : none); }
 #undef RET
   return -1;
 }

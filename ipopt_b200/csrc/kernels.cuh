@@ -53,4 +53,16 @@ struct DevNum {
   double tiny;      // zero-pivot threshold (scaled matrix)
 };
 
+// the sparse solve (b200ldlt_sparse_solve, solve_kernels.cu): the input of compact right-hand sides, the stage between
+// the two sweeps and the output at the selected variables
+__global__ void k_sps_in(int ncol, const int* __restrict__ pos, const int* __restrict__ bi, const int* __restrict__ perm,
+                         const double* __restrict__ scale, const double* __restrict__ b, int nbi, double* __restrict__ xp,
+                         long long ldx, int nfr, const int* __restrict__ fr, const long long* __restrict__ rows_ptr,
+                         double* __restrict__ cbv, long long ldcbv, int* __restrict__ done_f, long long ldf, int epoch);
+__global__ void k_sps_mid(int nz, const int* __restrict__ zpos, const long long* __restrict__ piv_big, double* __restrict__ xp,
+                          long long ldx, double* __restrict__ big, long long ldbig, int nfb, const int* __restrict__ fb,
+                          int* __restrict__ done_b, long long ldf, int epoch);
+__global__ void k_sps_out(int nxs, const int* __restrict__ xpos, const int* __restrict__ perm, const double* __restrict__ scale,
+                          const double* __restrict__ xp, long long ldx, double* __restrict__ out);
+
 }  // namespace b200

@@ -232,6 +232,62 @@ __global__ void k_inv_dot(int nent, const InvEnt* __restrict__ ent, const double
   if (l == 0) vals[t] = s;
 }
 
+// Sparse solve (b200ldlt_sparse_solve): job 0 of a block of compact right-hand sides with one pattern, swept forward over
+// the run set R_f of the pattern and backward over the run set R_b of the selection.  Column blockIdx.y = c of the sweep
+// state (x: leading dimension ldx, update vectors ldcbv, flags ldf); column c of b at b + c nbi.
+// k_sps_in: blocks [0, cdiv(ncol, 256)): x = P^T S b at the ncol positions of R_f, the scaled entry of b where b has one
+// (bi[j] >= 0: its index into the compact column; k_rhs_in's single multiply) and 0 elsewhere.  Blocks after that:
+// frontier front fr[q] (a child of R_f outside R_f), the column's slice of its update vector zeroed and its forward flag
+// set to this sweep's epoch, as in k_sfs_in.
+__global__ void k_sps_in(int ncol, const int* __restrict__ pos, const int* __restrict__ bi, const int* __restrict__ perm,
+                         const double* __restrict__ scale, const double* __restrict__ b, int nbi, double* __restrict__ xp,
+                         long long ldx, int nfr, const int* __restrict__ fr, const long long* __restrict__ rows_ptr,
+                         double* __restrict__ cbv, long long ldcbv, int* __restrict__ done_f, long long ldf, int epoch) {
+  const long long c = blockIdx.y;
+  const int nxb = (ncol + 255) / 256;
+  if ((int)blockIdx.x < nxb) {
+    const int j = blockIdx.x * 256 + threadIdx.x;
+    if (j < ncol) {
+      const int p = pos[j], q = bi[j];
+      xp[c * ldx + p] = q >= 0 ? scale[perm[p]] * b[c * nbi + q] : 0.0;
+    }
+    return;
+  }
+  if ((int)blockIdx.x - nxb >= nfr) return;
+  const int f = fr[blockIdx.x - nxb];
+  const long long r0 = rows_ptr[f], r1 = rows_ptr[f + 1];
+  for (long long e = r0 + threadIdx.x; e < r1; e += blockDim.x) cbv[c * ldcbv + e] = 0.0;
+  if (threadIdx.x == 0) done_f[c * ldf + f] = epoch;
+}
+// k_sps_mid, between the forward sweep and the backward sweep, under the backward epoch.  Blocks [0, cdiv(nz, 256)): the
+// forward result at the nz positions zpos (the positions the backward sweep reads that the forward sweep did not write)
+// set to 0, in x or in bigv through piv_big, wherever k_dinv writes it.  Blocks after that: the backward flag of
+// frontier front fb[q] (a parent of R_b outside R_b) set to this sweep's epoch, so that its children do not wait for it.
+__global__ void k_sps_mid(int nz, const int* __restrict__ zpos, const long long* __restrict__ piv_big, double* __restrict__ xp,
+                          long long ldx, double* __restrict__ big, long long ldbig, int nfb, const int* __restrict__ fb,
+                          int* __restrict__ done_b, long long ldf, int epoch) {
+  const long long c = blockIdx.y;
+  const int nzb = (nz + 255) / 256;
+  if ((int)blockIdx.x < nzb) {
+    const int j = blockIdx.x * 256 + threadIdx.x;
+    if (j < nz) {
+      const int p = zpos[j];
+      const long long q = piv_big[p];
+      if (q >= 0) big[c * ldbig + q] = 0.0; else xp[c * ldx + p] = 0.0;
+    }
+    return;
+  }
+  const int q = (blockIdx.x - nzb) * 256 + threadIdx.x;
+  if (q < nfb) done_b[c * ldf + fb[q]] = epoch;
+}
+// k_sps_out: out[c nxs + i] = S P x at the variable of pivot position xpos[i] (k_sol_out's single multiply)
+__global__ void k_sps_out(int nxs, const int* __restrict__ xpos, const int* __restrict__ perm, const double* __restrict__ scale,
+                          const double* __restrict__ xp, long long ldx, double* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long c = blockIdx.y;
+  if (i < nxs) { const int p = xpos[i]; out[c * nxs + i] = scale[perm[p]] * xp[c * ldx + p]; }
+}
+
 // r = b - A x from the original triplets (tests / bench parity helper)
 __global__ void k_residual_init(int n, const double* __restrict__ b, double* __restrict__ r) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
