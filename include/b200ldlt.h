@@ -148,11 +148,16 @@ int b200ldlt_enquire_indef(b200ldlt_handle h, int* pivot_var, int* pivot_type, d
  * nxi and xindex are host memory in both entry points (the pruned work lists are built on the host from the pattern).
  * Kernel launches: 2 + d + t, where d is the number of the B200_SOLVE_DIRECT bottom tree levels that hold a front of
  * the reach solved by the direct kernel, and t = 1 when the reach has a front above those levels (always, unless the
- * whole tree is made of direct fronts), else 0.  The first call after an analysis builds per-front indices into the
- * solve's work lists, and pinned and device staging for the pruned lists (about 28 bytes per variable plus 40 per
- * forward top task each); a handle that never makes the call allocates none of it.  Refused (nothing written to nxi,
- * xindex or x): nbi < 0 or nbi > n, a NULL pointer with nbi > 0, an index out of range or repeated.  nbi = 0 sets
- * *nxi = 0. */
+ * whole tree is made of direct fronts), else 0.
+ * Memory of the three calls that prune sweeps (this one, b200ldlt_sparse_solve and b200ldlt_inverse_entries): the first
+ * of them after an analysis builds, before its timing starts, host-side indices into the solve's forward and backward
+ * work lists and the marks of a pruned sweep (ints per front, per variable and per top task).  Each call stages its
+ * pruned lists and position lists in one pinned and device staging that the three calls share, which grows to the
+ * largest call and is freed by the next analysis.  A handle that never makes such a call allocates none of it.  Here the
+ * staging holds the pruned lists, 8 bytes per position of the run set and 4 per position of the reach; the host entry
+ * point copies b in and x out through the staging of the other host entry points.
+ * Refused (nothing written to nxi, xindex or x): nbi < 0 or nbi > n, a NULL pointer with nbi > 0, an index out of range
+ * or repeated.  nbi = 0 sets *nxi = 0. */
 int b200ldlt_sparse_fwd_solve(b200ldlt_handle h, int nbi, const int* bindex, const double* b, int* nxi, int* xindex, double* x);
 int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bindex, const double* d_b, int* nxi, int* xindex,
                                      double* d_x);
@@ -183,11 +188,9 @@ int b200ldlt_sparse_fwd_solve_device(b200ldlt_handle h, int nbi, const int* bind
  * hold a direct front of R_f, t_f = 1 when R_f has a front above them), d_b and t_b the same counts for R_b; a dense b
  * gives d_f = D and t_f = 1, a full selection d_b = D and t_b = 1 (D = the direct levels that hold any front).  With both
  * NULL: job 0's 4 + 2 D.  nbi = 0 is a zero b: d_f = t_f = 0.
- * Memory: the first call after an analysis builds sparse_fwd_solve's per-front indices (not its staging) and a host copy
- * of the backward top tasks indexed by front, before its timing starts; each call stages its pruned lists and position
- * lists (4 bytes per position of R_f twice, per zeroed position and per selected entry) in pinned and device staging
- * that grows to the largest call and is freed by the next analysis; a handle that never makes the call allocates none
- * of it.  symbolic_array "sparse_solve_fwd_run_set" and "sparse_solve_bwd_run_set" return the run sets of the last call
+ * Memory: as stated at b200ldlt_sparse_fwd_solve for the three calls that prune sweeps; here the staging holds both
+ * pruned lists and the position lists (4 bytes per position of R_f twice, per zeroed position and per selected
+ * entry).  symbolic_array "sparse_solve_fwd_run_set" and "sparse_solve_bwd_run_set" return the run sets of the last call
  * (every front for a dense b / a full selection), ascending; the call leaves "sparse_run_set", "inverse_run_set", the
  * factors, D and every later solve as they were.
  * Refused (FATAL_ERROR with "sparse_solve: <reason>", nothing written to x): nrhs < 0, nbi < 0 or nbi > n, nxs < 0; a
@@ -300,10 +303,10 @@ int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* 
  * enquire_indef reproduces every entry; an entry equals the same entry requested alone, whatever B200_SOLVE_BLOCK, as a
  * value (the y of a column swept in a block may differ from its y swept alone in the sign of a zero).
  * Kernel launches: sum over blocks b of (1 + d_b + t_b + 1), plus 1, with d_b and t_b counted as for sparse_fwd_solve on
- * the block's columns.  Memory: the first call after an analysis builds sparse_fwd_solve's per-front indices (not its
- * staging) and two ints per front; each call needs 12 bytes per element of the y store (sum over the columns of the
- * pivots on their paths to the root), 24 bytes per entry and per block its pruned lists, in pinned and device staging
- * that grows to the largest call and is freed by the next analysis.  symbolic_array "inverse_run_set" returns the union
+ * the block's columns.  Memory: as stated at b200ldlt_sparse_fwd_solve for the three calls that prune sweeps; here a
+ * call needs 12 bytes per element of the y store (sum over the columns of the pivots on their paths to the root), 24
+ * bytes per entry and per block its pruned lists, in the shared staging and a device y store that grows to the largest
+ * call and is freed by the next analysis.  symbolic_array "inverse_run_set" returns the union
  * of the run sets the last call swept.  The call leaves the factors, D, every later solve and "sparse_run_set" as they
  * were.  Refused (nothing written): nent < 0, a NULL pointer with nent > 0, an index out of range, and (FATAL_ERROR with
  * a message) a failed allocation of the staging or the y store.  nent = 0 is the no-columns case.

@@ -68,8 +68,8 @@ struct LinvPlan {
 
 // triangular-solve work of a set of fronts (solve_dataflow.cu): subtrees for k_solve_sub + task lists for k_solve_top
 struct SolvePlan {
-  // host copies of the forward lists as uploaded, one-element placeholders included (the sparse forward solve prunes them)
-  std::vector<SolveTask> tf;
+  // host copies of the lists as uploaded, one-element placeholders included (the pruned sweeps prune them)
+  std::vector<SolveTask> tf, tb;
   std::vector<int2> pairs;
   std::vector<SubDesc> subs;
   std::vector<int> meta, bundle;
@@ -111,65 +111,48 @@ struct LmulPlan {
   int width = 0;
 };
 
-// The pruned forward sweeps (b200ldlt_sparse_fwd_solve, b200ldlt_inverse_entries): per-front indices into the host copies
-// of the full plan's forward lists and the marks of one pruned sweep, built at the first such call after an analysis,
-// before that call's timing starts; and the staging of the sparse forward solve (pinned -> device, sized by the full
-// plan), allocated at its first call.  A handle that never makes either call allocates none of it.
-struct SparseFwdPlan {
+struct Solver;
+
+// Pinned -> device staging of the lists of a call (ListStaging::reserve / upload): h the pinned copy, d the device copy of
+// the same layout, ev the last copy out of h.  Grows to the largest call and lasts until the next analysis.
+struct ListStaging {
+  char* h = nullptr;
+  DevBuf<char> d;
+  cudaEvent_t ev = nullptr;
+  int reserve(Solver* sv, const char* call, size_t bytes);
+  int upload(Solver* sv, size_t bytes);
+  ~ListStaging() {
+    if (h) cudaFreeHost(h);
+    if (ev) cudaEventDestroy(ev);
+  }
+};
+
+// The calls that run pruned sweeps (b200ldlt_sparse_fwd_solve, b200ldlt_inverse_entries, b200ldlt_sparse_solve): per
+// front its indices into the host copies of the full plan's lists and, per direction, its top tasks; the marks of one
+// pruned sweep; each call's last run sets; the inverse entries' tree depths and path lengths and their y store; and the
+// one list staging the three calls share (each call ends in the synchronise of timed_call on the handle's one stream).
+// Built at the first such call after an analysis, before that call's timing starts; a handle that never makes one
+// allocates none of it.
+struct PrunedPlan {
   std::vector<int> dlev, didx;                 // by front: its direct level and index there, or -1
   std::vector<int> item_of, sub_of;            // by front: the subtree item / the subtree that walks it, or -1
-  std::vector<int> task_ptr, task_idx;         // by front (CSR): its forward top tasks, ascending
   std::vector<int> item_ptr, item_fr;          // by subtree item (CSR): the fronts its subtrees walk
   std::vector<int> iperm, sn_of;               // variable -> permuted column; position -> front
   std::vector<int> pos_bi;                     // position -> index into the compact b during a call, else -1
-  std::vector<unsigned> m_reach, m_run, m_fr, m_item, m_task;   // marks of the current call (== stamp)
-  std::vector<int> ord0, ord1;                 // per call: first / last slot of a run front in the pruned order
-  std::vector<int> last_run;                   // the run set of the last call, ascending (symbolic_array "sparse_run_set")
+  std::vector<int> depth, pathlen;             // by front: depth in the tree, pivots on its path to the root
+  std::vector<int> col_of;                     // inverse entries: variable -> its column in the current call, else -1
+  struct Dir {                                 // [0] forward (SolvePlan::tf), [1] backward (SolvePlan::tb)
+    std::vector<int> task_ptr, task_idx;       // by front (CSR): its top tasks, ascending
+    std::vector<unsigned> m_task;
+  } dir[2];
+  std::vector<unsigned> m_reach, m_run, m_fr, m_item;   // marks of the current sweep (== stamp)
+  std::vector<int> ord0, ord1;                 // per sweep: first / last slot of a run front in the pruned order
   unsigned stamp = 0;
-  char* h_buf = nullptr;                       // pinned staging, the layout of d_buf up to the output slice
-  DevBuf<char> d_buf;
-  cudaEvent_t ev_staged = nullptr;             // the last copy out of h_buf
-  ~SparseFwdPlan() {
-    if (h_buf) cudaFreeHost(h_buf);
-    if (ev_staged) cudaEventDestroy(ev_staged);
-  }
-};
-
-// Entries of A^-1 (b200ldlt_inverse_entries): per front its depth in the tree and the pivots on its path to the root;
-// the column of each variable during a call; the union of the run sets of the last call; the staging of a call (pinned
-// -> device: the entry list, the offsets and pivot positions of the y store, and per block its pruned lists, run-set
-// positions and column positions) and the values of the y store, both grown to the largest call.  Built at the first
-// call after an analysis, before its timing starts; a handle that never makes the call allocates none of it.
-struct InvPlan {
-  std::vector<int> depth, pathlen;             // by front
-  std::vector<int> col_of;                     // variable -> its column in the current call, else -1
-  std::vector<int> last_run;                   // symbolic_array "inverse_run_set"
-  char* h_buf = nullptr;
-  DevBuf<char> d_buf;
-  DevBuf<double> d_y;
-  cudaEvent_t ev_staged = nullptr;             // the last copy out of h_buf
-  ~InvPlan() {
-    if (h_buf) cudaFreeHost(h_buf);
-    if (ev_staged) cudaEventDestroy(ev_staged);
-  }
-};
-
-// The sparse solve (b200ldlt_sparse_solve): the host copy of the backward top tasks (SolvePlan::d_tb, copied back once)
-// and per front its entries there, the marks of a pruned backward sweep, the run sets of the last call, and the staging
-// of a call (pinned -> device: its pruned lists and position lists), grown to the largest call.  Built at the first call
-// after an analysis, before its timing starts; a handle that never makes the call allocates none of it.
-struct SparseSolvePlan {
-  std::vector<SolveTask> tb;
-  std::vector<int> task_ptr, task_idx;         // by front (CSR): its backward top tasks, ascending
-  std::vector<unsigned> m_task;
-  std::vector<int> last_fwd, last_bwd;         // symbolic_array "sparse_solve_fwd_run_set" / "sparse_solve_bwd_run_set"
-  char* h_buf = nullptr;
-  DevBuf<char> d_buf;
-  cudaEvent_t ev_staged = nullptr;             // the last copy out of h_buf
-  ~SparseSolvePlan() {
-    if (h_buf) cudaFreeHost(h_buf);
-    if (ev_staged) cudaEventDestroy(ev_staged);
-  }
+  // the run sets of each call's last run, ascending (symbolic_array "sparse_run_set", "inverse_run_set",
+  // "sparse_solve_fwd_run_set", "sparse_solve_bwd_run_set"); a call leaves the others' untouched
+  std::vector<int> last_sfs, last_inv, last_fwd, last_bwd;
+  ListStaging stg;
+  DevBuf<double> d_y;                          // inverse entries: the y store, grown to the largest call
 };
 
 // selected inversion (b200ldlt_selected_inverse, selinv_kernels.cu): per tree level the fronts of each launch and the tile
@@ -292,9 +275,7 @@ struct Analysis {
   DevBuf<long long> d_bigv_off;
   DevBuf<long long> d_piv_big;      // n : per pivot position, its index in bigv (pivots of big fronts) or -1 (partial solves)
   std::unique_ptr<LmulPlan> lmul;   // lmultiply: built at its first call
-  std::unique_ptr<SparseFwdPlan> sfs;   // sparse forward solve / inverse entries: built at the first such call
-  std::unique_ptr<InvPlan> inv;         // inverse entries: built at its first call
-  std::unique_ptr<SparseSolvePlan> sps; // sparse solve: built at its first call
+  std::unique_ptr<PrunedPlan> pruned;   // sparse forward solve / inverse entries / sparse solve: built at the first such call
   std::unique_ptr<SelInvPlan> selinv;   // selected inversion: built at its first call
   std::unique_ptr<EaPlan> ea;       // error analysis / condest: built at the first such call
   // zero pivots (b200ldlt_set_singular_action): the factor kernels append every forced zero pivot to d_zlist; with
@@ -794,7 +775,7 @@ static int build_solve_plan(Solver* sv, const Analysis& A, const std::vector<cha
   CU(SP.d_ccnt.alloc(std::max(ncidx, 1)));
   CU(cudaMemsetAsync(SP.d_ccnt.p, 0, SP.d_ccnt.n * sizeof(int), st));
   CU(SP.d_part.alloc(std::max<long long>(npart, 1) * 64));
-  SP.tf = std::move(tf); SP.pairs = std::move(pairs); SP.subs = std::move(subs);
+  SP.tf = std::move(tf); SP.tb = std::move(tb); SP.pairs = std::move(pairs); SP.subs = std::move(subs);
   SP.meta = std::move(meta); SP.bundle = std::move(bundle);
   return B200LDLT_SUCCESS;
 }
@@ -1788,10 +1769,10 @@ static int enqueue_lmul_columns(Solver* sv, int trans, int nrhs, const double* d
   });
 }
 
-// ---- pruned forward sweeps (b200ldlt_sparse_fwd_solve, b200ldlt_inverse_entries) -------------------------------------
+// ---- pruned sweeps (b200ldlt_sparse_fwd_solve, b200ldlt_inverse_entries, b200ldlt_sparse_solve) ----------------------
 // the top tasks T[0..nt) by front (CSR, ascending): a bundle's entry under each of its fronts
-static void index_tasks(const SolvePlan& SP, const std::vector<SolveTask>& T, int nt, int nsn, std::vector<int>& ptr,
-                        std::vector<int>& idx) {
+static void index_tasks(const SolvePlan& SP, const std::vector<SolveTask>& T, int nt, int nsn, PrunedPlan::Dir& D) {
+  std::vector<int>& ptr = D.task_ptr;
   ptr.assign(nsn + 1, 0);
   auto each_front = [&](const SolveTask& K, auto&& fn) {
     if (K.type == ST_SMALL) { for (int w = 0; w < K.blk; ++w) fn(SP.bundle[K.s + w]); }
@@ -1799,16 +1780,30 @@ static void index_tasks(const SolvePlan& SP, const std::vector<SolveTask>& T, in
   };
   for (int j = 0; j < nt; ++j) each_front(T[j], [&](int s) { ptr[s + 1]++; });
   for (int s = 0; s < nsn; ++s) ptr[s + 1] += ptr[s];
-  idx.resize(ptr[nsn]);
+  D.task_idx.resize(ptr[nsn]);
   std::vector<int> fill(ptr.begin(), ptr.end() - 1);
-  for (int j = 0; j < nt; ++j) each_front(T[j], [&](int s) { idx[fill[s]++] = j; });
+  for (int j = 0; j < nt; ++j) each_front(T[j], [&](int s) { D.task_idx[fill[s]++] = j; });
+  D.m_task.assign(std::max(nt, 1), 0);
 }
 
-// The per-front indices into the host copies of the handle's forward lists and the marks of a pruned sweep.
-static void build_sfs_plan(const Analysis& A, int n, SparseFwdPlan& P) {
+// PrunedPlan at the first pruned call after an analysis, before its timing starts: the per-front indices into the host
+// copies of the handle's lists, the marks, and the staging's event.  Fronts are numbered in postorder (a parent after
+// its children), so one pass from the last front down gives every front's depth and path length.
+static int pruned_state(Solver* sv, const char* call) {
+  Analysis& A = *sv->an;
+  if (A.pruned) return B200LDLT_SUCCESS;
   const Symbolic& S = A.S;
   const SolvePlan& SP = A.fronts.solve;
-  const int nsn = S.nsn;
+  const int nsn = S.nsn, n = sv->n;
+  std::unique_ptr<PrunedPlan> Q(new PrunedPlan());
+  PrunedPlan& P = *Q;
+  P.depth.assign(nsn, 0); P.pathlen.assign(nsn, 0);
+  for (int s = nsn - 1; s >= 0; --s) {
+    const int p = S.sn_parent[s];
+    if (p >= 0 && p <= s) { sv->err = std::string(call) + ": internal: the fronts are not in postorder"; return B200LDLT_FATAL_ERROR; }
+    P.depth[s] = p >= 0 ? P.depth[p] + 1 : 0;
+    P.pathlen[s] = S.k(s) + (p >= 0 ? P.pathlen[p] : 0);
+  }
   P.dlev.assign(nsn, -1); P.didx.assign(nsn, -1); P.item_of.assign(nsn, -1); P.sub_of.assign(nsn, -1);
   for (size_t l = 0; l < SP.direct_cnt.size(); ++l)
     for (int i = 0; i < SP.direct_cnt[l]; ++i) { const int s = SP.direct[l][i]; P.dlev[s] = (int)l; P.didx[s] = i; }
@@ -1824,62 +1819,69 @@ static void build_sfs_plan(const Analysis& A, int n, SparseFwdPlan& P) {
     }
     P.item_ptr.push_back((int)P.item_fr.size());
   }
-  index_tasks(SP, SP.tf, SP.ntf, nsn, P.task_ptr, P.task_idx);
+  index_tasks(SP, SP.tf, SP.ntf, nsn, P.dir[0]);
+  index_tasks(SP, SP.tb, SP.ntb, nsn, P.dir[1]);
   P.iperm.resize(n); P.sn_of.resize(n);
   for (int i = 0; i < n; ++i) P.iperm[S.perm[i]] = i;
   for (int s = 0; s < nsn; ++s) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) P.sn_of[p] = s;
   P.pos_bi.assign(n, -1);
+  P.col_of.assign(n, -1);
   P.m_reach.assign(nsn, 0); P.m_run.assign(nsn, 0); P.m_fr.assign(nsn, 0);
-  P.m_item.assign(std::max(SP.npair, 1), 0); P.m_task.assign(std::max(SP.ntf, 1), 0);
+  P.m_item.assign(std::max(SP.npair, 1), 0);
   P.ord0.assign(nsn, 0); P.ord1.assign(nsn, 0);
-}
-
-// SparseFwdPlan at the first pruned call after an analysis, before its timing starts; with `staging` (the sparse
-// forward solve) also its staging.
-static int sfs_state(Solver* sv, bool staging) {
-  Analysis& A = *sv->an;
-  const int n = sv->n;
-  if (!A.sfs) {
-    std::unique_ptr<SparseFwdPlan> P(new SparseFwdPlan());
-    build_sfs_plan(A, n, *P);
-    A.sfs = std::move(P);
-  }
-  SparseFwdPlan& P = *A.sfs;
-  if (!staging || P.h_buf) return B200LDLT_SUCCESS;
-  const SolvePlan& SP = A.fronts.solve;
-  long long ndirect = 0;
-  for (const int c : SP.direct_cnt) ndirect += c;
-  // staging: subtree items, top tasks, direct fronts, frontier, b, run-set positions and their b indices, output
-  // positions, and on the device the output slice
-  const size_t cap = 8 * (size_t)SP.npair + 8 * (size_t)n + sizeof(SolveTask) * (size_t)SP.ntf +
-                     4 * ((size_t)ndirect + 3 * (size_t)n + (size_t)A.S.nsn) + 8 * (size_t)n + 64;
-  if (!P.ev_staged) CU(cudaEventCreateWithFlags(&P.ev_staged, cudaEventDisableTiming));
-  CU(P.d_buf.alloc(cap));
-  CU(cudaHostAlloc((void**)&P.h_buf, cap, cudaHostAllocDefault));
+  CU(cudaEventCreateWithFlags(&P.stg.ev, cudaEventDisableTiming));
+  A.pruned = std::move(Q);
   return B200LDLT_SUCCESS;
 }
 
-// one sparse call, as prepared on the host: counts, staging offsets (bytes) and the pruned lists on the device
-struct SfsCall {
-  int ncol = 0, nxi = 0, nfr = 0;
-  size_t o_b = 0, o_pos = 0, o_bi = 0, o_xi = 0, o_fr = 0, o_x = 0, staged = 0;
-  PrunedLists pl{};
-};
+// The staging grown to `bytes` for this call, after the previous call's copy out of h is complete (h is rewritten next).
+// FATAL_ERROR with "<call>: ..." when the copy failed or the allocation fails (which leaves both buffers released).
+int ListStaging::reserve(Solver* sv, const char* call, size_t bytes) {
+  if (cudaEventSynchronize(ev) != cudaSuccess) {
+    sv->err = std::string(call) + ": staging copy failed";
+    return B200LDLT_FATAL_ERROR;
+  }
+  if (bytes <= d.n) return B200LDLT_SUCCESS;
+  d.release();
+  if (h) cudaFreeHost(h);
+  h = nullptr;
+  if (d.alloc(bytes) != cudaSuccess || cudaHostAlloc((void**)&h, bytes, cudaHostAllocDefault) != cudaSuccess) {
+    cudaGetLastError();
+    d.release();
+    h = nullptr;
+    sv->err = std::string(call) + ": cannot allocate the staging of " + std::to_string(bytes) + " bytes";
+    return B200LDLT_FATAL_ERROR;
+  }
+  return B200LDLT_SUCCESS;
+}
+
+// the first `bytes` of h to d on the handle's stream, and ev recorded after the copy
+int ListStaging::upload(Solver* sv, size_t bytes) {
+  CU(cudaMemcpyAsync(d.p, h, bytes, cudaMemcpyHostToDevice, sv->stream));
+  CU(cudaEventRecord(ev, sv->stream));
+  return B200LDLT_SUCCESS;
+}
 
 static inline size_t align8(size_t b) { return (b + 7) & ~(size_t)7; }
 
-// one pruned forward sweep as the host prepares it: the reach (ascending), the run set (the reach first), the subtree
-// items and top tasks it runs (ascending), per direct level the indices of its direct fronts (ascending), the frontier
+// the pivot positions of the fronts
+static int npos(const Symbolic& S, const std::vector<int>& fronts) {
+  int c = 0;
+  for (int s : fronts) c += S.sn_start[s + 1] - S.sn_start[s];
+  return c;
+}
+
+// one pruned sweep as the host prepares it: the reach (ascending), the run set (the reach first), the subtree items and
+// top tasks it runs (ascending), per direct level the indices of its direct fronts (ascending), the frontier
 struct PrunedSweep {
   std::vector<int> reach, run, items, tasks, fr;
   std::vector<std::vector<int>> dl;
 };
 
 // The run set of a pruned sweep, with stamp m: R's reach, run set, subtree items, top tasks and direct fronts (R.fr
-// cleared).  T is the sweep's top-task list, tptr / tidx its entries by front (CSR), mtask its marks.
-static void collect_run_set(SparseFwdPlan& P, const SolvePlan& SP, const Symbolic& S, const std::vector<SolveTask>& T,
-                            const std::vector<int>& tptr, const std::vector<int>& tidx, std::vector<unsigned>& mtask,
-                            unsigned m, const int* seed, int nseed, PrunedSweep& R) {
+// cleared).  T is the sweep's top-task list, D its entries by front and marks.
+static void collect_run_set(PrunedPlan& P, const SolvePlan& SP, const Symbolic& S, const std::vector<SolveTask>& T,
+                            PrunedPlan::Dir& D, unsigned m, const int* seed, int nseed, PrunedSweep& R) {
   const int nd = (int)SP.direct_cnt.size();
   std::vector<int>& reach = R.reach;
   std::vector<int>& run = R.run;
@@ -1898,10 +1900,10 @@ static void collect_run_set(SparseFwdPlan& P, const SolvePlan& SP, const Symboli
       P.m_item[it] = m; items.push_back(it);
       for (int e = P.item_ptr[it]; e < P.item_ptr[it + 1]; ++e) add(P.item_fr[e]);
     }
-    for (int e = tptr[s]; e < tptr[s + 1]; ++e) {
-      const int t = tidx[e];
-      if (mtask[t] == m) continue;
-      mtask[t] = m; tasks.push_back(t);
+    for (int e = D.task_ptr[s]; e < D.task_ptr[s + 1]; ++e) {
+      const int t = D.task_idx[e];
+      if (D.m_task[t] == m) continue;
+      D.m_task[t] = m; tasks.push_back(t);
       if (T[t].type == ST_SMALL) for (int w = 0; w < T[t].blk; ++w) add(SP.bundle[T[t].s + w]);
     }
   }
@@ -1913,64 +1915,72 @@ static void collect_run_set(SparseFwdPlan& P, const SolvePlan& SP, const Symboli
   for (auto& v : dl) std::sort(v.begin(), v.end());
 }
 
-// Host part of a pruned forward sweep from the pivot positions seed[0..nseed).  The reach (the fronts on the tree paths
-// from the fronts of the seeds to the root) gives the run set R: the reach, the fronts walked by a subtree item that
-// walks a reached front, and the fronts of a bundle that holds one (items and bundles are kept whole).  The pruned lists
-// take every entry of the handle's forward lists that belongs to a front of R, in list order.  F = the children of R
-// outside R.  Then the check that the pruned sweep cannot wait forever, before anything is launched: every front of R
-// owns work in the lists -- all of its top tasks, and all chunks of each chunked block (the arrival counters count modulo
-// the chunk count) -- and every child of a front of R is in F or runs EARLIER in the pruned order (the same subtree walk
-// counts: it is walked level by level).  FATAL_ERROR with "<call>: ..." when the check fails.
-static int prune_forward(Solver* sv, const char* call, const int* seed, int nseed, PrunedSweep& R) {
+// Host part of a pruned sweep (dir 0: forward over SolvePlan::tf, dir 1: backward over SolvePlan::tb) from the pivot
+// positions seed[0..nseed).  The reach (the fronts on the tree paths from the fronts of the seeds to the root) gives the
+// run set R: the reach, the fronts walked by a subtree item that walks a reached front, and the fronts of a bundle of
+// the direction's list that holds one (items and bundles are kept whole).  The pruned lists take every entry of the
+// handle's lists that belongs to a front of R, in list order.  The frontier R.fr: forward, the children of R outside R;
+// backward, the parents of R outside R (only item-mates and bundle-mates have one: their backward flags are stamped, so
+// those mates read stale x at ancestor positions; their outputs are never returned and nothing in the reach reads them).
+// Then the check that the pruned sweep cannot wait forever, before anything is launched: every front of R owns all of
+// its top tasks in the lists, each chunked block with all of its chunks, and a big front all of its blocks of both types
+// (FP and FC forward, BT and BX backward; the arrival and chunk counters count modulo); and every child (forward) or the
+// parent (backward) of a front of R is in the frontier or runs EARLIER in the pruned order -- forward: the direct levels
+// from the bottom up, subtree items, top tasks; backward: the reverse (the same subtree walk counts: it is walked level
+// by level, from its root down backward).  FATAL_ERROR with "<call>: ..." when the check fails.
+static int prune(Solver* sv, const char* call, int dir, const int* seed, int nseed, PrunedSweep& R) {
   Analysis& A = *sv->an;
-  SparseFwdPlan& P = *A.sfs;
+  PrunedPlan& P = *A.pruned;
   const SolvePlan& SP = A.fronts.solve;
   const Symbolic& S = A.S;
+  const bool fwd = dir == 0;
+  const std::vector<SolveTask>& T = fwd ? SP.tf : SP.tb;
+  PrunedPlan::Dir& D = P.dir[dir];
   const int nd = (int)SP.direct_cnt.size();
   const unsigned m = ++P.stamp;
-  collect_run_set(P, SP, S, SP.tf, P.task_ptr, P.task_idx, P.m_task, m, seed, nseed, R);
-  const std::vector<int>& run = R.run;
-  const std::vector<int>& items = R.items;
-  const std::vector<int>& tasks = R.tasks;
-  const std::vector<std::vector<int>>& dl = R.dl;
-  // pruned order: direct level l -> slot l, subtree item i -> nd + i, top task j -> nd + items + j
-  for (int s : run) { P.ord0[s] = INT_MAX; P.ord1[s] = -1; }
-  for (int l = 0; l < nd; ++l) for (int i : dl[l]) { const int s = SP.direct[l][i]; P.ord0[s] = P.ord1[s] = l; }
-  for (size_t i = 0; i < items.size(); ++i)
-    for (int e = P.item_ptr[items[i]]; e < P.item_ptr[items[i] + 1]; ++e) P.ord0[P.item_fr[e]] = P.ord1[P.item_fr[e]] = nd + (int)i;
-  for (size_t j = 0; j < tasks.size(); ++j) {
-    const SolveTask& T = SP.tf[tasks[j]];
-    const int o = nd + (int)(items.size() + j);
-    auto upd = [&](int s) { P.ord0[s] = std::min(P.ord0[s], o); P.ord1[s] = std::max(P.ord1[s], o); };
-    if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) upd(SP.bundle[T.s + w]);
-    else upd(T.s);
+  collect_run_set(P, SP, S, T, D, m, seed, nseed, R);
+  // pruned order: forward, direct level l -> slot l, subtree item i -> nd + i, top task j -> nd + items + j; backward,
+  // top task j -> slot j, subtree item i -> tasks + i, direct level l -> tasks + items + nd - 1 - l
+  const int nt = (int)R.tasks.size(), ni = (int)R.items.size();
+  const int o_item = fwd ? nd : nt, o_task = fwd ? nd + ni : 0;
+  auto o_level = [&](int l) { return fwd ? l : nt + ni + nd - 1 - l; };
+  for (int s : R.run) { P.ord0[s] = INT_MAX; P.ord1[s] = -1; }
+  auto upd = [&](int s, int o) { P.ord0[s] = std::min(P.ord0[s], o); P.ord1[s] = std::max(P.ord1[s], o); };
+  for (int l = 0; l < nd; ++l) for (int i : R.dl[l]) upd(SP.direct[l][i], o_level(l));
+  for (int i = 0; i < ni; ++i)
+    for (int e = P.item_ptr[R.items[i]]; e < P.item_ptr[R.items[i] + 1]; ++e) upd(P.item_fr[e], o_item + i);
+  for (int j = 0; j < nt; ++j) {
+    const SolveTask& K = T[R.tasks[j]];
+    if (K.type == ST_SMALL) for (int w = 0; w < K.blk; ++w) upd(SP.bundle[K.s + w], o_task + j);
+    else upd(K.s, o_task + j);
   }
-  for (int s : run) {
+  const int type_a = fwd ? ST_FP : ST_BT, type_b = fwd ? ST_FC : ST_BX;
+  for (int s : R.run) {
     bool ok = P.ord1[s] >= 0;
-    // all top tasks of the front are in the lists, each chunked block with all of its nq chunks, a big front with all
-    // of its FP and FC blocks
-    int nfp = 0, nfc = 0;
-    for (int e = P.task_ptr[s]; ok && e < P.task_ptr[s + 1]; ++e) {
-      const SolveTask& T = SP.tf[P.task_idx[e]];
-      ok = P.m_task[P.task_idx[e]] == m;
-      if (ok && (T.type == ST_FP || T.type == ST_FC) && T.q == 0) {
-        ok = e + T.nq <= P.task_ptr[s + 1];
-        for (int q = 1; ok && q < T.nq; ++q) {
-          const SolveTask& U = SP.tf[P.task_idx[e + q]];
-          ok = U.type == T.type && U.blk == T.blk && U.cidx == T.cidx && U.q == q && P.m_task[P.task_idx[e + q]] == m;
+    int na = 0, nb = 0;
+    for (int e = D.task_ptr[s]; ok && e < D.task_ptr[s + 1]; ++e) {
+      const SolveTask& K = T[D.task_idx[e]];
+      ok = D.m_task[D.task_idx[e]] == m;
+      if (ok && (K.type == type_a || K.type == type_b) && K.q == 0) {
+        ok = e + K.nq <= D.task_ptr[s + 1];
+        for (int q = 1; ok && q < K.nq; ++q) {
+          const SolveTask& U = T[D.task_idx[e + q]];
+          ok = U.type == K.type && U.blk == K.blk && U.cidx == K.cidx && U.q == q && D.m_task[D.task_idx[e + q]] == m;
         }
-        (T.type == ST_FP ? nfp : nfc) += 1;
+        (K.type == type_a ? na : nb) += 1;
       }
     }
     if (ok && S.f(s) > DF_MIDMAX && P.dlev[s] < 0 && P.item_of[s] < 0)
-      ok = nfp == (S.k(s) + DF_BLK - 1) / DF_BLK && nfc == (S.r(s) + DF_BLK - 1) / DF_BLK;
-    for (int e = S.child_ptr[s]; ok && e < S.child_ptr[s + 1]; ++e) {
-      const int c = S.child_idx[e];
+      ok = na == (S.k(s) + DF_BLK - 1) / DF_BLK && nb == ((fwd ? S.r(s) : S.k(s)) + DF_BLK - 1) / DF_BLK;
+    auto neighbour = [&](int c) {   // c runs earlier in the pruned order, or joins the frontier
       if (P.m_run[c] == m) ok = (P.sub_of[s] >= 0 && P.sub_of[c] == P.sub_of[s]) || P.ord1[c] < P.ord0[s];
       else if (P.m_fr[c] != m) { P.m_fr[c] = m; R.fr.push_back(c); }
-    }
+    };
+    if (fwd) for (int e = S.child_ptr[s]; ok && e < S.child_ptr[s + 1]; ++e) neighbour(S.child_idx[e]);
+    else if (ok && S.sn_parent[s] >= 0) neighbour(S.sn_parent[s]);
     if (!ok) {
-      sv->err = std::string(call) + ": the pruned sweep of front " + std::to_string(s) + " fails its dependency check (not launched)";
+      sv->err = std::string(call) + (fwd ? ": the pruned sweep" : ": the pruned backward sweep") + " of front " +
+                std::to_string(s) + " fails its dependency check (not launched)";
       return B200LDLT_FATAL_ERROR;
     }
   }
@@ -2010,117 +2020,100 @@ static size_t stage_pruned(const SolvePlan& SP, const std::vector<SolveTask>& T,
   return *o_fr + align8(4 * R.fr.size());
 }
 
-// Host part of a sparse forward solve: the pruned sweep of b's variables (prune_forward), and everything the device needs
-// in the pinned staging (b too when b_host).  FATAL_ERROR with a message, nothing written to the caller and nothing
-// launched, for a bad pattern or a failed check.
-static int sfs_prepare(Solver* sv, int nbi, const int* bindex, const double* b_host, SfsCall& C) {
-  Analysis& A = *sv->an;
-  SparseFwdPlan& P = *A.sfs;
-  const SolvePlan& SP = A.fronts.solve;
-  const Symbolic& S = A.S;
-  const int n = sv->n;
-  std::vector<int> seed(nbi);
-  for (int i = 0; i < nbi; ++i) {
-    const int v = bindex[i];
-    const char* bad = (v < 0 || v >= n) ? "sparse_fwd_solve: index out of range" : (P.pos_bi[P.iperm[v]] >= 0) ? "sparse_fwd_solve: index appears twice" : nullptr;
-    if (bad) {
-      for (int j = 0; j < i; ++j) P.pos_bi[P.iperm[bindex[j]]] = -1;
-      sv->err = bad;
-      return B200LDLT_FATAL_ERROR;
-    }
-    P.pos_bi[P.iperm[v]] = i;
-    seed[i] = P.iperm[v];
-  }
-  PrunedSweep R;
-  int rc = prune_forward(sv, "sparse_fwd_solve", seed.data(), nbi, R);
-  int nrc = 0, nxi = 0;
-  for (int s : R.run) nrc += S.sn_start[s + 1] - S.sn_start[s];
-  for (int s : R.reach) nxi += S.sn_start[s + 1] - S.sn_start[s];
-  // staging layout: the pruned lists, b, run-set positions and their b indices, output positions; the output slice
-  C.o_b = pruned_bytes(R);
-  C.o_pos = C.o_b + (b_host ? 8 * (size_t)nbi : 0);
-  C.o_bi = C.o_pos + 4 * (size_t)nrc; C.o_xi = C.o_bi + 4 * (size_t)nrc;
-  C.staged = C.o_xi + 4 * (size_t)nxi;
-  C.o_x = align8(C.staged);
-  if (rc == B200LDLT_SUCCESS && C.o_x + 8 * (size_t)n > P.d_buf.n) {
-    sv->err = "sparse_fwd_solve: staging too small";
-    rc = B200LDLT_FATAL_ERROR;
-  }
-  // (the previous call's copy out of the staging must be complete before it is rewritten)
-  if (rc == B200LDLT_SUCCESS && cudaEventSynchronize(P.ev_staged) != cudaSuccess) {
-    sv->err = "sparse_fwd_solve: staging copy failed";
-    rc = B200LDLT_FATAL_ERROR;
-  }
-  if (rc != B200LDLT_SUCCESS) {
-    for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = -1;
-    return rc;
-  }
-  char* h = P.h_buf;
-  {
-    int* pos = reinterpret_cast<int*>(h + C.o_pos);
-    int* bi = reinterpret_cast<int*>(h + C.o_bi);
-    int* xi = reinterpret_cast<int*>(h + C.o_xi);
-    int j = 0;
-    for (int s : R.run) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p, ++j) { pos[j] = p; bi[j] = P.pos_bi[p]; }
-    j = 0;
-    for (int s : R.reach) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) xi[j++] = p;
-  }
+// a compact b swept forward over a pruned run set R_f, as staged: R_f's ncol positions and their indices into the
+// compact column (offsets o_pos / o_bi), the frontier of nfr fronts and the pruned lists
+struct SparseFwd {
+  int ncol = 0, nfr = 0;
+  size_t o_pos = 0, o_bi = 0, o_fr = 0;
+  PrunedLists pl{};
+};
+
+// R_f's positions (the fronts of run, in order) to pos, and to bi for each its index into the compact b of nbi entries
+// at the pivot positions seed (-1: no entry)
+static void stage_positions(PrunedPlan& P, const Symbolic& S, const std::vector<int>& run, const int* seed, int nbi,
+                            int* pos, int* bi) {
+  for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = i;
+  int j = 0;
+  for (int s : run) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p, ++j) { pos[j] = p; bi[j] = P.pos_bi[p]; }
   for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = -1;
-  stage_pruned(SP, SP.tf, R, h, P.d_buf.p, 0, C.pl, &C.o_fr);
-  if (b_host) memcpy(h + C.o_b, b_host, 8 * (size_t)nbi);
-  P.last_run = R.run;
-  std::sort(P.last_run.begin(), P.last_run.end());
-  C.ncol = nrc; C.nxi = nxi; C.nfr = (int)R.fr.size();
+}
+
+// The forward stage of w compact columns (column c of b at b + c nbi) over the staged F: k_sps_in (x = P^T S b on R_f,
+// the frontier's update vectors and flags) and the forward sweep over the pruned lists, D^-1 applied or not.  Launches:
+// 1 + the direct levels that hold a front of R_f + 1 when R_f has a front outside them.
+static int sparse_forward(Solver* sv, SweepState& W, const SparseFwd& F, const double* b, int nbi, int w, bool apply_d) {
+  Analysis& A = *sv->an;
+  const char* d = A.pruned->stg.d.p;
+  A.solve_epoch++;
+  const unsigned g = std::max(1u, cdiv(F.ncol, 256) + (unsigned)F.nfr);
+  k_sps_in<<<dim3(g, w), 256, 0, sv->stream>>>(F.ncol, reinterpret_cast<const int*>(d + F.o_pos),
+                                               reinterpret_cast<const int*>(d + F.o_bi), A.d_perm.p, A.d_scale.p, b, nbi,
+                                               W.d_x.p, W.M.x, F.nfr, reinterpret_cast<const int*>(d + F.o_fr),
+                                               A.d_rows_ptr.p, W.d_cbv.p, W.M.cbv, W.d_done_f.p, W.M.nsn, A.solve_epoch);
+  ++sv->launches;
+  return launch_sweep(sv, A.fronts.solve, W, w, true, apply_d, &F.pl);
+}
+
+// ---- sparse forward solve (b200ldlt_sparse_fwd_solve) ----------------------------------------------------------------
+// one call as prepared on the host: the forward stage of b, and in the staging the output's y-store offsets {0, nxi}
+// and its nxi positions (the reach, ascending: xindex)
+struct SfsCall {
+  int nbi = 0, nxi = 0;
+  SparseFwd F;
+  size_t o_yoff = 0, o_xi = 0;
+};
+
+// Host part (arguments already checked): the pruned forward sweep of b's variables and everything the device needs in
+// the list staging.  FATAL_ERROR with a message, nothing written to the caller and nothing launched, for a failed check
+// or allocation.
+static int sfs_prepare(Solver* sv, int nbi, const int* bindex, SfsCall& C) {
+  Analysis& A = *sv->an;
+  PrunedPlan& P = *A.pruned;
+  const Symbolic& S = A.S;
+  std::vector<int> seed(nbi);
+  for (int i = 0; i < nbi; ++i) seed[i] = P.iperm[bindex[i]];
+  PrunedSweep R;
+  { const int rc = prune(sv, "sparse_fwd_solve", 0, seed.data(), nbi, R); if (rc != B200LDLT_SUCCESS) return rc; }
+  std::sort(R.run.begin(), R.run.end());
+  C.nbi = nbi;
+  C.F.ncol = npos(S, R.run); C.F.nfr = (int)R.fr.size();
+  C.nxi = npos(S, R.reach);
+  // staging layout: the pruned lists, run-set positions and their b indices, the y-store offsets, output positions
+  C.F.o_pos = pruned_bytes(R);
+  C.F.o_bi = C.F.o_pos + 4 * (size_t)C.F.ncol;
+  C.o_yoff = align8(C.F.o_bi + 4 * (size_t)C.F.ncol);
+  C.o_xi = C.o_yoff + 16;
+  { const int rc = P.stg.reserve(sv, "sparse_fwd_solve", C.o_xi + 4 * (size_t)C.nxi); if (rc != B200LDLT_SUCCESS) return rc; }
+  char* h = P.stg.h;
+  stage_pruned(A.fronts.solve, A.fronts.solve.tf, R, h, P.stg.d.p, 0, C.F.pl, &C.F.o_fr);
+  stage_positions(P, S, R.run, seed.data(), nbi, reinterpret_cast<int*>(h + C.F.o_pos), reinterpret_cast<int*>(h + C.F.o_bi));
+  const long long yoff[2] = {0, C.nxi};
+  memcpy(h + C.o_yoff, yoff, sizeof(yoff));
+  int* xi = reinterpret_cast<int*>(h + C.o_xi);
+  for (int s : R.reach) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *xi++ = p;
+  P.last_sfs = std::move(R.run);
   return B200LDLT_SUCCESS;
 }
 
-// Device part: the staged lists in, x = P^T S b on the run set and the frontier's update vectors / flags (k_sfs_in), the
-// forward sweep of job 1 over the pruned lists, the reached positions out (k_sfs_out).  Launches: 2 + the direct levels
-// that hold a front of the run set + 1 when the run set has a front outside them.
+// Device part: the staging in, the forward stage of job 1 (D^-1 left out) on the single-column state, and the reached
+// positions out through the y-store gather (k_inv_out, one column).  Launches: 2 + the direct levels that hold a front
+// of the run set + 1 when the run set has a front outside them.
 static int sfs_enqueue(Solver* sv, const SfsCall& C, const double* d_b, double* d_out) {
   Analysis& A = *sv->an;
-  SparseFwdPlan& P = *A.sfs;
-  cudaStream_t st = sv->stream;
+  PrunedPlan& P = *A.pruned;
   SweepState& W = A.sweep;
-  const char* d = P.d_buf.p;
-  CU(cudaMemcpyAsync(P.d_buf.p, P.h_buf, C.staged, cudaMemcpyHostToDevice, st));
-  CU(cudaEventRecord(P.ev_staged, st));
-  A.solve_epoch++;
-  k_sfs_in<<<cdiv(C.ncol, 256) + C.nfr, 256, 0, st>>>(C.ncol, reinterpret_cast<const int*>(d + C.o_pos),
-                                                      reinterpret_cast<const int*>(d + C.o_bi), A.d_perm.p, A.d_scale.p, d_b,
-                                                      W.d_x.p, reinterpret_cast<const int*>(d + C.o_fr), A.d_rows_ptr.p,
-                                                      W.d_cbv.p, W.d_done_f.p, A.solve_epoch);
-  ++sv->launches;
-  const int rc = launch_sweep(sv, A.fronts.solve, W, 1, true, false, &C.pl);
-  if (rc != B200LDLT_SUCCESS) return rc;
-  k_sfs_out<<<cdiv(C.nxi, 256), 256, 0, st>>>(C.nxi, reinterpret_cast<const int*>(d + C.o_xi), A.d_piv_big.p, W.d_x.p,
-                                             W.d_bigv.p, d_out);
+  const char* d = P.stg.d.p;
+  { const int rc = P.stg.upload(sv, C.o_xi + 4 * (size_t)C.nxi); if (rc != B200LDLT_SUCCESS) return rc; }
+  { const int rc = sparse_forward(sv, W, C.F, d_b, C.nbi, 1, false); if (rc != B200LDLT_SUCCESS) return rc; }
+  k_inv_out<<<dim3(cdiv(C.nxi, 256), 1), 256, 0, sv->stream>>>(0, reinterpret_cast<const long long*>(d + C.o_yoff),
+                                                               reinterpret_cast<const int*>(d + C.o_xi), A.d_piv_big.p,
+                                                               W.d_x.p, W.M.x, W.d_bigv.p, W.M.bigv, d_out);
   ++sv->launches;
   CU(cudaGetLastError());
   return B200LDLT_SUCCESS;
 }
 
 // ---- entries of A^-1 (b200ldlt_inverse_entries) ---------------------------------------------------------------------
-// InvPlan at the first call after an analysis, before its timing starts.  Fronts are numbered in postorder (a parent
-// after its children), so one pass from the last front down gives every front's depth and path length.
-static int inv_state(Solver* sv) {
-  Analysis& A = *sv->an;
-  if (A.inv) return B200LDLT_SUCCESS;
-  const Symbolic& S = A.S;
-  std::unique_ptr<InvPlan> Q(new InvPlan());
-  Q->depth.assign(S.nsn, 0); Q->pathlen.assign(S.nsn, 0);
-  for (int s = S.nsn - 1; s >= 0; --s) {
-    const int p = S.sn_parent[s];
-    if (p >= 0 && p <= s) { sv->err = "inverse_entries: internal: the fronts are not in postorder"; return B200LDLT_FATAL_ERROR; }
-    Q->depth[s] = p >= 0 ? Q->depth[p] + 1 : 0;
-    Q->pathlen[s] = S.k(s) + (p >= 0 ? Q->pathlen[p] : 0);
-  }
-  Q->col_of.assign(sv->n, -1);
-  CU(cudaEventCreateWithFlags(&Q->ev_staged, cudaEventDisableTiming));
-  A.inv = std::move(Q);
-  return B200LDLT_SUCCESS;
-}
-
 // one block of unit columns: columns [c0, c0 + w) of the call, its run set's ncol positions and frontier of nfr fronts,
 // the longest reach of its columns, staging offsets (bytes) and the pruned lists on the device
 struct InvBlock {
@@ -2137,28 +2130,27 @@ struct InvCall {
 
 // Host part of b200ldlt_inverse_entries.  The columns are the distinct variables of irow and jcol, sorted by pivot
 // position (neighbours in the tree share fronts) and cut into blocks of `width`; each block is one pruned forward sweep
-// (prune_forward, its dependency check included) of its unit columns.  Column c keeps y_c = L^-1 P^T S e_c on its reach,
-// the path from its front to the root (ascending positions), at [yoff[c], yoff[c + 1]) of the y store.  Entry (i, j)
-// reads the common suffix of y_i and y_j: the path from the lowest common ancestor of their fronts to the root, pathlen
-// of that front long (0 in different trees of the forest).  Everything the device needs goes to the pinned staging, each
-// block in a region of its own, so one copy carries the call.  FATAL_ERROR with a message, nothing written and nothing
-// launched, for a failed check or allocation.
+// (prune, its dependency check included) of its unit columns.  Column c keeps y_c = L^-1 P^T S e_c on its reach, the
+// path from its front to the root (ascending positions), at [yoff[c], yoff[c + 1]) of the y store.  Entry (i, j) reads
+// the common suffix of y_i and y_j: the path from the lowest common ancestor of their fronts to the root, pathlen of that
+// front long (0 in different trees of the forest).  Everything the device needs goes to the list staging, each block in
+// a region of its own, so one copy carries the call.  FATAL_ERROR with a message, nothing written and nothing launched,
+// for a failed check or allocation.
 static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, int width, InvCall& C) {
   Analysis& A = *sv->an;
-  const SparseFwdPlan& P = *A.sfs;
-  InvPlan& Q = *A.inv;
+  PrunedPlan& P = *A.pruned;
   const SolvePlan& SP = A.fronts.solve;
   const Symbolic& S = A.S;
   std::vector<int> cols;
   for (int t = 0; t < nent; ++t)
     for (const int v : {irow[t], jcol[t]})
-      if (Q.col_of[v] < 0) { Q.col_of[v] = 0; cols.push_back(v); }
+      if (P.col_of[v] < 0) { P.col_of[v] = 0; cols.push_back(v); }
   std::sort(cols.begin(), cols.end(), [&](int a, int b) { return P.iperm[a] < P.iperm[b]; });
   const int nc = (int)cols.size();
-  for (int c = 0; c < nc; ++c) Q.col_of[cols[c]] = c;
-  auto finish = [&](int rc) { for (const int v : cols) Q.col_of[v] = -1; return rc; };   // (col_of back to -1)
+  for (int c = 0; c < nc; ++c) P.col_of[cols[c]] = c;
+  auto finish = [&](int rc) { for (const int v : cols) P.col_of[v] = -1; return rc; };   // (col_of back to -1)
   std::vector<long long> yoff(nc + 1, 0);
-  for (int c = 0; c < nc; ++c) yoff[c + 1] = yoff[c] + Q.pathlen[P.sn_of[P.iperm[cols[c]]]];
+  for (int c = 0; c < nc; ++c) yoff[c + 1] = yoff[c] + P.pathlen[P.sn_of[P.iperm[cols[c]]]];
   const long long ny = yoff[nc];
   // the blocks, and the staging layout: entries, yoff, ypos, then per block its pruned lists, run-set positions and
   // column positions
@@ -2177,9 +2169,9 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
       seed[c] = P.iperm[cols[B.c0 + c]];
       B.maxlen = std::max(B.maxlen, (int)(yoff[B.c0 + c + 1] - yoff[B.c0 + c]));
     }
-    const int rc = prune_forward(sv, "inverse_entries", seed.data(), B.w, R[b]);
+    const int rc = prune(sv, "inverse_entries", 0, seed.data(), B.w, R[b]);
     if (rc != B200LDLT_SUCCESS) return finish(rc);
-    for (int s : R[b].run) B.ncol += S.sn_start[s + 1] - S.sn_start[s];
+    B.ncol = npos(S, R[b].run);
     B.nfr = (int)R[b].fr.size();
     run_all.insert(run_all.end(), R[b].run.begin(), R[b].run.end());
     B.o_lst = o;
@@ -2188,38 +2180,21 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
     o = align8(B.o_col + 4 * (size_t)B.w);
   }
   C.staged = o;
-  // the staging and the y store, grown to this call (a failed allocation leaves them released)
-  if (C.staged > Q.d_buf.n) {
-    Q.d_buf.release();
-    if (Q.h_buf) cudaFreeHost(Q.h_buf);
-    Q.h_buf = nullptr;
-    if (Q.d_buf.alloc(C.staged) != cudaSuccess || cudaHostAlloc((void**)&Q.h_buf, C.staged, cudaHostAllocDefault) != cudaSuccess) {
-      cudaGetLastError();
-      Q.d_buf.release();
-      Q.h_buf = nullptr;
-      sv->err = "inverse_entries: cannot allocate the staging of " + std::to_string(C.staged) + " bytes";
-      return finish(B200LDLT_FATAL_ERROR);
-    }
-  }
-  if ((size_t)ny > Q.d_y.n && Q.d_y.alloc(ny) != cudaSuccess) {
+  { const int rc = P.stg.reserve(sv, "inverse_entries", C.staged); if (rc != B200LDLT_SUCCESS) return finish(rc); }
+  if ((size_t)ny > P.d_y.n && P.d_y.alloc(ny) != cudaSuccess) {
     cudaGetLastError();
     sv->err = "inverse_entries: cannot allocate the y store of " + std::to_string(ny) + " doubles";
     return finish(B200LDLT_FATAL_ERROR);
   }
-  // (the previous call's copy out of the staging must be complete before it is rewritten)
-  if (cudaEventSynchronize(Q.ev_staged) != cudaSuccess) {
-    sv->err = "inverse_entries: staging copy failed";
-    return finish(B200LDLT_FATAL_ERROR);
-  }
-  char* h = Q.h_buf;
+  char* h = P.stg.h;
   InvEnt* he = reinterpret_cast<InvEnt*>(h + C.o_ent);
   for (int t = 0; t < nent; ++t) {
-    const int ci = Q.col_of[irow[t]], cj = Q.col_of[jcol[t]];
+    const int ci = P.col_of[irow[t]], cj = P.col_of[jcol[t]];
     int a = P.sn_of[P.iperm[irow[t]]], b = P.sn_of[P.iperm[jcol[t]]];
-    while (Q.depth[a] > Q.depth[b]) a = S.sn_parent[a];
-    while (Q.depth[b] > Q.depth[a]) b = S.sn_parent[b];
+    while (P.depth[a] > P.depth[b]) a = S.sn_parent[a];
+    while (P.depth[b] > P.depth[a]) b = S.sn_parent[b];
     while (a != b) { a = S.sn_parent[a]; b = S.sn_parent[b]; }   // (both -1 at once in different trees)
-    const int m = a >= 0 ? Q.pathlen[a] : 0;
+    const int m = a >= 0 ? P.pathlen[a] : 0;
     he[t] = InvEnt{yoff[ci + 1] - m, yoff[cj + 1] - m, m, 0};
   }
   memcpy(h + C.o_yoff, yoff.data(), 8 * (size_t)(nc + 1));
@@ -2229,7 +2204,7 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
       for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *yp++ = p;
   for (size_t b = 0; b < R.size(); ++b) {
     InvBlock& B = C.blk[b];
-    stage_pruned(SP, SP.tf, R[b], h, Q.d_buf.p, B.o_lst, B.pl, &B.o_fr);
+    stage_pruned(SP, SP.tf, R[b], h, P.stg.d.p, B.o_lst, B.pl, &B.o_fr);
     int* pos = reinterpret_cast<int*>(h + B.o_pos);
     for (int s : R[b].run) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *pos++ = p;
     int* cp = reinterpret_cast<int*>(h + B.o_col);
@@ -2237,7 +2212,7 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
   }
   std::sort(run_all.begin(), run_all.end());
   run_all.erase(std::unique(run_all.begin(), run_all.end()), run_all.end());
-  Q.last_run = std::move(run_all);
+  P.last_inv = std::move(run_all);
   return finish(B200LDLT_SUCCESS);
 }
 
@@ -2247,13 +2222,12 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
 // a front outside them), + 1.
 static int inv_enqueue(Solver* sv, const InvCall& C, double* out) {
   Analysis& A = *sv->an;
-  InvPlan& Q = *A.inv;
+  PrunedPlan& P = *A.pruned;
   cudaStream_t st = sv->stream;
-  const char* d = Q.d_buf.p;
+  const char* d = P.stg.d.p;
   const long long* yoff = reinterpret_cast<const long long*>(d + C.o_yoff);
   const int* ypos = reinterpret_cast<const int*>(d + C.o_ypos);
-  CU(cudaMemcpyAsync(Q.d_buf.p, Q.h_buf, C.staged, cudaMemcpyHostToDevice, st));
-  CU(cudaEventRecord(Q.ev_staged, st));
+  { const int rc = P.stg.upload(sv, C.staged); if (rc != B200LDLT_SUCCESS) return rc; }
   for (const InvBlock& B : C.blk) {
     SweepState& W = B.w == 1 ? A.sweep : *A.blk;
     A.solve_epoch++;
@@ -2265,10 +2239,10 @@ static int inv_enqueue(Solver* sv, const InvCall& C, double* out) {
     const int rc = launch_sweep(sv, A.fronts.solve, W, B.w, true, false, &B.pl);
     if (rc != B200LDLT_SUCCESS) return rc;
     k_inv_out<<<dim3(cdiv(B.maxlen, 256), B.w), 256, 0, st>>>(B.c0, yoff, ypos, A.d_piv_big.p, W.d_x.p, W.M.x,
-                                                              W.d_bigv.p, W.M.bigv, Q.d_y.p);
+                                                              W.d_bigv.p, W.M.bigv, P.d_y.p);
     ++sv->launches;
   }
-  k_inv_dot<<<cdiv(C.nent, 8), 256, 0, st>>>(C.nent, reinterpret_cast<const InvEnt*>(d + C.o_ent), Q.d_y.p, ypos,
+  k_inv_dot<<<cdiv(C.nent, 8), 256, 0, st>>>(C.nent, reinterpret_cast<const InvEnt*>(d + C.o_ent), P.d_y.p, ypos,
                                              A.d_ptype.p, A.d_dinv.p, A.d_doff.p, out);
   ++sv->launches;
   CU(cudaGetLastError());
@@ -2276,108 +2250,24 @@ static int inv_enqueue(Solver* sv, const InvCall& C, double* out) {
 }
 
 // ---- sparse solve (b200ldlt_sparse_solve) ---------------------------------------------------------------------------
-// SparseSolvePlan, and sparse_fwd_solve's per-front indices (not its staging), at the first call after an analysis,
-// before its timing starts.  The analysis keeps the backward top tasks on the device only: they are copied back here,
-// once, and indexed by front.
-static int sps_state(Solver* sv) {
-  { const int rc = sfs_state(sv, false); if (rc != B200LDLT_SUCCESS) return rc; }
-  Analysis& A = *sv->an;
-  if (A.sps) return B200LDLT_SUCCESS;
-  const SolvePlan& SP = A.fronts.solve;
-  std::unique_ptr<SparseSolvePlan> Q(new SparseSolvePlan());
-  Q->tb.resize(SP.ntb);
-  if (SP.ntb > 0) {
-    CU(cudaMemcpyAsync(Q->tb.data(), SP.d_tb.p, sizeof(SolveTask) * (size_t)SP.ntb, cudaMemcpyDeviceToHost, sv->stream));
-    CU(cudaStreamSynchronize(sv->stream));
-  }
-  index_tasks(SP, Q->tb, SP.ntb, A.S.nsn, Q->task_ptr, Q->task_idx);
-  Q->m_task.assign(std::max(SP.ntb, 1), 0);
-  CU(cudaEventCreateWithFlags(&Q->ev_staged, cudaEventDisableTiming));
-  A.sps = std::move(Q);
-  return B200LDLT_SUCCESS;
-}
-
-// Host part of a pruned backward sweep from the pivot positions seed[0..nseed) of the selected variables.  The reach (the
-// fronts on the tree paths from their fronts to the root) is ancestor-closed; the run set R_b adds the fronts walked by
-// a subtree item that walks a reached front and the fronts of a backward bundle that holds one (collect_run_set over
-// the backward list).  The frontier F_b (R.fr) = the parents of R_b outside R_b: only item-mates and bundle-mates have
-// one.  Their backward flags are stamped, so those mates read stale x at ancestor positions; their outputs are never
-// returned and nothing in the reach reads them.  Then the mirror of prune_forward's check, before anything is launched:
-// every front of R_b owns all of its backward top tasks -- each chunked block with all of its chunks, a big front with
-// all of its BT and BX blocks (bcnt_b and the chunk counters count modulo) -- and the parent of every front of R_b is a
-// root, in F_b, or runs EARLIER in the pruned backward order: top tasks, then subtree items (the same subtree walk
-// counts: it is walked from its root down), then the direct levels from the top down.  FATAL_ERROR with
-// "sparse_solve: ..." when the check fails.
-static int prune_backward(Solver* sv, const int* seed, int nseed, PrunedSweep& R) {
-  Analysis& A = *sv->an;
-  SparseFwdPlan& P = *A.sfs;
-  SparseSolvePlan& Q = *A.sps;
-  const SolvePlan& SP = A.fronts.solve;
-  const Symbolic& S = A.S;
-  const int nd = (int)SP.direct_cnt.size();
-  const unsigned m = ++P.stamp;
-  collect_run_set(P, SP, S, Q.tb, Q.task_ptr, Q.task_idx, Q.m_task, m, seed, nseed, R);
-  // pruned backward order: top task j -> slot j, subtree item i -> tasks + i, direct level l -> tasks + items + nd - 1 - l
-  const int nt = (int)R.tasks.size(), ni = (int)R.items.size();
-  for (int s : R.run) { P.ord0[s] = INT_MAX; P.ord1[s] = -1; }
-  auto upd = [&](int s, int o) { P.ord0[s] = std::min(P.ord0[s], o); P.ord1[s] = std::max(P.ord1[s], o); };
-  for (int j = 0; j < nt; ++j) {
-    const SolveTask& T = Q.tb[R.tasks[j]];
-    if (T.type == ST_SMALL) for (int w = 0; w < T.blk; ++w) upd(SP.bundle[T.s + w], j);
-    else upd(T.s, j);
-  }
-  for (int i = 0; i < ni; ++i)
-    for (int e = P.item_ptr[R.items[i]]; e < P.item_ptr[R.items[i] + 1]; ++e) upd(P.item_fr[e], nt + i);
-  for (int l = 0; l < nd; ++l) for (int i : R.dl[l]) upd(SP.direct[l][i], nt + ni + nd - 1 - l);
-  for (int s : R.run) {
-    bool ok = P.ord1[s] >= 0;
-    int nbt = 0, nbx = 0;
-    for (int e = Q.task_ptr[s]; ok && e < Q.task_ptr[s + 1]; ++e) {
-      const SolveTask& T = Q.tb[Q.task_idx[e]];
-      ok = Q.m_task[Q.task_idx[e]] == m;
-      if (ok && (T.type == ST_BT || T.type == ST_BX) && T.q == 0) {
-        ok = e + T.nq <= Q.task_ptr[s + 1];
-        for (int q = 1; ok && q < T.nq; ++q) {
-          const SolveTask& U = Q.tb[Q.task_idx[e + q]];
-          ok = U.type == T.type && U.blk == T.blk && U.cidx == T.cidx && U.q == q && Q.m_task[Q.task_idx[e + q]] == m;
-        }
-        (T.type == ST_BT ? nbt : nbx) += 1;
-      }
-    }
-    if (ok && S.f(s) > DF_MIDMAX && P.dlev[s] < 0 && P.item_of[s] < 0)
-      ok = nbt == (S.k(s) + DF_BLK - 1) / DF_BLK && nbx == (S.k(s) + DF_BLK - 1) / DF_BLK;
-    const int p = S.sn_parent[s];
-    if (ok && p >= 0) {
-      if (P.m_run[p] == m) ok = (P.sub_of[s] >= 0 && P.sub_of[p] == P.sub_of[s]) || P.ord1[p] < P.ord0[s];
-      else if (P.m_fr[p] != m) { P.m_fr[p] = m; R.fr.push_back(p); }
-    }
-    if (!ok) {
-      sv->err = "sparse_solve: the pruned backward sweep of front " + std::to_string(s) + " fails its dependency check (not launched)";
-      return B200LDLT_FATAL_ERROR;
-    }
-  }
-  return B200LDLT_SUCCESS;
-}
-
-// one sparse solve as prepared on the host: dense b (bindex NULL) / every entry (xsel NULL); the forward run set's
-// ncol positions and frontier of nfr fronts; the nz positions to zero and the nfb fronts of F_b between the sweeps; the
-// staging offsets (bytes) and the pruned lists on the device
+// one sparse solve as prepared on the host: dense b (bindex NULL) / every entry (xsel NULL); the forward stage of a
+// sparse b; the nz positions to zero and the nfb fronts of F_b between the sweeps; the staging offsets (bytes) and the
+// pruned backward lists on the device
 struct SpsCall {
   bool dense_b = false, all_x = false;
-  int nbi = 0, nxs = 0, ncol = 0, nfr = 0, nz = 0, nfb = 0;
-  size_t o_pos = 0, o_bi = 0, o_ffr = 0, o_z = 0, o_fb = 0, o_xpos = 0, staged = 0;
-  PrunedLists plf{}, plb{};
+  int nbi = 0, nxs = 0, nz = 0, nfb = 0;
+  SparseFwd F;
+  size_t o_z = 0, o_fb = 0, o_xpos = 0, staged = 0;
+  PrunedLists plb{};
 };
 
-// Host part of b200ldlt_sparse_solve (arguments already checked): one pruned forward sweep for the pattern of b
-// (prune_forward) and one pruned backward sweep for the selection (prune_backward), shared by every block of columns;
-// the positions to zero between the sweeps (R_b \ R_f with a sparse b; with a full selection everything outside R_f);
-// the output positions; all of it in the pinned staging, grown to this call.  FATAL_ERROR with a message, nothing
-// written and nothing launched, for a failed check or allocation.
+// Host part of b200ldlt_sparse_solve (arguments already checked): one pruned forward sweep for the pattern of b and one
+// pruned backward sweep for the selection (prune), shared by every block of columns; the positions to zero between the
+// sweeps (R_b \ R_f with a sparse b; with a full selection everything outside R_f); the output positions; all of it in
+// the list staging.  FATAL_ERROR with a message, nothing written and nothing launched, for a failed check or allocation.
 static int sps_prepare(Solver* sv, int nbi, const int* bindex, int nxs, const int* xsel, SpsCall& C) {
   Analysis& A = *sv->an;
-  SparseFwdPlan& P = *A.sfs;
-  SparseSolvePlan& Q = *A.sps;
+  PrunedPlan& P = *A.pruned;
   const SolvePlan& SP = A.fronts.solve;
   const Symbolic& S = A.S;
   const int nsn = S.nsn;
@@ -2385,7 +2275,7 @@ static int sps_prepare(Solver* sv, int nbi, const int* bindex, int nxs, const in
   std::vector<int> all;
   if (C.dense_b || C.all_x) { all.resize(nsn); for (int s = 0; s < nsn; ++s) all[s] = s; }
   if (C.dense_b && C.all_x) {   // job 0 itself
-    Q.last_fwd = all; Q.last_bwd = all;
+    P.last_fwd = all; P.last_bwd = all;
     return B200LDLT_SUCCESS;
   }
   PrunedSweep Rf, Rb;
@@ -2393,13 +2283,13 @@ static int sps_prepare(Solver* sv, int nbi, const int* bindex, int nxs, const in
   if (!C.dense_b) {
     seed.resize(nbi);
     for (int i = 0; i < nbi; ++i) seed[i] = P.iperm[bindex[i]];
-    const int rc = prune_forward(sv, "sparse_solve", seed.data(), nbi, Rf);
+    const int rc = prune(sv, "sparse_solve", 0, seed.data(), nbi, Rf);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   if (!C.all_x) {
     std::vector<int> sb(nxs);
     for (int i = 0; i < nxs; ++i) sb[i] = P.iperm[xsel[i]];
-    const int rc = prune_backward(sv, sb.data(), nxs, Rb);
+    const int rc = prune(sv, "sparse_solve", 1, sb.data(), nxs, Rb);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
   std::vector<int> runf = C.dense_b ? all : Rf.run, runb = C.all_x ? all : Rb.run;
@@ -2407,93 +2297,56 @@ static int sps_prepare(Solver* sv, int nbi, const int* bindex, int nxs, const in
   std::sort(runb.begin(), runb.end());
   std::vector<int> zf;   // fronts whose forward result is zeroed between the sweeps
   if (!C.dense_b) std::set_difference(runb.begin(), runb.end(), runf.begin(), runf.end(), std::back_inserter(zf));
-  if (!C.dense_b) for (int s : runf) C.ncol += S.sn_start[s + 1] - S.sn_start[s];
-  for (int s : zf) C.nz += S.sn_start[s + 1] - S.sn_start[s];
-  C.nfr = (int)Rf.fr.size(); C.nfb = (int)Rb.fr.size();
+  if (!C.dense_b) C.F.ncol = npos(S, runf);
+  C.nz = npos(S, zf);
+  C.F.nfr = (int)Rf.fr.size(); C.nfb = (int)Rb.fr.size();
   // staging layout: forward pruned lists, backward pruned lists, run-set positions and their b indices, zeroed
   // positions, output positions
-  C.o_pos = pruned_bytes(Rf) + pruned_bytes(Rb);
-  C.o_bi = C.o_pos + 4 * (size_t)C.ncol;
-  C.o_z = C.o_bi + 4 * (size_t)C.ncol;
+  C.F.o_pos = pruned_bytes(Rf) + pruned_bytes(Rb);
+  C.F.o_bi = C.F.o_pos + 4 * (size_t)C.F.ncol;
+  C.o_z = C.F.o_bi + 4 * (size_t)C.F.ncol;
   C.o_xpos = C.o_z + 4 * (size_t)C.nz;
   C.staged = align8(C.o_xpos + (C.all_x ? 0 : 4 * (size_t)nxs));
-  if (C.staged > Q.d_buf.n) {
-    Q.d_buf.release();
-    if (Q.h_buf) cudaFreeHost(Q.h_buf);
-    Q.h_buf = nullptr;
-    if (Q.d_buf.alloc(C.staged) != cudaSuccess || cudaHostAlloc((void**)&Q.h_buf, C.staged, cudaHostAllocDefault) != cudaSuccess) {
-      cudaGetLastError();
-      Q.d_buf.release();
-      Q.h_buf = nullptr;
-      sv->err = "sparse_solve: cannot allocate the staging of " + std::to_string(C.staged) + " bytes";
-      return B200LDLT_FATAL_ERROR;
-    }
-  }
-  // (the previous call's copy out of the staging must be complete before it is rewritten)
-  if (cudaEventSynchronize(Q.ev_staged) != cudaSuccess) {
-    sv->err = "sparse_solve: staging copy failed";
-    return B200LDLT_FATAL_ERROR;
-  }
-  char* h = Q.h_buf;
-  const char* d = Q.d_buf.p;
+  { const int rc = P.stg.reserve(sv, "sparse_solve", C.staged); if (rc != B200LDLT_SUCCESS) return rc; }
+  char* h = P.stg.h;
+  const char* d = P.stg.d.p;
   size_t o = 0;
-  if (!C.dense_b) o = stage_pruned(SP, SP.tf, Rf, h, d, o, C.plf, &C.o_ffr);
+  if (!C.dense_b) o = stage_pruned(SP, SP.tf, Rf, h, d, o, C.F.pl, &C.F.o_fr);
   if (!C.all_x) {
-    stage_pruned(SP, Q.tb, Rb, h, d, o, C.plb, &C.o_fb);
+    stage_pruned(SP, SP.tb, Rb, h, d, o, C.plb, &C.o_fb);
     int* xp = reinterpret_cast<int*>(h + C.o_xpos);
     for (int i = 0; i < nxs; ++i) xp[i] = P.iperm[xsel[i]];
   }
-  if (!C.dense_b) {
-    for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = i;
-    int* pos = reinterpret_cast<int*>(h + C.o_pos);
-    int* bi = reinterpret_cast<int*>(h + C.o_bi);
-    int j = 0;
-    for (int s : runf) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p, ++j) { pos[j] = p; bi[j] = P.pos_bi[p]; }
-    for (int i = 0; i < nbi; ++i) P.pos_bi[seed[i]] = -1;
-  }
+  if (!C.dense_b)
+    stage_positions(P, S, runf, seed.data(), nbi, reinterpret_cast<int*>(h + C.F.o_pos), reinterpret_cast<int*>(h + C.F.o_bi));
   int* zp = reinterpret_cast<int*>(h + C.o_z);
   for (int s : zf) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *zp++ = p;
-  Q.last_fwd = std::move(runf);
-  Q.last_bwd = std::move(runb);
+  P.last_fwd = std::move(runf);
+  P.last_bwd = std::move(runb);
   return B200LDLT_SUCCESS;
 }
 
 // Device part: the staging in, then per block of w columns (the blocked state, or the single-column state for w = 1):
-// the forward stage -- dense b: job 0's (k_rhs_in and the full sweep); sparse b: k_sps_in and job 0's forward sweep
-// (D^-1 applied, the rounding of the fused sweep) over the pruned lists -- then under the backward epoch k_sps_mid, the
-// backward sweep (pruned to R_b unless every entry is selected) and the output (k_sol_out for every entry, k_sps_out
-// for a selection).  Launches per block: 1 + d_f + t_f + 1 + d_b + t_b + 1; with a dense b and every entry selected the
-// block is job 0 itself (enqueue_solve): 4 + 2 D.
+// the forward stage -- dense b: job 0's (k_rhs_in and the full sweep); sparse b: sparse_forward with D^-1 applied (the
+// rounding of the fused sweep) -- then under the backward epoch k_sps_mid, the backward sweep (pruned to R_b unless
+// every entry is selected) and the output (k_sol_out for every entry, k_sps_out for a selection).  Launches per block:
+// 1 + d_f + t_f + 1 + d_b + t_b + 1; with a dense b and every entry selected the block is job 0 itself (enqueue_solve):
+// 4 + 2 D.
 static int sps_enqueue(Solver* sv, const SpsCall& C, int nrhs, bool blocked, const double* d_b, double* d_x) {
   Analysis& A = *sv->an;
-  SparseSolvePlan& Q = *A.sps;
+  PrunedPlan& P = *A.pruned;
   const SolvePlan& SP = A.fronts.solve;
   cudaStream_t st = sv->stream;
   const int n = sv->n;
-  const char* d = Q.d_buf.p;
+  const char* d = P.stg.d.p;
   const bool job0 = C.dense_b && C.all_x;
-  if (!job0) {
-    CU(cudaMemcpyAsync(Q.d_buf.p, Q.h_buf, C.staged, cudaMemcpyHostToDevice, st));
-    CU(cudaEventRecord(Q.ev_staged, st));
-  }
+  if (!job0) { const int rc = P.stg.upload(sv, C.staged); if (rc != B200LDLT_SUCCESS) return rc; }
   return for_blocks(nrhs, blocked ? A.blk->width : 1, [&](int c, int w) -> int {
     SweepState& W = w == 1 ? A.sweep : *A.blk;
     const double* b = d_b + (size_t)c * C.nbi;
     double* x = d_x + (size_t)c * C.nxs;
     if (job0) return enqueue_solve(sv, W, 0, b, x, w);
-    int rc;
-    if (C.dense_b) {
-      rc = forward(sv, SP, W, b, w);
-    } else {
-      A.solve_epoch++;
-      const unsigned g = std::max(1u, cdiv(C.ncol, 256) + (unsigned)C.nfr);
-      k_sps_in<<<dim3(g, w), 256, 0, st>>>(C.ncol, reinterpret_cast<const int*>(d + C.o_pos),
-                                           reinterpret_cast<const int*>(d + C.o_bi), A.d_perm.p, A.d_scale.p, b, C.nbi,
-                                           W.d_x.p, W.M.x, C.nfr, reinterpret_cast<const int*>(d + C.o_ffr), A.d_rows_ptr.p,
-                                           W.d_cbv.p, W.M.cbv, W.d_done_f.p, W.M.nsn, A.solve_epoch);
-      ++sv->launches;
-      rc = launch_sweep(sv, SP, W, w, true, true, &C.plf);
-    }
+    int rc = C.dense_b ? forward(sv, SP, W, b, w) : sparse_forward(sv, W, C.F, b, C.nbi, w, true);
     if (rc != B200LDLT_SUCCESS) return rc;
     A.solve_epoch++;
     const unsigned g = std::max(1u, cdiv(C.nz, 256) + cdiv(C.nfb, 256));
@@ -2789,29 +2642,37 @@ static int lmultiply(Solver* sv, int trans, int nrhs, const double* x, double* y
   return timed_call(sv, [&] { return enqueue_lmul_columns(sv, trans, nrhs, x, y); });
 }
 
+// The index-set check of the pruned calls: "index out of range" when an entry of idx[0..cnt) is outside [0, n), and
+// with `distinct` "bindex entry appears twice" when two are equal; nullptr when the set is good.
+static const char* bad_index_set(int n, int cnt, const int* idx, bool distinct) {
+  for (int i = 0; i < cnt; ++i)
+    if (idx[i] < 0 || idx[i] >= n) return "index out of range";
+  if (!distinct || cnt < 2) return nullptr;
+  std::vector<char> seen(n, 0);
+  for (int i = 0; i < cnt; ++i)
+    if (seen[idx[i]]++) return "bindex entry appears twice";
+  return nullptr;
+}
+
 // b200ldlt_sparse_fwd_solve (host == true: b and x in host memory) / _device
 static int sparse_fwd(Solver* sv, int nbi, const int* bindex, const double* b, bool host, int* nxi, int* xindex, double* x) {
-  if (nbi < 0 || nbi > sv->n) { sv->err = "sparse_fwd_solve: nbi must be 0..n"; return B200LDLT_FATAL_ERROR; }
-  if (nbi > 0 && (!bindex || !b || !nxi || !xindex || !x)) { sv->err = "sparse_fwd_solve: NULL argument"; return B200LDLT_FATAL_ERROR; }
+  const char* bad = (nbi < 0 || nbi > sv->n) ? "nbi must be 0..n"
+                  : nbi > 0 && (!bindex || !b || !nxi || !xindex || !x) ? "NULL argument"
+                  : bad_index_set(sv->n, nbi, bindex, true);
+  if (bad) { sv->err = std::string("sparse_fwd_solve: ") + bad; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "sparse_fwd_solve"); if (rc != B200LDLT_SUCCESS) return rc; }
   if (nbi == 0) {
     if (nxi) *nxi = 0;
     return no_columns(sv);
   }
-  { const int rc = sfs_state(sv, true); if (rc != B200LDLT_SUCCESS) return rc; }
+  { const int rc = pruned_state(sv, "sparse_fwd_solve"); if (rc != B200LDLT_SUCCESS) return rc; }
   SfsCall C;
-  { const int rc = sfs_prepare(sv, nbi, bindex, host ? b : nullptr, C); if (rc != B200LDLT_SUCCESS) return rc; }
-  SparseFwdPlan& P = *sv->an->sfs;
-  const double* d_b = host ? reinterpret_cast<const double*>(P.d_buf.p + C.o_b) : b;
-  double* d_x = host ? reinterpret_cast<double*>(P.d_buf.p + C.o_x) : x;
-  const int rc = timed_call(sv, [&]() -> int {
-    { const int rc2 = sfs_enqueue(sv, C, d_b, d_x); if (rc2 != B200LDLT_SUCCESS) return rc2; }
-    if (host) CU(cudaMemcpyAsync(P.h_buf + C.o_x, d_x, (size_t)C.nxi * sizeof(double), cudaMemcpyDeviceToHost, sv->stream));
-    return B200LDLT_SUCCESS;
-  });
+  { const int rc = sfs_prepare(sv, nbi, bindex, C); if (rc != B200LDLT_SUCCESS) return rc; }
+  // host: x at the start of the staging, b after it
+  const int rc = host ? staged_call(sv, b, nbi, x, C.nxi, [&](double* d) { return sfs_enqueue(sv, C, d + C.nxi, d); }, 0, C.nxi)
+                      : timed_call(sv, [&] { return sfs_enqueue(sv, C, b, x); });
   if (rc != B200LDLT_SUCCESS) return rc;
-  if (host) memcpy(x, P.h_buf + C.o_x, (size_t)C.nxi * sizeof(double));
-  memcpy(xindex, P.h_buf + C.o_xi, (size_t)C.nxi * sizeof(int));
+  memcpy(xindex, sv->an->pruned->stg.h + C.o_xi, sizeof(int) * (size_t)C.nxi);
   *nxi = C.nxi;
   return B200LDLT_SUCCESS;
 }
@@ -2819,13 +2680,12 @@ static int sparse_fwd(Solver* sv, int nbi, const int* bindex, const double* b, b
 // b200ldlt_inverse_entries (host == true: vals in host memory) / _device
 static int inverse_entries(Solver* sv, int nent, const int* irow, const int* jcol, double* vals, bool host) {
   const char* bad = nent < 0 ? "nent must be >= 0" : nent > 0 && (!irow || !jcol || !vals) ? "NULL argument" : nullptr;
-  for (int t = 0; !bad && t < nent; ++t)
-    if (irow[t] < 0 || irow[t] >= sv->n || jcol[t] < 0 || jcol[t] >= sv->n) bad = "index out of range";
+  if (!bad) bad = bad_index_set(sv->n, nent, irow, false);
+  if (!bad) bad = bad_index_set(sv->n, nent, jcol, false);
   if (bad) { sv->err = std::string("inverse_entries: ") + bad; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "inverse_entries"); if (rc != B200LDLT_SUCCESS) return rc; }
   if (nent == 0) return no_columns(sv);
-  { const int rc = sfs_state(sv, false); if (rc != B200LDLT_SUCCESS) return rc; }
-  { const int rc = inv_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
+  { const int rc = pruned_state(sv, "inverse_entries"); if (rc != B200LDLT_SUCCESS) return rc; }
   bool several = false;
   for (int t = 0; !several && t < nent; ++t) several = irow[t] != irow[0] || jcol[t] != irow[0];
   const bool blocked = several && block_solve_state(sv);
@@ -2843,19 +2703,12 @@ static int sparse_solve(Solver* sv, int nrhs, int nbi, const int* bindex, const 
                   : ((!b && nrhs > 0 && nbi > 0) || (!x && nrhs > 0 && nxs > 0)) ? "NULL argument"
                   : (!bindex && nbi != n) ? "a NULL bindex needs nbi = n" : (!xsel && nxs != n) ? "a NULL xsel needs nxs = n"
                   : nullptr;
-  if (!bad && bindex) {
-    std::vector<int> v(nbi);
-    if (nbi > 0) memcpy(v.data(), bindex, sizeof(int) * (size_t)nbi);
-    std::sort(v.begin(), v.end());
-    if (nbi > 0 && (v.front() < 0 || v.back() >= n)) bad = "index out of range";
-    else if (std::adjacent_find(v.begin(), v.end()) != v.end()) bad = "bindex entry appears twice";
-  }
-  for (int i = 0; !bad && xsel && i < nxs; ++i)
-    if (xsel[i] < 0 || xsel[i] >= n) bad = "index out of range";
+  if (!bad && bindex) bad = bad_index_set(n, nbi, bindex, true);
+  if (!bad && xsel) bad = bad_index_set(n, nxs, xsel, false);
   if (bad) { sv->err = std::string("sparse_solve: ") + bad; return B200LDLT_FATAL_ERROR; }
   { const int rc = factors_state(sv, "sparse_solve"); if (rc != B200LDLT_SUCCESS) return rc; }
   if (nrhs == 0 || nxs == 0) return no_columns(sv);
-  { const int rc = sps_state(sv); if (rc != B200LDLT_SUCCESS) return rc; }
+  { const int rc = pruned_state(sv, "sparse_solve"); if (rc != B200LDLT_SUCCESS) return rc; }
   const bool blocked = nrhs > 1 && block_solve_state(sv);
   SpsCall C;
   { const int rc = sps_prepare(sv, nbi, bindex, nxs, xsel, C); if (rc != B200LDLT_SUCCESS) return rc; }
@@ -3986,10 +3839,10 @@ int64_t b200ldlt_symbolic_array(b200ldlt_handle h, const char* name, int64_t* ou
   if (nm == "sn_level") RET(S.sn_level);
   if (nm == "level_ptr") RET(S.level_ptr);
   if (nm == "level_sn") RET(S.level_sn);
-  if (nm == "sparse_run_set") { static const std::vector<int> none; RET(A.sfs ? A.sfs->last_run : none); }
-  if (nm == "inverse_run_set") { static const std::vector<int> none; RET(A.inv ? A.inv->last_run : none); }
-  if (nm == "sparse_solve_fwd_run_set") { static const std::vector<int> none; RET(A.sps ? A.sps->last_fwd : none); }
-  if (nm == "sparse_solve_bwd_run_set") { static const std::vector<int> none; RET(A.sps ? A.sps->last_bwd : none); }
+  if (nm == "sparse_run_set") { static const std::vector<int> none; RET(A.pruned ? A.pruned->last_sfs : none); }
+  if (nm == "inverse_run_set") { static const std::vector<int> none; RET(A.pruned ? A.pruned->last_inv : none); }
+  if (nm == "sparse_solve_fwd_run_set") { static const std::vector<int> none; RET(A.pruned ? A.pruned->last_fwd : none); }
+  if (nm == "sparse_solve_bwd_run_set") { static const std::vector<int> none; RET(A.pruned ? A.pruned->last_bwd : none); }
 #undef RET
   return -1;
 }

@@ -8,11 +8,17 @@ code): build the other library into a directory of its own, then
 The dump holds the SHA-256 of the bytes of each array (the full arrays run to gigabytes) and the launch counts.
 
 What is dumped, per system (seeded generators and the golden systems of tests/golden):
-  * factor with use_graph 1 (and its replay), use_graph 0, B200_ONE_STREAM=1 and B200_SOLVE_BLOCK=1: status, inertia,
-    launches_factor, D^-1 (enquire_indef) and host solves of 1, 8 and 13 columns with launches_solve;
+  * factor with use_graph 1 (and its replay), use_graph 0, B200_ONE_STREAM=1, B200_SOLVE_BLOCK=1 and
+    B200_SOLVE_DIRECT=0: status, inertia, launches_factor, D^-1 (enquire_indef) and host solves of 1, 8 and 13 columns
+    with launches_solve;
   * on the use_graph 1 handle: device solves of 1, 8 and 13 columns, jobs 1..4 (host 1 and 13 columns, device 8),
-    lmultiply (trans 0 / 1, host 1 and 13, device 8), the sparse forward solve (host and device), selected inversion,
-    solve_refine_device and the Fredholm solve without zero pivots;
+    lmultiply (trans 0 / 1, host 1 and 13, device 8), selected inversion, solve_refine_device and the Fredholm solve
+    without zero pivots;
+  * on every handle of the first item, the calls that run pruned sweeps, host and device, each followed by the four run
+    sets of symbolic_array: the sparse forward solve; inverse_entries (a diagonal, an off-diagonal entry in both orders,
+    the first and last variable -- different trees on the two-component system --, and a block of 20 x 20 entries,
+    wider than the blocked-solve width); the sparse solve with 1 and 13 columns (sparse b with a selection, dense b with
+    a selection, sparse b with every entry, both NULL);
   * the Fredholm solve on kept singular factors, blocked and with B200_SOLVE_BLOCK=1 (host 1, 5 and 13 columns, device 5);
   * Schur mode with the root in each solve class: S_c, reduce and expand (host 1 and 11 columns, device 8);
   * the sharded factor and solve with 2 and 4 ranks emulated on one GPU, on two matrices.
@@ -54,6 +60,7 @@ def dump(lib, out):
     from ipopt_b200.sharded import ShardedLdlt
     from test_partial_solve import LARGE, SYSTEMS
     from test_fredholm import zeroed
+    from test_inverse_entries import two_components
     from test_schur import dense, pick_vars
 
     rec = {}
@@ -94,6 +101,58 @@ def dump(lib, out):
             put("%s/solve%d" % (key, w), X)
             launches(s, "%s/solve%d" % (key, w))
 
+    def run_sets(s, key):
+        for name in ("sparse_run_set", "inverse_run_set", "sparse_solve_fwd_run_set", "sparse_solve_bwd_run_set"):
+            put("%s/%s" % (key, name), s.symbolic(name))
+
+    def pruned_suite(s, key, dim, rng):
+        for k in (1, 5, min(50, dim)):
+            bi = np.sort(rng.choice(dim, k, replace=False)).astype(np.int32)
+            b = rng.standard_normal(k)
+            xi, x = s.sparse_fwd_solve(bi, b)
+            put("%s/sfs%d" % (key, k), xi, x)
+            launches(s, "%s/sfs%d" % (key, k))
+            run_sets(s, "%s/sfs%d" % (key, k))
+            Bd, Xd = dev(b), torch.zeros(dim, dtype=torch.float64, device="cuda")
+            xi = s.sparse_fwd_solve_device(bi, Bd.data_ptr(), Xd.data_ptr())
+            put("%s/sfs_dev%d" % (key, k), xi, Xd.cpu().numpy()[:len(xi)])
+            launches(s, "%s/sfs_dev%d" % (key, k))
+            run_sets(s, "%s/sfs_dev%d" % (key, k))
+        i, j = (int(v) for v in rng.choice(dim, 2, replace=False))
+        blk = rng.choice(dim, min(20, dim), replace=False)
+        bi, bj = np.meshgrid(blk, blk, indexing="ij")
+        sets = {"diag": ([i], [i]), "ij": ([i], [j]), "ji": ([j], [i]), "ends": ([0, dim - 1], [dim - 1, 0]),
+                "block20": (bi.ravel(), bj.ravel())}
+        for name, (irow, jcol) in sets.items():
+            irow, jcol = np.asarray(irow, np.int32), np.asarray(jcol, np.int32)
+            tag = "%s/inv_%s" % (key, name)
+            put(tag, s.inverse_entries(irow, jcol))
+            launches(s, tag)
+            run_sets(s, tag)
+            V = torch.zeros(len(irow), dtype=torch.float64, device="cuda")
+            assert s.inverse_entries_device(irow, jcol, V.data_ptr()) == SYMSOLVER_SUCCESS, s.last_error()
+            put(tag + "_dev", V.cpu().numpy())
+            launches(s, tag + "_dev")
+            run_sets(s, tag + "_dev")
+        bi = np.sort(rng.choice(dim, min(5, dim), replace=False)).astype(np.int32)
+        xs = rng.choice(dim, min(7, dim), replace=False).astype(np.int32)
+        for w in (1, 13):
+            for mode, (bindex, xsel) in (("sparse_sel", (bi, xs)), ("dense_sel", (None, xs)), ("sparse_all", (bi, None)),
+                                         ("dense_all", (None, None))):
+                nbi = dim if bindex is None else len(bindex)
+                nxs = dim if xsel is None else len(xsel)
+                B = rng.standard_normal((w, nbi))
+                tag = "%s/sps_%s_%d" % (key, mode, w)
+                put(tag, s.sparse_solve(bindex, B, xsel))
+                launches(s, tag)
+                run_sets(s, tag)
+                Bd, Xd = dev(B), torch.zeros(w * nxs, dtype=torch.float64, device="cuda")
+                assert s.sparse_solve_device(bindex, Bd.data_ptr(), xsel, Xd.data_ptr(), w) == SYMSOLVER_SUCCESS, \
+                    s.last_error()
+                put(tag + "_dev", Xd.cpu().numpy())
+                launches(s, tag + "_dev")
+                run_sets(s, tag + "_dev")
+
     def full_suite(s, key, dim, nnz, rng):
         for w in (1, 8, 13):
             X = dev(rng.standard_normal(dim * w))
@@ -118,16 +177,6 @@ def dump(lib, out):
             assert s.lmultiply_device(trans, X.data_ptr(), Y.data_ptr(), 8) == SYMSOLVER_SUCCESS, s.last_error()
             put("%s/lmul%d_dev8" % (key, trans), Y.cpu().numpy())
             launches(s, "%s/lmul%d_dev8" % (key, trans))
-        for k in (1, 5, min(50, dim)):
-            bi = np.sort(rng.choice(dim, k, replace=False)).astype(np.int32)
-            b = rng.standard_normal(k)
-            xi, x = s.sparse_fwd_solve(bi, b)
-            put("%s/sfs%d" % (key, k), xi, x)
-            launches(s, "%s/sfs%d" % (key, k))
-            Bd, Xd = dev(b), torch.zeros(dim, dtype=torch.float64, device="cuda")
-            xi = s.sparse_fwd_solve_device(bi, Bd.data_ptr(), Xd.data_ptr())
-            put("%s/sfs_dev%d" % (key, k), xi, Xd.cpu().numpy()[:len(xi)])
-            launches(s, "%s/sfs_dev%d" % (key, k))
         d, v = s.selected_inverse(True, True)
         put(key + "/selinv", d, v)
         launches(s, key + "/selinv")
@@ -143,10 +192,12 @@ def dump(lib, out):
     systems = {name: SYSTEMS[name] for name in ("MBndryCntrl1_30", "LukVlE1_1000", "random", "mbndry30_wzero")}
     systems["mbndry400"] = LARGE
     systems["mbndry60"] = lambda: mbndry_kkt(60, sigma_spread=3.0, seed=9)[:4]
+    systems["forest"] = two_components
     for name, make in systems.items():
         dim, irn, jcn, val = make()
         for tag, opts, sw in (("graph", {}, {}), ("nograph", {"use_graph": 0}, {}),
-                              ("onestream", {}, {"B200_ONE_STREAM": "1"}), ("block1", {}, {"B200_SOLVE_BLOCK": "1"})):
+                              ("onestream", {}, {"B200_ONE_STREAM": "1"}), ("block1", {}, {"B200_SOLVE_BLOCK": "1"}),
+                              ("direct0", {}, {"B200_SOLVE_DIRECT": "0"})):
             key = "%s/%s" % (name, tag)
             with env(**sw):
                 s = handle(dim, irn, jcn, val, **opts)
@@ -156,6 +207,7 @@ def dump(lib, out):
                 factor(s, key + "/again")
                 put(key + "/dinv", s.enquire_indef()[2])
                 host_solves(s, key, dim, rng)
+                pruned_suite(s, key, dim, rng)
                 if tag == "graph":
                     full_suite(s, key, dim, len(irn), rng)
                 s.close()
