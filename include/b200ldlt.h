@@ -291,9 +291,9 @@ int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* 
  * never straddles a front); i and j in different trees of the forest give exactly +0.
  * The columns (the distinct indices of irow and jcol) are sorted by pivot position and swept in blocks of up to
  * B200_SOLVE_BLOCK columns (the blocked state of the solves, allocated as a blocked solve does; B200_SOLVE_BLOCK=1 or
- * a failed allocation: one column per block), each block by job 1's forward sweep pruned to the union of its columns'
- * reaches as in sparse_fwd_solve (the same run sets, work lists and dependency check, which refuses a sweep that could
- * wait forever before anything is launched).
+ * a failed allocation: one column per block), each block by the forward stage of sparse_fwd_solve on its unit columns,
+ * pruned to the union of their reaches (the same run sets, work lists and dependency check, which refuses a sweep that
+ * could wait forever before anything is launched).
  * Summation order, pinned (every operation rounded on its own, no FMA): with a = y_i and b = y_j on the suffix, the TERM
  * at suffix offset o is d (a_o b_o) for a 1x1 pivot (d = D^-1 there), (d1 (a_o b_o) + d2 (a_o+1 b_o+1)) + e ((a_o b_o+1)
  * + (a_o+1 b_o)) for a 2x2 pivot opening at o (d1, d2 its diagonal and e its off-diagonal entry of D^-1), none at the
@@ -305,8 +305,9 @@ int b200ldlt_selected_inverse_device(b200ldlt_handle h, double* d_diag, double* 
  * Kernel launches: sum over blocks b of (1 + d_b + t_b + 1), plus 1, with d_b and t_b counted as for sparse_fwd_solve on
  * the block's columns.  Memory: as stated at b200ldlt_sparse_fwd_solve for the three calls that prune sweeps; here a
  * call needs 12 bytes per element of the y store (sum over the columns of the pivots on their paths to the root), 24
- * bytes per entry and per block its pruned lists, in the shared staging and a device y store that grows to the largest
- * call and is freed by the next analysis.  symbolic_array "inverse_run_set" returns the union
+ * bytes per entry, 8 w^2 bytes for the identity of the block width w, and per block its pruned lists and 8 bytes per
+ * position of its run set, in the shared staging and a device y store that grows to the largest call and is freed by
+ * the next analysis.  symbolic_array "inverse_run_set" returns the union
  * of the run sets the last call swept.  The call leaves the factors, D, every later solve and "sparse_run_set" as they
  * were.  Refused (nothing written): nent < 0, a NULL pointer with nent > 0, an index out of range, and (FATAL_ERROR with
  * a message) a failed allocation of the staging or the y store.  nent = 0 is the no-columns case.

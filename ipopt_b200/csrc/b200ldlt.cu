@@ -347,7 +347,6 @@ struct Solver {
   int tc_min_r = 0;                // fronts with r >= this use the tensor-core Schur path (0 = off)
   bool reanalyse = false;          // set by increase_quality after forced pivots: next factor re-runs the analysis on its values
   int n_reanalysed = 0;
-  long long n_factor = 0;
   bool reanalysed_since_raise = false;
   std::unique_ptr<Analysis> an;    // null: not analysed (none yet, a new pattern, or the last analysis failed)
   b200ldlt_info info;
@@ -1318,32 +1317,32 @@ __global__ void k_zero_pivots(int nz, const int* __restrict__ zpos, double* __re
   if (i < nz) { dinv[zpos[i]] = 0.0; zflag[zpos[i]] = 1; }
 }
 
-static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* num_neg) {
+// The outcome of a factorisation whose stream has drained (ev1 recorded after its last launch), from its counters (CNT_N
+// ints; on a sharded handle summed over the ranks): timing, launches and counts into info, the factors offered to the
+// solves or not, keep mode's D^+, the inertia and the return code.
+static int settle_factor(Solver* sv, const int* counters, int check_inertia, int expected_neg, int* num_neg) {
   Analysis& A = *sv->an;
   cudaStream_t st = sv->stream;
-  CU(cudaEventRecord(sv->ev1, st));
-  CU(cudaMemcpyAsync(sv->h_counters, A.d_counters.p, CNT_N * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
   float ms = 0;
   cudaEventElapsedTime(&ms, sv->ev0, sv->ev1);
   b200ldlt_info& I = sv->info;
   I.ms_factor_gpu = ms;
   I.launches_factor = sv->launches;
-  ++sv->n_factor;
-  I.num_neg = sv->h_counters[CNT_NEG];
-  I.num_forced = sv->h_counters[CNT_FORCED];
-  I.num_tiny = sv->h_counters[CNT_TINY];
-  I.num_growth = sv->h_counters[CNT_GROWTH];
-  I.num_2x2 = sv->h_counters[CNT_2X2];
+  I.num_neg = counters[CNT_NEG];
+  I.num_forced = counters[CNT_FORCED];
+  I.num_tiny = counters[CNT_TINY];
+  I.num_growth = counters[CNT_GROWTH];
+  I.num_2x2 = counters[CNT_2X2];
   // Factors of a matrix with a noise pivot (SINGULAR) are not offered to the solves, unless keep mode is on and every such
   // pivot is a zero pivot (its whole column noise): D_pp = 0 then describes the matrix, so dinv[p] is set to 0 (D^+) and
   // the pivot leaves the inertia.  A lifted zero (|pivot| <= tiny under a column that is not noise) never keeps factors.
   // With num_forced > 0 the factors (and the inertia reported) are those of a matrix perturbed by <= 1e-8 |column| in the
   // lifted pivots; the count is surfaced in b200ldlt_info and drives increase_quality (re-analysis with the current values).
+  // A sharded handle reads no zero list: its own holds only this rank's entries, while CNT_ZLIST counts all ranks'.
   A.factored = (I.num_tiny == 0);
   A.zpos.clear();
-  if (I.num_tiny > 0) {
-    const int nz = std::min(sv->h_counters[CNT_ZLIST], sv->n);
+  if (I.num_tiny > 0 && !A.shard.active) {
+    const int nz = std::min(counters[CNT_ZLIST], sv->n);
     std::vector<int> zl(nz);
     CU(cudaMemcpy(zl.data(), A.d_zlist.p, nz * sizeof(int), cudaMemcpyDeviceToHost));
     std::sort(zl.begin(), zl.end());
@@ -1359,7 +1358,7 @@ static int finish_factor(Solver* sv, int check_inertia, int expected_neg, int* n
       const bool keep = sv->keep_singular && sv->sc_vars.empty();   // (Schur mode keeps no singular factors)
       sv->err = "factor: SINGULAR: " + std::to_string(nz) + " zero pivot(s)" +
                 (keep ? "; factors kept with D^+ (zero pivots left out of the inertia)" : "; no factors kept");
-      if (keep && !A.shard.active && nz == I.num_tiny) {
+      if (keep && nz == I.num_tiny) {
         for (int e : zl) A.zpos.push_back(e >> 2);
         CU(A.d_zpos.upload(A.zpos, st));
         CU(cudaMemsetAsync(A.d_zflag.p, 0, sv->n, st));
@@ -1429,7 +1428,10 @@ static int do_factor(Solver* sv, const double* d_vals_ext, bool from_host, int c
     rc = enqueue_factor(sv, A.fronts, true);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
-  return finish_factor(sv, check_inertia, expected_neg, num_neg);
+  CU(cudaEventRecord(sv->ev1, st));
+  CU(cudaMemcpyAsync(sv->h_counters, A.d_counters.p, CNT_N * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return settle_factor(sv, sv->h_counters, check_inertia, expected_neg, num_neg);
 }
 
 __global__ void k_mark_flags(int* flags, const int* __restrict__ list, int n, int value) {
@@ -2039,8 +2041,10 @@ static void stage_positions(PrunedPlan& P, const Symbolic& S, const std::vector<
 }
 
 // The forward stage of w compact columns (column c of b at b + c nbi) over the staged F: k_sps_in (x = P^T S b on R_f,
-// the frontier's update vectors and flags) and the forward sweep over the pruned lists, D^-1 applied or not.  Launches:
-// 1 + the direct levels that hold a front of R_f + 1 when R_f has a front outside them.
+// the frontier's update vectors and flags) and the forward sweep over the pruned lists, D^-1 applied or not.  The one
+// forward stage of the three pruned calls: the sparse forward solve (one column), the sparse solve, and the entries of
+// A^-1 (unit columns: b is an identity).  Launches: 1 + the direct levels that hold a front of R_f + 1 when R_f has a
+// front outside them.
 static int sparse_forward(Solver* sv, SweepState& W, const SparseFwd& F, const double* b, int nbi, int w, bool apply_d) {
   Analysis& A = *sv->an;
   const char* d = A.pruned->stg.d.p;
@@ -2114,27 +2118,28 @@ static int sfs_enqueue(Solver* sv, const SfsCall& C, const double* d_b, double* 
 }
 
 // ---- entries of A^-1 (b200ldlt_inverse_entries) ---------------------------------------------------------------------
-// one block of unit columns: columns [c0, c0 + w) of the call, its run set's ncol positions and frontier of nfr fronts,
-// the longest reach of its columns, staging offsets (bytes) and the pruned lists on the device
+// one block of unit columns: columns [c0, c0 + w) of the call, the longest reach of its columns, and the forward stage
+// of its unit columns
 struct InvBlock {
-  int c0 = 0, w = 0, ncol = 0, nfr = 0, maxlen = 0;
-  size_t o_lst = 0, o_pos = 0, o_col = 0, o_fr = 0;
-  PrunedLists pl{};
+  int c0 = 0, w = 0, maxlen = 0;
+  SparseFwd F;
 };
-// one call as prepared on the host: the entry list, the y store's offsets (ncols + 1) and positions, the blocks
+// one call as prepared on the host: the entry list, the y store's offsets (ncols + 1) and positions, the identity of
+// order neye (the compact b of every block: column c of a block is column c of the identity), the blocks
 struct InvCall {
-  int nent = 0, ncols = 0;
-  size_t o_ent = 0, o_yoff = 0, o_ypos = 0, staged = 0;
+  int nent = 0, ncols = 0, neye = 0;
+  size_t o_ent = 0, o_yoff = 0, o_ypos = 0, o_eye = 0, staged = 0;
   std::vector<InvBlock> blk;
 };
 
 // Host part of b200ldlt_inverse_entries.  The columns are the distinct variables of irow and jcol, sorted by pivot
 // position (neighbours in the tree share fronts) and cut into blocks of `width`; each block is one pruned forward sweep
-// (prune, its dependency check included) of its unit columns.  Column c keeps y_c = L^-1 P^T S e_c on its reach, the
-// path from its front to the root (ascending positions), at [yoff[c], yoff[c + 1]) of the y store.  Entry (i, j) reads
-// the common suffix of y_i and y_j: the path from the lowest common ancestor of their fronts to the root, pathlen of that
-// front long (0 in different trees of the forest).  Everything the device needs goes to the list staging, each block in
-// a region of its own, so one copy carries the call.  FATAL_ERROR with a message, nothing written and nothing launched,
+// (prune, its dependency check included) of its unit columns, staged for sparse_forward with a compact b whose seeds are
+// the pivot positions of its columns and whose column c is column c of the staged identity.  Column c keeps
+// y_c = L^-1 P^T S e_c on its reach, the path from its front to the root (ascending positions), at [yoff[c], yoff[c + 1])
+// of the y store.  Entry (i, j) reads the common suffix of y_i and y_j: the path from the lowest common ancestor of
+// their fronts to the root, pathlen of that front long (0 in different trees of the forest).  Everything the device
+// needs goes to the list staging, each block in a region of its own, so one copy carries the call.  FATAL_ERROR with a message, nothing written and nothing launched,
 // for a failed check or allocation.
 static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, int width, InvCall& C) {
   Analysis& A = *sv->an;
@@ -2152,14 +2157,16 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
   std::vector<long long> yoff(nc + 1, 0);
   for (int c = 0; c < nc; ++c) yoff[c + 1] = yoff[c] + P.pathlen[P.sn_of[P.iperm[cols[c]]]];
   const long long ny = yoff[nc];
-  // the blocks, and the staging layout: entries, yoff, ypos, then per block its pruned lists, run-set positions and
-  // column positions
-  C.nent = nent; C.ncols = nc;
+  // the blocks, and the staging layout: entries, yoff, ypos, the identity, then per block its pruned lists, run-set
+  // positions and their indices into the block's columns
+  C.nent = nent; C.ncols = nc; C.neye = std::min(width, nc);
   C.o_ent = 0;
   C.o_yoff = align8(sizeof(InvEnt) * (size_t)nent);
   C.o_ypos = C.o_yoff + 8 * (size_t)(nc + 1);
-  size_t o = align8(C.o_ypos + 4 * (size_t)ny);
+  C.o_eye = align8(C.o_ypos + 4 * (size_t)ny);
+  size_t o = C.o_eye + 8 * (size_t)C.neye * C.neye;
   std::vector<PrunedSweep> R((nc + width - 1) / width);
+  std::vector<size_t> o_lst(R.size());
   std::vector<int> seed(width), run_all;
   C.blk.assign(R.size(), InvBlock());
   for (size_t b = 0; b < R.size(); ++b) {
@@ -2171,13 +2178,13 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
     }
     const int rc = prune(sv, "inverse_entries", 0, seed.data(), B.w, R[b]);
     if (rc != B200LDLT_SUCCESS) return finish(rc);
-    B.ncol = npos(S, R[b].run);
-    B.nfr = (int)R[b].fr.size();
+    B.F.ncol = npos(S, R[b].run);
+    B.F.nfr = (int)R[b].fr.size();
     run_all.insert(run_all.end(), R[b].run.begin(), R[b].run.end());
-    B.o_lst = o;
-    B.o_pos = o + pruned_bytes(R[b]);
-    B.o_col = B.o_pos + 4 * (size_t)B.ncol;
-    o = align8(B.o_col + 4 * (size_t)B.w);
+    o_lst[b] = o;
+    B.F.o_pos = o + pruned_bytes(R[b]);
+    B.F.o_bi = B.F.o_pos + 4 * (size_t)B.F.ncol;
+    o = align8(B.F.o_bi + 4 * (size_t)B.F.ncol);
   }
   C.staged = o;
   { const int rc = P.stg.reserve(sv, "inverse_entries", C.staged); if (rc != B200LDLT_SUCCESS) return finish(rc); }
@@ -2202,13 +2209,15 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
   for (int c = 0; c < nc; ++c)
     for (int s = P.sn_of[P.iperm[cols[c]]]; s >= 0; s = S.sn_parent[s])
       for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *yp++ = p;
+  double* eye = reinterpret_cast<double*>(h + C.o_eye);
+  std::fill(eye, eye + (size_t)C.neye * C.neye, 0.0);
+  for (int c = 0; c < C.neye; ++c) eye[(size_t)c * C.neye + c] = 1.0;
   for (size_t b = 0; b < R.size(); ++b) {
     InvBlock& B = C.blk[b];
-    stage_pruned(SP, SP.tf, R[b], h, P.stg.d.p, B.o_lst, B.pl, &B.o_fr);
-    int* pos = reinterpret_cast<int*>(h + B.o_pos);
-    for (int s : R[b].run) for (int p = S.sn_start[s]; p < S.sn_start[s + 1]; ++p) *pos++ = p;
-    int* cp = reinterpret_cast<int*>(h + B.o_col);
-    for (int c = 0; c < B.w; ++c) cp[c] = P.iperm[cols[B.c0 + c]];
+    stage_pruned(SP, SP.tf, R[b], h, P.stg.d.p, o_lst[b], B.F.pl, &B.F.o_fr);
+    for (int c = 0; c < B.w; ++c) seed[c] = P.iperm[cols[B.c0 + c]];
+    stage_positions(P, S, R[b].run, seed.data(), B.w, reinterpret_cast<int*>(h + B.F.o_pos),
+                    reinterpret_cast<int*>(h + B.F.o_bi));
   }
   std::sort(run_all.begin(), run_all.end());
   run_all.erase(std::unique(run_all.begin(), run_all.end()), run_all.end());
@@ -2216,7 +2225,7 @@ static int inv_prepare(Solver* sv, int nent, const int* irow, const int* jcol, i
   return finish(B200LDLT_SUCCESS);
 }
 
-// Device part: the staging in, then per block k_inv_in, the forward sweep of job 1 over its pruned lists (block width
+// Device part: the staging in, then per block the forward stage of job 1 (sparse_forward, D^-1 left out; block width
 // w: the blocked state, one column: the single-column state) and k_inv_out into the y store; then k_inv_dot to out.
 // Launches: sum over blocks of (2 + the direct levels that hold a front of the block's run set + 1 when the run set has
 // a front outside them), + 1.
@@ -2227,16 +2236,11 @@ static int inv_enqueue(Solver* sv, const InvCall& C, double* out) {
   const char* d = P.stg.d.p;
   const long long* yoff = reinterpret_cast<const long long*>(d + C.o_yoff);
   const int* ypos = reinterpret_cast<const int*>(d + C.o_ypos);
+  const double* eye = reinterpret_cast<const double*>(d + C.o_eye);
   { const int rc = P.stg.upload(sv, C.staged); if (rc != B200LDLT_SUCCESS) return rc; }
   for (const InvBlock& B : C.blk) {
     SweepState& W = B.w == 1 ? A.sweep : *A.blk;
-    A.solve_epoch++;
-    k_inv_in<<<dim3(cdiv(B.ncol, 256) + B.nfr, B.w), 256, 0, st>>>(
-        B.ncol, reinterpret_cast<const int*>(d + B.o_pos), reinterpret_cast<const int*>(d + B.o_col), A.d_perm.p,
-        A.d_scale.p, W.d_x.p, W.M.x, reinterpret_cast<const int*>(d + B.o_fr), A.d_rows_ptr.p, W.d_cbv.p, W.M.cbv,
-        W.d_done_f.p, W.M.nsn, A.solve_epoch);
-    ++sv->launches;
-    const int rc = launch_sweep(sv, A.fronts.solve, W, B.w, true, false, &B.pl);
+    const int rc = sparse_forward(sv, W, B.F, eye, C.neye, B.w, false);
     if (rc != B200LDLT_SUCCESS) return rc;
     k_inv_out<<<dim3(cdiv(B.maxlen, 256), B.w), 256, 0, st>>>(B.c0, yoff, ypos, A.d_piv_big.p, W.d_x.p, W.M.x,
                                                               W.d_bigv.p, W.M.bigv, P.d_y.p);
@@ -2377,20 +2381,18 @@ static int shard_setup(Solver* sv, int rank, int world) {
   H.cut_roots.clear(); H.top_fronts.clear();
   std::vector<char> take[2];
   take[0].assign(S.nsn, 0); take[1].assign(S.nsn, 0);
-  std::vector<int> mark_cut;
   for (int s = 0; s < S.nsn; ++s) {
     if (H.owner[s] < 0) { take[1][s] = (rank == 0); H.top_fronts.push_back(s); }
     else {
       take[0][s] = (H.owner[s] == rank);
       const int p = S.sn_parent[s];
-      if (p >= 0 && H.owner[p] < 0) { H.cut_roots.push_back(s); if (H.owner[s] != 0) mark_cut.push_back(s); }
+      if (p >= 0 && H.owner[p] < 0) H.cut_roots.push_back(s);
     }
   }
   for (int ph = 0; ph < 2; ++ph) {
     const int rc = build_front_plan(sv, A, take[ph], take[ph], H.part[ph]);
     if (rc != B200LDLT_SUCCESS) return rc;
   }
-  if (mark_cut.empty()) mark_cut.push_back(0), H.d_mark_cut.n = 0;
   {
     std::vector<int> mc;
     for (int s : H.cut_roots) if (H.owner[s] != 0) mc.push_back(s);
@@ -2578,12 +2580,13 @@ static int timed_call(Solver* sv, Enqueue&& enqueue, Drain&& drain = Drain()) {
 // chunks, so that the DMA of one chunk runs under the host copy of the next (the caller's array is pageable: Ipopt
 // allocates it per call, IpTSymLinearSolver.cpp:222-241).  The staging grows to the largest call and lasts until the
 // next analysis.  nwork: the staging holds at least that many doubles (device scratch of enqueue beyond in and out).
-// in_off: `in` is staged at that many doubles from the start (out always at the start).
+// in_off: `in` is staged at that many doubles from the start (out always at the start).  in2: a second input of nin2
+// doubles, staged directly after `in` in the same chunks.
 template <class Enqueue>
 static int staged_call(Solver* sv, const double* in, size_t nin, double* out, size_t nout, Enqueue&& enqueue,
-                       size_t nwork = 0, size_t in_off = 0) {
+                       size_t nwork = 0, size_t in_off = 0, const double* in2 = nullptr, size_t nin2 = 0) {
   Analysis& A = *sv->an;
-  const size_t need = std::max(std::max(in_off + nin, nout), nwork);
+  const size_t nall = nin + nin2, need = std::max(std::max(in_off + nall, nout), nwork);
   if (need > A.d_rhs.n) {
     A.d_rhs.release();
     if (A.h_rhs) cudaFreeHost(A.h_rhs);
@@ -2595,7 +2598,7 @@ static int staged_call(Solver* sv, const double* in, size_t nin, double* out, si
   double* h = A.h_rhs;
   double* d = A.d_rhs.p;
   auto chunk = [](size_t total) { return std::max<size_t>((total + 3) / 4, 32768); };   // at most 4: ev_chunk
-  const size_t ci = chunk(nin), co = chunk(nout);
+  const size_t ci = chunk(nall), co = chunk(nout);
   auto copy_out = [&]() -> int {
     for (size_t o = 0, k = 0; o < nout; o += co, ++k) {
       CU(cudaEventSynchronize(sv->ev_chunk[k]));
@@ -2604,9 +2607,13 @@ static int staged_call(Solver* sv, const double* in, size_t nin, double* out, si
     return B200LDLT_SUCCESS;
   };
   return timed_call(sv, [&]() -> int {
-    for (size_t o = 0; o < nin; o += ci) {
-      const size_t m = std::min(ci, nin - o);
-      memcpy(h + in_off + o, in + o, m * sizeof(double));
+    for (size_t o = 0; o < nall; o += ci) {
+      const size_t m = std::min(ci, nall - o);
+      for (size_t e = o; e < o + m;) {   // (a chunk may end in `in` and go on in in2)
+        const size_t k = std::min(o + m, e < nin ? nin : nall) - e;
+        memcpy(h + in_off + e, e < nin ? in + e : in2 + (e - nin), k * sizeof(double));
+        e += k;
+      }
       CU(cudaMemcpyAsync(d + in_off + o, h + in_off + o, m * sizeof(double), cudaMemcpyHostToDevice, st));
     }
     { const int rc = enqueue(d); if (rc != B200LDLT_SUCCESS) return rc; }
@@ -2812,10 +2819,8 @@ static int schur_solve(Solver* sv, const char* call, int nrhs, const double* b, 
   if (!host) return timed_call(sv, [&] { return enqueue_sc_columns(sv, nrhs, b, expand ? xs : nullptr, out, blocked); });
   if (!expand)   // in place in the staging: y of a block lands below the b of the blocks after it
     return staged_call(sv, b, nb, out, mb, [&](double* d) { return enqueue_sc_columns(sv, nrhs, d, nullptr, d, blocked); });
-  std::vector<double> in(nb + mb);   // b and xs side by side, one staged copy
-  std::copy(b, b + nb, in.begin());
-  std::copy(xs, xs + mb, in.begin() + nb);
-  return staged_call(sv, in.data(), nb + mb, out, nb, [&](double* d) { return enqueue_sc_columns(sv, nrhs, d, d + nb, d, blocked); });
+  return staged_call(sv, b, nb, out, nb, [&](double* d) { return enqueue_sc_columns(sv, nrhs, d, d + nb, d, blocked); },
+                     0, 0, xs, mb);
 }
 
 // ---- selected inversion (b200ldlt_selected_inverse) ----------------------------------------------------------------
@@ -3142,15 +3147,8 @@ static int error_analysis(Solver* sv, int nrhs, const double* b, const double* x
       return B200LDLT_SUCCESS;
     });
   };
-  int rc;
-  if (host) {
-    std::vector<double> in(2 * nb);
-    memcpy(in.data(), b, nb * sizeof(double));
-    memcpy(in.data() + nb, x, nb * sizeof(double));
-    rc = staged_call(sv, in.data(), 2 * nb, nullptr, 0, [&](double* d) { return enqueue(d, d + nb); });
-  } else {
-    rc = timed_call(sv, [&] { return enqueue(b, x); });
-  }
+  const int rc = host ? staged_call(sv, b, nb, nullptr, 0, [&](double* d) { return enqueue(d, d + nb); }, 0, 0, x, nb)
+                      : timed_call(sv, [&] { return enqueue(b, x); });
   if (rc != B200LDLT_SUCCESS) return rc;
   const double inf = INFINITY, anorm = ea_val(nrm[(size_t)EA_NRM * nrhs]);
   for (int c = 0; c < nrhs; ++c) {
@@ -3636,22 +3634,10 @@ int b200ldlt_shard_factor(b200ldlt_handle h, int phase, int from_host) {
 int b200ldlt_shard_factor_finish(b200ldlt_handle h, const int* counters_total, int check_inertia, int expected_neg, int* num_neg) {
   Solver* sv = (Solver*)h;
   if (!sv || !sv->an || !sv->an->shard.active || !counters_total) return B200LDLT_FATAL_ERROR;
-  Analysis& A = *sv->an;
   CU(cudaSetDevice(sv->dev));
   CU(cudaEventRecord(sv->ev1, sv->stream));
   CU(cudaStreamSynchronize(sv->stream));
-  cudaEventElapsedTime(&sv->info.ms_factor_gpu, sv->ev0, sv->ev1);
-  b200ldlt_info& I = sv->info;
-  I.launches_factor = sv->launches;
-  I.num_neg = counters_total[CNT_NEG]; I.num_forced = counters_total[CNT_FORCED]; I.num_tiny = counters_total[CNT_TINY];
-  I.num_growth = counters_total[CNT_GROWTH]; I.num_2x2 = counters_total[CNT_2X2];
-  sv->num_neg = I.num_neg;
-  if (num_neg) *num_neg = I.num_neg;
-  A.factored = (I.num_tiny == 0);
-  A.zpos.clear();
-  if (I.num_tiny > 0) return B200LDLT_SINGULAR;
-  if (check_inertia && I.num_neg != expected_neg) return B200LDLT_WRONG_INERTIA;
-  return B200LDLT_SUCCESS;
+  return settle_factor(sv, counters_total, check_inertia, expected_neg, num_neg);
 }
 
 /* phase 0: permute+scale rhs, forward sweep over my subtrees;  phase 1 (rank 0): forward + backward over the top;

@@ -53,8 +53,8 @@ struct DevNum {
   double tiny;      // zero-pivot threshold (scaled matrix)
 };
 
-// the sparse solve (b200ldlt_sparse_solve, solve_kernels.cu): the input of compact right-hand sides, the stage between
-// the two sweeps and the output at the selected variables
+// the sparse solve (b200ldlt_sparse_solve, solve_kernels.cu): the input of compact right-hand sides (the input of every
+// pruned forward sweep), the stage between the two sweeps and the output at the selected variables
 __global__ void k_sps_in(int ncol, const int* __restrict__ pos, const int* __restrict__ bi, const int* __restrict__ perm,
                          const double* __restrict__ scale, const double* __restrict__ b, int nbi, double* __restrict__ xp,
                          long long ldx, int nfr, const int* __restrict__ fr, const long long* __restrict__ rows_ptr,

@@ -129,30 +129,10 @@ __global__ void k_fred_out(int n, const int* __restrict__ perm, const double* __
   if (i < n) { const int o = perm[i]; x[oc * n + o] = scale[o] * xp[c * ldx + i]; }
 }
 
-// Entries of A^-1 (b200ldlt_inverse_entries): the sparse forward solve of a block of unit columns, column blockIdx.y = c
-// of the sweep state (x: leading dimension ldx, update vectors ldcbv, forward flags ldf).  Blocks [0, cdiv(ncol, 256)):
-// x at the ncol positions of the block's run set, scale (scale * 1.0, the multiply of k_sps_in) at colpos[c], the pivot
-// position of the column's variable, and 0 elsewhere.  Blocks after that: frontier front fr[q], the column's slice of its
-// update vector zeroed and its forward flag set to this sweep's epoch, as in k_sps_in.
-__global__ void k_inv_in(int ncol, const int* __restrict__ pos, const int* __restrict__ colpos, const int* __restrict__ perm,
-                         const double* __restrict__ scale, double* __restrict__ xp, long long ldx, const int* __restrict__ fr,
-                         const long long* __restrict__ rows_ptr, double* __restrict__ cbv, long long ldcbv,
-                         int* __restrict__ done_f, long long ldf, int epoch) {
-  const long long c = blockIdx.y;
-  const int nxb = (ncol + 255) / 256;
-  if ((int)blockIdx.x < nxb) {
-    const int j = blockIdx.x * 256 + threadIdx.x;
-    if (j < ncol) { const int p = pos[j]; xp[c * ldx + p] = p == colpos[c] ? scale[perm[p]] : 0.0; }
-    return;
-  }
-  const int f = fr[blockIdx.x - nxb];
-  const long long r0 = rows_ptr[f], r1 = rows_ptr[f + 1];
-  for (long long e = r0 + threadIdx.x; e < r1; e += blockDim.x) cbv[c * ldcbv + e] = 0.0;
-  if (threadIdx.x == 0) done_f[c * ldf + f] = epoch;
-}
-// The y store: column c0 + blockIdx.y of the call keeps its reach at [yoff[c], yoff[c + 1]), ypos the pivot positions and
-// y the sweep values there (see k_piv_out), read from column blockIdx.y of the sweep state.  Also the output of the
-// sparse forward solve: one column with yoff = {0, nxi}.
+// Entries of A^-1 (b200ldlt_inverse_entries), after the forward stage of a block of unit columns (k_sps_in and the
+// pruned sweep).  The y store: column c0 + blockIdx.y of the call keeps its reach at [yoff[c], yoff[c + 1]), ypos the
+// pivot positions and y the sweep values there (see k_piv_out), read from column blockIdx.y of the sweep state.  Also
+// the output of the sparse forward solve: one column with yoff = {0, nxi}.
 __global__ void k_inv_out(int c0, const long long* __restrict__ yoff, const int* __restrict__ ypos,
                           const long long* __restrict__ piv_big, const double* __restrict__ xp, long long ldx,
                           const double* __restrict__ big, long long ldbig, double* __restrict__ y) {
@@ -206,9 +186,10 @@ __global__ void k_inv_dot(int nent, const InvEnt* __restrict__ ent, const double
 // Sparse solve (b200ldlt_sparse_solve): job 0 of a block of compact right-hand sides with one pattern, swept forward over
 // the run set R_f of the pattern and backward over the run set R_b of the selection.  Column blockIdx.y = c of the sweep
 // state (x: leading dimension ldx, update vectors ldcbv, flags ldf); column c of b at b + c nbi.
-// k_sps_in (also the sparse forward solve's, one column): blocks [0, cdiv(ncol, 256)): x = P^T S b at the ncol
-// positions of R_f, the scaled entry of b where b has one (bi[j] >= 0: its index into the compact column; k_rhs_in's
-// single multiply) and 0 elsewhere.  Blocks after that: frontier front fr[q] (a child of R_f outside R_f), the column's
+// k_sps_in, the input of all three pruned calls (the sparse forward solve: one column; the entries of A^-1: b an
+// identity, whose entries the scaling, a power of two, multiplies exactly): blocks [0, cdiv(ncol, 256)): x = P^T S b at
+// the ncol positions of R_f, the scaled entry of b where b has one (bi[j] >= 0: its index into the compact column;
+// k_rhs_in's single multiply) and 0 elsewhere.  Blocks after that: frontier front fr[q] (a child of R_f outside R_f), the column's
 // slice of its update vector zeroed and its forward flag set to this sweep's epoch, so that its parent neither waits for
 // it nor adds anything from it.
 __global__ void k_sps_in(int ncol, const int* __restrict__ pos, const int* __restrict__ bi, const int* __restrict__ perm,

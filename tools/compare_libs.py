@@ -8,12 +8,13 @@ code): build the other library into a directory of its own, then
 The dump holds the SHA-256 of the bytes of each array (the full arrays run to gigabytes) and the launch counts.
 
 What is dumped, per system (seeded generators and the golden systems of tests/golden):
-  * factor with use_graph 1 (and its replay), use_graph 0, B200_ONE_STREAM=1, B200_SOLVE_BLOCK=1 and
-    B200_SOLVE_DIRECT=0: status, inertia, launches_factor, D^-1 (enquire_indef) and host solves of 1, 8 and 13 columns
-    with launches_solve;
+  * factor with use_graph 1 (and its replay), use_graph 0, B200_ONE_STREAM=1, B200_SOLVE_BLOCK=1, B200_SOLVE_BLOCK=3
+    and B200_SOLVE_DIRECT=0: status, inertia, launches_factor, D^-1 (enquire_indef) and host solves of 1, 8 and 13
+    columns with launches_solve;
   * on the use_graph 1 handle: device solves of 1, 8 and 13 columns, jobs 1..4 (host 1 and 13 columns, device 8),
-    lmultiply (trans 0 / 1, host 1 and 13, device 8), selected inversion, solve_refine_device and the Fredholm solve
-    without zero pivots;
+    lmultiply (trans 0 / 1, host 1 and 13, device 8), selected inversion, solve_refine_device, the Fredholm solve
+    without zero pivots, the error analysis (host 1 and 13 columns with and without the condition estimate, device 8)
+    and the refined solve (host 3 columns, device 1);
   * on every handle of the first item, the calls that run pruned sweeps, host and device, each followed by the four run
     sets of symbolic_array: the sparse forward solve; inverse_entries (a diagonal, an off-diagonal entry in both orders,
     the first and last variable -- different trees on the two-component system --, and a block of 20 x 20 entries,
@@ -186,6 +187,23 @@ def dump(lib, out):
         X, F, c = s.solve_fredholm(rng.standard_normal((dim, 3)), 1e-10)
         put(key + "/fred_nonsingular", X, F, c)
         launches(s, key + "/fred_nonsingular")
+        for w in (1, 13):
+            B, X = rng.standard_normal((dim, w)), rng.standard_normal((dim, w))
+            for cond in (0, 1):
+                e = s.error_analysis(B, X, cond)
+                put("%s/ea%d_cond%d" % (key, w, cond), *(e[k] for k in sorted(e)))
+                launches(s, "%s/ea%d_cond%d" % (key, w, cond))
+        Bd, Xd = dev(rng.standard_normal(dim * 8)), dev(rng.standard_normal(dim * 8))
+        st, e = s.error_analysis_device(Bd.data_ptr(), Xd.data_ptr(), 8)
+        put(key + "/ea_dev8", np.array([st]), *(e[k] for k in sorted(e)))
+        launches(s, key + "/ea_dev8")
+        X, r = s.solve_refined(rng.standard_normal((dim, 3)), 3)
+        put(key + "/refined3", X, *(r[k] for k in sorted(r)))
+        launches(s, key + "/refined3")
+        Bd, Xd = dev(rng.standard_normal(dim)), torch.zeros(dim, dtype=torch.float64, device="cuda")
+        st, r = s.solve_refined_device(Bd.data_ptr(), Xd.data_ptr(), 1, 3)
+        put(key + "/refined_dev1", np.array([st]), Xd.cpu().numpy(), *(r[k] for k in sorted(r)))
+        launches(s, key + "/refined_dev1")
         assert nnz == len(v)
 
     rng = np.random.default_rng(2024)
@@ -197,7 +215,7 @@ def dump(lib, out):
         dim, irn, jcn, val = make()
         for tag, opts, sw in (("graph", {}, {}), ("nograph", {"use_graph": 0}, {}),
                               ("onestream", {}, {"B200_ONE_STREAM": "1"}), ("block1", {}, {"B200_SOLVE_BLOCK": "1"}),
-                              ("direct0", {}, {"B200_SOLVE_DIRECT": "0"})):
+                              ("block3", {}, {"B200_SOLVE_BLOCK": "3"}), ("direct0", {}, {"B200_SOLVE_DIRECT": "0"})):
             key = "%s/%s" % (name, tag)
             with env(**sw):
                 s = handle(dim, irn, jcn, val, **opts)
