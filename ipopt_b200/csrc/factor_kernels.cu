@@ -18,8 +18,42 @@
 
 namespace b200 {
 
-#define BK_ALPHA 0.6403882032022076  // (1+sqrt(17))/8
 #define NB 32                        // panel width of the big-front path
+
+// The pivot rule of every dense-front LDL^T (factor_front_smem, warp_ldlt32, cta_ldlt32s): Bunch-Kaufman 1x1 / 2x2 pivots
+// among the candidate columns, each also held to the threshold u * max|column| over the whole front column.  The routines
+// search and reduce; these tests decide.  Column j: ajj = |a_jj|, lam = max |a_ij| over the other candidates (at row r),
+// gam = over the other rows; column r: arr = |a_rr|, sig / gamr likewise (without a_jr); cj / cr = max of columns j / r
+// outside rows j and r.  Macros, so that each routine compiles to exactly the expressions written here: operand order and
+// association are part of the factors' bits (fused multiply-adds follow the shape of each expression), and inline
+// functions changed the register allocation and schedule of the pivot loops.
+#define BK_ALPHA 0.6403882032022076  // (1+sqrt(17))/8
+#define PIV_NOISE 1e-12              // a forced column with |a_jj| and maximum <= this (scaled) is rounding noise
+#define PIV_LIFT 1e-8                // a forced pivot is lifted to PIV_LIFT * its column maximum
+#define PIV_ZERO 1.5e-8              // replaces a zero pivot, with its sign
+#define PIV_OK1(ajj, lam, gam, u, tiny) ((ajj) > (tiny) && (ajj) >= (u) * fmax(lam, gam))
+#define PIV_1X1_J(ok1, ajj, lam) ((ok1) && (ajj) >= BK_ALPHA * (lam))
+#define PIV_1X1_J_SIG(ok1, ajj, lam, sig) ((ok1) && (ajj) * (sig) >= BK_ALPHA * (lam) * (lam))
+#define PIV_1X1_R(arr, sig, gamr, u, tiny) ((arr) > (tiny) && (arr) >= BK_ALPHA * (sig) && (arr) >= (u) * fmax(sig, gamr))
+// 2x2 block [a b; b c]: adet = |ac - b^2|, aa = |a|, ab = |b|, ac = |c|
+#define PIV_2X2(lam, adet, aa, ab, ac, cj, cr, u, tiny)                                                                  \
+  ((lam) > (tiny) && (adet) > 0.0 && isfinite(adet) && ((ac) * (cj) + (ab) * (cr)) * (u) <= (adet) &&                  \
+   ((aa) * (cr) + (ab) * (cj)) * (u) <= (adet))
+// Forced pivots, once every remaining candidate failed (cmax = max(|a_jj|, column maximum)).  A zero pivot d (noise column,
+// |d| <= tiny, NaN) becomes +-PIV_ZERO (num_tiny, SINGULAR); any other is lifted to the threshold (static pivoting,
+// num_forced: |l_ij| <= 1e8, the factors of A perturbed by <= PIV_LIFT |column|, which iterative refinement absorbs).
+#define PIV_IS_NOISE(cmax) (!((cmax) > PIV_NOISE))
+#define PIV_IS_ZERO(d, noise, tiny) ((noise) || !(fabs(d) > (tiny)))
+#define PIV_ZEROED(d) (((d) < 0.0) ? -PIV_ZERO : PIV_ZERO)
+#define PIV_LIFTED(d, colmax) copysign(fmax(fabs(d), PIV_LIFT * (colmax)), d)
+// negative eigenvalues of the 2x2 pivot [a b; b c] with determinant det, added to c_neg
+#define PIV_COUNT_NEG2X2(c_neg, det, a) do { if ((det) < 0.0) (c_neg) += 1; else if ((a) < 0.0) (c_neg) += 2; } while (0)
+#define PIV_FLUSH(counters, c_neg, c_forced, c_tiny, c_2x2) do {                                                        \
+    if (c_neg) atomicAdd((counters) + CNT_NEG, c_neg);                                                                  \
+    if (c_forced) atomicAdd((counters) + CNT_FORCED, c_forced);                                                         \
+    if (c_tiny) atomicAdd((counters) + CNT_TINY, c_tiny);                                                               \
+    if (c_2x2) atomicAdd((counters) + CNT_2X2, c_2x2);                                                                  \
+  } while (0)
 
 // --------------------------------------------------------------------------------------------
 // small utility kernels
@@ -74,7 +108,7 @@ __global__ void k_fill(int n, double* x, double v) {
 }
 
 // --------------------------------------------------------------------------------------------
-// pivoted LDL^T of a dense symmetric front held in shared memory (full square storage).
+// pivoted LDL^T of a dense symmetric front held in shared memory (full square storage); pivot rule: the PIV_* tests.
 //   F   : f x f, leading dimension ld, LOWER triangle valid on entry (the strictly upper part is never read)
 //   k   : number of fully-summed (pivot) columns, candidates are rows/cols [0,k)
 //   lp  : k ints, out: pivot position t holds original local column lp[t]
@@ -85,14 +119,6 @@ __global__ void k_fill(int n, double* x, double v) {
 // off-diagonal of D and must be written out as 0) and F[k:, k:] holds the Schur complement.
 // All threads of the CTA must call this; blockDim.x is a multiple of 32.
 // --------------------------------------------------------------------------------------------
-__device__ __forceinline__ void warp_argmax(double& v, int& idx) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    double ov = __shfl_xor_sync(0xffffffffu, v, o);
-    int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-    if (ov > v || (ov == v && oi >= 0 && (idx < 0 || oi < idx))) { v = ov; idx = oi; }
-  }
-}
 __device__ __forceinline__ double warp_max(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
@@ -148,14 +174,12 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
     // ---------------- pivot decision by warp 0 ----------------
     if (warp == 0) {
       int type = 0, r = -1;
-      if (forced) {
-        // every remaining candidate failed the threshold test: force 1x1 pivots.  If the whole remaining
-        // column is rounding noise (scaled matrix, entries O(1)) the matrix is numerically singular.
+      if (forced) {   // noise is tested on the float-rounded maximum of column j, rows >= j
         double cm = 0.0;
         for (int i = j + lane; i < f; i += 32) cm = fmax(cm, fabs(F[i + j * ld]));
         cm = (double)wredux_max(__double2float_ru(cm));
         type = 1; r = j;
-        if (lane == 0) sh[4 * par + 2] = !(cm > 1e-12);
+        if (lane == 0) sh[4 * par + 2] = PIV_IS_NOISE(cm);
       } else {
         double lam = 0.0, gam = 0.0;
         int ridx = -1;
@@ -177,9 +201,9 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
           } else { lam = 0.0; ridx = -1; }
         }
         double ajj = fabs(F[j + j * ld]);
-        bool ok1 = (ajj > tiny) && (ajj >= u * fmax(lam, gam));
+        bool ok1 = PIV_OK1(ajj, lam, gam, u, tiny);
         if (lam == 0.0 || ridx < 0) { if (ok1) { type = 1; r = j; } }
-        else if (ok1 && ajj >= BK_ALPHA * lam) { type = 1; r = j; }
+        else if (PIV_1X1_J(ok1, ajj, lam)) { type = 1; r = j; }
         else {
           r = ridx;
           double sig = 0.0, gamr = 0.0, cj = 0.0, cr = 0.0;
@@ -192,14 +216,12 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
           sig = (double)wredux_max(__double2float_ru(sig)); gamr = (double)wredux_max(__double2float_ru(gamr));
           cj = (double)wredux_max(__double2float_ru(cj)); cr = (double)wredux_max(__double2float_ru(cr));
           double arr = fabs(F[r + r * ld]);
-          if (ok1 && ajj * sig >= BK_ALPHA * lam * lam) { type = 1; r = j; }
-          else if (arr > tiny && arr >= BK_ALPHA * sig && arr >= u * fmax(sig, gamr)) { type = 2; }
+          if (PIV_1X1_J_SIG(ok1, ajj, lam, sig)) { type = 1; r = j; }
+          else if (PIV_1X1_R(arr, sig, gamr, u, tiny)) { type = 2; }
           else {
             double a = F[j + j * ld], b = F[r + j * ld], c = F[r + r * ld];
             double det = a * c - b * b, adet = fabs(det);
-            if (lam > tiny && adet > 0.0 && isfinite(adet) &&
-                (fabs(c) * cj + fabs(b) * cr) * u <= adet && (fabs(a) * cr + fabs(b) * cj) * u <= adet)
-              type = 3;
+            if (PIV_2X2(lam, adet, fabs(a), fabs(b), fabs(c), cj, cr, u, tiny)) type = 3;
           }
         }
       }
@@ -228,14 +250,13 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
       // ---------------- 1x1 pivot at j ----------------
       double d = F[j + j * ld];
       if (forced) {
-        if (noise || !(fabs(d) > tiny)) {  // zero (or NaN) pivot: static perturbation, reported as SINGULAR
-          d = (d < 0.0) ? -1.5e-8 : 1.5e-8;
+        if (PIV_IS_ZERO(d, noise, tiny)) {
+          d = PIV_ZEROED(d);
           if (tid == 0) { ++c_tiny; zl_put(counters, zlist, pos0 + j, noise, d < 0.0); }
-        } else {
-          // static pivoting: lift the pivot to the threshold (see warp_ldlt32); cv2[j] holds max|column j|
+        } else {   // lifted against the exact maximum of column j below the diagonal
           double offmax = 0.0;
           for (int i = j + 1; i < f; ++i) offmax = fmax(offmax, fabs(F[i + j * ld]));
-          d = copysign(fmax(fabs(d), 1e-8 * offmax), d);
+          d = PIV_LIFTED(d, offmax);
           if (tid == 0) ++c_forced;
         }
       }
@@ -279,7 +300,7 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
         dinv[j] = da; dinv[j + 1] = db; doff[j] = dof; doff[j + 1] = 0.0;
         cv1[j] = da; cv1[j + 1] = db; cv2[j] = dof; cv2[j + 1] = 0.0;
         ++c_2x2;
-        if (det < 0.0) c_neg += 1; else if (a < 0.0) c_neg += 2;
+        PIV_COUNT_NEG2X2(c_neg, det, a);
       }
       // columns j, j+1 stay unscaled (see the 1x1 case): l = [c1 c2] D^-1 is formed on the fly
       const double* __restrict__ cj = F + j * ld;
@@ -338,12 +359,7 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
       }
     }
   }
-  if (tid == 0) {
-    if (c_neg) atomicAdd(counters + CNT_NEG, c_neg);
-    if (c_forced) atomicAdd(counters + CNT_FORCED, c_forced);
-    if (c_tiny) atomicAdd(counters + CNT_TINY, c_tiny);
-    if (c_2x2) atomicAdd(counters + CNT_2X2, c_2x2);
-  }
+  if (tid == 0) PIV_FLUSH(counters, c_neg, c_forced, c_tiny, c_2x2);
   __syncthreads();
 }
 
@@ -354,20 +370,10 @@ __device__ void factor_front_smem(double* F, int ld, int f, int k, int* lp, int*
 //   across lanes) so every register index is a compile-time constant: the pivot column is always a[0], a 2x2
 //   partner is first swapped to a[1], and after an elimination all columns shift left.
 //   Rows never move: the pivot row is reached with warp shuffles (F[g][c] = F[c][g] = lane cid[c]'s a[0]).
-// Same pivot rule as factor_front_smem (Bunch-Kaufman inside the candidates [0,k), threshold u against the
-// whole column, failed columns retried after the others, forced + flagged at the very end).
+// Pivot rule: the PIV_* tests; failed columns are retried after the others, forced + flagged at the very end.
 // Output: Lraw[i*33 + t] = L entry of original row i in pivot column t; order[t] = original index of pivot t;
 //         pt/dinv_s/doff_s per pivot; on exit a[c], c < f-k, holds the Schur complement column k+c for row i.
 // --------------------------------------------------------------------------------------------
-__device__ __forceinline__ void wred_max_idx(double& v, int& idx) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    double ov = __shfl_xor_sync(0xffffffffu, v, o);
-    int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-    if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
-  }
-}
-
 // Zero pivots of the register pivoting routines (warp_ldlt32, cta_ldlt32s).  Their pivot loops run at the edge of the
 // register file, so the forced branch only sets bit t (pivot t is a zero pivot) or bit 32 + t (a lifted zero) of a mask,
 // and the entries are appended after the loop.  cta_ldlt32s keeps the mask in place of its count c_tiny and appends the
@@ -432,13 +438,13 @@ __device__ void warp_ldlt32(double (&a)[32], double (&b)[32], const int f, const
     else lam = __shfl_sync(0xffffffffu, v0, r);                       // exact magnitude of the selected entry
     const double gam = fmax((double)gamf, __shfl_sync(0xffffffffu, gext, g0));
     const double ajj = fabs(__shfl_sync(0xffffffffu, a[0], g0));
-    const bool ok1 = (ajj > tiny) && (ajj >= u * fmax(lam, gam));
+    const bool ok1 = PIV_OK1(ajj, lam, gam, u, tiny);
     int type = 0;
     bool noise = false;
     const double colmax_f = fmax(lam, gam);
-    if (forced) { type = 1; noise = !(fmax(ajj, colmax_f) > 1e-12); }
+    if (forced) { type = 1; noise = PIV_IS_NOISE(fmax(ajj, colmax_f)); }
     else if (lam == 0.0 || r < 0) { if (ok1) type = 1; }
-    else if (ok1 && ajj >= BK_ALPHA * lam) type = 1;
+    else if (PIV_1X1_J(ok1, ajj, lam)) type = 1;
     else {
       // bring column r to position 1
       const int p = __shfl_sync(0xffffffffu, mypos, r);
@@ -470,8 +476,8 @@ __device__ void warp_ldlt32(double (&a)[32], double (&b)[32], const int f, const
       }
       const double crr = __shfl_sync(0xffffffffu, a[1], r);
       const double arr = fabs(crr);
-      if (ok1 && ajj * sig >= BK_ALPHA * lam * lam) type = 1;
-      else if (arr > tiny && arr >= BK_ALPHA * sig && arr >= u * fmax(sig, gamr)) {
+      if (PIV_1X1_J_SIG(ok1, ajj, lam, sig)) type = 1;
+      else if (PIV_1X1_R(arr, sig, gamr, u, tiny)) {
         // 1x1 on r: swap positions 0 and 1
         double x = a[0]; a[0] = a[1]; a[1] = x;
         if (TWO) { double y = b[0]; b[0] = b[1]; b[1] = y; }
@@ -481,9 +487,7 @@ __device__ void warp_ldlt32(double (&a)[32], double (&b)[32], const int f, const
       } else {
         const double pa = __shfl_sync(0xffffffffu, a[0], g0), pb = __shfl_sync(0xffffffffu, a[0], r);
         const double det = pa * crr - pb * pb, adet = fabs(det);
-        if (lam > tiny && adet > 0.0 && isfinite(adet) &&
-            (fabs(crr) * cj + fabs(pb) * cr) * u <= adet && (fabs(pa) * cr + fabs(pb) * cj) * u <= adet)
-          type = 3;
+        if (PIV_2X2(lam, adet, fabs(pa), fabs(pb), fabs(crr), cj, cr, u, tiny)) type = 3;
       }
     }
     if (type == 0) {
@@ -511,17 +515,11 @@ __device__ void warp_ldlt32(double (&a)[32], double (&b)[32], const int f, const
     if (type == 1) {
       double dd = __shfl_sync(0xffffffffu, a[0], g0);
       if (forced) {
-        if (noise || !(fabs(dd) > tiny)) {
-          dd = (dd < 0.0) ? -1.5e-8 : 1.5e-8; ++c_tiny;
+        if (PIV_IS_ZERO(dd, noise, tiny)) {
+          dd = PIV_ZEROED(dd); ++c_tiny;
           if (lane == 0) zl_mask[threadIdx.x >> 5] |= (noise ? 1ull : 1ull << 32) << t;
         }
-        else {
-          // static pivoting: a pivot that fails the threshold test everywhere in its supernode is lifted to the
-          // threshold (|l_ij| stays <= 1e8; the factors are those of a matrix perturbed by <= 1e-8 |column|,
-          // which the caller's iterative refinement absorbs).  Counted and reported in num_forced.
-          dd = copysign(fmax(fabs(dd), 1e-8 * colmax_f), dd);
-          ++c_forced;
-        }
+        else { dd = PIV_LIFTED(dd, colmax_f); ++c_forced; }
       }
       const double c0v = a[0];
       const double rinv = 1.0 / dd;
@@ -594,7 +592,7 @@ __device__ void warp_ldlt32(double (&a)[32], double (&b)[32], const int f, const
       if (lane == t) { my_order = g0; my_pt = 2; my_dinv = pc2 * idet; my_doff = -pb * idet; }
       if (lane == t + 1) { my_order = r; my_pt = 3; my_dinv = pa * idet; my_doff = 0.0; }
       ++c_2x2;
-      if (det < 0.0) c_neg += 1; else if (pa < 0.0) c_neg += 2;
+      PIV_COUNT_NEG2X2(c_neg, det, pa);
       alive &= ~((1u << g0) | (1u << r)); cand &= ~((1u << g0) | (1u << r));
 #pragma unroll
       for (int c = 0; c < 30; ++c) a[c] = a[c + 2];
@@ -610,12 +608,7 @@ __device__ void warp_ldlt32(double (&a)[32], double (&b)[32], const int f, const
     ++progress;
   }
   if (lane < k) { order[lane] = my_order; pt[lane] = my_pt; dinv_s[lane] = my_dinv; doff_s[lane] = my_doff; }
-  if (lane == 0) {
-    if (c_neg) atomicAdd(counters + CNT_NEG, c_neg);
-    if (c_forced) atomicAdd(counters + CNT_FORCED, c_forced);
-    if (c_tiny) atomicAdd(counters + CNT_TINY, c_tiny);
-    if (c_2x2) atomicAdd(counters + CNT_2X2, c_2x2);
-  }
+  if (lane == 0) PIV_FLUSH(counters, c_neg, c_forced, c_tiny, c_2x2);
   __syncwarp();
 }
 
@@ -1037,8 +1030,7 @@ __device__ __forceinline__ double fast_rcp(const double d) {
 // --------------------------------------------------------------------------------------------
 // cta_ldlt32s: pivoted LDL^T of a symmetric block of order f <= 32 (all f columns are candidates) by FOUR warps -- the
 // diagonal blocks of the big fronts are the serial chain of the factorisation, so what counts is the latency of ONE pivot
-// step.  Same pivoting rules as warp_ldlt32 (Bunch-Kaufman 1x1 / 2x2 with the threshold test against the whole front
-// column, failed columns retried after the others, forced pivots at the end), organised as follows:
+// step.  Pivot rule: the PIV_* tests (failed columns retried after the others, forced pivots at the end), as follows:
 //   * the block lives in shared memory As[c * 33 + i] = A[i][c] (full symmetric storage) NEXT to the owners' registers
 //     (warp w: columns 8w..8w+7, lane = row): after every update the owners store their live columns back, so any
 //     column -- the candidate AND a 2x2 partner -- is one conflict-free shared-memory read away: ONE barrier per pivot
@@ -1125,13 +1117,13 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
     bool ok1 = false;
     if (!no_1x1) {
       if (r >= 0) lam = fabs(cA[r]);                   // exact magnitude of the selected entry
-      ok1 = (ajj > tiny) && (ajj >= u * fmax(lam, gam));
+      ok1 = PIV_OK1(ajj, lam, gam, u, tiny);
       const double colmax_f = fmax(lam, gam);
       if (forced) {
         double dd = pa0;
-        const bool noise = !(fmax(ajj, colmax_f) > 1e-12);
-        if (noise || !(fabs(dd) > tiny)) { dd = (dd < 0.0) ? -1.5e-8 : 1.5e-8; zmask |= (noise ? 1ull : 1ull << 32) << t; }
-        else { dd = copysign(fmax(fabs(dd), 1e-8 * colmax_f), dd); ++c_forced; }
+        const bool noise = PIV_IS_NOISE(fmax(ajj, colmax_f));
+        if (PIV_IS_ZERO(dd, noise, tiny)) { dd = PIV_ZEROED(dd); zmask |= (noise ? 1ull : 1ull << 32) << t; }
+        else { dd = PIV_LIFTED(dd, colmax_f); ++c_forced; }
         apply1(a0, dd, 1.0 / dd, g0, pr0);
         continue;
       }
@@ -1140,7 +1132,7 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
         else parked |= 1u << g0;
         continue;
       }
-      if (ok1 && ajj >= BK_ALPHA * lam) { apply1(a0, pa0, rinv0, g0, pr0); continue; }
+      if (PIV_1X1_J(ok1, ajj, lam)) { apply1(a0, pa0, rinv0, g0, pr0); continue; }
     }
     // ---- second column: the arg-max partner r ----
     const double* __restrict__ cB = As + r * 33;
@@ -1173,15 +1165,14 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
     }
     if (!take22) {
       // exact sequence (identical decisions; reached when a float bound was inconclusive)
-      if (no_1x1) { lam = fabs(pb); ok1 = (ajj > tiny) && (ajj >= u * fmax(lam, gam)); }
+      if (no_1x1) { lam = fabs(pb); ok1 = PIV_OK1(ajj, lam, gam, u, tiny); }
       const double sig = (double)sigf;
       const double cjm = (double)cjf, cr = (double)crf;
       // Of the two columns read in this step one stays alive when the pivot is 1x1 (on g0 or on r) and is then rewritten
       // by its owner: in those two branches every warp must have finished reading before any store.
-      if (ok1 && ajj * sig >= BK_ALPHA * lam * lam) { __syncthreads(); apply1(a0, pa0, rinv0, g0, pr0); continue; }
-      if (arr > tiny && arr >= BK_ALPHA * sig && arr >= u * fmax(sig, ge_r)) { __syncthreads(); apply1(a1, crr, 1.0 / crr, r, pr1); continue; }   // 1x1 on r
-      take22 = lam > tiny && adet > 0.0 && isfinite(adet) &&
-               (arr * cjm + fabs(pb) * cr) * u <= adet && (ajj * cr + fabs(pb) * cjm) * u <= adet;
+      if (PIV_1X1_J_SIG(ok1, ajj, lam, sig)) { __syncthreads(); apply1(a0, pa0, rinv0, g0, pr0); continue; }
+      if (PIV_1X1_R(arr, sig, ge_r, u, tiny)) { __syncthreads(); apply1(a1, crr, 1.0 / crr, r, pr1); continue; }   // 1x1 on r
+      take22 = PIV_2X2(lam, adet, ajj, fabs(pb), arr, cjm, cr, u, tiny);
     }
     if (take22) {
       const double l1 = other ? n1 * idet : 0.0;
@@ -1199,7 +1190,7 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
         if (lane == t + 1) { my_order = r; my_pt = 3; my_dinv = pa0 * idet; my_doff = 0.0; }
       }
       ++c_2x2;
-      if (det < 0.0) c_neg += 1; else if (pa0 < 0.0) c_neg += 2;
+      PIV_COUNT_NEG2X2(c_neg, det, pa0);
       t += 2;
       ++progress;
       continue;
@@ -1208,12 +1199,7 @@ __device__ void cta_ldlt32s(double (&a)[8], const int f, const double u, const d
   }
   if (w == 0) {
     if (lane < f) { order[lane] = my_order; pt[lane] = my_pt; dinv_s[lane] = my_dinv; doff_s[lane] = my_doff; }
-    if (lane == 0) {
-      if (c_neg) atomicAdd(counters + CNT_NEG, c_neg);
-      if (c_forced) atomicAdd(counters + CNT_FORCED, c_forced);
-      if (zmask) atomicAdd(counters + CNT_TINY, __popcll(zmask));
-      if (c_2x2) atomicAdd(counters + CNT_2X2, c_2x2);
-    }
+    if (lane == 0) PIV_FLUSH(counters, c_neg, c_forced, __popcll(zmask), c_2x2);
   }
   __syncthreads();
   if (zmask && threadIdx.x == 0) zl_append(counters, zlist, zl_pos0[0], zmask, dinv_s);

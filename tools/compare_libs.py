@@ -1,16 +1,20 @@
 """Bit-for-bit comparison of two builds of libb200ldlt.so on the same seeded systems: every output array of every call
-that reads the factors, and every launch count.  Meant for changes that must not change a bit (refactors of the host
-code): build the other library into a directory of its own, then
+that reads the factors, every launch count and the pivoting counters of every factorisation.  Meant for changes that
+must not change a bit: refactors of the host code, and of the factor kernels, whose every front class (B200_NO_WARP2=1
+sends the fronts of order 33..64 through the shared-memory kernel) and forced-pivot path (lifted pivots, zero pivots,
+lifted zeros) is dumped.  Build the other library into a directory of its own, then
 
   python tools/compare_libs.py dump <libb200ldlt.so> <out.json>    (one process per library: one CUDA context each)
   python tools/compare_libs.py compare <a.json> <b.json>           (exit 1 on any difference)
 
-The dump holds the SHA-256 of the bytes of each array (the full arrays run to gigabytes) and the launch counts.
+The dump holds the SHA-256 of the bytes of each array (the full arrays run to gigabytes), the launch counts, and after
+every factorisation num_neg, num_forced, num_tiny, num_2x2 and num_growth.
 
-What is dumped, per system (seeded generators and the golden systems of tests/golden):
-  * factor with use_graph 1 (and its replay), use_graph 0, B200_ONE_STREAM=1, B200_SOLVE_BLOCK=1, B200_SOLVE_BLOCK=3
-    and B200_SOLVE_DIRECT=0: status, inertia, launches_factor, D^-1 (enquire_indef) and host solves of 1, 8 and 13
-    columns with launches_solve;
+What is dumped, per system (seeded generators, the golden systems of tests/golden and a tridiagonal whose pivots are
+lifted):
+  * factor with use_graph 1 (and its replay), use_graph 0, B200_ONE_STREAM=1, B200_SOLVE_BLOCK=1, B200_SOLVE_BLOCK=3,
+    B200_SOLVE_DIRECT=0 and B200_NO_WARP2=1: status, inertia, launches_factor, D^-1 (enquire_indef) and host solves of
+    1, 8 and 13 columns with launches_solve;
   * on the use_graph 1 handle: device solves of 1, 8 and 13 columns, jobs 1..4 (host 1 and 13 columns, device 8),
     lmultiply (trans 0 / 1, host 1 and 13, device 8), selected inversion, solve_refine_device, the Fredholm solve
     without zero pivots, the error analysis (host 1 and 13 columns with and without the condition estimate, device 8)
@@ -20,7 +24,11 @@ What is dumped, per system (seeded generators and the golden systems of tests/go
     the first and last variable -- different trees on the two-component system --, and a block of 20 x 20 entries,
     wider than the blocked-solve width); the sparse solve with 1 and 13 columns (sparse b with a selection, dense b with
     a selection, sparse b with every entry, both NULL);
-  * the Fredholm solve on kept singular factors, blocked and with B200_SOLVE_BLOCK=1 (host 1, 5 and 13 columns, device 5);
+  * the Fredholm solve on kept singular factors, blocked, with B200_SOLVE_BLOCK=1 and with B200_NO_WARP2=1 (host 1, 5
+    and 13 columns, device 5);
+  * the duplicated-constraint systems of tests/test_fredholm.py in keep mode, both orderings, default and
+    B200_NO_WARP2=1: status, last_error, the counters and the zero pivots where the factors are kept (a "lifted zero"
+    keeps none);
   * Schur mode with the root in each solve class: S_c, reduce and expand (host 1 and 11 columns, device 8);
   * the sharded factor and solve with 2 and 4 ranks emulated on one GPU, on two matrices.
 Needs a GPU, torch and the test helpers in tests/."""
@@ -33,6 +41,7 @@ import sys
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+COUNTERS = ("num_neg", "num_forced", "num_tiny", "num_2x2", "num_growth")
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
@@ -52,6 +61,19 @@ def env(**kw):
                 os.environ[k] = v
 
 
+def lifted_tridiagonal(n=2000):
+    """the system of tests/test_error_analysis.py::test_lifted_pivots_give_finite_estimates: a tiny diagonal under a unit
+    off-diagonal, whose factorisation lifts pivots (num_forced > 0)"""
+    irn = np.concatenate([np.arange(1, n + 1), np.arange(2, n + 1)]).astype(np.int32)
+    jcn = np.concatenate([np.arange(1, n + 1), np.arange(1, n)]).astype(np.int32)
+    val = np.concatenate([1e-10 * (1 + np.arange(n) % 3), np.ones(n - 1)])
+    return n, irn, jcn, val
+
+
+# (nx, nc, seed) of the duplicated-constraint systems (dup_kkt) of tests/test_fredholm.py::test_dependent_rows
+DEPENDENT_ROWS = [(40, 12, 0), (120, 40, 1), (300, 100, 2)]
+
+
 def dump(lib, out):
     import ipopt_b200.capi as capi
     capi.lib_path = lambda: os.path.abspath(lib)
@@ -60,7 +82,7 @@ def dump(lib, out):
     from ipopt_b200.kkt import mbndry_kkt
     from ipopt_b200.sharded import ShardedLdlt
     from test_partial_solve import LARGE, SYSTEMS
-    from test_fredholm import zeroed
+    from test_fredholm import dup_kkt, zeroed
     from test_inverse_entries import two_components
     from test_schur import dense, pick_vars
 
@@ -93,6 +115,8 @@ def dump(lib, out):
         st, neg = s.factor(False, 0)
         put(key + "/factor", np.array([st, neg]))
         launches(s, key + "/factor")
+        inf = s.info()
+        rec[key + "/factor#counters"] = [inf[k] for k in COUNTERS]
         return st
 
     def host_solves(s, key, dim, rng, widths=(1, 8, 13)):
@@ -211,11 +235,13 @@ def dump(lib, out):
     systems["mbndry400"] = LARGE
     systems["mbndry60"] = lambda: mbndry_kkt(60, sigma_spread=3.0, seed=9)[:4]
     systems["forest"] = two_components
+    systems["lifted"] = lifted_tridiagonal
     for name, make in systems.items():
         dim, irn, jcn, val = make()
         for tag, opts, sw in (("graph", {}, {}), ("nograph", {"use_graph": 0}, {}),
                               ("onestream", {}, {"B200_ONE_STREAM": "1"}), ("block1", {}, {"B200_SOLVE_BLOCK": "1"}),
-                              ("block3", {}, {"B200_SOLVE_BLOCK": "3"}), ("direct0", {}, {"B200_SOLVE_DIRECT": "0"})):
+                              ("block3", {}, {"B200_SOLVE_BLOCK": "3"}), ("direct0", {}, {"B200_SOLVE_DIRECT": "0"}),
+                              ("nowarp2", {}, {"B200_NO_WARP2": "1"})):
             key = "%s/%s" % (name, tag)
             with env(**sw):
                 s = handle(dim, irn, jcn, val, **opts)
@@ -233,7 +259,7 @@ def dump(lib, out):
 
     for system, k in (("random", 1), ("random", 3), ("mbndry400", 3)):
         dim, irn, jcn, val, rows = zeroed(system, k)
-        for tag, sw in (("blocked", {}), ("block1", {"B200_SOLVE_BLOCK": "1"})):
+        for tag, sw in (("blocked", {}), ("block1", {"B200_SOLVE_BLOCK": "1"}), ("nowarp2", {"B200_NO_WARP2": "1"})):
             key = "fred/%s_%d/%s" % (system, k, tag)
             with env(**sw):
                 s = handle(dim, irn, jcn, val, keep=1)
@@ -251,6 +277,21 @@ def dump(lib, out):
                 host_solves(s, key, dim, rng, (1, 8))
                 s.close()
         print("dumped fredholm", system, flush=True)
+
+    for nx, nc, seed in DEPENDENT_ROWS:
+        dim, irn, jcn, val, _ = dup_kkt(nx, nc, seed)
+        for ordering in (0, 1):
+            for tag, sw in (("default", {}), ("nowarp2", {"B200_NO_WARP2": "1"})):
+                key = "dependent/%d_%d_%d/o%d/%s" % (nx, nc, seed, ordering, tag)
+                with env(**sw):
+                    s = handle(dim, irn, jcn, val, keep=1, ordering=ordering)
+                    factor(s, key)
+                    err = s.last_error()
+                    rec[key + "/last_error"] = err
+                    if "no factors" not in err:
+                        put(key + "/zpos", s.enquire_zero_pivots())
+                    s.close()
+    print("dumped dependent rows", flush=True)
 
     for system, m in (("random", 20), ("random", 64), ("random_300_100", 150), ("random", 300)):
         dim, irn, jcn, val, A = dense(system)
@@ -305,8 +346,16 @@ def compare(a, b):
         B = json.load(f)
     bad = sorted(k for k in set(A) | set(B) if A.get(k) != B.get(k))
     n = sum(1 for k in A if k.endswith("#launches"))
-    print("%d entries (%d arrays, %d launch counts) compared, %d differ%s" % (
-        len(set(A) | set(B)), len(A) - n, n, len(bad), "" if not bad else ": " + ", ".join(bad[:20])))
+    c = sum(1 for k in A if k.endswith("#counters"))
+    print("%d entries (%d launch counts, %d factorisations' counters) compared, %d differ%s" % (
+        len(set(A) | set(B)), n, c, len(bad), "" if not bad else ": " + ", ".join(bad[:20])))
+
+    def nonzero(field, nowarp2):
+        i = COUNTERS.index(field)
+        return sum(1 for k, v in A.items() if k.endswith("#counters") and v[i] > 0 and ("/nowarp2/" in k) == nowarp2)
+    print("factorisations with num_forced > 0: %d default, %d B200_NO_WARP2=1; with num_tiny > 0: %d default, %d "
+          "B200_NO_WARP2=1" % (nonzero("num_forced", False), nonzero("num_forced", True), nonzero("num_tiny", False),
+                               nonzero("num_tiny", True)))
     return 1 if bad else 0
 
 
