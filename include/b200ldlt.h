@@ -471,6 +471,82 @@ int b200ldlt_solve_refined(b200ldlt_handle h, int nrhs, const double* b, double*
 int b200ldlt_solve_refined_device(b200ldlt_handle h, int nrhs, const double* d_b, double* d_x, int max_steps,
                                   double tol, b200ldlt_refined* out);
 
+/* ---- FGMRES preconditioned by the factors (cf. Arioli, Duff, Gratton and Pralet, SIAM J. Sci. Comput. 29 (2007);
+ * Carson and Higham's GMRES-IR; Pardiso iparm(4)) -----------------------------------------------------------------------
+ * Solves A_op x = b for nrhs columns by restarted, right-preconditioned flexible GMRES with M = job 0 as preconditioner,
+ * stopped by the componentwise backward error as b200ldlt_solve_refined stops.  M A_op = I + M (A_op - A_M), A_M the
+ * matrix job 0 inverts: with lifted pivots (info.num_forced > 0) or an altered D the difference has low rank, and with
+ * other values it is what the new values change, so GMRES converges where classical refinement (x <- x + M r, which
+ * needs the spectral radius of I - M A_op below 1) stagnates or diverges.
+ *   A_op   vals: nonzeros doubles in the triplet order given to b200ldlt_analyse, duplicates summed in triplet order as
+ *          the factorisation sums them (0.0 + v_0 + v_1 ...); vals == NULL is the matrix of the last factor call, bit for
+ *          bit the same as passing its values.  vals is in the memory of its entry point: host memory for
+ *          b200ldlt_solve_gmres (staged with b), device memory for _device.  A_op is not kept: the factors, the values
+ *          b200ldlt_refactor reuses and every other call are unaffected.
+ *   M      job 0's operator, as in the selected-inversion and error-analysis blocks above.
+ *   Omega: omega1, omega2, I1, I2, s, a_i, tau_i and the weights are those of b200ldlt_error_analysis with A := A_op;
+ *          r = b - A_op x is the double-double residual of b200ldlt_solve_refined, in its order.
+ *   Iterates: x_0 = job 0 on b (bit-identical to b200ldlt_solve).  The stopping rule of b200ldlt_solve_refined is applied
+ *          to each iterate x_k = x_0, x_1, ... exactly as stated there, with max_cycles in place of max_steps (status 0
+ *          converged, 1 stagnated with x_k or x_{k-1}, 2 max_cycles, 3 non-finite omega).  When the column goes on, one
+ *          restart cycle runs on A_op d = r_k (r_k the residual of the rule's iterate):
+ *            beta^2 = <r_k, r_k>, beta = sqrt(beta^2), v_0 = r_k (/) beta (per entry), g_0 = beta;
+ *            per step j = 0, 1, ...: z_j = job 0 on v_j (kept); w = A_op z_j (row i: lane l of a warp takes the row's
+ *              entries l, l + 32, ... of |A|'s row structure in order, t = t (+) (a_ij (*) z_j) from t = 0, then for
+ *              o = 16, 8, 4, 2, 1: t = t (+) t' of lane l xor o; w_i = lane 0's t);
+ *              CGS2: h1_q = <v_q, w> (q = 0..j), w_i = w_i (-) (h1_q (*) v_q,i) for q = 0..j in order;
+ *                    h2_q = <v_q, w> with that w, w_i = w_i (-) (h2_q (*) v_q,i) likewise;
+ *              h_q,j = h1_q (+) h2_q (q <= j), h_{j+1,j} = sqrt(<w, w>), v_{j+1} = w (/) h_{j+1,j} (per entry);
+ *            <a, b> is the fixed sum over P = min(ceil(n / 256), 264) CTAs of 256 threads: thread t of CTA p adds
+ *              a_i (*) b_i for i = 256 p + t, + 256 P, ... in order from 0.0; each warp a shuffle-xor tree (o = 16 .. 1,
+ *              t = t (+) t'); the CTA's 8 warps in order (t = w_0, t = t (+) w_k); the CTAs' partials in order from 0.0.
+ *            The host then rotates the column (every operation one rounded double operation, no FMA, no hypot):
+ *              for i < j with the earlier rotations (c_i, s_i): t = c_i h_i + s_i h_{i+1}, h_{i+1} = c_i h_{i+1} - s_i h_i,
+ *              h_i = t;  rho = sqrt(h_j h_j + h_{j+1} h_{j+1}), c_j = h_j / rho, s_j = h_{j+1} / rho, R_ij = h_i (i < j),
+ *              R_jj = rho;  g_{j+1} = -(s_j g_j), g_j = c_j g_j.
+ *            A step in which any h_{i,j} (i <= j + 1) or rho is not finite, or rho = 0, is a breakdown that is dropped:
+ *              the cycle ends with the steps before it.  Otherwise the step is kept, and the cycle ends after it when
+ *              h_{j+1,j} = 0 (a breakdown that is kept), |g_{j+1}| <= inner_tol (*) beta, or j + 1 = restart.  A beta that
+ *              is 0 or not finite (|r| beyond the range of its square) ends the cycle before its first step.
+ *            With m steps kept: y_i = (g_i (-) sum_{l = i+1}^{m-1} R_il y_l) (/) R_ii for i = m - 1 down to 0, the sum
+ *              subtracted term by term in ascending l;  d_i = 0 (+) y_0 z_0,i (+) ... (+) y_{m-1} z_{m-1},i in order,
+ *              each product rounded;  x_{k+1} = x_k (+) d, x_k kept for the rule's rollback.
+ *          So the returned omega never exceeds omega_first, and max_cycles = 0 returns job 0 with its omega.  In exact
+ *          arithmetic a cycle with M A_op = I + (rank k) ends within k + 1 steps.
+ *   Blocks: columns run in blocks of up to B200_SOLVE_BLOCK (8 by default) in lockstep by cycle and by Arnoldi step; each
+ *          iterate and each step works on the block's columns still active, packed into consecutive solve slots, as
+ *          b200ldlt_solve_refined packs them.  Every column's x and struct are bit-identical to a call on that column
+ *          alone, under any B200_SOLVE_BLOCK, between the two entry points and across calls.
+ * Kernel launches, with L0 = job 0's launches per block (4 + 2 D, 8 by default): 1 (the unique values of A_op) + per
+ * block L0 (x_0) + 3 E (per iterate: the row pass, the row classes and beta^2) + 2 (E - 1) (per cycle: v_0 and the
+ * update of x) + (L0 + 6) T (per Arnoldi step: job 0, the product with A_op, two dot and two update kernels, and the
+ * normalisation), where E is the largest nres of the block's columns and T the sum over the block's cycles of the most
+ * steps a column of the block took in that cycle.  One column: 1 + L0 + 5 nres - 2 + (L0 + 6) iters.  The call
+ * synchronises once per iterate (one D2H of the maxima and beta^2) and once per Arnoldi step (one D2H of the Hessenberg
+ * columns for the host's rotations and stopping decisions).
+ * Memory: that of b200ldlt_solve_refined for the block width, plus V (restart + 1 vectors) and Z (restart vectors) per
+ * column of the block, (2 restart + 1) 8 n bytes, and about 1.1 MB of reduction scratch; grown to the largest call and
+ * freed by the next analysis.  A failed allocation is a refusal with a message.  The host entry point stages
+ * 2 n nrhs doubles (x and a copy of b), plus nonzeros doubles when vals is given.
+ * b and x are n x nrhs, column-major; b and vals are not modified and x may not be b; out is nrhs structs in host memory
+ * for both entry points.  Timing (info.ms_solve_gpu, launches_solve) and refusals follow the solve family: no factors, a
+ * sharded handle, Schur mode; and nrhs < 0, restart < 1 or > 64, max_cycles < 0, tol or inner_tol < 0 or NaN, a NULL
+ * b, x or out with nrhs > 0, x == b.  Nothing is written on a refusal; nrhs = 0 is the no-columns case.  With kept
+ * singular factors the call runs and obeys the rule.  The call leaves the factors, D, the device values of the last
+ * factor call, later solves and the results of b200ldlt_error_analysis and b200ldlt_solve_refined as they were. */
+typedef struct b200ldlt_gmres {
+  double omega_first;    /* omega1 + omega2 of x_0 (job 0 on b) against A_op                                        */
+  double omega1, omega2; /* of the returned x                                                                        */
+  int cycles;            /* corrections (restart cycles) contained in the returned x                                 */
+  int iters;             /* Arnoldi steps (job-0 applications after x_0) the column took, rolled-back cycle included */
+  int status;            /* as b200ldlt_refined: 0 converged, 1 stagnated, 2 max_cycles, 3 non-finite omega          */
+  int nres;              /* residuals evaluated (cycles + 1, or cycles + 2 after a rollback)                         */
+} b200ldlt_gmres;
+int b200ldlt_solve_gmres(b200ldlt_handle h, int nrhs, const double* b, double* x, const double* vals, int restart,
+                         int max_cycles, double tol, double inner_tol, b200ldlt_gmres* out);
+int b200ldlt_solve_gmres_device(b200ldlt_handle h, int nrhs, const double* d_b, double* d_x, const double* d_vals,
+                                int restart, int max_cycles, double tol, double inner_tol, b200ldlt_gmres* out);
+
 /* <-> NumberOfNegEVals() (hpp:207) */
 int b200ldlt_num_neg(b200ldlt_handle h);
 /* <-> IncreaseQuality() (hpp:220): pivtol <- min(pivtolmax, pivtol^0.75); returns 0 if already at max.

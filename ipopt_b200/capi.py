@@ -63,6 +63,12 @@ class Refined(C.Structure):
                 ("status", C.c_int), ("nres", C.c_int)]
 
 
+class Gmres(C.Structure):
+    """b200ldlt_gmres: the outcome of FGMRES on one column (see include/b200ldlt.h)"""
+    _fields_ = [("omega_first", C.c_double), ("omega1", C.c_double), ("omega2", C.c_double), ("cycles", C.c_int),
+                ("iters", C.c_int), ("status", C.c_int), ("nres", C.c_int)]
+
+
 EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "b200ldlt_last_error",
             "b200ldlt_analyse", "b200ldlt_values_ptr", "b200ldlt_factor", "b200ldlt_factor_device",
             "b200ldlt_solve", "b200ldlt_solve_device", "b200ldlt_num_neg", "b200ldlt_increase_quality",
@@ -78,7 +84,8 @@ EXPORTED = ["b200ldlt_default_options", "b200ldlt_create", "b200ldlt_destroy", "
             "b200ldlt_schur_reduce_device", "b200ldlt_schur_expand", "b200ldlt_schur_expand_device",
             "b200ldlt_error_analysis", "b200ldlt_error_analysis_device", "b200ldlt_condest",
             "b200ldlt_inverse_entries", "b200ldlt_inverse_entries_device", "b200ldlt_solve_refined",
-            "b200ldlt_solve_refined_device", "b200ldlt_sparse_solve", "b200ldlt_sparse_solve_device"]
+            "b200ldlt_solve_refined_device", "b200ldlt_sparse_solve", "b200ldlt_sparse_solve_device",
+            "b200ldlt_solve_gmres", "b200ldlt_solve_gmres_device"]
 
 _lib = None
 
@@ -143,6 +150,10 @@ def load_library():
     L.b200ldlt_condest.argtypes = [vp, dp, dp, dp, ip]
     L.b200ldlt_solve_refined.argtypes = [vp, C.c_int, dp, dp, C.c_int, C.c_double, C.POINTER(Refined)]
     L.b200ldlt_solve_refined_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_double, C.POINTER(Refined)]
+    L.b200ldlt_solve_gmres.argtypes = [vp, C.c_int, dp, dp, dp, C.c_int, C.c_int, C.c_double, C.c_double,
+                                       C.POINTER(Gmres)]
+    L.b200ldlt_solve_gmres_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_double, C.c_double,
+                                              C.POINTER(Gmres)]
     L.b200ldlt_num_neg.argtypes = [vp]
     L.b200ldlt_increase_quality.argtypes = [vp]
     L.b200ldlt_get_info.argtypes = [vp, C.POINTER(Info)]
@@ -566,6 +577,43 @@ class B200Ldlt:
         st = self._L.b200ldlt_solve_refined_device(self._h, int(nrhs), C.c_void_p(d_b_ptr), C.c_void_p(d_x_ptr),
                                                    int(max_steps), float(tol), out)
         return st, self._refined_dict(out[:int(nrhs)])
+
+    # Defaults from tools/bench_gmres.py (DESIGN section 7 item 16): inner_tol 1e-10 was the fastest or tied on every
+    # system measured -- 1e-6 made the shifted systems take a second cycle, 1e-14 added a step everywhere; restart 20 was
+    # never reached there and bounds V and Z at 41 vectors per column of a block.
+    @staticmethod
+    def _gmres_dict(out):
+        return {k: np.array([getattr(o, k) for o in out], dtype=np.int32 if t is C.c_int else np.float64)
+                for k, t in Gmres._fields_}
+
+    def solve_gmres(self, B, vals=None, restart=20, max_cycles=10, tol=2.0 ** -52, inner_tol=1e-10):
+        """Solve A_op X = B (dim or dim x nrhs) by FGMRES preconditioned by the factors, stopped like solve_refined
+        (b200ldlt_solve_gmres).  vals: the nonzeros values of A_op in triplet order (None: the factored matrix).
+        Returns (X, dict of per-column arrays: omega_first, omega1, omega2, cycles, iters, status, nres).  Raises on a
+        refusal."""
+        B = np.asarray(B, dtype=np.float64)
+        Bm = np.asfortranarray(B.reshape(self.dim, -1, order="F"))
+        nrhs = Bm.shape[1]
+        X = np.zeros_like(Bm, order="F")
+        pv = None
+        if vals is not None:
+            vals = np.ascontiguousarray(vals, dtype=np.float64)
+            pv = _dptr(vals)
+        out = (Gmres * max(nrhs, 1))()
+        if self._L.b200ldlt_solve_gmres(self._h, nrhs, _dptr(Bm), _dptr(X), pv, int(restart), int(max_cycles),
+                                        float(tol), float(inner_tol), out) != SYMSOLVER_SUCCESS:
+            raise RuntimeError(self.last_error())
+        return X.reshape(B.shape, order="F"), self._gmres_dict(out[:nrhs])
+
+    def solve_gmres_device(self, d_b_ptr, d_x_ptr, nrhs=1, d_vals_ptr=None, restart=20, max_cycles=10,
+                           tol=2.0 ** -52, inner_tol=1e-10):
+        """The same on device arrays of dim x nrhs doubles (x written) and, if given, nonzeros device values.  Returns
+        (status, dict of per-column arrays)."""
+        out = (Gmres * max(int(nrhs), 1))()
+        st = self._L.b200ldlt_solve_gmres_device(self._h, int(nrhs), C.c_void_p(d_b_ptr), C.c_void_p(d_x_ptr),
+                                                 C.c_void_p(d_vals_ptr) if d_vals_ptr else None, int(restart),
+                                                 int(max_cycles), float(tol), float(inner_tol), out)
+        return st, self._gmres_dict(out[:int(nrhs)])
 
     def condest(self):
         """(kappa1, anorm1, ainv1, nprod): the 1-norm condition estimate ||A||_1 est||M||_1 (b200ldlt_condest).  Raises

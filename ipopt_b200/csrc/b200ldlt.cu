@@ -24,6 +24,7 @@
 #include "selinv_kernels.cu"
 #include "sc_kernels.cu"
 #include "ea_kernels.cu"
+#include "gmres_kernels.cu"
 #include "symbolic.hpp"
 
 namespace b200 {
@@ -181,11 +182,14 @@ struct SelInvPlan {
 // right-hand side r and s, overwritten by w1 and w2, and the reduced norms (grown to the largest call); the estimators'
 // input / product vectors and sign vectors (one column per estimator of a block) and the reduction scratch of
 // k_ea_post; for the refinement (b200ldlt_solve_refined) the solve slots of a block (r, then d) and the rollback copies
-// of its x.  Built at the first call after an analysis, before its timing starts; a handle that never makes the calls
-// allocates none of it.
+// of its x; for FGMRES (b200ldlt_solve_gmres) the Krylov vectors V and Z of each column of a block (grown to the largest
+// call), its Hessenberg columns, y, and the reduction scratch of the dots and norms.  Built at the first call after an
+// analysis, before its timing starts; a handle that never makes the calls allocates none of it.
 struct EaPlan {
   DevBuf<int> d_ptr, d_col, d_uid;
   DevBuf<double> d_uval, d_amax, d_rs, d_v, d_rf_d, d_rf_old;
+  DevBuf<double> d_gm_kv, d_gm_h, d_gm_y, d_gm_part;
+  DevBuf<unsigned> d_gm_cnt;
   DevBuf<unsigned long long> d_nrm;
   DevBuf<signed char> d_xi;
   DevBuf<EaPart> d_part;
@@ -3286,6 +3290,226 @@ static int solve_refined(Solver* sv, int nrhs, const double* b, double* x, int m
   return B200LDLT_SUCCESS;
 }
 
+// ---- FGMRES preconditioned by the factors (b200ldlt_solve_gmres) -----------------------------------------------------
+// One column's cycle on the host: beta, g, the Givens rotations and the rotated Hessenberg columns (rr[j * GM_RESTART_MAX
+// + i] = row i of column j), the steps kept (m) and whether it still steps.  The arithmetic is the header's, one
+// rounded double operation per written operation (the x86-64 host build has no FMA to contract into).
+struct GmCol {
+  double beta = 0.0;
+  double cs[GM_RESTART_MAX], sn[GM_RESTART_MAX], g[GM_RESTART_MAX + 1];
+  std::vector<double> rr = std::vector<double>((size_t)GM_RESTART_MAX * GM_RESTART_MAX);
+  int m = 0, iters = 0;
+  bool on = false;
+};
+
+// Arnoldi step j of G with its Hessenberg column h[0 .. j + 1]: the rotations, the stopping decision and G.m
+static void gm_step(GmCol& G, double* h, int j, int restart, double inner_tol) {
+  ++G.iters;
+  for (int i = 0; i < j; ++i) {
+    const double t = G.cs[i] * h[i] + G.sn[i] * h[i + 1];
+    h[i + 1] = G.cs[i] * h[i + 1] - G.sn[i] * h[i];
+    h[i] = t;
+  }
+  const double a = h[j], b = h[j + 1];
+  const double rho = std::sqrt(a * a + b * b);
+  bool finite = std::isfinite(rho) && rho != 0.0;
+  for (int i = 0; i <= j + 1; ++i) finite = finite && std::isfinite(h[i]);
+  if (!finite) { G.on = false; return; }   // the step is dropped: G.m stays j
+  G.cs[j] = a / rho;
+  G.sn[j] = b / rho;
+  double* r = G.rr.data() + (size_t)j * GM_RESTART_MAX;
+  for (int i = 0; i < j; ++i) r[i] = h[i];
+  r[j] = rho;
+  G.g[j + 1] = -(G.sn[j] * G.g[j]);
+  G.g[j] = G.cs[j] * G.g[j];
+  G.m = j + 1;
+  G.on = !(b == 0.0 || std::fabs(G.g[j + 1]) <= inner_tol * G.beta || G.m == restart);
+}
+
+// y = R^-1 g over G's m kept steps, back substitution with the row's terms in ascending column order
+static void gm_solve(const GmCol& G, double* y) {
+  for (int i = G.m - 1; i >= 0; --i) {
+    double t = G.g[i];
+    for (int l = i + 1; l < G.m; ++l) t = t - G.rr[(size_t)l * GM_RESTART_MAX + i] * y[l];
+    y[i] = t / G.rr[(size_t)i * GM_RESTART_MAX + i];
+  }
+}
+
+// b200ldlt_solve_gmres (host == true: b, x and vals in host memory) / _device
+static int solve_gmres(Solver* sv, int nrhs, const double* b, double* x, const double* vals, int restart, int max_cycles,
+                       double tol, double inner_tol, b200ldlt_gmres* out, bool host) {
+  const char* bad = nrhs < 0 ? "nrhs must be >= 0" : restart < 1 || restart > GM_RESTART_MAX ? "restart must be 1..64"
+                    : max_cycles < 0 ? "max_cycles must be >= 0" : !(tol >= 0.0) ? "tol must be >= 0"
+                    : !(inner_tol >= 0.0) ? "inner_tol must be >= 0" : nrhs > 0 && (!b || !x || !out) ? "NULL argument"
+                    : nrhs > 0 && b == x ? "x must not be b" : nullptr;
+  if (bad) { sv->err = std::string("solve_gmres: ") + bad; return B200LDLT_FATAL_ERROR; }
+  { const int rc = factors_state(sv, "solve_gmres"); if (rc != B200LDLT_SUCCESS) return rc; }
+  if (nrhs == 0) return no_columns(sv);
+  Analysis& A = *sv->an;
+  const int n = sv->n;
+  const size_t nb = (size_t)n * nrhs, nv = (size_t)sv->nnz;
+  const bool blocked = nrhs > 1 && block_solve_state(sv);
+  SweepState& W = blocked ? *A.blk : A.sweep;
+  const int width = blocked ? W.width : 1;
+  { const int rc = ea_state(sv, width, 0); if (rc != B200LDLT_SUCCESS) return rc; }
+  EaPlan& P = *A.ea;
+  cudaStream_t st = sv->stream;
+  const int parts = ea_parts(n);
+  if (P.d_rf_d.n < (size_t)n * width) { CU(P.d_rf_d.alloc((size_t)n * width)); CU(P.d_rf_old.alloc((size_t)n * width)); }
+  if (!P.d_gm_h.n) {
+    CU(P.d_gm_h.alloc((size_t)MS_NB_MAX * GM_H));
+    CU(P.d_gm_y.alloc((size_t)MS_NB_MAX * GM_RESTART_MAX));
+    CU(P.d_gm_part.alloc((size_t)MS_NB_MAX * GM_Q * parts));
+    CU(P.d_gm_cnt.alloc((size_t)MS_NB_MAX * GM_Q));
+    CU(cudaMemsetAsync(P.d_gm_cnt.p, 0, (size_t)MS_NB_MAX * GM_Q * sizeof(unsigned), st));
+  }
+  const size_t kv = (size_t)(2 * restart + 1) * n;   // V (restart + 1 vectors) and Z (restart) of one column
+  if (P.d_gm_kv.n < kv * width && P.d_gm_kv.alloc(kv * width) != cudaSuccess) {
+    cudaGetLastError();
+    sv->err = "solve_gmres: cannot allocate the Krylov vectors (" + std::to_string(8.0 * kv * width / 1e6) + " MB)";
+    return B200LDLT_FATAL_ERROR;
+  }
+  double* const gkv = P.d_gm_kv.p;   // the Krylov vectors of column c at gkv + c gld, its Hessenberg column at ghb + c GM_H
+  double* const ghb = P.d_gm_h.p;
+  const long long gld = (long long)kv;
+  std::vector<RfCol> R(nrhs);
+  std::vector<int> iters(nrhs, 0);
+  std::vector<GmCol> G(width);
+  std::vector<double> hh((size_t)width * GM_H), yy((size_t)MS_NB_MAX * GM_RESTART_MAX);
+  std::vector<unsigned long long> nrm((size_t)EA_NRM * width + 1);
+  // x_held: d_x already holds b (the host staging); d_op: the caller's values of A_op, or the factored ones
+  auto enqueue = [&](const double* d_b, double* d_x, const double* d_op, bool x_held) -> int {
+    const long long nu = A.S.nnz_u;
+    k_sum_dups<<<cdiv(nu, 256), 256, 0, st>>>(nu, A.d_useg_ptr.p, A.d_useg_src.p, d_op, P.d_uval.p);
+    ++sv->launches;
+    const unsigned g = std::min<unsigned>(cdiv(n, EA_WARPS), EA_ROW_CTAS);
+    return for_blocks(nrhs, width, [&](int c0, int w) -> int {
+      const double* bb = d_b + (size_t)c0 * n;
+      double* xb = d_x + (size_t)c0 * n;
+      if (!x_held) CU(cudaMemcpyAsync(xb, bb, (size_t)n * w * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      { const int rc = enqueue_solve(sv, W, 0, xb, xb, w); if (rc != B200LDLT_SUCCESS) return rc; }
+      RfCols act;
+      int na = w;
+      for (int s = 0; s < w; ++s) act.c[s] = s;
+      for (int k = 0;; ++k) {
+        // r (double-double) of the unfinished columns into the slots, s, the omegas and beta^2 = ||r||^2; one D2H each
+        CU(cudaMemsetAsync(P.d_nrm.p, 0, ((size_t)EA_NRM * na + 1) * sizeof(unsigned long long), st));
+        k_ea_rows<true><<<dim3(g, na), EA_THREADS, 0, st>>>(n, na, P.d_ptr.p, P.d_col.p, P.d_uid.p, P.d_uval.p, bb, xb,
+                                                            P.d_rs.p, P.d_amax.p, P.d_nrm.p, act, P.d_rf_d.p);
+        k_ea_class<true><<<dim3(cdiv(n, EA_THREADS), na), EA_THREADS, 0, st>>>(n, bb, P.d_amax.p, P.d_rs.p, P.d_nrm.p, act,
+                                                                               P.d_rf_d.p);
+        GmSlots sl;   // the residuals in the solve slots
+        for (int s = 0; s < na; ++s) { sl.v[s] = s; sl.h[s] = act.c[s]; }
+        k_gm_update<true><<<dim3(parts, na), EA_THREADS, 0, st>>>(n, -1, 0, sl, P.d_rf_d.p, n, ghb, P.d_gm_part.p, P.d_gm_cnt.p);
+        sv->launches += 3;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(nrm.data(), P.d_nrm.p, (size_t)EA_NRM * na * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(hh.data(), P.d_gm_h.p, (size_t)GM_H * w * sizeof(double), cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        // the rule per column; a finished column that returns x_{k-1} gets it back, the others' r close up
+        RfCols next;
+        int nn = 0;
+        for (int s = 0; s < na; ++s) {
+          const int c = act.c[s];
+          const int v = rf_rule(R[c0 + c], ea_val(nrm[(size_t)EA_NRM * s + EA_W1]), ea_val(nrm[(size_t)EA_NRM * s + EA_W2]), k,
+                                max_cycles, tol);
+          if (v == 2)
+            CU(cudaMemcpyAsync(xb + (size_t)c * n, P.d_rf_old.p + (size_t)c * n, (size_t)n * sizeof(double),
+                               cudaMemcpyDeviceToDevice, st));
+          if (v != 0) continue;
+          if (nn != s)
+            CU(cudaMemcpyAsync(P.d_rf_d.p + (size_t)nn * n, P.d_rf_d.p + (size_t)s * n, (size_t)n * sizeof(double),
+                               cudaMemcpyDeviceToDevice, st));
+          next.c[nn++] = c;
+        }
+        if (nn == 0) return B200LDLT_SUCCESS;
+        // one cycle: v_0 = r / beta into the slots and V, then the Arnoldi steps of the columns still stepping in lockstep
+        int slot[MS_NB_MAX];
+        for (int s = 0; s < nn; ++s) {
+          const int c = next.c[s];
+          sl.v[s] = sl.h[s] = c;
+          GmCol& C = G[c];
+          C.beta = std::sqrt(hh[(size_t)GM_H * c + GM_Q - 1]);
+          C.g[0] = C.beta;
+          C.m = 0;
+          C.iters = 0;
+          C.on = std::isfinite(C.beta) && C.beta != 0.0;
+          slot[c] = s;
+        }
+        k_gm_scale<<<dim3(cdiv(n, EA_THREADS), nn), EA_THREADS, 0, st>>>(n, -1, 0, sl, gkv, gld, ghb, P.d_rf_d.p);
+        ++sv->launches;
+        CU(cudaGetLastError());
+        for (int j = 0;; ++j) {
+          GmSlots sa;
+          int on[MS_NB_MAX], ns = 0;
+          for (int s = 0; s < nn; ++s) {
+            const int c = next.c[s];
+            if (!G[c].on) continue;
+            if (slot[c] != ns)
+              CU(cudaMemcpyAsync(P.d_rf_d.p + (size_t)ns * n, P.d_rf_d.p + (size_t)slot[c] * n, (size_t)n * sizeof(double),
+                                 cudaMemcpyDeviceToDevice, st));
+            slot[c] = ns;
+            sa.v[ns] = sa.h[ns] = c;
+            on[ns++] = c;
+          }
+          if (ns == 0) break;
+          // z_j = job 0 on v_j, w = A_op z_j, CGS2 against v_0 .. v_j, ||w||, v_{j+1} = w / ||w||
+          { const int rc = enqueue_solve(sv, W, 0, P.d_rf_d.p, P.d_rf_d.p, ns); if (rc != B200LDLT_SUCCESS) return rc; }
+          k_gm_apply<<<dim3(g, ns), EA_THREADS, 0, st>>>(n, restart, j, P.d_ptr.p, P.d_col.p, P.d_uid.p, P.d_uval.p,
+                                                         P.d_rf_d.p, sa, gkv, gld, ghb);
+          for (int pass = 0; pass < 2; ++pass) {
+            k_gm_dot<<<dim3(parts, ns, j + 1), EA_THREADS, 0, st>>>(n, j, pass * GM_Q, sa, gkv, gld, ghb, P.d_gm_part.p, P.d_gm_cnt.p);
+            if (pass == 0) k_gm_update<false><<<dim3(parts, ns), EA_THREADS, 0, st>>>(n, j, 0, sa, gkv, gld, ghb, P.d_gm_part.p, P.d_gm_cnt.p);
+            else k_gm_update<true><<<dim3(parts, ns), EA_THREADS, 0, st>>>(n, j, GM_Q, sa, gkv, gld, ghb, P.d_gm_part.p, P.d_gm_cnt.p);
+          }
+          k_gm_scale<<<dim3(cdiv(n, EA_THREADS), ns), EA_THREADS, 0, st>>>(n, j, GM_Q, sa, gkv, gld, ghb, P.d_rf_d.p);
+          sv->launches += 6;
+          CU(cudaGetLastError());
+          CU(cudaMemcpyAsync(hh.data(), P.d_gm_h.p, (size_t)GM_H * w * sizeof(double), cudaMemcpyDeviceToHost, st));
+          CU(cudaStreamSynchronize(st));
+          for (int s = 0; s < ns; ++s) {
+            const double* hc = hh.data() + (size_t)GM_H * on[s];
+            double h[GM_RESTART_MAX + 1];
+            for (int i = 0; i <= j; ++i) h[i] = hc[i] + hc[GM_Q + i];
+            h[j + 1] = std::sqrt(hc[GM_Q + GM_Q - 1]);
+            gm_step(G[on[s]], h, j, restart, inner_tol);
+          }
+        }
+        // x_{k+1} = x_k (+) Z y, x_k kept for a rollback
+        GmFinal f;
+        for (int s = 0; s < nn; ++s) {
+          const int c = next.c[s];
+          f.c[s] = c;
+          f.m[s] = G[c].m;
+          iters[c0 + c] += G[c].iters;
+          gm_solve(G[c], yy.data() + (size_t)s * GM_RESTART_MAX);
+        }
+        CU(cudaMemcpyAsync(P.d_gm_y.p, yy.data(), (size_t)nn * GM_RESTART_MAX * sizeof(double), cudaMemcpyHostToDevice, st));
+        k_gm_final<<<dim3(cdiv(n, EA_THREADS), nn), EA_THREADS, 0, st>>>(n, restart, sl, gkv, gld, ghb, f, P.d_gm_y.p, xb, P.d_rf_old.p);
+        ++sv->launches;
+        CU(cudaGetLastError());
+        act = next;
+        na = nn;
+      }
+    });
+  };
+  int rc;
+  if (host) {
+    // the staging holds x (b on entry, the solution on exit), the caller's values if any, then a copy of b
+    const size_t nin2 = vals ? nv : 0;
+    rc = staged_call(sv, b, nb, x, nb, [&](double* d) -> int {
+      CU(cudaMemcpyAsync(d + nb + nin2, d, nb * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      return enqueue(d + nb + nin2, d, vals ? d + nb : sv->d_vals.p, true);
+    }, 2 * nb + nin2, 0, vals, nin2);
+  } else {
+    rc = timed_call(sv, [&] { return enqueue(b, x, vals ? vals : sv->d_vals.p, false); });
+  }
+  if (rc != B200LDLT_SUCCESS) return rc;
+  for (int c = 0; c < nrhs; ++c)
+    out[c] = b200ldlt_gmres{R[c].first, R[c].om1, R[c].om2, R[c].steps, iters[c], R[c].status, R[c].nres};
+  return B200LDLT_SUCCESS;
+}
+
 // b200ldlt_condest: ||A||_1 from the row pass, est ||M||_1 by one estimator through the single-column state
 static int condest(Solver* sv, double* kappa1, double* anorm1, double* ainv1, int* nprod) {
   if (!kappa1) { sv->err = "condest: NULL kappa1"; return B200LDLT_FATAL_ERROR; }
@@ -3506,6 +3730,20 @@ int b200ldlt_solve_refined_device(b200ldlt_handle h, int nrhs, const double* d_b
   Solver* sv = (Solver*)h;
   if (!sv) return B200LDLT_FATAL_ERROR;
   return solve_refined(sv, nrhs, d_b, d_x, max_steps, tol, out, false);
+}
+
+int b200ldlt_solve_gmres(b200ldlt_handle h, int nrhs, const double* b, double* x, const double* vals, int restart,
+                         int max_cycles, double tol, double inner_tol, b200ldlt_gmres* out) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return solve_gmres(sv, nrhs, b, x, vals, restart, max_cycles, tol, inner_tol, out, true);
+}
+
+int b200ldlt_solve_gmres_device(b200ldlt_handle h, int nrhs, const double* d_b, double* d_x, const double* d_vals,
+                                int restart, int max_cycles, double tol, double inner_tol, b200ldlt_gmres* out) {
+  Solver* sv = (Solver*)h;
+  if (!sv) return B200LDLT_FATAL_ERROR;
+  return solve_gmres(sv, nrhs, d_b, d_x, d_vals, restart, max_cycles, tol, inner_tol, out, false);
 }
 
 int b200ldlt_condest(b200ldlt_handle h, double* kappa1, double* anorm1, double* ainv1, int* nprod) {
